@@ -93,6 +93,11 @@ struct dsact_cnn_handle {
   dsact_replay rb;
   bool rb_bound = false;
   int64_t dev_rb_size = -1;
+  // what the last phase 1 ran on (phase 2 reads the same rows and noise)
+  int32_t pending_batch = 0;
+  dsact_batch pending = {};
+  const float *pending_eps1 = nullptr, *pending_z3 = nullptr, *pending_z4 = nullptr;
+  DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   int64_t total;
   float* Wp() const { return reinterpret_cast<float*>(buf.workspace); }
   void layout() {
@@ -364,6 +369,248 @@ static void cnn_conv_backward(dsact_cnn_handle* h, const CnnGeom& g, const float
   c.check();
 }
 
+// ---- the DSAC-T step in three phases --------------------------------------------------------------------------------
+// dsact_cnn_step runs them back to back on its own rows; the data-parallel step (dsact_cnn_dp_step) runs the critic-std
+// exchange between phases 1 and 2 and the gradient exchange between phase 2 and the update.
+struct CnnFeats { const float *P, *T, *Q[4]; };   // head inputs: pi(s), pi'(s'), Q1/Q2 features of s, Q1'/Q2' features of s'
+static CnnFeats cnn_feats(const dsact_cnn_handle* h, const dsact_batch& bt) {
+  // without a conv stack (the MLP approximators with separate heads) the feature is the observation itself
+  float* W = h->Wp();
+  const bool enc = h->pi.nconv > 0;
+  const int qL = h->q.nconv;
+  CnnFeats f;
+  f.P = enc ? W + h->convP[h->pi.nconv] : bt.obs;
+  f.T = enc ? W + h->convT[h->pi.nconv] : bt.obs2;
+  for (int k = 0; k < 2; ++k) {
+    f.Q[k] = enc ? W + h->convQ[k][qL] : bt.obs;
+    f.Q[2 + k] = enc ? W + h->convQ[2 + k][qL] : bt.obs2;
+  }
+  return f;
+}
+
+// phase 1: clear the step's accumulators and gradients, noise, the encoder forwards, the policy heads, the critics on
+// (s, a), sample_kernel (whose y = 1 half leaves the local critic-std sums in state[ST_STDSUM..+1]), the targets and the
+// mean heads of the critics on (s, a~)
+static void cnn_enqueue_phase1(dsact_cnn_handle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
+  const dsact_cnn_config& cf = h->cfg;
+  const CnnGeom &q = h->q, &pi = h->pi;
+  const int B = bt.batch, A = cf.act_dim;
+  float* W = h->Wp();
+  float* P = h->buf.params; float* T = h->buf.targets; float* G = h->buf.grads;
+  float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
+  float* Tq[2] = {T, T + q.n}; float* Tpi = T + 2 * q.n;
+  const long long n_all = 2 * q.n + pi.n + 1;
+  {
+    int blocks = (int)((n_all / 4 + 255) / 256); if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms; if (blocks < 1) blocks = 1;
+    launch_k(begin_step_kernel, blocks, 256, 0, c, h->buf.state, G, n_all); c.done();
+  }
+  const float *eps1, *eps2, *z3, *z4;
+  if (noise) { eps1 = noise->eps1; eps2 = noise->eps2; z3 = noise->z3; z4 = noise->z4; }
+  else {
+    const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
+    int blocks = (total / 2 + 255) / 256; if (blocks < 1) blocks = 1;
+    launch_k(noise_kernel, blocks, 256, 0, c, W + h->eps1, W + h->eps2, W + h->z3, W + h->z4, B, A, h->seed, (const float*)h->buf.state); c.done();
+    eps1 = W + h->eps1; eps2 = W + h->eps2; z3 = W + h->z3; z4 = W + h->z4;
+  }
+  h->pending = bt; h->pending_batch = B;
+  h->pending_eps1 = eps1; h->pending_z3 = z3; h->pending_z4 = z4;
+
+  // ---- encoders: pi(s), pi'(s'), Q_k features of s, Q'_k features of s'
+  cnn_conv_forward(h, pi, Ppi, bt.obs, h->convP, B, c);
+  cnn_conv_forward(h, pi, Tpi, bt.obs2, h->convT, B, c);
+  for (int k = 0; k < 2; ++k) {
+    cnn_conv_forward(h, q, Pq[k], bt.obs, h->convQ[k], B, c);
+    cnn_conv_forward(h, q, Tq[k], bt.obs2, h->convQ[2 + k], B, c);
+  }
+  const CnnFeats f = cnn_feats(h, bt);
+
+  // ---- policy heads: logits = (mean | log_std), the layout sample_kernel reads (networks/cnn.py:233-240)
+  {
+    std::vector<CnnHeadFwd> v;
+    for (int hd = 0; hd < pi.nheads; ++hd) {
+      v.push_back({Ppi + pi.head_off[hd], f.P, pi.F, nullptr, 0, &h->hb[hd], true, W + h->logitsP + hd * A, 2 * A});
+      v.push_back({Tpi + pi.head_off[hd], f.T, pi.F, nullptr, 0, &h->hb[2 + hd], false, W + h->logitsT + hd * A, 2 * A});
+    }
+    cnn_heads_forward(h, pi.head, v, B, c);
+    if (pi.ls_row >= 0) {   // std_type "parameter": log_std columns = the learnable row
+      int blocks = (B * A + 255) / 256; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
+      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + h->logitsP, 2 * A, A, (const float*)(Ppi + pi.ls_row), B, A); c.done();
+      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + h->logitsT, 2 * A, A, (const float*)(Tpi + pi.ls_row), B, A); c.done();
+    }
+  }
+  // ---- critics on (s, a): out = (mean, raw std) packed [B,2] (networks/cnn.py:454-461; softplus is applied by the loss kernels)
+  {
+    std::vector<CnnHeadFwd> v;
+    for (int k = 0; k < 2; ++k)
+      for (int hd = 0; hd < q.nheads; ++hd)
+        v.push_back({Pq[k] + q.head_off[hd], f.Q[k], q.F, bt.act, A, &h->hb[4 + 2 * k + hd], true, W + h->outQ[k] + hd, 2});
+    cnn_heads_forward(h, q.head, v, B, c);
+  }
+  {
+    SampleArgs a;
+    a.logits[0] = W + h->logitsP; a.logits[1] = W + h->logitsT;
+    a.eps[0] = eps1; a.eps[1] = eps2;
+    a.act[0] = W + h->new_act; a.act[1] = W + h->act2;
+    a.logp[0] = W + h->logp_new; a.logp[1] = W + h->logp2;
+    a.hi = h->buf.act_high; a.lo = h->buf.act_low; a.state = h->buf.state;
+    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
+    a.img[0] = ImgOut{nullptr, 0, 1, 0}; a.img[1] = ImgOut{nullptr, 0, 1, 0};
+    a.out_q[0] = W + h->outQ[0]; a.out_q[1] = W + h->outQ[1];
+    a.advance_rng = noise ? 0 : 1;
+    int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
+    launch_k(sample_kernel, dim3(blocks, 2), 256, 0, c, a); c.done();
+  }
+  // ---- targets on (s', a') and the mean heads of the critics on (s, a~)
+  {
+    std::vector<CnnHeadFwd> v;
+    for (int k = 0; k < 2; ++k)
+      for (int hd = 0; hd < q.nheads; ++hd)
+        v.push_back({Tq[k] + q.head_off[hd], f.Q[2 + k], q.F, W + h->act2, A, &h->hb[8 + 2 * k + hd], false, W + h->outQ[2 + k] + hd, 2});
+    for (int k = 0; k < 2; ++k)
+      v.push_back({Pq[k] + q.head_off[0], f.Q[k], q.F, W + h->new_act, A, &h->hb[12 + k], true, W + h->outQ[4 + k], 2});
+    cnn_heads_forward(h, q.head, v, B, c);
+  }
+  c.check();
+}
+
+// phase 2: losses, the head and encoder backward passes, and phase2_tail_kernel, on the rows phase 1 ran.  Every batch
+// mean is a sum over these rows times 1/global_batch; phase2_tail_kernel keeps rows = B (this shard), so that the log_alpha
+// gradient it writes is this rank's additive share -(sum_local logp + B * H) / global_batch (see tail_grad_log_alpha).
+static void cnn_enqueue_phase2(dsact_cnn_handle* h, int64_t global_batch, Ctx& c) {
+  const dsact_cnn_config& cf = h->cfg;
+  const CnnGeom &q = h->q, &pi = h->pi;
+  const dsact_batch& bt = h->pending;
+  const int B = bt.batch, A = cf.act_dim;
+  float* W = h->Wp();
+  float* P = h->buf.params; float* G = h->buf.grads;
+  float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
+  float* Gq[2] = {G, G + q.n}; float* Gpi = G + 2 * q.n;
+  const bool enc = pi.nconv > 0;
+  const CnnFeats f = cnn_feats(h, bt);
+
+  // ---- losses and head-output gradients
+  const float inv_gb = (float)(1.0 / (double)global_batch);
+  StepScalars sc;
+  sc.tau_b = (float)cf.tau_b; sc.alpha_fixed = (float)cf.alpha_fixed; sc.inv_global_batch = inv_gb;
+  sc.auto_alpha = cf.auto_alpha; sc.log_alpha = P + 2 * q.n + pi.n;
+  {
+    LossArgs a;
+    a.sc = sc;
+    a.rew = bt.rew; a.done = bt.done; a.z3 = h->pending_z3; a.z4 = h->pending_z4;
+    a.logp2 = W + h->logp2; a.logp_new = W + h->logp_new;
+    for (int k = 0; k < 2; ++k) {
+      a.out_q[k] = W + h->outQ[k]; a.out_qt[k] = W + h->outQ[2 + k]; a.out_qa[k] = W + h->outQ[4 + k];
+      a.d_out_q[k] = W + h->dOut[k]; a.d_out_qa[k] = W + h->dOut[4 + k];
+      a.gbias_q[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];          // output bias of the mean head
+      a.gbias_q_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
+      a.img_q[k] = ImgOut{nullptr, 0, 1, 0}; a.img_qa[k] = ImgOut{nullptr, 0, 1, 0};
+    }
+    a.state = h->buf.state; a.B = B; a.gamma = (float)cf.gamma; a.inv_global_batch = inv_gb;
+    int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
+    launch_k(loss_kernel, blocks, 64, 0, c, a); c.done();
+  }
+  auto zero = [&](float* p, long long n) {
+    int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
+    launch_k(zero_kernel, blocks, 256, 0, c, p, n); c.done();
+  };
+  zero(W + h->dfeat[0], (long long)B * pi.F);
+  zero(W + h->dfeat[1], (long long)B * q.F);
+  zero(W + h->dfeat[2], (long long)B * q.F);
+  zero(W + h->dfa[0], (long long)B * (q.F + A));
+  zero(W + h->dfa[1], (long long)B * (q.F + A));
+  // ---- critic backward through both heads (feature gradient accumulated over the heads), actor path through the mean head
+  {
+    std::vector<CnnHeadBwd> v;
+    for (int k = 0; k < 2; ++k)
+      for (int hd = 0; hd < q.nheads; ++hd)   // d(feature|act): only the feature part is used (replayed actions carry no gradient)
+        v.push_back({Pq[k] + q.head_off[hd], Gq[k] + q.head_off[hd], f.Q[k], q.F, bt.act, A, &h->hb[4 + 2 * k + hd],
+                     W + h->dOut[k] + hd, 2, nullptr});
+    for (int k = 0; k < 2; ++k)
+      v.push_back({Pq[k] + q.head_off[0], nullptr, f.Q[k], q.F, W + h->new_act, A, &h->hb[12 + k], W + h->dOut[4 + k], 2, W + h->dfa[k]});
+    cnn_heads_backward(h, q.head, v, B, c);
+  }
+  // feature gradients of the critics: the layer-0 input gradient of both heads, feature columns only.  The generic
+  // backward above skipped it for the critic passes (din = null): do it here with the feature-width problem
+  for (int k = 0; k < 2 && enc; ++k) {
+    GemmGroup gd;
+    gd.n = 0;
+    for (int hd = 0; hd < q.nheads; ++hd) {
+      GemmProb p = prob_zero();
+      const Net& net = q.head;
+      p.A[0] = W + h->hb[4 + 2 * k + hd].dz[0]; p.lda[0] = net.s[1]; p.K[0] = net.s[1];
+      p.B[0] = Pq[k] + q.head_off[hd] + net.w[0]; p.ldb[0] = net.s[0];
+      p.M = B; p.N = q.F; p.C = W + h->dfeat[1 + k]; p.ldc = q.F; p.epi = EPI_ATOMIC;
+      gd.p[gd.n++] = p;
+    }
+    launch_simt(h->num_sms, gd, V_DGRAD, c); c.done();
+  }
+  // dL/da~ through critic k = the action columns of dfa[k]: compact them for policy_grad_kernel
+  for (int k = 0; k < 2; ++k) {
+    const cudaError_t e = cudaMemcpy2DAsync(W + h->dAct[k], sizeof(float) * A, W + h->dfa[k] + q.F, sizeof(float) * (q.F + A),
+                                            sizeof(float) * A, B, cudaMemcpyDeviceToDevice, c.s);
+    if (e != cudaSuccess && c.err == cudaSuccess) c.err = e;
+  }
+  {
+    PolicyGradArgs a;
+    a.logits = W + h->logitsP; a.eps = h->pending_eps1; a.d_act1 = W + h->dAct[0]; a.d_act2 = W + h->dAct[1];
+    a.hi = h->buf.act_high; a.lo = h->buf.act_low;
+    a.d_logits = W + h->dlogits; a.state = h->buf.state;
+    a.gbias = Gpi + pi.head_off[0] + pi.head.b[pi.head.L];        // output bias of the mean head [A]
+    a.gbias_ls = pi.ls_row >= 0 ? Gpi + pi.ls_row : (pi.nheads == 2 ? Gpi + pi.head_off[1] + pi.head.b[pi.head.L] : nullptr);   // log_std head / row [A]
+    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
+    a.inv_global_batch = inv_gb;
+    a.img = ImgOut{nullptr, 0, 1, 0};
+    a.sc = sc;
+    int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;
+    launch_k(policy_grad_kernel, blocks, 256, sizeof(float) * 2 * A, c, a); c.done();
+  }
+  {
+    std::vector<CnnHeadBwd> v;
+    for (int hd = 0; hd < pi.nheads; ++hd)
+      v.push_back({Ppi + pi.head_off[hd], Gpi + pi.head_off[hd], f.P, pi.F, nullptr, 0, &h->hb[hd], W + h->dlogits + hd * A, 2 * A,
+                   enc ? W + h->dfeat[0] : nullptr});
+    cnn_heads_backward(h, pi.head, v, B, c);
+  }
+  // ---- encoders backward
+  if (enc) {
+    cnn_conv_backward(h, pi, Ppi, Gpi, bt.obs, h->convP, W + h->dfeat[0], B, c);
+    for (int k = 0; k < 2; ++k) cnn_conv_backward(h, q, Pq[k], Gq[k], bt.obs, h->convQ[k], W + h->dfeat[1 + k], B, c);
+  }
+
+  // ---- end of backward bookkeeping: log_alpha gradient (this shard's share), mean_std EMA commit, the Adam scalars
+  const AdamHyper hy{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
+  launch_k(phase2_tail_kernel, 1, 32, 0, c, G + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, hy, 1); c.done();
+  c.check();
+}
+
+// Adam / Polyak on `grads` (dp = false), or on the rank-ordered sum of every rank's exchange block (dp = true).
+// scalars_ready: 1 = phase 2 of this step wrote the Adam scalars; 0 = apply_kernel forms them (a handle that only receives
+// gradients never runs phase 2)
+static void cnn_enqueue_apply(dsact_cnn_handle* h, Ctx& c, int scalars_ready, bool dp) {
+  const dsact_cnn_config& cf = h->cfg;
+  const long long n_all = 2 * h->q.n + h->pi.n + 1;
+  ApplyArgs a;
+  memset(&a, 0, sizeof(a));
+  a.params = h->buf.params; a.targets = h->buf.targets; a.grads = h->buf.grads; a.m = h->buf.adam_m; a.v = h->buf.adam_v;
+  a.state = h->buf.state;
+  a.n_q2 = 2 * h->q.n; a.n_all = n_all;
+  a.delay_update = cf.delay_update; a.auto_alpha = cf.auto_alpha;
+  a.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2}; a.scalars_ready = scalars_ready;
+  a.eps = (float)cf.adam_eps; a.tau = (float)cf.tau;
+  a.omb1 = (float)(1.0 - cf.adam_beta1); a.b2f = (float)cf.adam_beta2; a.omb2 = (float)(1.0 - cf.adam_beta2);
+  a.g_lo = 0; a.g_hi = (n_all + 3) / 4; a.finish = 1;
+  int blocks = (int)(((n_all + 3) / 4 + 255) / 256); if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
+  if (dp) {
+    a.dp_timeout_ns = dp_timeout_ns(); a.dp_wait_kind = 2;
+    dp_apply_args(h->dp, a);
+    launch_k(apply_kernel<2>, blocks, 256, 0, c, a);
+  } else {
+    launch_k(apply_kernel<0>, blocks, 256, 0, c, a);
+  }
+  c.done();
+  c.check();
+}
+
 #include "v1_step.cuh"
 
 extern "C" {
@@ -405,7 +652,11 @@ int dsact_cnn_create(const dsact_cnn_config* cfg, int device, dsact_cnn_handle**
   return DSACT_OK;
 }
 
-void dsact_cnn_destroy(dsact_cnn_handle* h) { delete h; }
+void dsact_cnn_destroy(dsact_cnn_handle* h) {
+  if (!h) return;
+  if (h->dp.buf) { cudaSetDevice(h->device); dp_peer_release(h->dp); }
+  delete h;
+}
 
 int dsact_cnn_bind(dsact_cnn_handle* h, const dsact_buffers* b) {
   if (!h || !b) return fail(DSACT_EINVAL, "null argument");
@@ -499,208 +750,145 @@ int dsact_cnn_replay_sample(dsact_cnn_handle* h, int32_t batch, int64_t size, co
   return DSACT_OK;
 }
 
-int dsact_cnn_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration, void* stream) {
+static int cnn_check_batch(const dsact_cnn_handle* h, const dsact_batch* batch) {
   if (!h || !h->bound) return fail(DSACT_ESTATE, "dsact_cnn_bind has not been called");
   if (!batch || !batch->obs || !batch->act || !batch->rew || !batch->obs2 || !batch->done) return fail(DSACT_EINVAL, "null batch pointer");
   if (batch->batch < 1 || batch->batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch %d outside [1, max_batch=%d]", batch->batch, h->cfg.max_batch);
-  int rc = check_noise(noise);
-  if (rc) return rc;
+  return DSACT_OK;
+}
+static int cnn_sync_iteration(dsact_cnn_handle* h, int64_t iteration, cudaStream_t s) {
+  if (iteration < 0 || iteration > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
+  if (h->dev_iter != iteration) { set_iter_kernel<<<1, 32, 0, s>>>(h->buf.state, (int)iteration); CUDA_TRY(cudaGetLastError()); }
+  return DSACT_OK;
+}
+// the split and data-parallel entry points implement DSAC_V2 (DSAC-T); DSAC_V1 (algo 1) has local steps only
+static int cnn_check_v2(const dsact_cnn_handle* h) {
+  if (!h) return fail(DSACT_EINVAL, "null handle");
+  if (h->cfg.algo != 0) return fail(DSACT_EINVAL, "DSAC_V1 handles (algo 1) have no split or data-parallel update");
+  return DSACT_OK;
+}
+static int cnn_finish(dsact_cnn_handle* h, Ctx& c) {
+  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
+  h->launches += c.launches;
+  return DSACT_OK;
+}
+
+int dsact_cnn_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration, void* stream) {
+  int rc = cnn_check_batch(h, batch);
+  if (rc || (rc = check_noise(noise))) return rc;
   if (iteration < 0 || iteration > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
-  if (h->dev_iter != iteration) { set_iter_kernel<<<1, 32, 0, s>>>(h->buf.state, (int)iteration); CUDA_TRY(cudaGetLastError()); }
-  const dsact_cnn_config& cf = h->cfg;
-  if (cf.algo == 1) return cnn_step_v1(h, batch, noise, iteration, s);
-  const CnnGeom &q = h->q, &pi = h->pi;
-  const int B = batch->batch, A = cf.act_dim;
-  float* W = h->Wp();
-  float* P = h->buf.params; float* T = h->buf.targets; float* G = h->buf.grads;
-  float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
-  float* Tq[2] = {T, T + q.n}; float* Tpi = T + 2 * q.n;
-  float* Gq[2] = {G, G + q.n}; float* Gpi = G + 2 * q.n;
+  if ((rc = cnn_sync_iteration(h, iteration, s))) return rc;
+  if (h->cfg.algo == 1) return cnn_step_v1(h, batch, noise, iteration, s);
   Ctx c{s, 0, cudaSuccess};
   c.pdl = false;
-  const long long n_all = 2 * q.n + pi.n + 1;
-  {
-    int blocks = (int)((n_all / 4 + 255) / 256); if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(begin_step_kernel, blocks, 256, 0, c, h->buf.state, G, n_all); c.done();
-  }
-  const float *eps1, *eps2, *z3, *z4;
-  if (noise) { eps1 = noise->eps1; eps2 = noise->eps2; z3 = noise->z3; z4 = noise->z4; }
-  else {
-    const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
-    int blocks = (total / 2 + 255) / 256; if (blocks < 1) blocks = 1;
-    launch_k(noise_kernel, blocks, 256, 0, c, W + h->eps1, W + h->eps2, W + h->z3, W + h->z4, B, A, h->seed, (const float*)h->buf.state); c.done();
-    eps1 = W + h->eps1; eps2 = W + h->eps2; z3 = W + h->z3; z4 = W + h->z4;
-  }
+  cnn_enqueue_phase1(h, *batch, noise, c);
+  cnn_enqueue_phase2(h, batch->batch, c);
+  cnn_enqueue_apply(h, c, 1, false);
+  if ((rc = cnn_finish(h, c))) return rc;
+  h->dev_iter = iteration + 1;
+  return DSACT_OK;
+}
 
-  // ---- encoders: pi(s), pi'(s'), Q_k features of s, Q'_k features of s'
-  cnn_conv_forward(h, pi, Ppi, batch->obs, h->convP, B, c);
-  cnn_conv_forward(h, pi, Tpi, batch->obs2, h->convT, B, c);
-  for (int k = 0; k < 2; ++k) {
-    cnn_conv_forward(h, q, Pq[k], batch->obs, h->convQ[k], B, c);
-    cnn_conv_forward(h, q, Tq[k], batch->obs2, h->convQ[2 + k], B, c);
-  }
-  // without a conv stack (the MLP approximators with separate heads) the feature is the observation itself
-  const bool enc = pi.nconv > 0;
-  const float* featP = enc ? W + h->convP[pi.nconv] : batch->obs;
-  const float* featT = enc ? W + h->convT[pi.nconv] : batch->obs2;
-  const float* featQ[4] = {enc ? W + h->convQ[0][q.nconv] : batch->obs, enc ? W + h->convQ[1][q.nconv] : batch->obs,
-                           enc ? W + h->convQ[2][q.nconv] : batch->obs2, enc ? W + h->convQ[3][q.nconv] : batch->obs2};
+int dsact_cnn_grad_phase1(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
+  int rc = cnn_check_v2(h);
+  if (rc || (rc = cnn_check_batch(h, batch)) || (rc = check_noise(noise))) return rc;
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = false;
+  cnn_enqueue_phase1(h, *batch, noise, c);
+  return cnn_finish(h, c);
+}
 
-  // ---- policy heads: logits = (mean | log_std), the layout sample_kernel reads (networks/cnn.py:233-240)
-  {
-    std::vector<CnnHeadFwd> v;
-    for (int hd = 0; hd < pi.nheads; ++hd) {
-      v.push_back({Ppi + pi.head_off[hd], featP, pi.F, nullptr, 0, &h->hb[hd], true, W + h->logitsP + hd * A, 2 * A});
-      v.push_back({Tpi + pi.head_off[hd], featT, pi.F, nullptr, 0, &h->hb[2 + hd], false, W + h->logitsT + hd * A, 2 * A});
-    }
-    cnn_heads_forward(h, pi.head, v, B, c);
-    if (pi.ls_row >= 0) {   // std_type "parameter": log_std columns = the learnable row
-      int blocks = (B * A + 255) / 256; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + h->logitsP, 2 * A, A, (const float*)(Ppi + pi.ls_row), B, A); c.done();
-      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + h->logitsT, 2 * A, A, (const float*)(Tpi + pi.ls_row), B, A); c.done();
-    }
-  }
-  // ---- critics on (s, a): out = (mean, raw std) packed [B,2] (networks/cnn.py:454-461; softplus is applied by the loss kernels)
-  {
-    std::vector<CnnHeadFwd> v;
-    for (int k = 0; k < 2; ++k)
-      for (int hd = 0; hd < q.nheads; ++hd)
-        v.push_back({Pq[k] + q.head_off[hd], featQ[k], q.F, batch->act, A, &h->hb[4 + 2 * k + hd], true, W + h->outQ[k] + hd, 2});
-    cnn_heads_forward(h, q.head, v, B, c);
-  }
-  {
-    SampleArgs a;
-    a.logits[0] = W + h->logitsP; a.logits[1] = W + h->logitsT;
-    a.eps[0] = eps1; a.eps[1] = eps2;
-    a.act[0] = W + h->new_act; a.act[1] = W + h->act2;
-    a.logp[0] = W + h->logp_new; a.logp[1] = W + h->logp2;
-    a.hi = h->buf.act_high; a.lo = h->buf.act_low; a.state = h->buf.state;
-    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
-    a.img[0] = ImgOut{nullptr, 0, 1, 0}; a.img[1] = ImgOut{nullptr, 0, 1, 0};
-    a.out_q[0] = W + h->outQ[0]; a.out_q[1] = W + h->outQ[1];
-    a.advance_rng = noise ? 0 : 1;
-    int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-    launch_k(sample_kernel, dim3(blocks, 2), 256, 0, c, a); c.done();
-  }
-  // ---- targets on (s', a') and the mean heads of the critics on (s, a~)
-  {
-    std::vector<CnnHeadFwd> v;
-    for (int k = 0; k < 2; ++k)
-      for (int hd = 0; hd < q.nheads; ++hd)
-        v.push_back({Tq[k] + q.head_off[hd], featQ[2 + k], q.F, W + h->act2, A, &h->hb[8 + 2 * k + hd], false, W + h->outQ[2 + k] + hd, 2});
-    for (int k = 0; k < 2; ++k)
-      v.push_back({Pq[k] + q.head_off[0], featQ[k], q.F, W + h->new_act, A, &h->hb[12 + k], true, W + h->outQ[4 + k], 2});
-    cnn_heads_forward(h, q.head, v, B, c);
-  }
+int dsact_cnn_grad_phase2(dsact_cnn_handle* h, int64_t global_batch, void* stream) {
+  int rc = cnn_check_v2(h);
+  if (rc) return rc;
+  if (!h->bound) return fail(DSACT_ESTATE, "not bound");
+  if (h->pending_batch < 1) return fail(DSACT_ESTATE, "dsact_cnn_grad_phase2 without a preceding dsact_cnn_grad_phase1");
+  if (global_batch < h->pending_batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, h->pending_batch);
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = false;
+  cnn_enqueue_phase2(h, global_batch, c);
+  return cnn_finish(h, c);
+}
 
-  // ---- losses and head-output gradients
-  const float invB = (float)(1.0 / (double)B);
-  StepScalars sc;
-  sc.tau_b = (float)cf.tau_b; sc.alpha_fixed = (float)cf.alpha_fixed; sc.inv_global_batch = invB;
-  sc.auto_alpha = cf.auto_alpha; sc.log_alpha = P + 2 * q.n + pi.n;
-  {
-    LossArgs a;
-    a.sc = sc;
-    a.rew = batch->rew; a.done = batch->done; a.z3 = z3; a.z4 = z4;
-    a.logp2 = W + h->logp2; a.logp_new = W + h->logp_new;
-    for (int k = 0; k < 2; ++k) {
-      a.out_q[k] = W + h->outQ[k]; a.out_qt[k] = W + h->outQ[2 + k]; a.out_qa[k] = W + h->outQ[4 + k];
-      a.d_out_q[k] = W + h->dOut[k]; a.d_out_qa[k] = W + h->dOut[4 + k];
-      a.gbias_q[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];          // output bias of the mean head
-      a.gbias_q_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
-      a.img_q[k] = ImgOut{nullptr, 0, 1, 0}; a.img_qa[k] = ImgOut{nullptr, 0, 1, 0};
-    }
-    a.state = h->buf.state; a.B = B; a.gamma = (float)cf.gamma; a.inv_global_batch = invB;
-    int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-    launch_k(loss_kernel, blocks, 64, 0, c, a); c.done();
-  }
-  auto zero = [&](float* p, long long n) {
-    int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(zero_kernel, blocks, 256, 0, c, p, n); c.done();
-  };
-  zero(W + h->dfeat[0], (long long)B * pi.F);
-  zero(W + h->dfeat[1], (long long)B * q.F);
-  zero(W + h->dfeat[2], (long long)B * q.F);
-  zero(W + h->dfa[0], (long long)B * (q.F + A));
-  zero(W + h->dfa[1], (long long)B * (q.F + A));
-  // ---- critic backward through both heads (feature gradient accumulated over the heads), actor path through the mean head
-  {
-    std::vector<CnnHeadBwd> v;
-    for (int k = 0; k < 2; ++k)
-      for (int hd = 0; hd < q.nheads; ++hd)   // d(feature|act): only the feature part is used (replayed actions carry no gradient)
-        v.push_back({Pq[k] + q.head_off[hd], Gq[k] + q.head_off[hd], featQ[k], q.F, batch->act, A, &h->hb[4 + 2 * k + hd],
-                     W + h->dOut[k] + hd, 2, nullptr});
-    for (int k = 0; k < 2; ++k)
-      v.push_back({Pq[k] + q.head_off[0], nullptr, featQ[k], q.F, W + h->new_act, A, &h->hb[12 + k], W + h->dOut[4 + k], 2, W + h->dfa[k]});
-    cnn_heads_backward(h, q.head, v, B, c);
-  }
-  // feature gradients of the critics: the layer-0 input gradient of both heads, feature columns only.  The generic
-  // backward above skipped it for the critic passes (din = null): do it here with the feature-width problem
-  for (int k = 0; k < 2 && enc; ++k) {
-    GemmGroup gd;
-    gd.n = 0;
-    for (int hd = 0; hd < q.nheads; ++hd) {
-      GemmProb p = prob_zero();
-      const Net& net = q.head;
-      p.A[0] = W + h->hb[4 + 2 * k + hd].dz[0]; p.lda[0] = net.s[1]; p.K[0] = net.s[1];
-      p.B[0] = Pq[k] + q.head_off[hd] + net.w[0]; p.ldb[0] = net.s[0];
-      p.M = B; p.N = q.F; p.C = W + h->dfeat[1 + k]; p.ldc = q.F; p.epi = EPI_ATOMIC;
-      gd.p[gd.n++] = p;
-    }
-    launch_simt(h->num_sms, gd, V_DGRAD, c); c.done();
-  }
-  // dL/da~ through critic k = the action columns of dfa[k]: compact them for policy_grad_kernel
-  for (int k = 0; k < 2; ++k) {
-    CUDA_TRY(cudaMemcpy2DAsync(W + h->dAct[k], sizeof(float) * A, W + h->dfa[k] + q.F, sizeof(float) * (q.F + A), sizeof(float) * A, B,
-                               cudaMemcpyDeviceToDevice, s));
-  }
-  {
-    PolicyGradArgs a;
-    a.logits = W + h->logitsP; a.eps = eps1; a.d_act1 = W + h->dAct[0]; a.d_act2 = W + h->dAct[1];
-    a.hi = h->buf.act_high; a.lo = h->buf.act_low;
-    a.d_logits = W + h->dlogits; a.state = h->buf.state;
-    a.gbias = Gpi + pi.head_off[0] + pi.head.b[pi.head.L];        // output bias of the mean head [A]
-    a.gbias_ls = pi.ls_row >= 0 ? Gpi + pi.ls_row : (pi.nheads == 2 ? Gpi + pi.head_off[1] + pi.head.b[pi.head.L] : nullptr);   // log_std head / row [A]
-    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
-    a.inv_global_batch = invB;
-    a.img = ImgOut{nullptr, 0, 1, 0};
-    a.sc = sc;
-    int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(policy_grad_kernel, blocks, 256, sizeof(float) * 2 * A, c, a); c.done();
-  }
-  {
-    std::vector<CnnHeadBwd> v;
-    for (int hd = 0; hd < pi.nheads; ++hd)
-      v.push_back({Ppi + pi.head_off[hd], Gpi + pi.head_off[hd], featP, pi.F, nullptr, 0, &h->hb[hd], W + h->dlogits + hd * A, 2 * A,
-                   enc ? W + h->dfeat[0] : nullptr});
-    cnn_heads_backward(h, pi.head, v, B, c);
-  }
-  // ---- encoders backward
-  if (enc) {
-    cnn_conv_backward(h, pi, Ppi, Gpi, batch->obs, h->convP, W + h->dfeat[0], B, c);
-    for (int k = 0; k < 2; ++k) cnn_conv_backward(h, q, Pq[k], Gq[k], batch->obs, h->convQ[k], W + h->dfeat[1 + k], B, c);
-  }
+int dsact_cnn_compute_grads(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
+  int rc = cnn_check_v2(h);
+  if (rc || (rc = cnn_check_batch(h, batch)) || (rc = check_noise(noise))) return rc;
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = false;
+  cnn_enqueue_phase1(h, *batch, noise, c);
+  cnn_enqueue_phase2(h, batch->batch, c);
+  return cnn_finish(h, c);
+}
 
-  // ---- end of backward bookkeeping + Adam / Polyak
-  AdamHyper hy{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-  launch_k(phase2_tail_kernel, 1, 32, 0, c, G + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, hy, 1); c.done();
-  {
-    ApplyArgs a;
-    memset(&a, 0, sizeof(a));
-    a.params = P; a.targets = T; a.grads = G; a.m = h->buf.adam_m; a.v = h->buf.adam_v; a.state = h->buf.state;
-    a.n_q2 = 2 * q.n; a.n_all = n_all;
-    a.delay_update = cf.delay_update; a.auto_alpha = cf.auto_alpha;
-    a.hy = hy; a.scalars_ready = 1;
-    a.eps = (float)cf.adam_eps; a.tau = (float)cf.tau;
-    a.omb1 = (float)(1.0 - cf.adam_beta1); a.b2f = (float)cf.adam_beta2; a.omb2 = (float)(1.0 - cf.adam_beta2);
-    a.g_lo = 0; a.g_hi = (n_all + 3) / 4; a.finish = 1;
-    int blocks = (int)(((n_all + 3) / 4 + 255) / 256); if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-    launch_k(apply_kernel<0>, blocks, 256, 0, c, a); c.done();
+int dsact_cnn_apply(dsact_cnn_handle* h, int64_t iteration, void* stream) {
+  int rc = cnn_check_v2(h);
+  if (rc) return rc;
+  if (!h->bound) return fail(DSACT_ESTATE, "not bound");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = cnn_sync_iteration(h, iteration, s))) return rc;
+  Ctx c{s, 0, cudaSuccess};
+  c.pdl = false;
+  cnn_enqueue_apply(h, c, 0, false);
+  if ((rc = cnn_finish(h, c))) return rc;
+  h->dev_iter = iteration + 1;
+  return DSACT_OK;
+}
+
+// ---- data parallelism over peer memory (dp_peer.cuh; the same exchange buffer and kernels as dsact_dp_*) -------------
+int dsact_cnn_dp_export(dsact_cnn_handle* h, void* handle_out, int64_t* bytes_out) {
+  int rc = cnn_check_v2(h);
+  if (rc) return rc;
+  if (!handle_out) return fail(DSACT_EINVAL, "null argument");
+  return dp_peer_export(h->dp, h->device, 2 * h->q.n + h->pi.n + 1, handle_out, bytes_out);
+}
+
+int dsact_cnn_dp_connect(dsact_cnn_handle* h, int32_t rank, int32_t world, const void* handles) {
+  int rc = cnn_check_v2(h);
+  if (rc) return rc;
+  if (!handles) return fail(DSACT_EINVAL, "null argument");
+  if (!h->bound) return fail(DSACT_ESTATE, "dsact_cnn_bind has not been called");
+  if (!h->dp.buf) return fail(DSACT_ESTATE, "dsact_cnn_dp_export has not been called");
+  return dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
+}
+
+// One data-parallel update on this rank's shard, eager on the caller's stream: phase 1, critic-std sums exchanged,
+// phase 2 scaled by 1/global_batch, the local gradients into this rank's exchange block, logged sums exchanged (also the
+// "every block is complete" barrier), [reduce-scatter from 6 ranks up], Adam on the rank-ordered global sum.
+// Every rank must call it for the same iteration.
+int dsact_cnn_dp_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t global_batch, int64_t iteration,
+                      void* stream) {
+  int rc = cnn_check_v2(h);
+  if (rc || (rc = cnn_check_batch(h, batch)) || (rc = check_noise(noise))) return rc;
+  if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_cnn_dp_connect has not been called");
+  if (global_batch < batch->batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch->batch);
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = cnn_sync_iteration(h, iteration, s))) return rc;
+  Ctx c{s, 0, cudaSuccess};
+  c.pdl = false;
+  float* state = h->buf.state;
+  cnn_enqueue_phase1(h, *batch, noise, c);
+  enqueue_dp_exchange(h->dp, state, 0, c);
+  cnn_enqueue_phase2(h, global_batch, c);
+  {   // phase 2 already wrote the log_alpha share: a plain copy of the flat gradients into this rank's block
+    const long long n = 2 * h->q.n + h->pi.n + 1;
+    TailArgs none;
+    memset(&none, 0, sizeof(none));
+    int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
+    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF, (const float*)h->buf.grads, (const float*)h->buf.grads, n, 0,
+             4LL, (const float*)state, none);
+    c.done();
   }
-  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
-  h->launches += c.launches;
+  enqueue_dp_exchange(h->dp, state, 1, c);
+  if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, state, 2 * h->q.n, h->num_sms, c, 0);
+  cnn_enqueue_apply(h, c, 1, true);
+  if ((rc = cnn_finish(h, c))) return rc;
   h->dev_iter = iteration + 1;
   return DSACT_OK;
 }

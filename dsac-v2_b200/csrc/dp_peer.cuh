@@ -42,6 +42,17 @@ struct DpComm {
   int rank, world;
 };
 
+// Host-side exchange state of one handle (MLP or head-wise engine): the buffer it exports, the peers' buffers as opened
+// here, and the rank map the kernels take.  Export / connect / release are in engine.cu (dp_peer_*).
+struct DpPeer {
+  float* buf = nullptr;                   // this rank's exchange buffer (cudaMalloc, exported with CUDA IPC)
+  void* opened[DP_MAX_RANKS] = {};        // peers' buffers as opened here
+  DpComm comm = {};
+  bool ready = false;                     // dp_peer_connect succeeded
+  long long n_params = 0;                 // length of the flat gradient buffer the blocks mirror
+  long long npad() const { return (n_params + 3) / 4 * 4; }   // a block, padded to whole float4 groups
+};
+
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }

@@ -154,11 +154,7 @@ struct dsact_handle {
   cudaEvent_t ev_fork, ev_join;
   cudaEvent_t ev_pro_fork, ev_pro_join;   // prologue branch (weight images, noise, clears) beside the replay gather
   cudaEvent_t ev_dp_fork, ev_dp_join;     // std-sum exchange of the data-parallel step beside the second forward chain
-  // peer-memory data parallelism (dp_peer.cuh)
-  float* dp_buf = nullptr;            // this rank's exchange buffer (cudaMalloc, exported with CUDA IPC)
-  void* dp_opened[DP_MAX_RANKS] = {}; // peers' buffers as opened here
-  DpComm dp = {};
-  bool dp_ready = false;
+  DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   // host-minibatch staging (dsact_stage_host): two device sets + a private copy stream
   float* stage_buf[2] = {nullptr, nullptr};
   int64_t stage_floats = 0;
@@ -784,33 +780,101 @@ static bool dp_split_enabled() {
   static const bool on = getenv("DSACT_DP_SPLIT") && getenv("DSACT_DP_SPLIT")[0] == '1';
   return on;
 }
-static bool dp_two_shot(const dsact_handle* h) {
+static bool dp_two_shot(const DpPeer& dp) {
   static const char* e = getenv("DSACT_DP_TWO_SHOT");
   if (e && (e[0] == '0' || e[0] == '1')) return e[0] == '1';
-  return h->dp.world >= 6;
+  return dp.comm.world >= 6;
 }
-static long long dp_npad(const dsact_handle* h) { return (2 * h->q.n + h->pi.n + 1 + 3) / 4 * 4; }
 // `part`: 0 = the whole buffer, 1 = the critics' groups [0, n_q2 / 4) (kind-4 flags), 2 = the rest (kind-2 flags)
-static void enqueue_dp_reduce_scatter(dsact_handle* h, Ctx& c, int part = 0) {
-  const long long g_all = dp_npad(h) / 4, g_q = (2 * h->q.n) / 4;
+static void enqueue_dp_reduce_scatter(const DpPeer& dp, const float* state, long long n_q2, int num_sms, Ctx& c, int part = 0) {
+  const long long g_all = dp.npad() / 4, g_q = n_q2 / 4;
   const long long G0 = part == 2 ? g_q : 0, G1 = part == 1 ? g_q : g_all;
-  const long long groups = G1 - G0, per = (groups + h->dp.world - 1) / h->dp.world;
+  const long long groups = G1 - G0, per = (groups + dp.comm.world - 1) / dp.comm.world;
   DpSlice sl;
-  sl.g_lo = G0 + per * h->dp.rank;
+  sl.g_lo = G0 + per * dp.comm.rank;
   sl.g_hi = sl.g_lo + per < G1 ? sl.g_lo + per : G1;
   if (sl.g_lo > G1) sl.g_lo = G1;
-  sl.red_off = DP_GRADS_OFF + dp_npad(h);
-  sl.ticket = reinterpret_cast<int*>(h->dp_buf) + DP_TICKET + (part == 1 ? 1 : 0);   // block ticket of this launch
+  sl.red_off = DP_GRADS_OFF + dp.npad();
+  sl.ticket = reinterpret_cast<int*>(dp.buf) + DP_TICKET + (part == 1 ? 1 : 0);   // block ticket of this launch
   sl.flag_kind = part == 1 ? 4 : 2;
-  int blocks = (int)((per + 255) / 256); if (blocks < 1) blocks = 1; if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms;
-  launch_k(dp_reduce_scatter_kernel, blocks, 256, 0, c, h->dp, sl, (const float*)h->buf.state);
+  int blocks = (int)((per + 255) / 256); if (blocks < 1) blocks = 1; if (blocks > 2 * num_sms) blocks = 2 * num_sms;
+  launch_k(dp_reduce_scatter_kernel, blocks, 256, 0, c, dp.comm, sl, state);
   c.done();
+}
+static void enqueue_dp_reduce_scatter(dsact_handle* h, Ctx& c, int part = 0) {
+  enqueue_dp_reduce_scatter(h->dp, h->buf.state, 2 * h->q.n, h->num_sms, c, part);
 }
 
 // One exchange of the peer-memory data-parallel path (dp_peer.cuh): kind 0 = critic-std sums, 1 = logged sums.
-static void enqueue_dp_exchange(dsact_handle* h, int kind, Ctx& c) {
-  launch_k(dp_exchange_kernel, 1, 32 * h->dp.world, 0, c, h->dp, h->buf.state, kind, dp_timeout_ns());
+static void enqueue_dp_exchange(const DpPeer& dp, float* state, int kind, Ctx& c) {
+  launch_k(dp_exchange_kernel, 1, 32 * dp.comm.world, 0, c, dp.comm, state, kind, dp_timeout_ns());
   c.done();
+}
+static void enqueue_dp_exchange(dsact_handle* h, int kind, Ctx& c) { enqueue_dp_exchange(h->dp, h->buf.state, kind, c); }
+
+// apply_kernel<2>'s view of the exchange: the reduced block in this rank's own memory once every rank's kind-2 (kind-4)
+// flag is here (two-shot), or every rank's block, summed in rank order (one-shot)
+static void dp_apply_args(const DpPeer& dp, ApplyArgs& a) {
+  if (dp_two_shot(dp)) {
+    a.dp_world = 1;
+    a.dp_grads[0] = dp.buf + DP_GRADS_OFF + dp.npad();
+    a.dp_own = dp.buf; a.dp_wait_world = dp.comm.world;
+  } else {
+    a.dp_world = dp.comm.world;
+    for (int r = 0; r < dp.comm.world; ++r) a.dp_grads[r] = dp.comm.peer[r] + DP_GRADS_OFF;
+  }
+}
+
+// ---- exchange-buffer setup shared by dsact_dp_* and dsact_cnn_dp_* ----------------------------------------------
+static int dp_peer_export(DpPeer& dp, int device, long long n_params, void* handle_out, int64_t* bytes_out) {
+  CUDA_TRY(cudaSetDevice(device));
+  dp.n_params = n_params;
+  // header + this rank's gradient block + the reduced block of the two-shot exchange
+  const size_t bytes = sizeof(float) * (size_t)(DP_GRADS_OFF + 2 * dp.npad());
+  if (!dp.buf) {
+    CUDA_TRY(cudaMalloc(&dp.buf, bytes));
+    CUDA_TRY(cudaMemset(dp.buf, 0, bytes));
+  }
+  cudaIpcMemHandle_t ipc;
+  CUDA_TRY(cudaIpcGetMemHandle(&ipc, dp.buf));
+  static_assert(sizeof(ipc) == DSACT_IPC_HANDLE_BYTES, "IPC handle size");
+  memcpy(handle_out, &ipc, sizeof(ipc));
+  if (bytes_out) *bytes_out = (int64_t)bytes;
+  return DSACT_OK;
+}
+
+static int dp_peer_connect(DpPeer& dp, int device, float* state, int32_t rank, int32_t world, const void* handles) {
+  if (!dp.buf) return fail(DSACT_ESTATE, "the exchange buffer has not been exported (dp_export)");
+  if (world < 2 || world > DP_MAX_RANKS || rank < 0 || rank >= world) return fail(DSACT_EINVAL, "rank %d / world %d outside [2, %d]", rank, world, DP_MAX_RANKS);
+  CUDA_TRY(cudaSetDevice(device));
+  CUDA_TRY(cudaDeviceSynchronize());
+  dp.ready = false;
+  for (int r = 0; r < DP_MAX_RANKS; ++r)
+    if (dp.opened[r]) { cudaIpcCloseMemHandle(dp.opened[r]); dp.opened[r] = nullptr; }
+  dp.comm.rank = rank; dp.comm.world = world;
+  for (int r = 0; r < world; ++r) {
+    if (r == rank) { dp.comm.peer[r] = dp.buf; continue; }
+    cudaIpcMemHandle_t ipc;
+    memcpy(&ipc, static_cast<const char*>(handles) + (size_t)r * sizeof(ipc), sizeof(ipc));
+    void* p = nullptr;
+    cudaError_t e = cudaIpcOpenMemHandle(&p, ipc, cudaIpcMemLazyEnablePeerAccess);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(DSACT_ECUDA, "cudaIpcOpenMemHandle(rank %d): %s", r, cudaGetErrorString(e)); }
+    dp.opened[r] = p;
+    dp.comm.peer[r] = static_cast<float*>(p);
+  }
+  // every rank starts at epoch 0 with clear flags (the caller synchronises the ranks after this call)
+  CUDA_TRY(cudaMemset(dp.buf, 0, sizeof(float) * DP_GRADS_OFF));
+  CUDA_TRY(cudaMemset(state + ST_DP_EPOCH, 0, sizeof(float)));
+  CUDA_TRY(cudaMemset(state + ST_DP_ERR, 0, sizeof(float)));
+  CUDA_TRY(cudaDeviceSynchronize());
+  dp.ready = true;
+  return DSACT_OK;
+}
+
+static void dp_peer_release(DpPeer& dp) {
+  for (int r = 0; r < DP_MAX_RANKS; ++r) if (dp.opened[r]) cudaIpcCloseMemHandle(dp.opened[r]);
+  if (dp.buf) cudaFree(dp.buf);
+  dp = DpPeer();
 }
 
 // `dp_std_exchange`: the std sums are complete once sample_kernel has run, one whole forward chain before the loss needs
@@ -1064,11 +1128,11 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
         const long long nq = (2 * q.n) / 4 * 4;   // whole float4 groups of the critics' span
         int blocks = (int)((nq / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
         TailArgs none; memset(&none, 0, sizeof(none));
-        launch_k(dp_grad_fold_kernel, blocks, 256, 0, cs, h->dp_buf + DP_GRADS_OFF, (const float*)G_, (const float*)(W + ar.slabs), nq,
+        launch_k(dp_grad_fold_kernel, blocks, 256, 0, cs, h->dp.buf + DP_GRADS_OFF, (const float*)G_, (const float*)(W + ar.slabs), nq,
                  ar.nslabs, (long long)ar.slab_stride, (const float*)h->buf.state, none);
         cs.done();
         enqueue_dp_exchange(h, 3, cs);
-        if (dp_two_shot(h)) enqueue_dp_reduce_scatter(h, cs, 1);
+        if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h, cs, 1);
         enqueue_apply(h, cs, false, true, early_apply, 1);
         h->apply_early = true;
       } else if (early_apply) {   // Adam + Polyak of both critics beside the policy backward: every critic gradient is final here
@@ -1132,7 +1196,7 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
     const long long lo = h->apply_early ? (2 * q.n) / 4 * 4 : 0;   // the critics' groups went out on the side branch
     const long long n = 2 * q.n + pi.n + 1 - lo;
     int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp_buf + DP_GRADS_OFF + lo, (const float*)G_ + lo, (const float*)(tc ? W + ar.slabs : G_) + lo, n,
+    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF + lo, (const float*)G_ + lo, (const float*)(tc ? W + ar.slabs : G_) + lo, n,
              tc ? ar.nslabs : 0, (long long)(tc ? ar.slab_stride : 4), (const float*)h->buf.state, tail_args(h, global_batch, B, fold_tail));
     c.done();
   }
@@ -1166,14 +1230,7 @@ static void enqueue_apply(dsact_handle* h, Ctx& c, bool reduce_slabs = false, bo
   a.dp_own = nullptr; a.dp_wait_world = 0; a.dp_timeout_ns = dp_timeout_ns();
   for (int r = 0; r < 8; ++r) a.dp_grads[r] = nullptr;
   a.dp_wait_kind = part == 1 ? 4 : 2;
-  if (dp && dp_two_shot(h)) {   // the reduced block in this rank's own memory, once every rank's kind-2 (kind-4) flag is here
-    a.dp_world = 1;
-    a.dp_grads[0] = h->dp_buf + DP_GRADS_OFF + dp_npad(h);
-    a.dp_own = h->dp_buf; a.dp_wait_world = h->dp.world;
-  } else if (dp) {
-    a.dp_world = h->dp.world;
-    for (int r = 0; r < h->dp.world; ++r) a.dp_grads[r] = h->dp.peer[r] + DP_GRADS_OFF;
-  }
+  if (dp) dp_apply_args(h->dp, a);
   a.eps = (float)cf.adam_eps; a.tau = (float)cf.tau;
   a.omb1 = (float)(1.0 - cf.adam_beta1); a.b2f = (float)cf.adam_beta2; a.omb2 = (float)(1.0 - cf.adam_beta2);
   a.slabs = nullptr; a.nslabs = 0; a.slab_stride = 0;
@@ -1393,8 +1450,7 @@ void dsact_destroy(dsact_handle* h) {
   cudaEventDestroy(h->ev_pro_join);
   cudaEventDestroy(h->ev_dp_fork);
   cudaEventDestroy(h->ev_dp_join);
-  for (int r = 0; r < DP_MAX_RANKS; ++r) if (h->dp_opened[r]) cudaIpcCloseMemHandle(h->dp_opened[r]);
-  if (h->dp_buf) cudaFree(h->dp_buf);
+  dp_peer_release(h->dp);
   for (int t = 0; t < 2; ++t) {
     if (h->stage_buf[t]) cudaFree(h->stage_buf[t]);
     if (h->ev_stage_ready[t]) cudaEventDestroy(h->ev_stage_ready[t]);
@@ -1693,49 +1749,16 @@ int dsact_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_
 // ---- data parallelism over peer memory (dp_peer.cuh) ------------------------------------------------------------
 int dsact_dp_export(dsact_handle* h, void* handle_out, int64_t* bytes_out) {
   if (!h || !handle_out) return fail(DSACT_EINVAL, "null argument");
-  CUDA_TRY(cudaSetDevice(h->device));
-  // header + this rank's gradient block + the reduced block of the two-shot exchange
-  const size_t bytes = sizeof(float) * (size_t)(DP_GRADS_OFF + 2 * ((2 * h->q.n + h->pi.n + 1 + 3) / 4 * 4));
-  if (!h->dp_buf) {
-    CUDA_TRY(cudaMalloc(&h->dp_buf, bytes));
-    CUDA_TRY(cudaMemset(h->dp_buf, 0, bytes));
-  }
-  cudaIpcMemHandle_t ipc;
-  CUDA_TRY(cudaIpcGetMemHandle(&ipc, h->dp_buf));
-  static_assert(sizeof(ipc) == DSACT_IPC_HANDLE_BYTES, "IPC handle size");
-  memcpy(handle_out, &ipc, sizeof(ipc));
-  if (bytes_out) *bytes_out = (int64_t)bytes;
-  return DSACT_OK;
+  return dp_peer_export(h->dp, h->device, 2 * h->q.n + h->pi.n + 1, handle_out, bytes_out);
 }
 
 int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* handles) {
   if (!h || !handles) return fail(DSACT_EINVAL, "null argument");
   if (!h->bound) return fail(DSACT_ESTATE, "dsact_bind has not been called");
-  if (!h->dp_buf) return fail(DSACT_ESTATE, "dsact_dp_export has not been called");
-  if (world < 2 || world > DP_MAX_RANKS || rank < 0 || rank >= world) return fail(DSACT_EINVAL, "rank %d / world %d outside [2, %d]", rank, world, DP_MAX_RANKS);
-  CUDA_TRY(cudaSetDevice(h->device));
-  CUDA_TRY(cudaDeviceSynchronize());
-  drop_graphs(h);
-  for (int r = 0; r < DP_MAX_RANKS; ++r)
-    if (h->dp_opened[r]) { cudaIpcCloseMemHandle(h->dp_opened[r]); h->dp_opened[r] = nullptr; }
-  h->dp.rank = rank; h->dp.world = world;
-  for (int r = 0; r < world; ++r) {
-    if (r == rank) { h->dp.peer[r] = h->dp_buf; continue; }
-    cudaIpcMemHandle_t ipc;
-    memcpy(&ipc, static_cast<const char*>(handles) + (size_t)r * sizeof(ipc), sizeof(ipc));
-    void* p = nullptr;
-    cudaError_t e = cudaIpcOpenMemHandle(&p, ipc, cudaIpcMemLazyEnablePeerAccess);
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(DSACT_ECUDA, "cudaIpcOpenMemHandle(rank %d): %s", r, cudaGetErrorString(e)); }
-    h->dp_opened[r] = p;
-    h->dp.peer[r] = static_cast<float*>(p);
-  }
-  // every rank starts at epoch 0 with clear flags (the caller synchronises the ranks after this call)
-  CUDA_TRY(cudaMemset(h->dp_buf, 0, sizeof(float) * DP_GRADS_OFF));
-  CUDA_TRY(cudaMemset(h->buf.state + ST_DP_EPOCH, 0, sizeof(float)));
-  CUDA_TRY(cudaMemset(h->buf.state + ST_DP_ERR, 0, sizeof(float)));
-  CUDA_TRY(cudaDeviceSynchronize());
-  h->dp_ready = true;
-  return DSACT_OK;
+  if (!h->dp.buf) return fail(DSACT_ESTATE, "dsact_dp_export has not been called");
+  const int rc = dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
+  if (rc == DSACT_OK) drop_graphs(h);   // captured data-parallel steps hold the previous peer map
+  return rc;
 }
 
 // One data-parallel update as one submission: forward, std-sum exchange, losses + backward scaled by 1/global_batch,
@@ -1744,7 +1767,7 @@ int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* 
                   void* stream) {
   int rc = check_batch(h, batch);
   if (rc || (rc = check_noise(noise))) return rc;
-  if (!h->dp_ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
+  if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (global_batch < batch->batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch->batch);
   CUDA_TRY(cudaSetDevice(h->device));
   if ((rc = sync_iteration(h, iteration, (cudaStream_t)stream))) return rc;
@@ -1761,7 +1784,7 @@ int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* 
     enqueue_phase2(h, bt, global_batch, c, REDUCE_DP, ta.enabled, early ? &ta : nullptr, true);
     const bool split = h->apply_early;   // the critics' part went out (and was applied) beside the policy backward
     enqueue_dp_exchange(h, 1, c);
-    if (dp_two_shot(h)) enqueue_dp_reduce_scatter(h, c, split ? 2 : 0);
+    if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h, c, split ? 2 : 0);
     enqueue_apply(h, c, false, true, &ta);
   });
   if (rc) return rc;
@@ -1773,7 +1796,7 @@ int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* 
 int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
                          int64_t global_batch, int64_t iteration, void* stream) {
   if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if (!h->dp_ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
+  if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
   if (global_batch < batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch);
   int rc = check_noise(noise);
@@ -1796,7 +1819,7 @@ int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int
     enqueue_phase2(h, bt, global_batch, c, REDUCE_DP, ta.enabled, early ? &ta : nullptr, true);
     const bool split = h->apply_early;
     enqueue_dp_exchange(h, 1, c);
-    if (dp_two_shot(h)) enqueue_dp_reduce_scatter(h, c, split ? 2 : 0);
+    if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h, c, split ? 2 : 0);
     enqueue_apply(h, c, false, true, &ta);
   });
   if (rc) return rc;

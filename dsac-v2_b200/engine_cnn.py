@@ -86,6 +86,7 @@ class CnnEngine:
             check(self.lib.dsact_cnn_set_carry(self.h, -1.0, -1.0, 0, 0, self._stream()))
             self._stats_host = torch.zeros(_lib.NUM_STATS, dtype=torch.float32).pin_memory()
         self.last_batch = 0
+        self.dp_world = 0          # > 1 once dp_connect has mapped the peers
 
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -165,23 +166,74 @@ class CnnEngine:
         return out
 
     # ---- the path -------------------------------------------------------------------------------------------------------
+    def _args(self, data: Dict[str, torch.Tensor], noise):
+        """ctypes batch / noise of a minibatch (image observations [B, C, H, W]); the device copies stay referenced until
+        the next call, which is after the kernels reading them were enqueued."""
+        t = {k: data[k].to(device=self.device, dtype=torch.float32).contiguous() for k in ("obs", "act", "rew", "obs2", "done")}
+        B = t["obs"].shape[0]
+        c = self.cfg
+        if t["obs"][0].numel() != self.obs_elems or t["obs2"].shape != t["obs"].shape or t["act"].shape != (B, c.act_dim):
+            raise ValueError("minibatch shapes do not match the configured observation / action shape")
+        b = Batch(t["obs"].data_ptr(), t["act"].data_ptr(), t["rew"].data_ptr(), t["obs2"].data_ptr(), t["done"].data_ptr(), B, None)
+        n = None
+        if noise is not None:
+            nz = [torch.as_tensor(x).to(device=self.device, dtype=torch.float32).contiguous() for x in noise]
+            n = C.byref(Noise(*(x.data_ptr() for x in nz)))
+            self._keep_noise = nz
+        self._keep = t
+        return b, n
+
     def step(self, data: Dict[str, torch.Tensor], iteration: int, noise=None):
         """DSAC_V2.local_update (reference dsac_v2.py:102-105) with image observations [B, C, H, W] on the device."""
         with torch.cuda.device(self.device):
-            t = {k: data[k].to(device=self.device, dtype=torch.float32).contiguous() for k in ("obs", "act", "rew", "obs2", "done")}
-            B = t["obs"].shape[0]
-            c = self.cfg
-            if t["obs"][0].numel() != self.obs_elems or t["obs2"].shape != t["obs"].shape or t["act"].shape != (B, c.act_dim):
-                raise ValueError("minibatch shapes do not match the configured observation / action shape")
-            b = Batch(t["obs"].data_ptr(), t["act"].data_ptr(), t["rew"].data_ptr(), t["obs2"].data_ptr(), t["done"].data_ptr(), B, None)
-            n = None
-            if noise is not None:
-                nz = [torch.as_tensor(x).to(device=self.device, dtype=torch.float32).contiguous() for x in noise]
-                n = C.byref(Noise(*(x.data_ptr() for x in nz)))
-                self._keep_noise = nz
-            self._keep = t
+            b, n = self._args(data, noise)
             check(self.lib.dsact_cnn_step(self.h, C.byref(b), n, int(iteration), self._stream()))
-        self.last_batch = B
+        self.last_batch = b.batch
+
+    # ---- split form (get_remote_update_info / remote_update) and data parallelism: the signatures of engine.Engine ------
+    def compute_grads(self, data, noise=None):
+        with torch.cuda.device(self.device):
+            b, n = self._args(data, noise)
+            check(self.lib.dsact_cnn_compute_grads(self.h, C.byref(b), n, self._stream()))
+        self.last_batch = b.batch
+
+    def grad_phase1(self, data, noise=None):
+        with torch.cuda.device(self.device):
+            b, n = self._args(data, noise)
+            check(self.lib.dsact_cnn_grad_phase1(self.h, C.byref(b), n, self._stream()))
+        self.last_batch = b.batch
+
+    def grad_phase2(self, global_batch: int):
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_cnn_grad_phase2(self.h, int(global_batch), self._stream()))
+
+    def apply(self, iteration: int):
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_cnn_apply(self.h, int(iteration), self._stream()))
+
+    def dp_export(self) -> bytes:
+        """Allocate this rank's exchange buffer; its CUDA IPC handle (to be handed to every other rank)."""
+        buf = C.create_string_buffer(_lib.IPC_HANDLE_BYTES)
+        n = C.c_int64(0)
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_cnn_dp_export(self.h, buf, C.byref(n)))
+        return buf.raw
+
+    def dp_connect(self, rank: int, handles: Sequence[bytes]):
+        """Map every rank's exchange buffer (`handles` in rank order, one per rank including this one)."""
+        blob = b"".join(handles)
+        if len(blob) != _lib.IPC_HANDLE_BYTES * len(handles):
+            raise ValueError("malformed IPC handle list")
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_cnn_dp_connect(self.h, int(rank), len(handles), blob))
+        self.dp_world = len(handles)
+
+    def dp_step(self, data, iteration: int, global_batch: int, noise=None):
+        """dsact_cnn_step on this rank's shard with the exchanges done in-kernel over peer memory."""
+        with torch.cuda.device(self.device):
+            b, n = self._args(data, noise)
+            check(self.lib.dsact_cnn_dp_step(self.h, C.byref(b), n, int(global_batch), int(iteration), self._stream()))
+        self.last_batch = b.batch
 
     # ---- device replay ring (flattened image rows) ---------------------------------------------------------------------
     @property
@@ -238,4 +290,6 @@ class CnnEngine:
         with torch.cuda.device(self.device):
             check(self.lib.dsact_cnn_read_stats(self.h, int(global_batch or self.last_batch), self._stats_host.data_ptr(), self._stream()))
             torch.cuda.current_stream(self.device).synchronize()
+        if float(self._stats_host[14]) != 0.0:   # include/dsact.h: slot 14 = 1 + rank of a peer that never arrived (dp_step)
+            raise _lib.DsactError(f"data-parallel exchange timed out waiting for rank {int(self._stats_host[14]) - 1}")
         return dict(zip(STAT_KEYS, self._stats_host.tolist()))

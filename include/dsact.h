@@ -265,6 +265,21 @@ int dsact_cnn_replay_bind(dsact_cnn_handle *h, const dsact_replay *rb);
 int dsact_cnn_replay_add(dsact_cnn_handle *h, const float *obs, const float *obs2, const float *act, const float *rew,
                          const float *done, const float *logp, int64_t n, int64_t ptr, void *stream);
 int dsact_cnn_replay_sample(dsact_cnn_handle *h, int32_t batch, int64_t size, const int64_t *idx, dsact_batch *out, void *stream);
+/* Split form and data-parallel replicas of the head-wise DSAC-T step, with the semantics of their MLP-engine namesakes:
+ * dsact_cnn_grad_phase1 (forwards; local critic-std sums in state[DSACT_STATE_STDSUM..+1]), dsact_cnn_grad_phase2 (losses
+ * and backward passes with means over `global_batch` >= the phase-1 batch; the log_alpha gradient is this shard's additive
+ * share), dsact_cnn_compute_grads (= phase 1 + phase 2 on its own rows), dsact_cnn_apply (Adam / Polyak on whatever
+ * `grads` holds; also on a handle that never ran phase 2).  dsact_cnn_dp_export / _connect / _step: the peer-memory
+ * exchange of dsact_dp_* (same buffer layout, kernels, rank-ordered sums, timeout and tb_info slot 14), eager on
+ * `stream`.  dsact_cnn_step = phase 1 + phase 2 + apply.  DSAC_V1 handles (algo = 1) return DSACT_EINVAL from all seven. */
+int dsact_cnn_grad_phase1(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, void *stream);
+int dsact_cnn_grad_phase2(dsact_cnn_handle *h, int64_t global_batch, void *stream);
+int dsact_cnn_compute_grads(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, void *stream);
+int dsact_cnn_apply(dsact_cnn_handle *h, int64_t iteration, void *stream);
+int dsact_cnn_dp_export(dsact_cnn_handle *h, void *handle_out, int64_t *bytes_out);
+int dsact_cnn_dp_connect(dsact_cnn_handle *h, int32_t rank, int32_t world, const void *handles);
+int dsact_cnn_dp_step(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, int64_t global_batch,
+                      int64_t iteration, void *stream);
 
 /* introspection for tests/bench: number of kernel launches (graph nodes included)
  * submitted by this handle so far, and by the most recent entry-point call */
