@@ -525,14 +525,15 @@ __device__ __forceinline__ void pgrad_elem(const PolicyGradArgs& a, int row, int
 __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
   pdl_sync();
   extern __shared__ float gb[];   // [2A] block-local bias-gradient sums
-  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5, warp = threadIdx.x >> 5;
   const int A = a.A;
   for (int i = threadIdx.x; i < 2 * A; i += blockDim.x) gb[i] = 0.f;
   __syncthreads();
   const float coef = step_alpha(a.sc) * a.inv_global_batch;  // dL/dlogp
-  for (int j = lane; j < A; j += 32) {
+  for (int j0 = 0; j0 < A; j0 += 32) {   // block-uniform loop (barriers inside)
+    const int j = j0 + lane;
     float gb_mean = 0.f, gb_ls = 0.f;
-    for (int row = blockIdx.x * wpb + (threadIdx.x >> 5); row < a.B; row += gridDim.x * wpb) {
+    for (int row = blockIdx.x * wpb + warp; j < A && row < a.B; row += gridDim.x * wpb) {
       float gu, gls;
       pgrad_elem(a, row, j, coef, gu, gls);
       a.d_logits[(size_t)row * 2 * A + j] = gu;
@@ -542,10 +543,13 @@ __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
       gb_mean += gu;
       gb_ls += gls;
     }
-    atomicAdd(&gb[j], gb_mean);
-    atomicAdd(&gb[A + j], gb_ls);
+    // the warps add their partial sums in warp order, so the block's sum does not depend on warp timing (with at most
+    // two blocks, as for batches up to 16 rows, the bias gradient is then the same bits on every run)
+    for (int w = 0; w < wpb; ++w) {
+      if (warp == w && j < A) { gb[j] += gb_mean; gb[A + j] += gb_ls; }
+      __syncthreads();
+    }
   }
-  __syncthreads();
   for (int i = threadIdx.x; i < 2 * A; i += blockDim.x) atomicAdd((a.gbias_ls && i >= A) ? a.gbias_ls + (i - A) : a.gbias + i, gb[i]);
 }
 

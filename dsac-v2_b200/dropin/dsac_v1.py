@@ -4,9 +4,13 @@
 
 * `ApproxContainer`: `q`, `q_target`, `policy`, `policy_target` (the same `networks.mlp` / `networks.cnn` classes as
   DSAC-T) + `log_alpha`; on a CUDA device the parameters are views into the engine's flat buffers [q | policy | log_alpha].
+  Approximators: MLP with policy std_type "mlp_shared" / "mlp_separated" / "parameter", or CNN (`type_1` / `type_2`,
+  one conv_type for both networks, as in example_train/dsacv1_cnn_carracing_offasync.py).
 * `DSAC_V1.local_update(data, iteration) -> tb_info` runs the whole update in the CUDA library; no CPU fallback.
   `get_remote_update_info` / `remote_update` (the gradient-message seam of the reference's asynchronous trainers) are not
   part of this engine and raise.
+* `full_state_dict` / `load_full_state_dict`: weights, Adam moments and counters, the device generator's state, in the
+  "dsact-full-state-1" format of `dsac_v2.DSAC_V2` (what `OffSerialTrainer` writes with `dsact_full_checkpoint`).
 
 Extra kwargs: `dsact_noise` = "device" (default) | "reference" (draw eps1, eps2 and the three z's of one update from torch's
 CPU generator in the reference's order), `dsact_max_batch`, `seed`.
@@ -23,6 +27,8 @@ import torch.nn as nn
 import networks.cnn as _cnn
 import networks.mlp as _mlp
 from dsact_host import TB_TAGS as tb_tags
+from dsact_host import full_state_dict as _full_state
+from dsact_host import load_full_state_dict as _load_full_state
 from dsact_host import net_kwargs
 
 from dsac_v2_b200 import _lib
@@ -43,10 +49,6 @@ class ApproxContainer(nn.Module):
         if q_args["apprfunc"] != pi_args["apprfunc"]:
             raise NotImplementedError("value and policy approximators must be of the same type (both MLP or both CNN)")
         cnn = q_args["apprfunc"] == "CNN"
-        if cnn:   # the engine's DSAC_V1 step is wired for encoders too, but only the MLP configuration is pinned to the reference
-            raise NotImplementedError("DSAC_V1 on the CUDA engine: MLP approximators (the CNN configuration is not validated)")
-        if pi_args["std_type"] != "mlp_shared":   # same reason: wired in the engine (pi_std 0 / 1 with algo = 1), no reference golden
-            raise NotImplementedError("DSAC_V1 on the CUDA engine: policy std_type 'mlp_shared' (the reference's default for DSAC_V1)")
         mod = _cnn if cnn else _mlp
         q_cls, pi_cls = getattr(mod, q_args["name"], None), getattr(mod, pi_args["name"], None)
         if q_cls is None or pi_cls is None:
@@ -183,6 +185,15 @@ class DSAC_V1:
         tb = {k: vals[i] for k, i in _V1_KEYS}
         tb[tb_tags["alg_time"]] = (time.time() - t0) * 1000
         return tb
+
+    # ---- full training state (the reference saves weights only, training/trainer.py:137-152) ----
+    def full_state_dict(self) -> dict:
+        """Everything a bit-for-bit resume needs beyond `networks.state_dict()`: Adam moments and step counters, the
+        device generator's seed/counter."""
+        return _full_state(self.networks)
+
+    def load_full_state_dict(self, state: dict) -> None:
+        _load_full_state(self.networks, state)
 
     def get_remote_update_info(self, data: Dict, iteration: int):
         raise NotImplementedError("DSAC_V1 on the CUDA engine: local_update only (no gradient-message seam)")

@@ -31,6 +31,8 @@ import torch.nn as nn
 import networks.cnn as _cnn
 import networks.mlp as _mlp
 from dsact_host import TB_TAGS as tb_tags
+from dsact_host import full_state_dict as _full_state
+from dsact_host import load_full_state_dict as _load_full_state
 from dsact_host import net_kwargs
 
 from dsac_v2_b200 import _lib, dp
@@ -322,32 +324,10 @@ class DSAC_V2:
     def full_state_dict(self) -> dict:
         """Everything a bit-for-bit resume needs beyond the 53-key `networks.state_dict()`: Adam moments and step
         counters, the mean_std EMA pair, the device generator's seed/counter."""
-        eng = self.networks.engine()
-        st = eng.state.detach().cpu()
-        ints = st[:16].view(torch.int32)
-        return {
-            "format": "dsact-full-state-1",
-            "networks": self.networks.state_dict(),
-            "adam_m": eng.adam_m.detach().cpu().clone(),
-            "adam_v": eng.adam_v.detach().cpu().clone(),
-            "mean_std": [float(st[0]), float(st[1])],
-            "adam_steps": [int(ints[8]), int(ints[9])],
-            "rng_counter": int(ints[10]) & 0xFFFFFFFF,
-            "rng_seed": int(getattr(eng, "_seed", 0)),
-        }
+        return _full_state(self.networks)
 
     def load_full_state_dict(self, state: dict) -> None:
-        if state.get("format") != "dsact-full-state-1":
-            raise ValueError("not a dsact full-state checkpoint")
-        self.networks.load_state_dict(state["networks"])
-        eng = self.networks.engine()
-        with torch.no_grad():
-            eng.adam_m.copy_(state["adam_m"])
-            eng.adam_v.copy_(state["adam_v"])
-            ints = eng.state[:16].view(torch.int32)
-            ints[10] = int(state["rng_counter"]) - (1 << 32 if int(state["rng_counter"]) >= (1 << 31) else 0)
-        eng.set_carry(state["mean_std"][0], state["mean_std"][1], state["adam_steps"][0], state["adam_steps"][1])
-        eng.seed(state["rng_seed"])
+        _load_full_state(self.networks, state)
 
     # ---- reference interface ------------------------------------------------------
     def local_update(self, data: Dict, iteration: int) -> dict:

@@ -120,6 +120,43 @@ class ActionDistributionMixin:
         return dist
 
 
+FULL_STATE_FORMAT = "dsact-full-state-1"
+
+
+def full_state_dict(networks) -> dict:
+    """Everything a bit-for-bit resume needs beyond `networks.state_dict()`: Adam moments and step counters, the
+    mean_std EMA pair, the device generator's seed/counter.  `networks` is an `ApproxContainer` of `dsac_v2` or
+    `dsac_v1`; both engines keep these in the same state slots (include/dsact.h)."""
+    eng = networks.engine()
+    st = eng.state.detach().cpu()
+    ints = st[:16].view(torch.int32)
+    return {
+        "format": FULL_STATE_FORMAT,
+        "networks": networks.state_dict(),
+        "adam_m": eng.adam_m.detach().cpu().clone(),
+        "adam_v": eng.adam_v.detach().cpu().clone(),
+        "mean_std": [float(st[0]), float(st[1])],
+        "adam_steps": [int(ints[8]), int(ints[9])],
+        "rng_counter": int(ints[10]) & 0xFFFFFFFF,
+        "rng_seed": int(getattr(eng, "_seed", 0)),
+    }
+
+
+def load_full_state_dict(networks, state: dict) -> None:
+    """Restore what `full_state_dict` saved into the networks' engine."""
+    if state.get("format") != FULL_STATE_FORMAT:
+        raise ValueError("not a dsact full-state checkpoint")
+    networks.load_state_dict(state["networks"])
+    eng = networks.engine()
+    with torch.no_grad():
+        eng.adam_m.copy_(state["adam_m"])
+        eng.adam_v.copy_(state["adam_v"])
+        ints = eng.state[:16].view(torch.int32)
+        ints[10] = int(state["rng_counter"]) - (1 << 32 if int(state["rng_counter"]) >= (1 << 31) else 0)
+    eng.set_carry(state["mean_std"][0], state["mean_std"][1], state["adam_steps"][0], state["adam_steps"][1])
+    eng.seed(state["rng_seed"])
+
+
 def net_kwargs(kind: str, kwargs: dict) -> dict:
     """Per-network constructor arguments out of the flat kwargs dict; same keys and
     defaults as reference utils/common_utils.py:48-89 (MLP branch)."""

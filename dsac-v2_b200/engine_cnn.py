@@ -276,6 +276,13 @@ class CnnEngine:
                 "act": view(out.act, B * A, (B, A)), "rew": view(out.rew, B, (B,)), "done": view(out.done, B, (B,)),
                 "logp": view(out.logp, B, (B,))}
 
+    def set_carry(self, mean_std1=-1.0, mean_std2=-1.0, adam_steps_q=0, adam_steps_pi=0):
+        """The state one update carries to the next besides weights and Adam moments: the mean_std EMA pair (-1 = not
+        started; unused by DSAC_V1) and the Adam step counters of the critic and policy optimizers."""
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_cnn_set_carry(self.h, float(mean_std1), float(mean_std2), int(adam_steps_q),
+                                               int(adam_steps_pi), self._stream()))
+
     def seed(self, seed: int):
         self._seed = int(seed) & (2 ** 64 - 1)
         check(self.lib.dsact_cnn_seed(self.h, self._seed))

@@ -230,13 +230,28 @@ def make_weights_std(cfg: dict, std_type: str, seed: int = 0) -> dict:
 
 
 # ---- DSAC_V1 (reference dsac_v1.py; SURVEY.md §8f rank 4) --------------------------------------------------------------
-def make_weights_v1(cfg: dict, seed: int = 0) -> dict:
-    """`make_weights` in the schema of `dsac_v1.ApproxContainer` (:17-52): one critic `q.q.*`, `policy.policy.*`, targets."""
-    w = make_weights(cfg, seed)
+def to_v1_schema(weights: dict) -> dict:
+    """DSAC-T weights in the schema of `dsac_v1.ApproxContainer` (:17-52): critic `q1` (and its target) becomes the one
+    critic `q`, `q2` is dropped, the policy and its target are kept."""
     out = {}
-    for k, v in w.items():
+    for k, v in weights.items():
         if k.startswith("q1"):
             out["q" + k[2:]] = v.copy()
         elif k.startswith("policy"):
             out[k] = v.copy()
     return out
+
+
+def make_weights_v1(cfg: dict, seed: int = 0) -> dict:
+    """`make_weights` in the V1 schema: one critic `q.q.*`, `policy.policy.*`, targets."""
+    return to_v1_schema(make_weights(cfg, seed))
+
+
+def make_cnn_weights_v1(cfg: dict, seed: int = 0) -> dict:
+    """`make_cnn_weights` in the V1 schema: `q.conv.*`, `q.mean.*`, `q.log_std.*`, the CNN policy, targets."""
+    return to_v1_schema(make_cnn_weights(cfg, seed))
+
+
+def make_weights_std_v1(cfg: dict, std_type: str, seed: int = 0) -> dict:
+    """`make_weights_std` in the V1 schema: one critic `q.q.*`, the policy of `std_type`, targets."""
+    return to_v1_schema(make_weights_std(cfg, std_type, seed))

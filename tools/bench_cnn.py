@@ -4,9 +4,11 @@ observations) at a fixed global batch (default 1024).  --gpus N > 1 spawns one p
 batch and runs the peer-memory data-parallel step (`CnnEngine.dp_step`).  Device-resident minibatches; prints one JSON line
 with steps/s, the card's name, power limit and the clocks during the timed region, and whether the replicas ended
 bit-identical (checksums all-gathered, as bench.py's replica check does).  With --cpu (one GPU only), the oracle port on
-the host cores for the same step.
+the host cores for the same step.  --algorithm DSAC_V1 times the older algorithm's update (one critic, fixed TD bound;
+the reference's example_train/dsacv1_cnn_carracing_offasync.py) with the same encoder and heads, on one GPU: DSAC_V1 has
+no data-parallel step.
 
-    python tools/bench_cnn.py [--gpus 1] [--batch 1024] [--steps 20] [--warmup 3] [--cpu]
+    python tools/bench_cnn.py [--algorithm DSAC_V2|DSAC_V1] [--gpus 1] [--batch 1024] [--steps 20] [--warmup 3] [--cpu]
 """
 import argparse
 import json
@@ -49,10 +51,12 @@ def run(rank, world, a, out_path):
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
     lo, hi = dp.shard_rows(a.batch, rank, world)
     B = hi - lo
-    c = make_cnn_config(cfg["obs_dim"], cfg["act_dim"], t["kernels"], t["channels"], t["strides"], t["heads"], max_batch=B)
+    v1 = a.algorithm == "DSAC_V1"
+    c = make_cnn_config(cfg["obs_dim"], cfg["act_dim"], t["kernels"], t["channels"], t["strides"], t["heads"], max_batch=B,
+                        algo=a.algorithm)
     lim = torch.full((cfg["act_dim"],), cfg["act_lim"])
     eng = CnnEngine(c, dev, lim, -lim)
-    eng.load_weights(synth.make_cnn_weights(cfg))
+    eng.load_weights(synth.make_cnn_weights_v1(cfg) if v1 else synth.make_cnn_weights(cfg))
     if dist is not None and not dp.connect_peers(eng, dist):
         raise SystemExit("the ranks could not map each other's exchange buffers (peer transport unavailable)")
     g = torch.Generator(device=dev).manual_seed(3 + rank)
@@ -85,9 +89,10 @@ def run(rank, world, a, out_path):
         dist.all_gather(gathered, cs)
         identical = all(bool(torch.equal(x, gathered[0])) for x in gathered)
     if rank == 0:
-        out = {"metric": "DSAC-T gradient-steps/sec, CNN encoder (carracing type_2, 3x96x96), global batch %d on %d GPU(s)" % (a.batch, world),
+        name = "DSAC_V1" if v1 else "DSAC-T"
+        out = {"metric": "%s gradient-steps/sec, CNN encoder (carracing type_2, 3x96x96), global batch %d on %d GPU(s)" % (name, a.batch, world),
                "value": 1000.0 / ms, "unit": "steps/s", "ms_per_step": ms, "steps": a.steps, "warmup": a.warmup, "dtype": "f32",
-               "data": "synthetic", "gpus": world, "transport": "peer" if world > 1 else None,
+               "algorithm": a.algorithm, "data": "synthetic", "gpus": world, "transport": "peer" if world > 1 else None,
                "config": {"workload": "gym_carracing shapes, conv(4,3,3,3,3,3)/(8..256) + mean/log_std heads [256,256,256], fp32 direct convolutions",
                           "batch": a.batch, "shard_rows": [dp.shard_rows(a.batch, r, world)[1] - dp.shard_rows(a.batch, r, world)[0] for r in range(world)]},
                "card": card(0), "clocks_rank0": clocks.summary(), "finite": bool(all(v == v for v in stats.values())),
@@ -109,6 +114,7 @@ def _spawned(rank, world, a, out_path):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--algorithm", choices=("DSAC_V2", "DSAC_V1"), default="DSAC_V2")
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--batch", type=int, default=1024, help="global batch (split over the GPUs)")
     ap.add_argument("--steps", type=int, default=20)
@@ -116,10 +122,14 @@ def main():
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--port", type=int, default=29400 + os.getpid() % 1000)
     a = ap.parse_args()
+    if a.algorithm == "DSAC_V1" and a.gpus > 1:
+        raise SystemExit("--algorithm DSAC_V1 runs on one GPU: DSAC_V1 has no data-parallel step (use --gpus 1)")
     if a.gpus < 1 or a.gpus > torch.cuda.device_count():
         raise SystemExit(f"--gpus {a.gpus}: this host has {torch.cuda.device_count()} CUDA device(s)")
     if a.cpu and a.gpus > 1:
         raise SystemExit("--cpu compares against one GPU: use it with --gpus 1")
+    if a.algorithm == "DSAC_V1" and a.cpu:
+        raise SystemExit("--cpu times the DSAC-T step only: use it without --algorithm DSAC_V1")
     with tempfile.TemporaryDirectory() as tmp:
         out_path = os.path.join(tmp, "result.json")
         if a.gpus == 1:
