@@ -601,7 +601,7 @@ static void cnn_enqueue_apply(dsact_cnn_handle* h, Ctx& c, int scalars_ready, bo
   a.g_lo = 0; a.g_hi = (n_all + 3) / 4; a.finish = 1;
   int blocks = (int)(((n_all + 3) / 4 + 255) / 256); if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
   if (dp) {
-    a.dp_timeout_ns = dp_timeout_ns(); a.dp_wait_kind = 2;
+    a.dp_timeout_ns = dp_timeout_ns();
     dp_apply_args(h->dp, a);
     launch_k(apply_kernel<2>, blocks, 256, 0, c, a);
   } else {
@@ -886,7 +886,7 @@ int dsact_cnn_dp_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact
     c.done();
   }
   enqueue_dp_exchange(h->dp, state, 1, c);
-  if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, state, 2 * h->q.n, h->num_sms, c, 0);
+  if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, state, h->num_sms, c);
   cnn_enqueue_apply(h, c, 1, true);
   if ((rc = cnn_finish(h, c))) return rc;
   h->dev_iter = iteration + 1;

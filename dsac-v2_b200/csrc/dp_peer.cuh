@@ -4,18 +4,16 @@
 // no NCCL launch between the phases.
 //
 // Per rank one cudaMalloc'd exchange buffer (floats):
-//   [0, 128)                      arrival flags (uint32 epochs): flag[kind * 16 + source_rank]; words 96, 97: block tickets
+//   [0, 128)                      arrival flags (uint32 epochs): flag[kind * 16 + source_rank]; word 96: block ticket
 //   [128, 128 + 2*2*R*32)         small payloads: small[kind][parity][source_rank][32]
 //   [DP_GRADS_OFF, + n_params)    this rank's local gradient sum of the running step
 //   [DP_GRADS_OFF + n_pad, + n_params)  the global gradient sum ("reduced" block; two-shot exchange only, see below)
 // kind 0 = after the forward passes (2 std sums, SUM), kind 1 = before Adam (16 logged sums SUM + 2 minima MIN; it is
-// also the "local gradients are complete" barrier), kind 3 = "the critics' gradients are complete" (no payload): the
-// critics' part of the exchange and of the update runs on a side branch beside the policy backward (SURVEY.md §8e:
-// "Q1|Q2 grads when critic backward completes, pi grads + log_alpha grad after actor backward"), kinds 2 / 4 = the
-// reduced slices of the two-shot exchange have arrived (policy part / critics' part).  Every rank pushes its payload into every peer's buffer, raises
-// its flag there (release, system scope) and polls only its own memory.  Reductions run in rank order on every rank,
-// so the replicas stay bit-identical.  Reuse is safe without further barriers: a rank overwrites its gradient block
-// in phase 2 of step t+1, i.e. after the kind-0 barrier of t+1, which every peer reaches only after its apply of t.
+// also the "local gradients are complete" barrier), kind 2 = the reduced slices of the two-shot exchange have arrived
+// (no payload).  Every rank pushes its payload into every peer's buffer, raises its flag there (release, system scope)
+// and polls only its own memory.  Reductions run in rank order on every rank, so the replicas stay bit-identical.
+// Reuse is safe without further barriers: a rank overwrites its gradient block in phase 2 of step t+1, i.e. after the
+// kind-0 barrier of t+1, which every peer reaches only after its apply of t.
 //
 // Gradient exchange, two variants.  ONE-SHOT (world < 6): apply_kernel reads every rank's block through NVLink and sums
 // in rank order — (N-1) x n floats cross the links per rank.  TWO-SHOT (world >= 6, dp_reduce_scatter_kernel): rank r
@@ -31,8 +29,8 @@
 namespace dsact {
 
 constexpr int DP_MAX_RANKS = 8;
-constexpr int DP_FLAGS = 128;   // 6 kinds x 16 ranks of arrival flags, then the block tickets of the reduce-scatter launches
-constexpr int DP_TICKET = 96;   // header words 96, 97
+constexpr int DP_FLAGS = 128;   // kinds 0-2 x 16 ranks of arrival flags, then the block ticket of the reduce-scatter launch
+constexpr int DP_TICKET = 96;   // header word 96
 constexpr int DP_SMALL = 32;
 constexpr int DP_SMALL_OFF = DP_FLAGS;
 constexpr int DP_GRADS_OFF = 2048;   // floats; 8 KiB header
@@ -85,7 +83,7 @@ __global__ void dp_exchange_kernel(const DpComm c, float* __restrict__ state, in
   int* sti = reinterpret_cast<int*>(state);
   const uint32_t e = (uint32_t)sti[ST_DP_EPOCH] + (kind == 0 ? 1u : 0u);
   const int par = (int)(e & 1u);
-  const int n = kind == 0 ? 2 : (kind == 1 ? 18 : 0);   // kind 3: arrival only
+  const int n = kind == 0 ? 2 : 18;
   float* src = kind == 0 ? state + ST_STDSUM : state + ST_ACC;   // (the 2 minima sit at ST_ACC + 16, 17)
   const int t = threadIdx.x, p = t >> 5, i = t & 31;
   // 1. push my payload into every rank's small[kind][par][my rank][...]
@@ -150,7 +148,6 @@ struct DpSlice {
   long long g_lo, g_hi;      // float4 groups of this rank's slice
   long long red_off;         // floats from a rank's buffer base to its reduced block
   int* ticket;               // zero-initialised int in this rank's buffer header
-  int flag_kind;             // 2 (policy part or the whole buffer) or 4 (critics' part)
 };
 __global__ void __launch_bounds__(256) dp_reduce_scatter_kernel(const DpComm c, const DpSlice sl, const float* __restrict__ state) {
   pdl_sync();
@@ -176,15 +173,15 @@ __global__ void __launch_bounds__(256) dp_reduce_scatter_kernel(const DpComm c, 
     if (atomicAdd(sl.ticket, 1) == (int)gridDim.x - 1) {
       *sl.ticket = 0;
       __threadfence_system();
-      for (int r = 0; r < c.world; ++r) st_release_sys(reinterpret_cast<uint32_t*>(c.peer[r]) + sl.flag_kind * 16 + c.rank, e);
+      for (int r = 0; r < c.world; ++r) st_release_sys(reinterpret_cast<uint32_t*>(c.peer[r]) + 2 * 16 + c.rank, e);
     }
   }
 }
 
 // apply_kernel's side of the two-shot exchange: one thread per block waits until every rank's kind-2 flag of this epoch
 // has arrived in this rank's own memory (the reduced block is then complete).  Returns false on timeout.
-__device__ __forceinline__ bool dp_wait_reduced(const float* own_buf, int world, uint32_t epoch, unsigned long long timeout_ns, int kind) {
-  const uint32_t* flags = reinterpret_cast<const uint32_t*>(own_buf) + kind * 16;
+__device__ __forceinline__ bool dp_wait_reduced(const float* own_buf, int world, uint32_t epoch, unsigned long long timeout_ns) {
+  const uint32_t* flags = reinterpret_cast<const uint32_t*>(own_buf) + 2 * 16;
   const unsigned long long t0 = dp_time_ns();
   for (int r = 0; r < world; ++r)
     while ((int32_t)(ld_acquire_sys(flags + r) - epoch) < 0) {

@@ -118,7 +118,6 @@ struct Arena {
       // batch split of the weight-gradient GEMMs: at most 4 slabs of >= 256 rows (more slabs mean more partial tiles to
       // write and to fold in apply)
       nslabs = (int)(B / 256); if (nslabs > 4) nslabs = 4; if (nslabs < 1) nslabs = 1;
-      if (getenv("DSACT_WG_SLABS")) { const int v = atoi(getenv("DSACT_WG_SLABS")); if (v >= 1 && v <= 16 && v * 128 <= B) nslabs = v; }   // tuning aid
       slab_stride = (2 * q.n + pi.n + 1 + 3) / 4 * 4;
       slabs = take((int64_t)nslabs * slab_stride);
     }
@@ -170,7 +169,7 @@ struct dsact_handle {
   int32_t last_launches;
   bool tc() const { return cfg.gemm_mode != DSACT_GEMM_FP32; }
   bool fused() const {  // layer-chain kernel: every layer must fit one 256-column wgmma accumulator / A operand
-    if (!tc() || getenv("DSACT_NO_FUSE")) return false;
+    if (!tc()) return false;
     for (int j = 1; j <= q.L + 1; ++j) if (q.s[j] > 256) return false;
     for (int j = 1; j <= pi.L + 1; ++j) if (pi.s[j] > 256) return false;
     for (int j = 1; j <= q.L; ++j) if (q.s[j] % 8) return false;    // hidden widths: multiples of 8 (the validated shapes)
@@ -200,7 +199,7 @@ struct Ctx {
   cudaError_t err;
   Prof* prof = nullptr;
   cudaStream_t side = nullptr;   // optional second stream for an independent branch (null: serialise on `s`)
-  bool pdl = true;               // programmatic dependent launch for this enqueue (off in fp32 mode, see pdl_enabled)
+  bool pdl = true;               // programmatic dependent launch for this enqueue (off in fp32 mode, see launch_k)
   void check() { cudaError_t e = cudaGetLastError(); if (e != cudaSuccess && err == cudaSuccess) err = e; }
   void done(int cls = CLS_OTHER, double flops = 0.0) {
     launches++;
@@ -216,14 +215,8 @@ struct Ctx {
 };
 
 // Every kernel goes out with the programmatic-dependent-launch attribute (each kernel begins with griddepcontrol.wait),
-// so that inside the captured graph a kernel's launch and prologue overlap its predecessor's tail (tools/pdl_ab.sh
-// compares both).  DSACT_PDL=0 turns it off.  The fp32 SIMT mode launches without it: its multi-wave GEMM grids would
-// lose SM slots to early-launched dependents.
-static bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("DSACT_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
+// so that inside the captured graph a kernel's launch and prologue overlap its predecessor's tail.  The fp32 SIMT mode
+// launches without it: its multi-wave GEMM grids would lose SM slots to early-launched dependents.
 template <typename... KArgs, typename... Args>
 static void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Ctx& c, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -231,7 +224,7 @@ static void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = (pdl_enabled() && c.pdl) ? 1 : 0;
+  cfg.attrs = at; cfg.numAttrs = c.pdl ? 1 : 0;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
   if (e != cudaSuccess && c.err == cudaSuccess) c.err = e;
 }
@@ -308,7 +301,6 @@ static void launch_tc(dsact_handle* h, Group& G, int variant, Ctx& c, int max_ct
     int ctas = 0;
     for (int i = 0; i < G.n; ++i) ctas += ((G.prob(i).M + TC_BM - 1) / TC_BM) * ((G.prob(i).N + 127) / 128) * (G.wg_slab ? G.wg_nslabs : h->ar.nslabs);
     if (ctas * 2 <= h->num_sms) wg_bn = 64;
-    if (getenv("DSACT_WG_BN")) { const int v = atoi(getenv("DSACT_WG_BN")); if (v == 64 || v == 128 || v == 256) wg_bn = v; }   // tuning aid
   }
   for (int i = 0; i < G.n; ++i) {
     const GemmProb& s = G.prob(i);
@@ -681,10 +673,6 @@ static void enqueue_noise(dsact_handle* h, int B, Ctx& c) {
   launch_k(noise_kernel, blocks, 256, 0, c, W + ar.eps1, W + ar.eps2, W + ar.z3, W + ar.z4, B, A, h->seed, h->buf.state);
   c.done();
 }
-static bool prologue_merged() {   // DSACT_PROLOGUE_MERGE=0: separate clear / image / noise launches (A/B aid)
-  static const bool off = getenv("DSACT_PROLOGUE_MERGE") && getenv("DSACT_PROLOGUE_MERGE")[0] == '0';
-  return !off;
-}
 static void enqueue_prologue(dsact_handle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged,
                              bool with_noise = true) {
   const dsact_config& cf = h->cfg;
@@ -701,10 +689,10 @@ static void enqueue_prologue(dsact_handle* h, const dsact_batch& bt, const dsact
   const long long n_grads = 2 * q.n + pi.n + 1;
   int zero_blocks = (int)((n_grads / 4 + 255) / 256); if (zero_blocks > 2 * h->num_sms) zero_blocks = 2 * h->num_sms; if (zero_blocks < 1) zero_blocks = 1;
   const bool want_noise = !nz && with_noise;
-  const bool merged = tc && prologue_merged();   // tensor-core modes: clears + images + noise as one launch
-  if (!merged) { launch_k(begin_step_kernel, zero_blocks, 256, 0, c, h->buf.state, h->buf.grads, n_grads); c.done(); }
+  if (!tc) { launch_k(begin_step_kernel, zero_blocks, 256, 0, c, h->buf.state, h->buf.grads, n_grads); c.done(); }
 
-  if (tc) {  // refresh the weight images (the caller may have written params/targets through its views) + inputs
+  if (tc) {  // refresh the weight images (the caller may have written params/targets through its views) + inputs; the clears
+             // and the device noise ride in the same launch
     ImgBatch ib;
     for (int n = 0; n < 2; ++n)
       for (int j = 0; j <= q.L; ++j) {
@@ -729,26 +717,22 @@ static void enqueue_prologue(dsact_handle* h, const dsact_batch& bt, const dsact
       ib.add(bt.obs2, O, h->img(ar.i_obs2, B), B, O);
       ib.add(bt.act, A, h->img(ar.i_act, B), B, A);
     }
-    if (merged) {
-      PrologueArgs pa;
-      memset(&pa, 0, sizeof(pa));
-      pa.zero_blocks = zero_blocks;
-      pa.state = h->buf.state; pa.grads = h->buf.grads; pa.n_grads = n_grads;
-      pa.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-      if (want_noise) {
-        const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
-        pa.noise_blocks = (total / 2 + 255) / 256; if (pa.noise_blocks < 1) pa.noise_blocks = 1;
-        pa.eps1 = W + ar.eps1; pa.eps2 = W + ar.eps2; pa.z3 = W + ar.z3; pa.z4 = W + ar.z4;
-        pa.B = B; pa.A = A; pa.seed = h->seed;
-      }
-      ib.launch(h, c, &pa);
-    } else {
-      ib.launch(h, c);
+    PrologueArgs pa;
+    memset(&pa, 0, sizeof(pa));
+    pa.zero_blocks = zero_blocks;
+    pa.state = h->buf.state; pa.grads = h->buf.grads; pa.n_grads = n_grads;
+    pa.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
+    if (want_noise) {
+      const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
+      pa.noise_blocks = (total / 2 + 255) / 256; if (pa.noise_blocks < 1) pa.noise_blocks = 1;
+      pa.eps1 = W + ar.eps1; pa.eps2 = W + ar.eps2; pa.z3 = W + ar.z3; pa.z4 = W + ar.z4;
+      pa.B = B; pa.A = A; pa.seed = h->seed;
     }
+    ib.launch(h, c, &pa);
   }
 
   // device noise; the counter it reads is stepped by sample_kernel, once every reader of this step has run
-  if (want_noise && !merged) enqueue_noise(h, B, c);
+  if (want_noise && !tc) enqueue_noise(h, B, c);
   c.check();
 }
 
@@ -772,37 +756,20 @@ static unsigned long long dp_timeout_ns() {
       (unsigned long long)(getenv("DSACT_DP_TIMEOUT_MS") ? atoll(getenv("DSACT_DP_TIMEOUT_MS")) : 10000) * 1000000ull;
   return t;
 }
-// two-shot gradient exchange (dp_peer.cuh) from 6 ranks up, one-shot below (fewer barriers); DSACT_DP_TWO_SHOT=0/1 overrides
-// DSACT_DP_SPLIT=1: the critics' part of the gradient exchange and of the update on the side branch, beside the policy
-// backward (SURVEY.md 8e's overlap).  Replicas stay bit-identical in both exchange variants; the data-parallel overhead is
-// barrier skew and launch count, which a second exchange adds to.  Default: one exchange.
-static bool dp_split_enabled() {
-  static const bool on = getenv("DSACT_DP_SPLIT") && getenv("DSACT_DP_SPLIT")[0] == '1';
-  return on;
-}
-static bool dp_two_shot(const DpPeer& dp) {
-  static const char* e = getenv("DSACT_DP_TWO_SHOT");
-  if (e && (e[0] == '0' || e[0] == '1')) return e[0] == '1';
-  return dp.comm.world >= 6;
-}
-// `part`: 0 = the whole buffer, 1 = the critics' groups [0, n_q2 / 4) (kind-4 flags), 2 = the rest (kind-2 flags)
-static void enqueue_dp_reduce_scatter(const DpPeer& dp, const float* state, long long n_q2, int num_sms, Ctx& c, int part = 0) {
-  const long long g_all = dp.npad() / 4, g_q = n_q2 / 4;
-  const long long G0 = part == 2 ? g_q : 0, G1 = part == 1 ? g_q : g_all;
-  const long long groups = G1 - G0, per = (groups + dp.comm.world - 1) / dp.comm.world;
+// two-shot gradient exchange (dp_peer.cuh) from 6 ranks up, one-shot below (fewer barriers).  Replicas stay bit-identical
+// in both variants.
+static bool dp_two_shot(const DpPeer& dp) { return dp.comm.world >= 6; }
+static void enqueue_dp_reduce_scatter(const DpPeer& dp, const float* state, int num_sms, Ctx& c) {
+  const long long groups = dp.npad() / 4, per = (groups + dp.comm.world - 1) / dp.comm.world;
   DpSlice sl;
-  sl.g_lo = G0 + per * dp.comm.rank;
-  sl.g_hi = sl.g_lo + per < G1 ? sl.g_lo + per : G1;
-  if (sl.g_lo > G1) sl.g_lo = G1;
+  sl.g_lo = per * dp.comm.rank;
+  sl.g_hi = sl.g_lo + per < groups ? sl.g_lo + per : groups;
+  if (sl.g_lo > groups) sl.g_lo = groups;
   sl.red_off = DP_GRADS_OFF + dp.npad();
-  sl.ticket = reinterpret_cast<int*>(dp.buf) + DP_TICKET + (part == 1 ? 1 : 0);   // block ticket of this launch
-  sl.flag_kind = part == 1 ? 4 : 2;
+  sl.ticket = reinterpret_cast<int*>(dp.buf) + DP_TICKET;
   int blocks = (int)((per + 255) / 256); if (blocks < 1) blocks = 1; if (blocks > 2 * num_sms) blocks = 2 * num_sms;
   launch_k(dp_reduce_scatter_kernel, blocks, 256, 0, c, dp.comm, sl, state);
   c.done();
-}
-static void enqueue_dp_reduce_scatter(dsact_handle* h, Ctx& c, int part = 0) {
-  enqueue_dp_reduce_scatter(h->dp, h->buf.state, 2 * h->q.n, h->num_sms, c, part);
 }
 
 // One exchange of the peer-memory data-parallel path (dp_peer.cuh): kind 0 = critic-std sums, 1 = logged sums.
@@ -812,8 +779,8 @@ static void enqueue_dp_exchange(const DpPeer& dp, float* state, int kind, Ctx& c
 }
 static void enqueue_dp_exchange(dsact_handle* h, int kind, Ctx& c) { enqueue_dp_exchange(h->dp, h->buf.state, kind, c); }
 
-// apply_kernel<2>'s view of the exchange: the reduced block in this rank's own memory once every rank's kind-2 (kind-4)
-// flag is here (two-shot), or every rank's block, summed in rank order (one-shot)
+// apply_kernel<2>'s view of the exchange: the reduced block in this rank's own memory once every rank's kind-2 flag is
+// here (two-shot), or every rank's block, summed in rank order (one-shot)
 static void dp_apply_args(const DpPeer& dp, ApplyArgs& a) {
   if (dp_two_shot(dp)) {
     a.dp_world = 1;
@@ -1005,27 +972,27 @@ static void enqueue_phase1(dsact_handle* h, const dsact_batch& bt, const dsact_n
   c.check();
 }
 
-// `defer_reduce`: the caller enqueues enqueue_apply(.., reduce_slabs = true) next, which folds the split slabs itself
+// the apply of a single-call step can fold the weight-gradient split slabs itself (apply_kernel<1>)
 static bool slabs_foldable(const dsact_handle* h) {
   return h->tc() && ((uintptr_t)(h->W() + h->ar.slabs) & 15) == 0 && ((uintptr_t)h->buf.grads & 15) == 0;
 }
-enum { REDUCE_INPLACE = 0, REDUCE_DEFER = 1, REDUCE_DP = 2 };   // where the weight-gradient slabs get folded
-static TailArgs tail_args(const dsact_handle* h, int64_t global_batch, int rows, bool enabled) {
+static TailArgs tail_args(const dsact_handle* h, int64_t global_batch, int rows) {
   const Net &q = h->q, &pi = h->pi;
   TailArgs t;
   t.sc.tau_b = (float)h->cfg.tau_b; t.sc.alpha_fixed = (float)h->cfg.alpha_fixed;
   t.sc.inv_global_batch = (float)(1.0 / (double)global_batch);
   t.sc.auto_alpha = h->cfg.auto_alpha; t.sc.log_alpha = h->buf.params + 2 * q.n + pi.n;
-  t.target_entropy = -(float)h->cfg.act_dim; t.rows = rows; t.enabled = enabled ? 1 : 0;
+  t.target_entropy = -(float)h->cfg.act_dim; t.rows = rows; t.enabled = 1;
   return t;
 }
-// `fold_tail`: the caller's next kernels (dp_grad_fold / apply) do the end-of-backward bookkeeping, no phase2_tail launch
-static void enqueue_apply(dsact_handle* h, Ctx& c, bool reduce_slabs, bool dp, const TailArgs* tail, int part);
-// `early_apply` (single-GPU fused steps with the folded tail): update the critics on the side branch as soon as their
-// weight gradients are complete, beside the policy backward; the caller's enqueue_apply then does the rest.
-static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t global_batch, Ctx& c, int reduce_mode = REDUCE_INPLACE,
-                           bool fold_tail = false, const TailArgs* early_apply = nullptr, bool dp_early = false) {
-  const bool defer_reduce = reduce_mode != REDUCE_INPLACE;
+static void enqueue_apply(dsact_handle* h, Ctx& c, const TailArgs* tail, bool dp, int part);
+// `tail` == null (split API): the weight-gradient slabs are folded into the gradient buffer here and phase2_tail_kernel
+// closes the backward.  Otherwise (single-call steps) the kernels that follow do both: enqueue_apply (dp = false), or
+// dp_grad_fold into this rank's exchange block (dp = true).  Single-GPU fused steps also update the critics on the side
+// branch as soon as their weight gradients are complete, beside the policy backward; the caller's enqueue_apply then
+// does the rest.
+static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t global_batch, Ctx& c, const TailArgs* tail = nullptr,
+                           bool dp = false) {
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
@@ -1064,33 +1031,18 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
   const Ten t_obs = ten(bt.obs, ar.i_obs), t_act = ten(bt.act, ar.i_act);
 
   // wave C: critic passes 0,1 (dgrad + wgrad) and actor passes 4,5 (dgrad only), top layer down.
-  // The freeze trick of the reference (dsac_v2.py:166-181) makes the two backward passes independent.  Default: one
-  // 4-pass dgrad chain, then the critics' weight gradients as a side branch beside the policy backward.  Opt-in
-  // (DSACT_BWD_SPLIT=1): the critics' own backward (dgrad chain 0,1 -> their weight gradients) as a side branch beside
-  // the whole actor path (dgrad chain 4,5 -> policy_grad -> policy dgrad chain -> policy weight gradients): two half-wave
-  // chain launches against an earlier start of the policy path.
+  // The freeze trick of the reference (dsac_v2.py:166-181) makes the two backward passes independent: one 4-pass dgrad
+  // chain, then the critics' weight gradients as a side branch beside the policy backward.
   Group gw;  // every weight-gradient problem of the two critics
   const bool fused = h->fused();
-  static const bool split_on = getenv("DSACT_BWD_SPLIT") && getenv("DSACT_BWD_SPLIT")[0] == '1';
-  const bool two_branches = fused && c.side != nullptr && split_on;
-  Ctx cs{c.side, 0, cudaSuccess};
-  cs.pdl = c.pdl;
-  if (two_branches) {
-    cudaEventRecord(h->ev_fork, c.s);
-    cudaStreamWaitEvent(c.side, h->ev_fork, 0);
-  }
-  if (fused) {  // dgrad as chain launches: dz stays in tensor memory between layers
-    auto chain_of = [&](int pp0, int pp1, Ctx& cx) {
-      ChainBuild cb(h->passes());
-      for (int pp = pp0; pp < pp1; ++pp) {
-        const int p = passes[pp], k = p & 1;
-        chain_dgrad_pass(cb, h, q, ar.i_wq[k], h->img(ar.i_dOut[p], B), B, cf.act_q, ar.zQ[p], p < 2 ? Gq[k] : nullptr,
-                         p < 2 ? ar.i_dzQ[p] : nullptr, p < 2 ? nullptr : W + ar.dAct[k], ar.kpad_q0, A);
-      }
-      launch_chain(h, cb, CLS_GEMM_DGRAD, cx);
-    };
-    if (two_branches) { chain_of(0, 2, cs); chain_of(2, 4, c); }
-    else chain_of(0, 4, c);
+  if (fused) {  // dgrad as one chain launch: dz stays on chip between layers
+    ChainBuild cb(h->passes());
+    for (int pp = 0; pp < 4; ++pp) {
+      const int p = passes[pp], k = p & 1;
+      chain_dgrad_pass(cb, h, q, ar.i_wq[k], h->img(ar.i_dOut[p], B), B, cf.act_q, ar.zQ[p], p < 2 ? Gq[k] : nullptr,
+                       p < 2 ? ar.i_dzQ[p] : nullptr, p < 2 ? nullptr : W + ar.dAct[k], ar.kpad_q0, A);
+    }
+    launch_chain(h, cb, CLS_GEMM_DGRAD, c);
   }
   for (int j = q.L; j >= 1; --j) {
     Group gd;
@@ -1115,28 +1067,17 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
         add_dgrad(gd, q, 0, weight(h, q, Pq[k], 0, ar.i_wq[k][0]), O, ar.kpad_q0, A, ten(W + ar.dzQ[4 + k][0], ar.i_dzQ[4 + k][0]),
                   ten(W + ar.dAct[k], none), nullptr, nullptr, B, 0);
     }
-    if (!two_branches && fused && c.side != nullptr) {   // one 4-pass chain on the main branch, the critics' weight gradients beside the policy backward
+    if (fused && c.side != nullptr) {   // the critics' weight gradients beside the policy backward
       cudaEventRecord(h->ev_fork, c.s);
       cudaStreamWaitEvent(c.side, h->ev_fork, 0);
-    }
-    if (fused && c.side != nullptr) {
+      Ctx cs{c.side, 0, cudaSuccess};
+      cs.pdl = c.pdl;
       // the policy backward chain needs ceil(B/128) whole SMs: keep them free of weight-gradient CTAs
       const int chain_ctas = (B + TC_BM - 1) / TC_BM;
       const int cap = h->num_sms - chain_ctas;
       launch_group(h, gw, V_WGRAD, cs, cap >= h->num_sms / 2 ? cap : 0);
-      if (early_apply && dp_early) {   // data parallel: the critics' blocks are exchanged and applied here, beside the policy backward
-        const long long nq = (2 * q.n) / 4 * 4;   // whole float4 groups of the critics' span
-        int blocks = (int)((nq / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
-        TailArgs none; memset(&none, 0, sizeof(none));
-        launch_k(dp_grad_fold_kernel, blocks, 256, 0, cs, h->dp.buf + DP_GRADS_OFF, (const float*)G_, (const float*)(W + ar.slabs), nq,
-                 ar.nslabs, (long long)ar.slab_stride, (const float*)h->buf.state, none);
-        cs.done();
-        enqueue_dp_exchange(h, 3, cs);
-        if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h, cs, 1);
-        enqueue_apply(h, cs, false, true, early_apply, 1);
-        h->apply_early = true;
-      } else if (early_apply) {   // Adam + Polyak of both critics beside the policy backward: every critic gradient is final here
-        enqueue_apply(h, cs, true, false, early_apply, 1);
+      if (tail && !dp && slabs_foldable(h)) {   // Adam + Polyak of both critics beside the policy backward: every critic gradient is final here
+        enqueue_apply(h, cs, tail, false, 1);
         h->apply_early = true;
       }
       cudaEventRecord(h->ev_join, c.side);
@@ -1182,39 +1123,31 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
   launch_group(h, gwp, V_WGRAD, c);
 
   if (h->join_pending) { cudaStreamWaitEvent(c.s, h->ev_join, 0); h->join_pending = false; }
-  if (tc && reduce_mode != REDUCE_DP && !(defer_reduce && slabs_foldable(h))) {  // fold the weight-gradient split slabs into the flat gradient buffer
+  if (tc && !dp && !(tail && slabs_foldable(h))) {  // fold the weight-gradient split slabs into the flat gradient buffer
     const long long n = 2 * q.n + pi.n + 1;
     int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
     launch_k(grad_reduce_kernel, blocks, 256, 0, c, G_, W + ar.slabs, n, ar.nslabs, (long long)ar.slab_stride); c.done();
   }
-  AdamHyper hy{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-  if (!fold_tail) {
-    launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, hy, defer_reduce ? 1 : 0);
+  if (!tail) {
+    AdamHyper hy{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
+    launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, hy, 0);
     c.done();
   }
-  if (reduce_mode == REDUCE_DP) {  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
-    const long long lo = h->apply_early ? (2 * q.n) / 4 * 4 : 0;   // the critics' groups went out on the side branch
-    const long long n = 2 * q.n + pi.n + 1 - lo;
+  if (dp) {  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
+    const long long n = 2 * q.n + pi.n + 1;
     int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF + lo, (const float*)G_ + lo, (const float*)(tc ? W + ar.slabs : G_) + lo, n,
-             tc ? ar.nslabs : 0, (long long)(tc ? ar.slab_stride : 4), (const float*)h->buf.state, tail_args(h, global_batch, B, fold_tail));
+    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF, (const float*)G_, (const float*)(tc ? W + ar.slabs : G_), n,
+             tc ? ar.nslabs : 0, (long long)(tc ? ar.slab_stride : 4), (const float*)h->buf.state, *tail);
     c.done();
   }
   c.check();
 }
 
-static bool fold_tail_enabled() {   // DSACT_FOLD_TAIL=0: keep the separate phase2_tail launch (A/B aid)
-  static const bool off = getenv("DSACT_FOLD_TAIL") && getenv("DSACT_FOLD_TAIL")[0] == '0';
-  return !off;
-}
-// `tail` != null: this apply also does the end-of-backward bookkeeping of the step (see TailArgs)
+// `tail` != null: this apply also does the end-of-backward bookkeeping of the step (see TailArgs) and, single-GPU, folds
+// the weight-gradient split slabs.  `dp`: the gradients are the rank-ordered sum of the exchange blocks.
 // `part`: 0 = the whole flat buffer; 1 = the critics' span only, without closing the step (launched beside the policy
 // backward, see enqueue_phase2); 2 = everything after that span + the end-of-step bookkeeping
-static bool apply_split_enabled() {   // DSACT_APPLY_SPLIT=0: one apply launch after the whole backward (A/B aid)
-  static const bool off = getenv("DSACT_APPLY_SPLIT") && getenv("DSACT_APPLY_SPLIT")[0] == '0';
-  return !off;
-}
-static void enqueue_apply(dsact_handle* h, Ctx& c, bool reduce_slabs = false, bool dp = false, const TailArgs* tail = nullptr, int part = 0) {
+static void enqueue_apply(dsact_handle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
   const dsact_config& cf = h->cfg;
   if (part == 0 && h->apply_early) { part = 2; h->apply_early = false; }   // phase 2 already updated the critics
   ApplyArgs a;
@@ -1223,21 +1156,20 @@ static void enqueue_apply(dsact_handle* h, Ctx& c, bool reduce_slabs = false, bo
   a.n_q2 = 2 * h->q.n; a.n_all = 2 * h->q.n + h->pi.n + 1;
   a.delay_update = cf.delay_update; a.auto_alpha = cf.auto_alpha;
   a.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-  a.scalars_ready = (reduce_slabs || dp) ? 1 : 0;   // single-call steps: the phase-2 tail of this very step computed them
   memset(&a.tail, 0, sizeof(a.tail));
-  if (tail && tail->enabled) { a.tail = *tail; a.scalars_ready = 2; }   // folded tail: scalars precomputed by the previous apply if stamped
+  a.scalars_ready = 0;   // split API: formed here
+  if (tail) { a.tail = *tail; a.scalars_ready = 2; }   // single-call steps: precomputed by the previous apply / prologue if stamped
   a.dp_world = 0;
   a.dp_own = nullptr; a.dp_wait_world = 0; a.dp_timeout_ns = dp_timeout_ns();
   for (int r = 0; r < 8; ++r) a.dp_grads[r] = nullptr;
-  a.dp_wait_kind = part == 1 ? 4 : 2;
   if (dp) dp_apply_args(h->dp, a);
   a.eps = (float)cf.adam_eps; a.tau = (float)cf.tau;
   a.omb1 = (float)(1.0 - cf.adam_beta1); a.b2f = (float)cf.adam_beta2; a.omb2 = (float)(1.0 - cf.adam_beta2);
   a.slabs = nullptr; a.nslabs = 0; a.slab_stride = 0;
-  if (reduce_slabs && !dp && slabs_foldable(h)) { a.slabs = h->W() + h->ar.slabs; a.nslabs = h->ar.nslabs; a.slab_stride = h->ar.slab_stride; }
+  if (tail && !dp && slabs_foldable(h)) { a.slabs = h->W() + h->ar.slabs; a.nslabs = h->ar.nslabs; a.slab_stride = h->ar.slab_stride; }
   const int64_t g_all = (a.n_all + 3) / 4, g_q = a.n_q2 / 4;   // a group straddling the critic / policy boundary goes with part 2
   a.g_lo = part == 2 ? g_q : 0; a.g_hi = part == 1 ? g_q : g_all; a.finish = part == 1 ? 0 : 1;
-  a.next_scalars = (h->tc() && prologue_merged()) ? 0 : 1;   // the merged prologue of every step forms them itself
+  a.next_scalars = h->tc() ? 0 : 1;   // the tensor-core modes' prologue (step_prologue_kernel) forms them itself
   int blocks = (int)((a.g_hi - a.g_lo + 255) / 256);   // one 4-element group per thread
   if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
   if (blocks < 1) blocks = 1;
@@ -1247,6 +1179,21 @@ static void enqueue_apply(dsact_handle* h, Ctx& c, bool reduce_slabs = false, bo
   else launch_k(apply_kernel<0>, blocks, 256, 0, c, a);
   c.done();
   c.check();
+}
+
+// One whole update of the single-call steps: phase 1, phase 2 over `global_batch` rows, then (dp) the logged-sum exchange
+// (also the "every rank's block is complete" barrier) and the reduce-scatter from 6 ranks up, then Adam / Polyak.
+// `dp`: the gradients and statistics are reduced over the peers (dsact_dp_connect) instead of locally.
+static void enqueue_update(dsact_handle* h, const dsact_batch& bt, const dsact_noise* nz, int64_t global_batch, bool dp,
+                           bool inputs_imaged, bool prologue_forked, Ctx& c) {
+  enqueue_phase1(h, bt, nz, c, inputs_imaged, prologue_forked, dp);
+  const TailArgs ta = tail_args(h, global_batch, bt.batch);
+  enqueue_phase2(h, bt, global_batch, c, &ta, dp);
+  if (dp) {
+    enqueue_dp_exchange(h, 1, c);
+    if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, h->buf.state, h->num_sms, c);
+  }
+  enqueue_apply(h, c, &ta, dp);
 }
 
 // `images_only`: the caller is a fused tensor-core step, which reads obs / obs2 / act through their bf16 images alone
@@ -1566,13 +1513,7 @@ int dsact_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noi
   const bool imaged = take_arena_images(h, bt);
   GraphKey skey = make_key(K_STEP, &bt, np, bt.batch);
   skey.size = imaged ? 1 : 0;
-  rc = run(h, (cudaStream_t)stream, skey, [&](Ctx& c) {
-    enqueue_phase1(h, bt, np, c, imaged);
-    const TailArgs ta = tail_args(h, bt.batch, bt.batch, fold_tail_enabled());
-    const bool early = ta.enabled && h->fused() && slabs_foldable(h) && apply_split_enabled();
-    enqueue_phase2(h, bt, bt.batch, c, REDUCE_DEFER, ta.enabled, early ? &ta : nullptr);
-    enqueue_apply(h, c, true, false, &ta);
-  });
+  rc = run(h, (cudaStream_t)stream, skey, [&](Ctx& c) { enqueue_update(h, bt, np, bt.batch, false, imaged, false, c); });
   if (rc) return rc;
   h->pending = bt; h->pending_batch = bt.batch;
   h->dev_iter = iteration + 1;
@@ -1733,11 +1674,7 @@ int dsact_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_
     const bool forked = fork_prologue(h, bt, np, c, true);   // weight images, noise, clears: beside the gather
     enqueue_gather(h, batch, idx, c, h->fused());
     if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-    enqueue_phase1(h, bt, np, c, true, forked);  // device noise (np == null): phase1 advances the counter after the join
-    const TailArgs ta = tail_args(h, batch, batch, fold_tail_enabled());
-    const bool early = ta.enabled && h->fused() && slabs_foldable(h) && apply_split_enabled();
-    enqueue_phase2(h, bt, batch, c, REDUCE_DEFER, ta.enabled, early ? &ta : nullptr);
-    enqueue_apply(h, c, true, false, &ta);
+    enqueue_update(h, bt, np, batch, false, true, forked, c);  // device noise (np == null): phase1 advances the counter after the join
   });
   if (rc) return rc;
   h->pending = bt; h->pending_batch = batch;
@@ -1777,16 +1714,7 @@ int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* 
   const bool imaged = take_arena_images(h, bt);
   GraphKey key = make_key(K_DP_STEP, &bt, np, global_batch);
   key.size = imaged ? 1 : 0;
-  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) {
-    enqueue_phase1(h, bt, np, c, imaged, false, true);
-    const TailArgs ta = tail_args(h, global_batch, bt.batch, fold_tail_enabled());
-    const bool early = ta.enabled && h->fused() && slabs_foldable(h) && dp_split_enabled();
-    enqueue_phase2(h, bt, global_batch, c, REDUCE_DP, ta.enabled, early ? &ta : nullptr, true);
-    const bool split = h->apply_early;   // the critics' part went out (and was applied) beside the policy backward
-    enqueue_dp_exchange(h, 1, c);
-    if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h, c, split ? 2 : 0);
-    enqueue_apply(h, c, false, true, &ta);
-  });
+  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) { enqueue_update(h, bt, np, global_batch, true, imaged, false, c); });
   if (rc) return rc;
   h->pending = bt; h->pending_batch = bt.batch;
   h->dev_iter = iteration + 1;
@@ -1813,14 +1741,7 @@ int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int
     const bool forked = fork_prologue(h, bt, np, c, true);
     enqueue_gather(h, batch, idx, c, h->fused());
     if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-    enqueue_phase1(h, bt, np, c, true, forked, true);
-    const TailArgs ta = tail_args(h, global_batch, bt.batch, fold_tail_enabled());
-    const bool early = ta.enabled && h->fused() && slabs_foldable(h) && dp_split_enabled();
-    enqueue_phase2(h, bt, global_batch, c, REDUCE_DP, ta.enabled, early ? &ta : nullptr, true);
-    const bool split = h->apply_early;
-    enqueue_dp_exchange(h, 1, c);
-    if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h, c, split ? 2 : 0);
-    enqueue_apply(h, c, false, true, &ta);
+    enqueue_update(h, bt, np, global_batch, true, true, forked, c);
   });
   if (rc) return rc;
   h->pending = bt; h->pending_batch = batch;
@@ -1848,10 +1769,7 @@ int dsact_profile_step(dsact_handle* h, const dsact_batch* batch, const dsact_no
   cudaEvent_t e0;
   CUDA_TRY(cudaEventCreate(&e0));
   CUDA_TRY(cudaEventRecord(e0, s));
-  enqueue_phase1(h, bt, np, c);
-  const TailArgs ta = tail_args(h, bt.batch, bt.batch, fold_tail_enabled());
-  enqueue_phase2(h, bt, bt.batch, c, REDUCE_DEFER, ta.enabled);
-  enqueue_apply(h, c, true, false, &ta);
+  enqueue_update(h, bt, np, bt.batch, false, false, false, c);   // no side stream: the critics' update is not split off
   cudaError_t e = cudaStreamSynchronize(s);
   memset(out, 0, sizeof(*out));
   cudaEvent_t prev = e0;

@@ -606,7 +606,7 @@ struct ApplyArgs {
   int64_t n_all;     // 2*n_q + n_pi + 1
   int delay_update, auto_alpha;
   AdamHyper hy;
-  int scalars_ready;   // state[ST_ADAM_SC..] was written by phase2_tail_kernel of this step
+  int scalars_ready;   // the Adam scalars: 0 = formed here, 1 = phase2_tail_kernel of this step wrote them, 2 = stamped (see below)
   float omb1, b2f, omb2, eps, tau;  // (float)(1-beta1), (float)beta2, (float)(1-beta2) formed in double on the host
   // tensor-core modes, single-call steps: the weight-gradient split slabs are folded in here (grads += sum of slabs, stored
   // back so that the caller's .grad views hold the totals) instead of by a separate grad_reduce launch
@@ -620,7 +620,6 @@ struct ApplyArgs {
   // kind-2 flags in `dp_own` first
   const float* dp_own;
   int dp_wait_world;
-  int dp_wait_kind;   // 2, or 4 for the critics' part
   unsigned long long dp_timeout_ns;
   // 4-element groups [g_lo, g_hi) of the flat buffers this launch updates; `finish`: its last block closes the step
   // (counters, EMA commit, next Adam scalars).  A step may update the critics' span early, beside the policy backward,
@@ -629,7 +628,7 @@ struct ApplyArgs {
   int finish;
   int next_scalars;   // the finishing block also precomputes the NEXT step's Adam scalars (steps whose prologue does not)
 };
-__device__ __forceinline__ bool dp_wait_reduced(const float* own_buf, int world, uint32_t epoch, unsigned long long timeout_ns, int kind);
+__device__ __forceinline__ bool dp_wait_reduced(const float* own_buf, int world, uint32_t epoch, unsigned long long timeout_ns);
 // torch.optim.Adam single-tensor step (amsgrad / weight decay off)
 __device__ __forceinline__ float adam_update(float w, float g, float& m, float& v, float step_size, float bc2_sqrt,
                                              float omb1, float b2, float omb2, float eps) {
@@ -657,7 +656,7 @@ __global__ void __launch_bounds__(256, 4) apply_kernel(const __grid_constant__ A
     adam_scalars(sti, a.hy, sh);
   }
   if (MODE == 2 && a.dp_wait_world > 0 && threadIdx.x == 32) {   // two-shot exchange: the reduced block is complete
-    if (!dp_wait_reduced(a.dp_own, a.dp_wait_world, (uint32_t)sti[ST_DP_EPOCH], a.dp_timeout_ns, a.dp_wait_kind))
+    if (!dp_wait_reduced(a.dp_own, a.dp_wait_world, (uint32_t)sti[ST_DP_EPOCH], a.dp_timeout_ns))
       reinterpret_cast<int*>(a.state)[ST_DP_ERR] = 1 + a.dp_wait_world;   // (no single rank to name)
   }
   __syncthreads();

@@ -197,13 +197,18 @@ def test_bf16x3_tensor_core_path_matches_reference_golden(golden_dir, name):
     eng.close()
 
 
+# a hidden layer wider than 256: the chain kernel does not take it, so the tensor-core modes run the per-layer GEMM path
+WIDE = dict(obs_dim=7, act_dim=3, hidden=(264, 40), act_lim=1.0)
+
+
 @pytest.mark.parametrize("mode", ["bf16x3", "fp32"])
-@pytest.mark.parametrize("cfg_name,batch,steps", [("humanoid", 65536, 2), ("halfcheetah", 8192, 3)])
+@pytest.mark.parametrize("cfg_name,batch,steps", [("humanoid", 65536, 2), ("halfcheetah", 8192, 3), ("wide", 40, 3)])
 def test_large_batches_match_oracle(cfg_name, batch, steps, mode):
     """The largest configurations of BASELINE.json (config 4's 65536-row sweep point; config 3's 8192 rows per GPU):
-    multi-wave chain launches and the bounded weight-gradient launches, against the pinned oracle on the same inputs."""
+    multi-wave chain launches and the bounded weight-gradient launches, against the pinned oracle on the same inputs.
+    `wide` (WIDE) is the per-layer tensor-core step, which shapes outside the chain kernel's range take."""
     from oracle.dsact_oracle import TB_KEYS, from_config
-    cfg = synth.CONFIGS[cfg_name]
+    cfg = WIDE if cfg_name == "wide" else synth.CONFIGS[cfg_name]
     eng = make_engine(cfg, batch, use_graph=True, gemm_mode=mode)
     orc = from_config(cfg, synth.make_weights(cfg), **synth.HYPER)
     torch.set_num_threads(min(16, os.cpu_count() or 4))
