@@ -143,6 +143,7 @@ SYMBOLS = {
     "dsact_profile_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_void_p, C.POINTER(Profile)]),
     "dsact_launch_count": (C.c_int64, [C.c_void_p]),
     "dsact_last_call_launches": (C.c_int32, [C.c_void_p]),
+    "dsact_cnn_test_conv": (C.c_int, [C.c_int32] * 8 + [C.c_void_p] * 7 + [C.c_int32] * 4 + [C.c_void_p]),
     "dsact_test_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                   C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
 }

@@ -244,65 +244,156 @@ static void cnn_heads_backward(dsact_cnn_handle* h, const Net& net, std::vector<
   c.check();
 }
 
+// The kernel variant one convolution layer runs with; 0 in a field = the engine's choice (conv_layer_*).  `r`: output
+// positions per thread of conv_fwd8_kernel (1, 2, 4); `cob`: output channels per conv_wgrad_kernel block (1, 4, 8);
+// `slabs`: row slabs of the weight gradient; `channels`: 8 (conv_fwd8 / conv_dgrad8) or 1 (conv_fwd / conv_dgrad)
+// channels per thread.  With a field set, a layer whose window is its whole input runs the direct kernels too.
+struct ConvPick { int r = 0, cob = 0, slabs = 0, channels = 0; };
+
 template <int R>
-static void launch_conv_fwd8(const ConvShape& s, long long rows, size_t smem, Ctx& c, const float* x, const float* w, const float* b, float* y) {
+static int launch_conv_fwd8(const ConvShape& s, long long rows, size_t smem, Ctx& c, const float* x, const float* w, const float* b, float* y) {
   const dim3 grid((unsigned)((rows + 128 * R - 1) / (128 * R)), s.Cout / 8);
   switch (s.K) {
-    case 1: launch_k(conv_fwd8_kernel<1, R>, grid, 128, smem, c, x, w, b, y, s); break;
-    case 2: launch_k(conv_fwd8_kernel<2, R>, grid, 128, smem, c, x, w, b, y, s); break;
-    case 3: launch_k(conv_fwd8_kernel<3, R>, grid, 128, smem, c, x, w, b, y, s); break;
-    case 4: launch_k(conv_fwd8_kernel<4, R>, grid, 128, smem, c, x, w, b, y, s); break;
-    default:   // 8x8 window (type_1's first layer): one position per thread (64 taps in registers)
-      if constexpr (R == 1) launch_k(conv_fwd8_kernel<8, 1>, grid, 128, smem, c, x, w, b, y, s);
-      break;
+    case 1: launch_k(conv_fwd8_kernel<1, R>, grid, 128, smem, c, x, w, b, y, s); return DSACT_OK;
+    case 2: launch_k(conv_fwd8_kernel<2, R>, grid, 128, smem, c, x, w, b, y, s); return DSACT_OK;
+    case 3: launch_k(conv_fwd8_kernel<3, R>, grid, 128, smem, c, x, w, b, y, s); return DSACT_OK;
+    case 4: launch_k(conv_fwd8_kernel<4, R>, grid, 128, smem, c, x, w, b, y, s); return DSACT_OK;
+    case 8:   // 8x8 window (type_1's first layer): one position per thread (64 taps in registers)
+      if constexpr (R == 1) { launch_k(conv_fwd8_kernel<8, 1>, grid, 128, smem, c, x, w, b, y, s); return DSACT_OK; }
+      return fail(DSACT_EINVAL, "conv forward: the 8x8 window runs one position per thread (R = %d requested)", R);
+    default: return fail(DSACT_EINVAL, "conv forward: no kernel for a %dx%d window", s.K, s.K);
   }
 }
 
 // a layer whose window is its whole input is a linear layer over the flattened [Cin*K*K] sample (its NCHW order)
 static bool conv_is_linear(const ConvShape& s) { return s.Hin == s.K && s.Win == s.K; }
+static bool conv_pick_default(const ConvPick& pk) { return !pk.r && !pk.cob && !pk.slabs && !pk.channels; }
+
+// y = relu(conv(x, w) + b) of one layer
+static int conv_layer_fwd(int num_sms, const ConvShape& s, const float* x, const float* w, const float* b, float* y, const ConvPick& pk, Ctx& c) {
+  const long long rows = (long long)s.B * s.Hout * s.Wout;
+  const size_t smem8 = sizeof(float) * 8 * s.Cin * s.K * s.K;
+  if (pk.cob || pk.slabs) return fail(DSACT_EINVAL, "conv forward: cob / slabs are weight-gradient choices");
+  if (conv_pick_default(pk) && conv_is_linear(s)) {
+    GemmGroup G; G.n = 0;
+    GemmProb p = prob_zero();
+    const int kin = s.Cin * s.K * s.K;
+    p.A[0] = x; p.lda[0] = kin; p.K[0] = kin; p.B[0] = w; p.ldb[0] = kin;
+    p.M = s.B; p.N = s.Cout; p.C = y; p.ldc = s.Cout; p.bias = b; p.act = ACT_RELU; p.epi = EPI_BIAS_ACT;
+    G.p[G.n++] = p;
+    launch_simt(num_sms, G, V_FWD, c);
+    return DSACT_OK;
+  }
+  const bool fits8 = s.Cout % 8 == 0 && smem8 <= 48 * 1024;   // eight output channels per thread, 1 / 2 / 4 positions
+  const int channels = pk.channels ? pk.channels : fits8 ? 8 : 1;
+  if (channels == 8) {
+    if (!fits8) return fail(DSACT_EINVAL, "conv forward: 8 channels per thread needs Cout %% 8 == 0 and Cin*K*K*32 B <= 48 KiB");
+    const long long wave = 2LL * num_sms * 128;
+    const int r = pk.r ? pk.r : s.K > 4 ? 1 : rows >= 4 * wave ? 4 : rows >= 2 * wave ? 2 : 1;
+    if (r == 4) return launch_conv_fwd8<4>(s, rows, smem8, c, x, w, b, y);
+    if (r == 2) return launch_conv_fwd8<2>(s, rows, smem8, c, x, w, b, y);
+    if (r == 1) return launch_conv_fwd8<1>(s, rows, smem8, c, x, w, b, y);
+    return fail(DSACT_EINVAL, "conv forward: R must be 1, 2 or 4");
+  }
+  if (channels != 1 || pk.r > 1) return fail(DSACT_EINVAL, "conv forward: channels per thread 8 or 1 (one position per thread)");
+  const size_t smem1 = sizeof(float) * s.Cin * s.K * s.K;
+  if (smem1 > 48 * 1024) return fail(DSACT_EINVAL, "conv forward: Cin*K*K*4 B above 48 KiB");
+  dim3 grid((unsigned)((rows + 127) / 128), s.Cout);
+  launch_k(conv_fwd_kernel, grid, 128, smem1, c, x, w, b, y, s);
+  return DSACT_OK;
+}
+
+template <int COB>
+static int launch_conv_wgrad(const ConvShape& s, int slabs, Ctx& c, const float* dy, const float* x, float* dw, float* db) {
+  const dim3 grid(s.Cin, s.Cout / COB, slabs);
+  switch (s.K) {
+    case 1: launch_k(conv_wgrad_kernel<1, COB>, grid, 256, 0, c, dy, x, dw, db, s); return DSACT_OK;
+    case 2: launch_k(conv_wgrad_kernel<2, COB>, grid, 256, 0, c, dy, x, dw, db, s); return DSACT_OK;
+    case 3: launch_k(conv_wgrad_kernel<3, COB>, grid, 256, 0, c, dy, x, dw, db, s); return DSACT_OK;
+    case 4:
+      if constexpr (COB <= 4) { launch_k(conv_wgrad_kernel<4, COB>, grid, 256, 0, c, dy, x, dw, db, s); return DSACT_OK; }
+      return fail(DSACT_EINVAL, "conv weight gradient: a 4x4 window takes at most 4 output channels per block (COB = %d)", COB);
+    case 8:   // 64 taps x 1 channel
+      if constexpr (COB == 1) { launch_k(conv_wgrad_kernel<8, 1>, grid, 256, 0, c, dy, x, dw, db, s); return DSACT_OK; }
+      return fail(DSACT_EINVAL, "conv weight gradient: an 8x8 window takes 1 output channel per block (COB = %d)", COB);
+    default: return fail(DSACT_EINVAL, "conv weight gradient: no kernel for a %dx%d window", s.K, s.K);
+  }
+}
+
+// dw += corr(x, dy), db += sum(dy) of one layer (dy: gradient of its pre-activation)
+static int conv_layer_wgrad(int num_sms, const ConvShape& s, const float* dy, const float* x, float* dw, float* db, const ConvPick& pk, Ctx& c) {
+  const long long rows = (long long)s.B * s.Hout * s.Wout;
+  if (pk.r || pk.channels) return fail(DSACT_EINVAL, "conv weight gradient: R / channels are forward and dgrad choices");
+  if (conv_pick_default(pk) && conv_is_linear(s)) {   // dW = dz^T x through the GEMM
+    GemmGroup gw; gw.n = 0;
+    GemmProb p = prob_zero();
+    const int kin = s.Cin * s.K * s.K;
+    p.A[0] = dy; p.lda[0] = s.Cout; p.K[0] = s.B; p.B[0] = x; p.ldb[0] = kin;
+    p.M = s.Cout; p.N = kin; p.C = dw; p.ldc = kin; p.epi = EPI_ATOMIC;
+    gw.p[gw.n++] = p;
+    launch_simt(num_sms, gw, V_WGRAD, c); c.done();
+    launch_k(colsum_rows_kernel, (s.Cout + 31) / 32, dim3(32, 8), 0, c, dy, s.B, s.Cout, db);
+    return DSACT_OK;
+  }
+  // K*K*cob accumulators per thread; slabs: >= 32 rows per thread, enough blocks for ~4 per SM
+  const int cob = pk.cob ? pk.cob : s.K > 4 ? 1 : (s.Cout % 8 == 0 && s.K <= 3) ? 8 : s.Cout % 4 == 0 ? 4 : 1;
+  if (s.Cout % cob != 0) return fail(DSACT_EINVAL, "conv weight gradient: Cout %d is no multiple of COB %d", s.Cout, cob);
+  long long slabs = pk.slabs;
+  if (!slabs) {
+    const int base = s.Cin * (s.Cout / cob);
+    slabs = (4LL * num_sms + base - 1) / base;
+    const long long cap = (rows + 256 * 32 - 1) / (256 * 32);
+    if (slabs > cap) slabs = cap;
+    if (slabs < 1) slabs = 1;
+  }
+  if (slabs < 1 || slabs > 65535) return fail(DSACT_EINVAL, "conv weight gradient: 1..65535 slabs");
+  if (cob == 8) return launch_conv_wgrad<8>(s, (int)slabs, c, dy, x, dw, db);
+  if (cob == 4) return launch_conv_wgrad<4>(s, (int)slabs, c, dy, x, dw, db);
+  if (cob == 1) return launch_conv_wgrad<1>(s, (int)slabs, c, dy, x, dw, db);
+  return fail(DSACT_EINVAL, "conv weight gradient: COB must be 1, 4 or 8");
+}
+
+// dx = convT(dy, w) (.) [x > 0] of one layer (x: its input, the ReLU output of the layer below).  conv_dgrad8_kernel needs
+// the CNN_DGRAD_SMEM opt-in of dsact_cnn_create / dsact_cnn_test_conv.
+static int conv_layer_dgrad(int num_sms, const ConvShape& s, const float* dy, const float* w, const float* x, float* dx, const ConvPick& pk, Ctx& c) {
+  const long long rin = (long long)s.B * s.Hin * s.Win;
+  const size_t smem8 = sizeof(float) * 8 * s.Cout * s.K * s.K;
+  if (pk.r > 1 || pk.cob || pk.slabs) return fail(DSACT_EINVAL, "conv dgrad: one input position per thread; cob / slabs are weight-gradient choices");
+  if (conv_pick_default(pk) && conv_is_linear(s)) {   // dx = dz W (.) [x > 0]
+    GemmGroup G; G.n = 0;
+    GemmProb p = prob_zero();
+    const int kin = s.Cin * s.K * s.K;
+    p.A[0] = dy; p.lda[0] = s.Cout; p.K[0] = s.Cout; p.B[0] = w; p.ldb[0] = kin;
+    p.M = s.B; p.N = kin; p.C = dx; p.ldc = kin; p.epi = EPI_DACT; p.Zin = x; p.ldz = kin; p.act = ACT_RELU;
+    G.p[G.n++] = p;
+    launch_simt(num_sms, G, V_DGRAD, c);
+    return DSACT_OK;
+  }
+  const bool fits8 = s.Cin % 8 == 0 && smem8 <= (size_t)CNN_DGRAD_SMEM;
+  const int channels = pk.channels ? pk.channels : fits8 ? 8 : 1;
+  if (channels == 8) {
+    if (!fits8) return fail(DSACT_EINVAL, "conv dgrad: 8 channels per thread needs Cin %% 8 == 0 and Cout*K*K*32 B <= 96 KiB");
+    dim3 grid((unsigned)((rin + 127) / 128), s.Cin / 8);
+    launch_k(conv_dgrad8_kernel, grid, 128, smem8, c, dy, w, x, dx, s, 1);
+    return DSACT_OK;
+  }
+  if (channels != 1) return fail(DSACT_EINVAL, "conv dgrad: channels per thread 8 or 1");
+  dim3 grid((unsigned)((rin + 127) / 128), s.Cin);
+  launch_k(conv_dgrad_kernel, grid, 128, 0, c, dy, w, x, dx, s, 1);
+  return DSACT_OK;
+}
+
+static void conv_note(int rc, Ctx& c) { if (rc != DSACT_OK && c.err == cudaSuccess) c.err = cudaErrorInvalidValue; }
 
 static void cnn_conv_forward(dsact_cnn_handle* h, const CnnGeom& g, const float* params, const float* img, const int64_t* acts, int B, Ctx& c) {
   float* W = h->Wp();
   const float* x = img;
   for (int j = 0; j < g.nconv; ++j) {
-    const ConvShape s = g.shape(j, B);
-    const long long rows = (long long)B * s.Hout * s.Wout;
-    const size_t smem8 = sizeof(float) * 8 * s.Cin * s.K * s.K;
-    if (conv_is_linear(s)) {
-      GemmGroup G; G.n = 0;
-      GemmProb p = prob_zero();
-      const int kin = s.Cin * s.K * s.K;
-      p.A[0] = x; p.lda[0] = kin; p.K[0] = kin; p.B[0] = params + g.cw[j]; p.ldb[0] = kin;
-      p.M = B; p.N = s.Cout; p.C = W + acts[j + 1]; p.ldc = s.Cout; p.bias = params + g.cb[j]; p.act = ACT_RELU; p.epi = EPI_BIAS_ACT;
-      G.p[G.n++] = p;
-      launch_simt(h->num_sms, G, V_FWD, c);
-    } else if (s.Cout % 8 == 0 && smem8 <= 48 * 1024) {   // eight output channels per thread, 1 / 2 / 4 positions
-      const long long wave = 2LL * h->num_sms * 128;
-      const float *w = params + g.cw[j], *b = params + g.cb[j];
-      if (s.K > 4) launch_conv_fwd8<1>(s, rows, smem8, c, x, w, b, W + acts[j + 1]);
-      else if (rows >= 4 * wave) launch_conv_fwd8<4>(s, rows, smem8, c, x, w, b, W + acts[j + 1]);
-      else if (rows >= 2 * wave) launch_conv_fwd8<2>(s, rows, smem8, c, x, w, b, W + acts[j + 1]);
-      else launch_conv_fwd8<1>(s, rows, smem8, c, x, w, b, W + acts[j + 1]);
-    } else {
-      dim3 grid((unsigned)((rows + 127) / 128), s.Cout);
-      launch_k(conv_fwd_kernel, grid, 128, sizeof(float) * s.Cin * s.K * s.K, c, x, params + g.cw[j], params + g.cb[j], W + acts[j + 1], s);
-    }
+    conv_note(conv_layer_fwd(h->num_sms, g.shape(j, B), x, params + g.cw[j], params + g.cb[j], W + acts[j + 1], ConvPick(), c), c);
     c.done();
     x = W + acts[j + 1];
   }
   c.check();
-}
-
-template <int COB>
-static void launch_conv_wgrad(const ConvShape& s, int slabs, Ctx& c, const float* dy, const float* x, float* dw, float* db) {
-  const dim3 grid(s.Cin, s.Cout / COB, slabs);
-  switch (s.K) {
-    case 1: launch_k(conv_wgrad_kernel<1, COB>, grid, 256, 0, c, dy, x, dw, db, s); break;
-    case 2: launch_k(conv_wgrad_kernel<2, COB>, grid, 256, 0, c, dy, x, dw, db, s); break;
-    case 3: launch_k(conv_wgrad_kernel<3, COB>, grid, 256, 0, c, dy, x, dw, db, s); break;
-    case 4: if constexpr (COB <= 4) launch_k(conv_wgrad_kernel<4, COB>, grid, 256, 0, c, dy, x, dw, db, s); break;
-    default: if constexpr (COB == 1) launch_k(conv_wgrad_kernel<8, 1>, grid, 256, 0, c, dy, x, dw, db, s); break;   // 64 taps x 1 channel
-  }
 }
 
 // backward through one encoder: `gtop` = dL/d(feature) [B, F] (consumed); gparams was cleared by begin_step_kernel
@@ -320,48 +411,11 @@ static void cnn_conv_backward(dsact_cnn_handle* h, const CnnGeom& g, const float
   for (int j = g.nconv - 1; j >= 0; --j) {
     const ConvShape s = g.shape(j, B);
     const float* x = j == 0 ? img : W + acts[j];
-    const long long rows = (long long)B * s.Hout * s.Wout;
-    if (conv_is_linear(s)) {   // dW = dz^T x through the GEMM
-      GemmGroup gw; gw.n = 0;
-      GemmProb p = prob_zero();
-      const int kin = s.Cin * s.K * s.K;
-      p.A[0] = gcur; p.lda[0] = s.Cout; p.K[0] = B; p.B[0] = x; p.ldb[0] = kin;
-      p.M = s.Cout; p.N = kin; p.C = gparams + g.cw[j]; p.ldc = kin; p.epi = EPI_ATOMIC;
-      gw.p[gw.n++] = p;
-      launch_simt(h->num_sms, gw, V_WGRAD, c); c.done();
-      launch_k(colsum_rows_kernel, (s.Cout + 31) / 32, dim3(32, 8), 0, c, (const float*)gcur, B, s.Cout, gparams + g.cb[j]); c.done();
-    } else {
-      // slabs: >= 32 rows per thread, enough blocks for ~4 per SM
-      const int cob = s.K > 4 ? 1 : (s.Cout % 8 == 0 && s.K <= 3) ? 8 : s.Cout % 4 == 0 ? 4 : 1;   // K*K*cob accumulators per thread
-      const int base = s.Cin * (s.Cout / cob);
-      long long slabs = (4LL * h->num_sms + base - 1) / base;
-      const long long cap = (rows + 256 * 32 - 1) / (256 * 32);
-      if (slabs > cap) slabs = cap;
-      if (slabs < 1) slabs = 1;
-      if (cob == 8) launch_conv_wgrad<8>(s, (int)slabs, c, gcur, x, gparams + g.cw[j], gparams + g.cb[j]);
-      else if (cob == 4) launch_conv_wgrad<4>(s, (int)slabs, c, gcur, x, gparams + g.cw[j], gparams + g.cb[j]);
-      else launch_conv_wgrad<1>(s, (int)slabs, c, gcur, x, gparams + g.cw[j], gparams + g.cb[j]);
-      c.done();
-    }
+    conv_note(conv_layer_wgrad(h->num_sms, s, gcur, x, gparams + g.cw[j], gparams + g.cb[j], ConvPick(), c), c);
+    c.done();
     if (j > 0) {
       float* gnext = bufs[flip]; flip ^= 1;
-      const long long rin = (long long)B * s.Hin * s.Win;
-      const size_t smem8 = sizeof(float) * 8 * s.Cout * s.K * s.K;
-      if (conv_is_linear(s)) {   // dx = dz W (.) [x > 0]
-        GemmGroup G; G.n = 0;
-        GemmProb p = prob_zero();
-        const int kin = s.Cin * s.K * s.K;
-        p.A[0] = gcur; p.lda[0] = s.Cout; p.K[0] = s.Cout; p.B[0] = params + g.cw[j]; p.ldb[0] = kin;
-        p.M = B; p.N = kin; p.C = gnext; p.ldc = kin; p.epi = EPI_DACT; p.Zin = x; p.ldz = kin; p.act = ACT_RELU;
-        G.p[G.n++] = p;
-        launch_simt(h->num_sms, G, V_DGRAD, c);
-      } else if (s.Cin % 8 == 0 && smem8 <= (size_t)CNN_DGRAD_SMEM) {
-        dim3 grid((unsigned)((rin + 127) / 128), s.Cin / 8);
-        launch_k(conv_dgrad8_kernel, grid, 128, smem8, c, (const float*)gcur, params + g.cw[j], x, gnext, s, 1);
-      } else {
-        dim3 grid((unsigned)((rin + 127) / 128), s.Cin);
-        launch_k(conv_dgrad_kernel, grid, 128, 0, c, (const float*)gcur, params + g.cw[j], x, gnext, s, 1);
-      }
+      conv_note(conv_layer_dgrad(h->num_sms, s, gcur, params + g.cw[j], x, gnext, ConvPick(), c), c);
       c.done();
       gcur = gnext;
     }
@@ -890,6 +944,40 @@ int dsact_cnn_dp_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact
   cnn_enqueue_apply(h, c, 1, true);
   if ((rc = cnn_finish(h, c))) return rc;
   h->dev_iter = iteration + 1;
+  return DSACT_OK;
+}
+
+int dsact_cnn_test_conv(int32_t op, int32_t batch, int32_t cin, int32_t hin, int32_t win, int32_t cout, int32_t k, int32_t stride,
+                        const float* x, const float* w, const float* b, const float* dy, float* out, float* dw, float* db,
+                        int32_t r, int32_t cob, int32_t slabs, int32_t channels, void* stream) {
+  if (op < 0 || op > 2) return fail(DSACT_EINVAL, "op must be 0 (forward), 1 (weight gradient) or 2 (dgrad)");
+  if (batch < 1 || cin < 1 || cout < 1 || k < 1 || stride < 1 || hin < k || win < k) return fail(DSACT_EINVAL, "bad layer shape");
+  if (r < 0 || cob < 0 || slabs < 0 || channels < 0) return fail(DSACT_EINVAL, "negative kernel choice");
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  cudaDeviceProp prop;
+  CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
+  if (prop.major != 9 || prop.minor != 0) return fail(DSACT_EARCH, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major, prop.minor);
+  CUDA_TRY(cudaFuncSetAttribute(conv_dgrad8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CNN_DGRAD_SMEM));
+  ConvShape s;
+  s.B = batch; s.Cin = cin; s.Hin = hin; s.Win = win; s.Cout = cout; s.K = k; s.S = stride;
+  s.Hout = (hin - k) / stride + 1; s.Wout = (win - k) / stride + 1;
+  ConvPick pk; pk.r = r; pk.cob = cob; pk.slabs = slabs; pk.channels = channels;
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  int rc;
+  if (op == 0) {
+    if (!x || !w || !b || !out) return fail(DSACT_EINVAL, "forward needs x, w, b, out");
+    rc = conv_layer_fwd(prop.multiProcessorCount, s, x, w, b, out, pk, c);
+  } else if (op == 1) {
+    if (!x || !dy || !dw || !db) return fail(DSACT_EINVAL, "weight gradient needs x, dy, dw, db");
+    rc = conv_layer_wgrad(prop.multiProcessorCount, s, dy, x, dw, db, pk, c);
+  } else {
+    if (!x || !w || !dy || !out) return fail(DSACT_EINVAL, "dgrad needs x, w, dy, out");
+    rc = conv_layer_dgrad(prop.multiProcessorCount, s, dy, w, x, out, pk, c);
+  }
+  if (rc) return rc;
+  c.check();
+  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
   return DSACT_OK;
 }
 

@@ -304,6 +304,18 @@ int dsact_profile_step(dsact_handle *h, const dsact_batch *batch, const dsact_no
 int dsact_test_gemm(dsact_handle *h, int32_t variant, const float *A, int32_t lda, const float *B, int32_t ldb,
                     const float *bias, float *C, int32_t ldc, int32_t M, int32_t N, int32_t K, void *stream);
 
+/* Test hook of the head-wise engine's convolution kernels: one layer (NCHW, square k x k window, stride, no padding) on
+ * caller buffers, enqueued on `stream` of the current device.
+ *  op 0 (forward)        : out[B,cout,hout,wout] = relu(conv(x, w) + b)
+ *  op 1 (weight gradient): dw[cout,cin,k,k] += corr(x, dy), db[cout] += sum(dy)   (dy: gradient of the pre-activation)
+ *  op 2 (dgrad)          : out[B,cin,hin,win] = convT(dy, w) (.) [x > 0]
+ * r, cob, slabs, channels: 0 = the engine's choice; otherwise positions per thread of the forward (1, 2, 4), output
+ * channels per weight-gradient block (1, 4, 8), row slabs of the weight gradient, and channels per thread of the forward /
+ * dgrad kernels (8 or 1).  DSACT_EINVAL for a combination that has no kernel. */
+int dsact_cnn_test_conv(int32_t op, int32_t batch, int32_t cin, int32_t hin, int32_t win, int32_t cout, int32_t k, int32_t stride,
+                        const float *x, const float *w, const float *b, const float *dy, float *out, float *dw, float *db,
+                        int32_t r, int32_t cob, int32_t slabs, int32_t channels, void *stream);
+
 #define DSACT_STATE_STDSUM 4   /* state[4], state[5]: local sums of critic std (phase1 -> phase2) */
 #define DSACT_STATE_ACC 16     /* state[16..47]: per-step accumulators (sums first, then mins) */
 #define DSACT_STATE_STATS 48   /* state[48..63]: finalised tb_info */

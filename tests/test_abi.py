@@ -111,3 +111,11 @@ def test_head_wise_layouts_match_the_dropin_modules(variant):
     sizes = dict(net.named_parameters())
     assert all(tuple(sizes[e[0]].shape) == tuple(e[4]) and sizes[e[0]].numel() == e[3] for e in schema)
     assert [e[1] for e in schema] == [k for k, p in net.named_parameters() if not p.requires_grad]
+
+
+def test_conv_test_hook_rejects_bad_arguments_before_touching_a_device():
+    lib = _lib.load()
+    null = None
+    for op, shape in ((3, (2, 8, 9, 9, 8, 3, 1)), (0, (2, 8, 2, 9, 8, 3, 1)), (1, (0, 8, 9, 9, 8, 3, 1))):
+        assert lib.dsact_cnn_test_conv(op, *shape, null, null, null, null, null, null, null, 0, 0, 0, 0, null) == -1
+        assert lib.dsact_last_error()
