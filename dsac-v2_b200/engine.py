@@ -82,7 +82,10 @@ def _f32c(t: torch.Tensor, device) -> torch.Tensor:
 class Engine:
     """One handle bound to flat torch-owned buffers on one CUDA device."""
 
-    def __init__(self, cfg: Config, device: torch.device, act_high: torch.Tensor, act_low: torch.Tensor):
+    def __init__(self, cfg: Config, device: torch.device, act_high: torch.Tensor, act_low: torch.Tensor, *,
+                 workspace_fill: float = 0.0):
+        """`workspace_fill`: the value the scratch workspace holds when it is bound.  No step depends on it: every region a
+        step reads is written first by that step, or by dsact_bind (arena_views()["slabs"])."""
         if not torch.cuda.is_available():
             raise _lib.DsactError("the DSAC-T update engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
@@ -99,7 +102,8 @@ class Engine:
             self.params, self.targets = z(L.n_params), z(L.n_targets)
             self.grads, self.adam_m, self.adam_v = z(L.n_params), z(L.n_params), z(L.n_params)
             self.state = z(L.state_floats)
-            self.workspace = torch.zeros(int(L.workspace_bytes) // 4 + 64, dtype=torch.float32, device=self.device)
+            self.workspace = torch.full((int(L.workspace_bytes) // 4 + 64,), float(workspace_fill), dtype=torch.float32,
+                                        device=self.device)
             self.act_high = _f32c(torch.as_tensor(act_high).reshape(-1), self.device).clone()
             self.act_low = _f32c(torch.as_tensor(act_low).reshape(-1), self.device).clone()
             h = C.c_void_p()
@@ -189,15 +193,30 @@ class Engine:
         return Batch(t["obs"].data_ptr(), t["act"].data_ptr(), t["rew"].data_ptr(), t["obs2"].data_ptr(),
                      t["done"].data_ptr(), B, None)
 
-    def _noise_slots(self, B):
+    def arena_views(self, batch: Optional[int] = None) -> Dict[str, torch.Tensor]:
+        """Views of the arena slots the device generator writes, for the first `batch` rows (default max_batch): `idx`
+        (int64 [B], the replay indices the last index-drawing gather recorded) and the noise `eps1`, `eps2` [B, A],
+        `z3`, `z4` [B] (device noise, or host noise staged there); and `slabs`, the one region dsact_bind initialises.
+        Offsets follow Arena::build (csrc/engine.cu)."""
         O, A, r64 = self.cfg.obs_dim, self.cfg.act_dim, lambda n: (n + 63) // 64 * 64
         mb = self.cfg.max_batch
-        off = 2 * r64(mb * O) + r64(mb * A) + 3 * r64(mb) + r64(2 * mb)  # obs obs2 act rew done logp idx
-        out = []
-        for n, shape in ((A, (B, A)), (A, (B, A)), (1, (B,)), (1, (B,))):
-            out.append(self._ws_view[off:off + B * n].view(shape))
+        B = mb if batch is None else int(batch)
+        off = 2 * r64(mb * O) + r64(mb * A) + 3 * r64(mb)  # obs obs2 act rew done logp
+        out = {"idx": self._ws_view[off:off + 2 * B].view(torch.int64)}
+        off += r64(2 * mb)
+        for name, n, shape in (("eps1", A, (B, A)), ("eps2", A, (B, A)), ("z3", 1, (B,)), ("z4", 1, (B,))):
+            out[name] = self._ws_view[off:off + B * n].view(shape)
             off += r64(mb * n)
+        # the tensor-core modes' weight-gradient split slabs, the arena's last region: dsact_bind zeroes them, because
+        # their bias entries are read by the fold and never written by a kernel
+        end = int(self.layout.workspace_bytes) // 4
+        n = r64(min(max(mb // 256, 1), 4) * ((int(self.layout.n_params) + 3) // 4 * 4)) if self.cfg.gemm_mode else 0
+        out["slabs"] = self._ws_view[end - n:end]
         return out
+
+    def _noise_slots(self, B):
+        v = self.arena_views(B)
+        return [v[k] for k in ("eps1", "eps2", "z3", "z4")]
 
     def _noise(self, noise, B):
         if noise is None:

@@ -56,7 +56,8 @@ def make_heads_config(obs_dim: int, act_dim: int, hidden: Sequence[int], std_typ
 class CnnEngine:
     """One `dsact_cnn_handle` bound to flat torch-owned buffers on one CUDA device."""
 
-    def __init__(self, cfg: CnnConfig, device, act_high, act_low):
+    def __init__(self, cfg: CnnConfig, device, act_high, act_low, *, workspace_fill: float = 0.0):
+        """`workspace_fill`: the value the scratch workspace holds when it is bound (see `engine.Engine`)."""
         if not torch.cuda.is_available():
             raise _lib.DsactError("the DSAC-T update engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib, self.cfg = _lib.load(), cfg
@@ -71,7 +72,8 @@ class CnnEngine:
             self.params, self.targets = z(lay.n_params), z(lay.n_targets)
             self.grads, self.adam_m, self.adam_v = z(lay.n_params), z(lay.n_params), z(lay.n_params)
             self.state = z(lay.state_floats)
-            self.workspace = z(int(lay.workspace_bytes) // 4 + 64)
+            self.workspace = torch.full((int(lay.workspace_bytes) // 4 + 64,), float(workspace_fill), dtype=torch.float32,
+                                        device=self.device)
             off = (-self.workspace.data_ptr() % 256) // 4
             self._ws_view = self.workspace[off:]
             self.act_high = torch.as_tensor(act_high, dtype=torch.float32).reshape(-1).to(self.device).clone()
@@ -275,6 +277,32 @@ class CnnEngine:
         return {"obs": view(out.obs, B * self.obs_elems, img), "obs2": view(out.obs2, B * self.obs_elems, img),
                 "act": view(out.act, B * A, (B, A)), "rew": view(out.rew, B, (B,)), "done": view(out.done, B, (B,)),
                 "logp": view(out.logp, B, (B,))}
+
+    def arena_views(self, batch: Optional[int] = None) -> Dict[str, torch.Tensor]:
+        """Views of the arena slots the device generator writes, for the first `batch` rows (default max_batch): `idx`
+        (int64 [B]) and `eps1`, `eps2` [B, A], `z3`, `z4` [B].  Offsets follow dsact_cnn_handle::layout
+        (csrc/cnn_engine.cuh), counted back from the end of the workspace: the replay minibatch and its indices come last,
+        and between them and the noise lie the critic outputs, the action gradients, the feature gradients and the two
+        conv-backward buffers."""
+        c, r64 = self.cfg, lambda n: (n + 63) // 64 * 64
+        mb, A, O = c.max_batch, c.act_dim, self.obs_elems
+        B = mb if batch is None else int(batch)
+        cin, hh, ww, big = c.channels, c.height, c.width, 0
+        for j in range(c.n_conv):
+            k, st = c.conv_kernel[j], c.conv_stride[j]
+            cin, hh, ww = c.conv_channels[j], (hh - k) // st + 1, (ww - k) // st + 1
+            big = max(big, cin * hh * ww)
+        F = cin * hh * ww
+        end = int(self.layout.workspace_bytes) // 4
+        idx = end - r64(2 * mb)
+        r_obs = idx - 3 * r64(mb) - r64(mb * A) - 2 * r64(mb * O)
+        z4 = r_obs - 2 * r64(mb * big) - 2 * r64(mb * (F + A)) - 3 * r64(mb * F) - 2 * r64(mb * A) - 12 * r64(2 * mb) - r64(mb)
+        z3 = z4 - r64(mb)
+        eps2 = z3 - r64(mb * A)
+        eps1 = eps2 - r64(mb * A)
+        v = self._ws_view
+        return {"idx": v[idx:idx + 2 * B].view(torch.int64), "eps1": v[eps1:eps1 + B * A].view(B, A),
+                "eps2": v[eps2:eps2 + B * A].view(B, A), "z3": v[z3:z3 + B], "z4": v[z4:z4 + B]}
 
     def set_carry(self, mean_std1=-1.0, mean_std2=-1.0, adam_steps_q=0, adam_steps_pi=0):
         """The state one update carries to the next besides weights and Adam moments: the mean_std EMA pair (-1 = not

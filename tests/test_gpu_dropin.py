@@ -343,7 +343,6 @@ def test_device_generator_is_seeded_from_the_run_seed():
         data = {k: torch.from_numpy(v).cuda() for k, v in synth.make_batch(cfg, B, 0).items()}
         alg.local_update(data, 0)
         torch.cuda.synchronize()
-        off = 2 * ((B * cfg["obs_dim"] + 63) // 64 * 64) + (B * cfg["act_dim"] + 63) // 64 * 64 + 3 * ((B + 63) // 64 * 64) + (2 * B + 63) // 64 * 64
-        outs.append(eng._ws_view[off:off + B * cfg["act_dim"]].clone())
+        outs.append(eng.arena_views(B)["eps1"].clone())
     assert not torch.equal(outs[0], outs[1])
     assert torch.equal(outs[0], outs[2])

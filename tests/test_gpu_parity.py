@@ -155,13 +155,7 @@ def test_device_noise_statistics():
     eng2.step(b, 0, None)
     np.testing.assert_allclose(stats_vec(eng2), s1, rtol=1e-5)
     # the generated noise itself sits in the arena: N(0,1)
-    A = cfg["act_dim"]
-    lay = eng.layout
-    ws = eng._ws_view
-    O = cfg["obs_dim"]
-    r64 = lambda n: (n + 63) // 64 * 64
-    off = 2 * r64(B * O) + r64(B * A) + 3 * r64(B) + r64(2 * B)
-    eps1 = ws[off:off + B * A]
+    eps1 = eng.arena_views(B)["eps1"]
     assert abs(eps1.mean().item()) < 0.02 and abs(eps1.std().item() - 1.0) < 0.02
     assert abs((eps1 ** 4).mean().item() - 3.0) < 0.2
     eng.close(); eng2.close()
