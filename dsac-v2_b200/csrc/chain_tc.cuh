@@ -7,7 +7,9 @@
 // layer takes A from SHARED MEMORY: the epilogue of layer j writes act(z_j) (or dz_j) as bf16 hi/lo pairs, in the
 // 128-byte-swizzled K-major layout wgmma reads, into the operand buffer, so hidden activations never leave the SM
 // unless the backward pass needs them (act' for the dgrad chain, images for wgrad).
-// The weight tiles of layer j+1 are prefetched by the TMA warp while the epilogue of layer j runs.
+// The weight tiles of layer j+1 are prefetched by the TMA warp while the epilogue of layer j runs.  The MMAs of a k-block
+// issue back to back and one k-block stays in flight while the next is issued; the layer width (64, 128, 192 or 256) is
+// a compile-time parameter of each layer's body, dispatched once per layer.
 //
 // Shared memory: [ B ring: stages x planes x stage_b ][ operand buffer: planes x 4 k-blocks x 8 KiB (layer 0: its A
 // ring) ][ 16-float scratch row per MMA thread ][ barriers ].
@@ -26,10 +28,8 @@ struct ChainLayer {
   CUtensorMap mapB;          // weight image; forward: K-major (box = bn rows), dgrad: MN-major (box = 64 x 64)
   int kblocks[2];            // k-blocks of 64; layer 0 may have two A segments, later layers use [0] only
   int kB0[2];                // offset of each segment along B's reduction dimension
-  int K;                     // reduction length of layers >= 1 (= width of the previous layer)
   int N, bn;                 // outputs; tile width (multiple of 16, <= 256)
-  int b_mn;
-  int epi, act;              // EPI_BIAS_ACT | EPI_DACT | EPI_STORE
+  int epi, act;             // EPI_BIAS_ACT | EPI_DACT | EPI_STORE
   const float* bias;
   float* Zout;               // forward: act'(pre-activation) store, ld = N (null: not needed by a backward pass)
   const float* Zin;          // dgrad: act'(pre-activation) of the layer below, ld = N
@@ -56,7 +56,80 @@ inline int chain_smem_bytes(int stages, int planes, int stage_b) {
   return stages * planes * stage_b + planes * CH_OPND_PLANE + TC_SCRATCH + 2 * stages * 8 + 1024;
 }
 
-template <bool PLANES2>
+// One layer on the MMA warpgroup, 64 x (64 NB) outputs: the MMAs with one k-block in flight (the ring slot of k-block kb is
+// released once kb + 1 has been issued and kb has retired), the epilogue on the accumulator registers, and the next
+// layer's A operand.  (stage, phase) is the consumer's position in the B ring, carried from layer to layer.
+template <bool PLANES2, bool B_MN, int NB>
+__device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass& P, int j, uint8_t* ringB, uint8_t* opnd,
+                                            float* row, int stages, int stage_b, uint64_t* full, uint64_t* empty, int m0,
+                                            int& stage, uint32_t& phase) {
+  constexpr int planes = PLANES2 ? 2 : 1;
+  const ChainLayer& Lj = P.L[j];
+  const int lane = threadIdx.x & 31, r_lo = (threadIdx.x >> 5) * 16 + (lane >> 2);   // this thread's rows r_lo, r_lo + 8
+  const int nkb = Lj.kblocks[0] + Lj.kblocks[1];
+  float acc[128];
+#pragma unroll
+  for (int i = 0; i < 32 * NB; ++i) acc[i] = 0.f;
+  int prev = -1;
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait(&full[stage], phase);
+    if (j == 0 && kb == 0 && threadIdx.x == 0) TC_STAMP(2);
+    const uint32_t sB = smem_u32(ringB + (size_t)stage * planes * stage_b);
+    // layer 0: the ring slot of this stage; later layers: k-block kb of the operand buffer
+    const uint32_t sA = smem_u32(opnd) + (uint32_t)(j == 0 ? stage * planes * TC_STAGE_A : kb * TC_STAGE_A);
+    const uint32_t a_plane = j == 0 ? TC_STAGE_A : CH_OPND_PLANE;
+    wg_fence();
+    // All four k16 steps, also in a partial last k-block: past K the operand buffer holds the zeros the previous
+    // epilogue wrote and TMA zero-fills B, so the extra products add exact zeros.
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k) {
+      const uint32_t b_off = B_MN ? k * 2048 : k * 32;
+      const uint64_t b_hi = make_desc(sB + b_off, B_MN ? 8192 : 16, 1024);
+      const uint64_t b_lo = make_desc(sB + stage_b + b_off, B_MN ? 8192 : 16, 1024);
+      const uint64_t a_hi = make_desc(sA + k * 32, 16, 1024);
+      const uint64_t a_lo = make_desc(sA + a_plane + k * 32, 16, 1024);
+      wgmma_step<NB, 0, B_MN, PLANES2>(acc, a_hi, b_hi, a_lo, b_lo);
+    }
+    wg_commit();
+    wg_wait<1>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);   // this warp's share of k-block kb - 1 retired
+    prev = stage;
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+  wg_wait<0>();
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+  if (threadIdx.x == 0) TC_STAMP(8 + 3 * j);   // MMAs of layer j retired
+  EpiArgs E;
+  E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.N; E.ldz = Lj.N;
+  E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
+  E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
+  epi_frag<PLANES2, NB>(acc, E, m0, 0, row);
+  if (threadIdx.x == 0) TC_STAMP(9 + 3 * j);
+  if (j + 1 < P.n_layers) {
+    // next layer's A operand: bf16 hi/lo pairs at (row, column) of the swizzled K-major k-block tiles
+    // (16-byte chunk index ^= row & 7).  Every warp's MMAs of this layer have retired before anyone overwrites.
+    wg_bar();
+#pragma unroll
+    for (int i = 0; i < 8 * NB; ++i) {
+      const int c = 8 * i + 2 * (lane & 3), cc = c & 63;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r_lo + 8 * h;
+        uint32_t whi, wlo;
+        split_pack2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], whi, wlo);
+        const uint32_t off = (uint32_t)((c >> 6) * TC_STAGE_A + r * 128 + ((((cc >> 3) ^ (r & 7)) << 4) | ((cc & 7) * 2)));
+        *reinterpret_cast<uint32_t*>(opnd + off) = whi;
+        if (PLANES2) *reinterpret_cast<uint32_t*>(opnd + CH_OPND_PLANE + off) = wlo;
+      }
+    }
+    fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads
+    wg_bar();
+  }
+  if (threadIdx.x == 0) TC_STAMP(10 + 3 * j);
+}
+
+// B_MN: the weight tiles are MN-major (dgrad chains); forward chains read them K-major.
+template <bool PLANES2, bool B_MN>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_constant__ ChainGroup g, int stages, int stage_b) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // keeps the shared address space (LDS/STS)
@@ -106,8 +179,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_co
       for (int j = 0; j < nl; ++j) {
         const ChainLayer& Lj = P.L[j];
         const int nkb = Lj.kblocks[0] + Lj.kblocks[1];
-        const int b_boxes = Lj.b_mn ? (Lj.bn + 63) / 64 : 1;
-        const uint32_t b_bytes = Lj.b_mn ? (uint32_t)b_boxes * 8192 : (uint32_t)Lj.bn * 128;
+        const int b_boxes = B_MN ? (Lj.bn + 63) / 64 : 1;
+        const uint32_t b_bytes = B_MN ? (uint32_t)b_boxes * 8192 : (uint32_t)Lj.bn * 128;
         const uint32_t tx = planes * (b_bytes + (j == 0 ? (uint32_t)TC_STAGE_A : 0u));
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
@@ -119,7 +192,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_co
           for (int pl = 0; pl < planes; ++pl) {
             if (j == 0)  // A ring slot = B ring slot: reuse is ordered by the same empty barrier
               tma_load_3d(opnd + (size_t)(stage * planes + pl) * TC_STAGE_A, &P.mapA[seg], &full[stage], kloc, m0, pl);
-            if (Lj.b_mn) {
+            if (B_MN) {
               for (int i = 0; i < b_boxes; ++i) tma_load_3d(sB + pl * stage_b + i * 8192, &Lj.mapB, &full[stage], 64 * i, kB, pl);
             } else {
               tma_load_3d(sB + pl * stage_b, &Lj.mapB, &full[stage], kB, 0, pl);
@@ -131,71 +204,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_co
     }
   } else {
     // ===== MMA warpgroup: per layer the MMAs, then the epilogue on the accumulator registers, which also writes the
-    // next layer's operand =====
-    const int wl = threadIdx.x, r_lo = (wl >> 5) * 16 + (lane >> 2);   // this thread's rows r_lo, r_lo + 8 of the block
-    float* row = scratch + wl * 16;
+    // next layer's operand; the tile width is dispatched once per layer =====
+    float* row = scratch + threadIdx.x * 16;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[128];
     for (int j = 0; j < nl; ++j) {
-      const ChainLayer& Lj = P.L[j];
-      const int nkb = Lj.kblocks[0] + Lj.kblocks[1];
-      const int nb = (Lj.bn + 63) / 64;
-#pragma unroll
-      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        if (j == 0 && kb == 0 && threadIdx.x == 0) TC_STAMP(2);
-        const uint32_t sB = smem_u32(ringB + (size_t)stage * planes * stage_b);
-        // layer 0: the ring slot of this stage; later layers: k-block kb of the operand buffer
-        const uint32_t sA = smem_u32(opnd) + (uint32_t)(j == 0 ? stage * planes * TC_STAGE_A : kb * TC_STAGE_A);
-        const uint32_t a_plane = j == 0 ? TC_STAGE_A : CH_OPND_PLANE;
-        const int ksteps = j == 0 ? 4 : min(4, (Lj.K - kb * TC_BK + 15) / 16);
-        wg_fence();
-        for (int k = 0; k < ksteps; ++k) {
-          const uint32_t b_off = Lj.b_mn ? k * 2048 : k * 32;
-          const uint64_t b_hi = make_desc(sB + b_off, Lj.b_mn ? 8192 : 16, 1024);
-          const uint64_t b_lo = make_desc(sB + stage_b + b_off, Lj.b_mn ? 8192 : 16, 1024);
-          const uint64_t a_hi = make_desc(sA + k * 32, 16, 1024);
-          const uint64_t a_lo = make_desc(sA + a_plane + k * 32, 16, 1024);
-          if (Lj.b_mn) wgmma_step<0, 1>(acc, nb, planes == 2, a_hi, b_hi, a_lo, b_lo);
-          else wgmma_step<0, 0>(acc, nb, planes == 2, a_hi, b_hi, a_lo, b_lo);
-        }
-        wg_commit();
-        wg_wait_all();
-        if (lane == 0) mbar_arrive(&empty[stage]);
-        if (++stage == stages) { stage = 0; phase ^= 1; }
+      switch ((P.L[j].bn + 63) / 64) {
+        case 1: chain_layer<PLANES2, B_MN, 1>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
+        case 2: chain_layer<PLANES2, B_MN, 2>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
+        case 3: chain_layer<PLANES2, B_MN, 3>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
+        default: chain_layer<PLANES2, B_MN, 4>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
       }
-      if (threadIdx.x == 0) TC_STAMP(8 + 3 * j);   // MMAs of layer j retired
-      EpiArgs E;
-      E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.N; E.ldz = Lj.N;
-      E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
-      E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
-      epi_frag<PLANES2>(acc, nb, E, m0, 0, row);
-      if (threadIdx.x == 0) TC_STAMP(9 + 3 * j);
-      if (j + 1 < nl) {
-        // next layer's A operand: bf16 hi/lo pairs at (row, column) of the swizzled K-major k-block tiles
-        // (16-byte chunk index ^= row & 7).  Every warp's MMAs of this layer have retired before anyone overwrites.
-        wg_bar();
-        uint8_t* const o = opnd;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (i >= 8 * nb) break;
-          const int c = 8 * i + 2 * (lane & 3), cc = c & 63;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r_lo + 8 * h;
-            uint32_t whi, wlo;
-            split_pack2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], whi, wlo);
-            const uint32_t off = (uint32_t)((c >> 6) * TC_STAGE_A + r * 128 + ((((cc >> 3) ^ (r & 7)) << 4) | ((cc & 7) * 2)));
-            *reinterpret_cast<uint32_t*>(o + off) = whi;
-            if (PLANES2) *reinterpret_cast<uint32_t*>(o + CH_OPND_PLANE + off) = wlo;
-          }
-        }
-        fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads
-        wg_bar();
-      }
-      if (threadIdx.x == 0) TC_STAMP(10 + 3 * j);
     }
   }
 

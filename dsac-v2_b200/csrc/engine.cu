@@ -545,6 +545,7 @@ static Wt weight(const dsact_handle* h, const Net& net, const float* base, int j
 struct ChainBuild {
   ChainGroup g;
   int grid = 0, stage_b = 16 * 128;
+  int b_mn = -1;   // B orientation, one per launch: forward chains K-major, dgrad chains MN-major
   double flops = 0.0;
   bool ok = true;
   explicit ChainBuild(int passes) { memset(&g, 0, sizeof(g)); g.passes = passes; }
@@ -558,9 +559,12 @@ struct ChainBuild {
   }
   ChainLayer& layer(ChainPass& P, const Img& wimg, bool b_mn, int N, int K0, int K1, int kB1) {
     ChainLayer& L = P.L[P.n_layers++];
-    L.N = N; L.bn = (N + 15) / 16 * 16; L.b_mn = b_mn ? 1 : 0;
+    L.N = N; L.bn = (N + 15) / 16 * 16;
+    const int o = b_mn ? 1 : 0;
+    if (this->b_mn >= 0 && this->b_mn != o) ok = false;   // the kernel takes one B orientation per launch
+    this->b_mn = o;
     L.kblocks[0] = (K0 + TC_BK - 1) / TC_BK; L.kblocks[1] = (K1 + TC_BK - 1) / TC_BK;
-    L.kB0[0] = 0; L.kB0[1] = kB1; L.K = K0;
+    L.kB0[0] = 0; L.kB0[1] = kB1;
     ok = ok && make_map(&L.mapB, wimg, b_mn ? 64 : L.bn);
     const int sb = (L.bn + 63) / 64 * 8192;   // the wgmma N (64 multiple) reads that many rows of a K-major tile
     if (sb > stage_b) stage_b = sb;
@@ -580,12 +584,19 @@ static void launch_chain(dsact_handle* h, ChainBuild& cb, int cls, Ctx& c) {
   const int stages = planes == 2 ? 2 : 4;   // layer 0's A ring lives in the 4-k-block operand buffer
   const int smem = chain_smem_bytes(stages, planes, cb.stage_b);
   if (!h->chain_attr_done) {
-    cudaFuncSetAttribute(tc_chain_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(tc_chain_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc_chain_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc_chain_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc_chain_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc_chain_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     h->chain_attr_done = true;
   }
-  if (planes == 2) launch_k(tc_chain_kernel<true>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
-  else launch_k(tc_chain_kernel<false>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+  if (planes == 2) {
+    if (cb.b_mn) launch_k(tc_chain_kernel<true, true>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+    else launch_k(tc_chain_kernel<true, false>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+  } else {
+    if (cb.b_mn) launch_k(tc_chain_kernel<false, true>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+    else launch_k(tc_chain_kernel<false, false>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+  }
   c.done(cls, cb.flops);
   c.check();
   if (debug && cb.g.dbg) {
@@ -878,7 +889,7 @@ static void enqueue_phase1(dsact_handle* h, const dsact_batch& bt, const dsact_n
 
   const bool fused = h->fused();
   const Img i_none;
-  if (fused) {  // wave A as ONE launch: each CTA runs a 128-row block through every layer of its pass
+  if (fused) {  // wave A as ONE launch: each CTA runs a 64-row block through every layer of its pass
     ChainBuild cb(h->passes());
     chain_fwd_pass(cb, h, pi, PIb[0], ar.i_wpi[0], t_obs.im, O, i_none, 0, 0, B, cf.act_pi, ar.zP, ar.i_hP, W + ar.logitsP);
     chain_fwd_pass(cb, h, pi, PIb[1], ar.i_wpi[1], t_obs2.im, O, i_none, 0, 0, B, cf.act_pi, nullptr, nullptr, W + ar.logitsT);
@@ -1072,7 +1083,7 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
       cudaStreamWaitEvent(c.side, h->ev_fork, 0);
       Ctx cs{c.side, 0, cudaSuccess};
       cs.pdl = c.pdl;
-      // the policy backward chain needs ceil(B/128) whole SMs: keep them free of weight-gradient CTAs
+      // the policy backward chain needs ceil(B/64) whole SMs: keep them free of weight-gradient CTAs
       const int chain_ctas = (B + TC_BM - 1) / TC_BM;
       const int cap = h->num_sms - chain_ctas;
       launch_group(h, gw, V_WGRAD, cs, cap >= h->num_sms / 2 ? cap : 0);

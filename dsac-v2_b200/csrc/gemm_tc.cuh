@@ -112,7 +112,8 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>   // at most N committed wgmma groups of this warp still in flight
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, %0;" ::"n"(TC_MMA_THREADS) : "memory"); }   // the MMA warpgroup only
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -128,28 +129,22 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
   return d;
 }
 
-// One k16 step of a 64 x (64 nb) tile: hi*hi, and with two planes also hi*lo + lo*hi.  nb is warp-uniform.
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_step(float (&d)[128], int nb, bool three, uint64_t a_hi, uint64_t b_hi, uint64_t a_lo,
-                                           uint64_t b_lo) {
-  switch (nb) {
-    case 1:
-      wgmma_n64<TA, TB>(d, a_hi, b_hi);
-      if (three) { wgmma_n64<TA, TB>(d, a_hi, b_lo); wgmma_n64<TA, TB>(d, a_lo, b_hi); }
-      break;
-    case 2:
-      wgmma_n128<TA, TB>(d, a_hi, b_hi);
-      if (three) { wgmma_n128<TA, TB>(d, a_hi, b_lo); wgmma_n128<TA, TB>(d, a_lo, b_hi); }
-      break;
-    case 3:
-      wgmma_n192<TA, TB>(d, a_hi, b_hi);
-      if (three) { wgmma_n192<TA, TB>(d, a_hi, b_lo); wgmma_n192<TA, TB>(d, a_lo, b_hi); }
-      break;
-    default:
-      wgmma_n256<TA, TB>(d, a_hi, b_hi);
-      if (three) { wgmma_n256<TA, TB>(d, a_hi, b_lo); wgmma_n256<TA, TB>(d, a_lo, b_hi); }
-      break;
-  }
+// One m64 x (64 NB) x k16 wgmma.
+template <int NB, int TA, int TB>
+__device__ __forceinline__ void wgmma_nb(float (&d)[128], uint64_t a, uint64_t b) {
+  if constexpr (NB == 1) wgmma_n64<TA, TB>(d, a, b);
+  else if constexpr (NB == 2) wgmma_n128<TA, TB>(d, a, b);
+  else if constexpr (NB == 3) wgmma_n192<TA, TB>(d, a, b);
+  else wgmma_n256<TA, TB>(d, a, b);
+}
+
+// One k16 step of a 64 x (64 NB) tile: hi*hi, and with two planes also hi*lo + lo*hi.
+// The tile width is a compile-time constant of the whole MMA loop and epilogue: with a runtime width the accumulator
+// is read and written on paths ptxas cannot prove uniform, and it then waits for every wgmma before issuing the next.
+template <int NB, int TA, int TB, bool PLANES2>
+__device__ __forceinline__ void wgmma_step(float (&d)[128], uint64_t a_hi, uint64_t b_hi, uint64_t a_lo, uint64_t b_lo) {
+  wgmma_nb<NB, TA, TB>(d, a_hi, b_hi);
+  if constexpr (PLANES2) { wgmma_nb<NB, TA, TB>(d, a_hi, b_lo); wgmma_nb<NB, TA, TB>(d, a_lo, b_hi); }
 }
 
 __device__ __forceinline__ unsigned long long gtime() {
@@ -278,20 +273,19 @@ struct EpiArgs {
   long long img_plane;
 };
 
-// Epilogue of the warpgroup's 64 x (64 nb) accumulator, element (0, 0) = output (m0, n0), straight from the wgmma
+// Epilogue of the warpgroup's 64 x (64 NB) accumulator, element (0, 0) = output (m0, n0), straight from the wgmma
 // fragment: acc[16 g + t] sits in row ra (t & 2 == 0) or ra + 8, column n0 + 32 g + 8 (t >> 2) + 2 (lane & 3) + (t & 1).
 // Columns >= N leave as zeros (they are the next layer's K padding and the image padding).  On return acc holds the
 // result.  `row`: this thread's 16-float shared-memory row (generic activations).
-template <bool PLANES2>
-__device__ __forceinline__ void epi_frag(float (&acc)[128], int nb, const EpiArgs& E, int m0, int n0, float* row) {
+template <bool PLANES2, int NB>
+__device__ __forceinline__ void epi_frag(float (&acc)[128], const EpiArgs& E, int m0, int n0, float* row) {
   const int wl = threadIdx.x & (TC_MMA_THREADS - 1), lane = threadIdx.x & 31;
   const int ra = m0 + (wl >> 5) * 16 + (lane >> 2);
   const bool ok0 = ra < E.M, ok1 = ra + 8 < E.M;
   const int cq = n0 + 2 * (lane & 3);
   const int img_w = (E.N + 7) / 8 * 8;
 #pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    if (g >= 2 * nb) break;
+  for (int g = 0; g < 2 * NB; ++g) {
     float v[16], d[16];
 #pragma unroll
     for (int t = 0; t < 16; ++t) v[t] = acc[16 * g + t];
@@ -354,6 +348,53 @@ __device__ __forceinline__ void epi_frag(float (&acc)[128], int nb, const EpiArg
 #pragma unroll
     for (int t = 0; t < 16; ++t) acc[16 * g + t] = v[t];
   }
+}
+
+// MMA warpgroup of one 64 x (64 NB) tile: the MMAs, one k-block of them kept in flight (the slot of k-block kb is
+// released once kb + 1 has been issued and kb has retired), then the epilogue on the accumulator registers.
+template <bool A_MN, bool B_MN, bool PLANES2, int NB>
+__device__ __forceinline__ void gemm_tile_mma(const TcGroup& g, const TcProb& P, uint8_t* smem, int stages, int stage_b,
+                                              uint64_t* full, uint64_t* empty, int kb_begin, int kb_end, int ks, int m0, int n0) {
+  constexpr int planes = PLANES2 ? 2 : 1;
+  const int stage_bytes = planes * (TC_STAGE_A + stage_b);
+  const int lane = threadIdx.x & 31;
+  float acc[128];
+#pragma unroll
+  for (int i = 0; i < 32 * NB; ++i) acc[i] = 0.f;
+  int stage = 0, prev = -1;
+  uint32_t phase = 0;
+  for (int kb = kb_begin; kb < kb_end; ++kb) {
+    mbar_wait(&full[stage], phase);
+    if (kb == kb_begin && threadIdx.x == 0) TC_STAMP(2);
+    const uint32_t sA = smem_u32(smem + (size_t)stage * stage_bytes);
+    const uint32_t sB = sA + planes * TC_STAGE_A;
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k) {
+      const uint32_t a_off = A_MN ? k * 2048 : k * 32;
+      const uint32_t b_off = B_MN ? k * 2048 : k * 32;
+      const uint64_t a_hi = make_desc(sA + a_off, A_MN ? 8192 : 16, 1024);
+      const uint64_t b_hi = make_desc(sB + b_off, B_MN ? 8192 : 16, 1024);
+      const uint64_t a_lo = make_desc(sA + TC_STAGE_A + a_off, A_MN ? 8192 : 16, 1024);
+      const uint64_t b_lo = make_desc(sB + stage_b + b_off, B_MN ? 8192 : 16, 1024);
+      wgmma_step<NB, A_MN, B_MN, PLANES2>(acc, a_hi, b_hi, a_lo, b_lo);
+    }
+    wg_commit();
+    wg_wait<1>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);  // this warp's share of k-block kb - 1 retired
+    prev = stage;
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+  wg_wait<0>();
+  if (threadIdx.x == 0) TC_STAMP(3);
+  wg_bar();   // every MMA of the tile retired: the pipeline smem is dead and serves as the activation scratch
+  if (threadIdx.x == 0) TC_STAMP(4);
+  EpiArgs E;
+  E.epi = P.epi; E.act = P.act; E.M = P.M; E.N = P.N; E.ldc = P.ldc; E.ldz = P.ldz;
+  E.bias = P.bias; E.Zout = P.Zout; E.Zin = P.Zin; E.colsum = P.colsum;
+  E.C = P.C ? P.C + (P.epi == EPI_PARTIAL ? (size_t)ks * P.split_stride : 0) : nullptr;
+  E.img = P.img; E.img_pitch = P.img_pitch; E.img_plane = P.img_plane;
+  epi_frag<PLANES2, NB>(acc, E, m0, n0, reinterpret_cast<float*>(smem) + threadIdx.x * 16);
 }
 
 // A_MN / B_MN: operand is MN-major (reduction dimension strided in global memory).
@@ -437,43 +478,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_kernel(const __grid_con
       }
     }
   } else {
-    // ===== MMA warpgroup, then the epilogue on the accumulator registers =====
-    const int nb = (bn + 63) / 64;   // wgmma N = 64 nb; columns >= bn are never stored
-    float acc[128];
-#pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
-      mbar_wait(&full[stage], phase);
-      if (kb == kb_begin && threadIdx.x == 0) TC_STAMP(2);
-      const uint32_t sA = smem_u32(smem + (size_t)stage * stage_bytes);
-      const uint32_t sB = sA + planes * TC_STAGE_A;
-      wg_fence();
-#pragma unroll
-      for (int k = 0; k < TC_BK / 16; ++k) {
-        const uint32_t a_off = A_MN ? k * 2048 : k * 32;
-        const uint32_t b_off = B_MN ? k * 2048 : k * 32;
-        const uint64_t a_hi = make_desc(sA + a_off, A_MN ? 8192 : 16, 1024);
-        const uint64_t b_hi = make_desc(sB + b_off, B_MN ? 8192 : 16, 1024);
-        const uint64_t a_lo = make_desc(sA + TC_STAGE_A + a_off, A_MN ? 8192 : 16, 1024);
-        const uint64_t b_lo = make_desc(sB + stage_b + b_off, B_MN ? 8192 : 16, 1024);
-        wgmma_step<A_MN, B_MN>(acc, nb, planes == 2, a_hi, b_hi, a_lo, b_lo);
-      }
-      wg_commit();
-      wg_wait_all();
-      if (lane == 0) mbar_arrive(&empty[stage]);  // smem slot reusable once this warp's share of the MMAs retired
-      if (++stage == stages) { stage = 0; phase ^= 1; }
+    // ===== MMA warpgroup: wgmma N = 64 nb; columns >= bn are never stored =====
+    switch ((bn + 63) / 64) {
+      case 1: gemm_tile_mma<A_MN, B_MN, PLANES2, 1>(g, P, smem, stages, stage_b, full, empty, kb_begin, kb_end, ks, m0, n0); break;
+      case 2: gemm_tile_mma<A_MN, B_MN, PLANES2, 2>(g, P, smem, stages, stage_b, full, empty, kb_begin, kb_end, ks, m0, n0); break;
+      case 3: gemm_tile_mma<A_MN, B_MN, PLANES2, 3>(g, P, smem, stages, stage_b, full, empty, kb_begin, kb_end, ks, m0, n0); break;
+      default: gemm_tile_mma<A_MN, B_MN, PLANES2, 4>(g, P, smem, stages, stage_b, full, empty, kb_begin, kb_end, ks, m0, n0); break;
     }
-    if (threadIdx.x == 0) TC_STAMP(3);
-    wg_bar();   // every MMA of the tile retired: the pipeline smem is dead and serves as the activation scratch
-    if (threadIdx.x == 0) TC_STAMP(4);
-    EpiArgs E;
-    E.epi = P.epi; E.act = P.act; E.M = P.M; E.N = P.N; E.ldc = P.ldc; E.ldz = P.ldz;
-    E.bias = P.bias; E.Zout = P.Zout; E.Zin = P.Zin; E.colsum = P.colsum;
-    E.C = P.C ? P.C + (P.epi == EPI_PARTIAL ? (size_t)ks * P.split_stride : 0) : nullptr;
-    E.img = P.img; E.img_pitch = P.img_pitch; E.img_plane = P.img_plane;
-    epi_frag<PLANES2>(acc, nb, E, m0, n0, reinterpret_cast<float*>(smem) + threadIdx.x * 16);
   }
 
   if (lane == 0 && warp < 4) { if (g.dbg) atomicMax(&g.dbg[(size_t)blockIdx.x * TC_DBG_SLOTS + 5], gtime()); }
