@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DSACT_LIB: kernel-development aid (A/B of two builds on one GPU box); the product is libdsact.so beside this file
 LIB_PATH = os.environ.get("DSACT_LIB") or os.path.join(_HERE, "libdsact.so")
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 MAX_HIDDEN = 6
 NUM_STATS = 16
 
@@ -62,7 +62,9 @@ class CnnConfig(C.Structure):
 
 class Layout(C.Structure):
     _fields_ = [("n_q", C.c_int64), ("n_pi", C.c_int64), ("n_params", C.c_int64), ("n_targets", C.c_int64),
-                ("workspace_bytes", C.c_int64), ("state_floats", C.c_int64), ("max_batch", C.c_int64)]
+                ("workspace_bytes", C.c_int64), ("state_floats", C.c_int64), ("max_batch", C.c_int64),
+                ("off_idx", C.c_int64), ("off_eps1", C.c_int64), ("off_eps2", C.c_int64), ("off_z3", C.c_int64),
+                ("off_z4", C.c_int64), ("off_slabs", C.c_int64), ("slab_floats", C.c_int64)]
 
 
 _fp = C.c_void_p  # device pointers travel as integers
@@ -124,22 +126,6 @@ SYMBOLS = {
                                        C.c_void_p]),
     "dsact_cnn_query_layout": (C.c_int, [C.POINTER(CnnConfig), C.POINTER(Layout)]),
     "dsact_cnn_create": (C.c_int, [C.POINTER(CnnConfig), C.c_int, C.POINTER(C.c_void_p)]),
-    "dsact_cnn_destroy": (None, [C.c_void_p]),
-    "dsact_cnn_bind": (C.c_int, [C.c_void_p, C.POINTER(Buffers)]),
-    "dsact_cnn_set_carry": (C.c_int, [C.c_void_p, C.c_float, C.c_float, C.c_int64, C.c_int64, C.c_void_p]),
-    "dsact_cnn_replay_bind": (C.c_int, [C.c_void_p, C.POINTER(Replay)]),
-    "dsact_cnn_replay_add": (C.c_int, [C.c_void_p] + [C.c_void_p] * 6 + [C.c_int64, C.c_int64, C.c_void_p]),
-    "dsact_cnn_replay_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Batch), C.c_void_p]),
-    "dsact_cnn_seed": (C.c_int, [C.c_void_p, C.c_uint64]),
-    "dsact_cnn_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_void_p]),
-    "dsact_cnn_read_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
-    "dsact_cnn_grad_phase1": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_void_p]),
-    "dsact_cnn_grad_phase2": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
-    "dsact_cnn_compute_grads": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_void_p]),
-    "dsact_cnn_apply": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
-    "dsact_cnn_dp_export": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
-    "dsact_cnn_dp_connect": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
-    "dsact_cnn_dp_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_profile_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_void_p, C.POINTER(Profile)]),
     "dsact_launch_count": (C.c_int64, [C.c_void_p]),
     "dsact_last_call_launches": (C.c_int32, [C.c_void_p]),

@@ -1,5 +1,5 @@
 // DSAC-T update with the reference's CNN approximators (BASELINE config 5; reference networks/cnn.py:30-53 conv stack,
-// :151-240 StochaPolicy, :383-461 ActionValueDistri).  Included at the end of engine.cu: it reuses the grouped fp32 GEMM
+// :151-240 StochaPolicy, :383-461 ActionValueDistri).  Included by engine.cu before its C ABI: it reuses the grouped fp32 GEMM
 // launcher, the loss / sample / policy-gradient kernels and apply_kernel of the MLP engine; what is new here is the conv
 // stack (conv.cuh) and the two-head wiring (separate `mean` and `log_std` MLPs per network, their outputs packed into the
 // [B,2] / [B,2A] arrays the loss kernels read, by strided GEMM outputs).
@@ -75,14 +75,9 @@ constexpr int CNN_DGRAD_SMEM = 96 * 1024;   // opt-in dynamic shared memory of c
 
 struct CnnHeadBuf { int64_t z[DSACT_MAX_HIDDEN], h[DSACT_MAX_HIDDEN], dz[DSACT_MAX_HIDDEN]; };
 
-struct dsact_cnn_handle {
+struct HeadsHandle : dsact_handle {
   dsact_cnn_config cfg;
-  int device, num_sms;
   CnnGeom q, pi;
-  dsact_buffers buf;
-  bool bound = false;
-  uint64_t seed = 0x5DEECE66Dull;
-  int64_t dev_iter = -1, launches = 0;
   // arena (floats from the workspace base)
   int64_t convP[DSACT_MAX_CONV + 1], convT[DSACT_MAX_CONV + 1], convQ[4][DSACT_MAX_CONV + 1];   // activations 1..nconv
   CnnHeadBuf hb[14];   // 0,1 pi mean/ls; 2,3 pi'; 4..7 Q1,Q2 (s,a) mean/ls; 8..11 Q1',Q2'; 12,13 mean head of Q1,Q2 on (s,a~)
@@ -90,16 +85,8 @@ struct dsact_cnn_handle {
   int64_t dfeat[3], dfa[2];   // dL/dfeature of pi, Q1, Q2; dL/d(feature|act) scratch of the actor path
   int64_t ga, gb;             // conv-backward ping-pong buffers (largest activation)
   int64_t r_obs, r_obs2, r_act, r_rew, r_done, r_logp, r_idx;   // gathered replay minibatch
-  dsact_replay rb;
-  bool rb_bound = false;
-  int64_t dev_rb_size = -1;
-  // what the last phase 1 ran on (phase 2 reads the same rows and noise)
-  int32_t pending_batch = 0;
-  dsact_batch pending = {};
-  const float *pending_eps1 = nullptr, *pending_z3 = nullptr, *pending_z4 = nullptr;
-  DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   int64_t total;
-  float* Wp() const { return reinterpret_cast<float*>(buf.workspace); }
+  HeadsHandle() : dsact_handle(ENGINE_HEADS) {}
   void layout() {
     const int64_t B = cfg.max_batch, A = cfg.act_dim;
     int64_t off = 0;
@@ -129,12 +116,19 @@ struct dsact_cnn_handle {
 };
 
 // critics: two heads of one output (networks/cnn.py) or one head of two (networks/mlp.py:113-127); policy: mean and
-// log_std heads (networks/cnn.py, mlp.py std_type "mlp_separated") or a mean head + learnable row (std_type "parameter")
-static void cnn_build_nets(dsact_cnn_handle* h) {
-  const dsact_cnn_config& c = h->cfg;
+// log_std heads (networks/cnn.py, mlp.py std_type "mlp_separated") or a mean head + learnable row (std_type "parameter").
+// Also lays out the arena and sets the shell's sizes.
+static void cnn_setup(HeadsHandle* h, const dsact_cnn_config& c) {
   const bool q1 = c.q_heads == 1, row = c.pi_std == 1, shared = c.pi_std == 2;
+  h->cfg = c;
   h->q.build(c, c.act_dim, q1 ? 2 : 1, q1 ? 1 : 2, false);
   h->pi.build(c, 0, shared ? 2 * c.act_dim : c.act_dim, (row || shared) ? 1 : 2, row);
+  h->layout();
+  h->obs_elems = (int64_t)c.channels * c.height * c.width;
+  h->act_dim = c.act_dim;
+  h->max_batch = c.max_batch;
+  h->v1 = c.algo == 1;
+  h->n_params = (h->v1 ? 1 : 2) * h->q.n + h->pi.n + 1;   // DSAC_V1 has one critic
 }
 
 static int cnn_validate(const dsact_cnn_config* c) {
@@ -167,8 +161,8 @@ struct CnnHeadFwd {
   bool keep_z;
   float* out; int out_ld;       // head output column(s) inside a packed array
 };
-static void cnn_heads_forward(dsact_cnn_handle* h, const Net& net, std::vector<CnnHeadFwd>& P, int B, Ctx& c) {
-  float* W = h->Wp();
+static void cnn_heads_forward(HeadsHandle* h, const Net& net, std::vector<CnnHeadFwd>& P, int B, Ctx& c) {
+  float* W = h->W();
   for (int j = 0; j <= net.L; ++j) {
     size_t i0 = 0;
     while (i0 < P.size()) {
@@ -204,8 +198,8 @@ struct CnnHeadBwd {
   const float* dout; int dout_ld;   // dL/d(head output) inside a packed array
   float* din;            // [B, k0 + k1] dL/d(layer-0 input), accumulated (+=), or null
 };
-static void cnn_heads_backward(dsact_cnn_handle* h, const Net& net, std::vector<CnnHeadBwd>& P, int B, Ctx& c) {
-  float* W = h->Wp();
+static void cnn_heads_backward(HeadsHandle* h, const Net& net, std::vector<CnnHeadBwd>& P, int B, Ctx& c) {
+  float* W = h->W();
   for (int j = net.L; j >= 0; --j) {
     GemmGroup gw, gd;
     gw.n = gd.n = 0;
@@ -385,8 +379,8 @@ static int conv_layer_dgrad(int num_sms, const ConvShape& s, const float* dy, co
 
 static void conv_note(int rc, Ctx& c) { if (rc != DSACT_OK && c.err == cudaSuccess) c.err = cudaErrorInvalidValue; }
 
-static void cnn_conv_forward(dsact_cnn_handle* h, const CnnGeom& g, const float* params, const float* img, const int64_t* acts, int B, Ctx& c) {
-  float* W = h->Wp();
+static void cnn_conv_forward(HeadsHandle* h, const CnnGeom& g, const float* params, const float* img, const int64_t* acts, int B, Ctx& c) {
+  float* W = h->W();
   const float* x = img;
   for (int j = 0; j < g.nconv; ++j) {
     conv_note(conv_layer_fwd(h->num_sms, g.shape(j, B), x, params + g.cw[j], params + g.cb[j], W + acts[j + 1], ConvPick(), c), c);
@@ -397,9 +391,9 @@ static void cnn_conv_forward(dsact_cnn_handle* h, const CnnGeom& g, const float*
 }
 
 // backward through one encoder: `gtop` = dL/d(feature) [B, F] (consumed); gparams was cleared by begin_step_kernel
-static void cnn_conv_backward(dsact_cnn_handle* h, const CnnGeom& g, const float* params, float* gparams, const float* img,
+static void cnn_conv_backward(HeadsHandle* h, const CnnGeom& g, const float* params, float* gparams, const float* img,
                               const int64_t* acts, float* gtop, int B, Ctx& c) {
-  float* W = h->Wp();
+  float* W = h->W();
   float* gcur = gtop;
   float* bufs[2] = {W + h->ga, W + h->gb};
   int flip = 0;
@@ -424,12 +418,12 @@ static void cnn_conv_backward(dsact_cnn_handle* h, const CnnGeom& g, const float
 }
 
 // ---- the DSAC-T step in three phases --------------------------------------------------------------------------------
-// dsact_cnn_step runs them back to back on its own rows; the data-parallel step (dsact_cnn_dp_step) runs the critic-std
+// dsact_step runs them back to back on its own rows; the data-parallel step (dsact_dp_step) runs the critic-std
 // exchange between phases 1 and 2 and the gradient exchange between phase 2 and the update.
 struct CnnFeats { const float *P, *T, *Q[4]; };   // head inputs: pi(s), pi'(s'), Q1/Q2 features of s, Q1'/Q2' features of s'
-static CnnFeats cnn_feats(const dsact_cnn_handle* h, const dsact_batch& bt) {
+static CnnFeats cnn_feats(const HeadsHandle* h, const dsact_batch& bt) {
   // without a conv stack (the MLP approximators with separate heads) the feature is the observation itself
-  float* W = h->Wp();
+  float* W = h->W();
   const bool enc = h->pi.nconv > 0;
   const int qL = h->q.nconv;
   CnnFeats f;
@@ -445,11 +439,11 @@ static CnnFeats cnn_feats(const dsact_cnn_handle* h, const dsact_batch& bt) {
 // phase 1: clear the step's accumulators and gradients, noise, the encoder forwards, the policy heads, the critics on
 // (s, a), sample_kernel (whose y = 1 half leaves the local critic-std sums in state[ST_STDSUM..+1]), the targets and the
 // mean heads of the critics on (s, a~)
-static void cnn_enqueue_phase1(dsact_cnn_handle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
+static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
   const dsact_cnn_config& cf = h->cfg;
   const CnnGeom &q = h->q, &pi = h->pi;
   const int B = bt.batch, A = cf.act_dim;
-  float* W = h->Wp();
+  float* W = h->W();
   float* P = h->buf.params; float* T = h->buf.targets; float* G = h->buf.grads;
   float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
   float* Tq[2] = {T, T + q.n}; float* Tpi = T + 2 * q.n;
@@ -530,12 +524,12 @@ static void cnn_enqueue_phase1(dsact_cnn_handle* h, const dsact_batch& bt, const
 // phase 2: losses, the head and encoder backward passes, and phase2_tail_kernel, on the rows phase 1 ran.  Every batch
 // mean is a sum over these rows times 1/global_batch; phase2_tail_kernel keeps rows = B (this shard), so that the log_alpha
 // gradient it writes is this rank's additive share -(sum_local logp + B * H) / global_batch (see tail_grad_log_alpha).
-static void cnn_enqueue_phase2(dsact_cnn_handle* h, int64_t global_batch, Ctx& c) {
+static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
   const dsact_cnn_config& cf = h->cfg;
   const CnnGeom &q = h->q, &pi = h->pi;
   const dsact_batch& bt = h->pending;
   const int B = bt.batch, A = cf.act_dim;
-  float* W = h->Wp();
+  float* W = h->W();
   float* P = h->buf.params; float* G = h->buf.grads;
   float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
   float* Gq[2] = {G, G + q.n}; float* Gpi = G + 2 * q.n;
@@ -640,7 +634,7 @@ static void cnn_enqueue_phase2(dsact_cnn_handle* h, int64_t global_batch, Ctx& c
 // Adam / Polyak on `grads` (dp = false), or on the rank-ordered sum of every rank's exchange block (dp = true).
 // scalars_ready: 1 = phase 2 of this step wrote the Adam scalars; 0 = apply_kernel forms them (a handle that only receives
 // gradients never runs phase 2)
-static void cnn_enqueue_apply(dsact_cnn_handle* h, Ctx& c, int scalars_ready, bool dp) {
+static void cnn_enqueue_apply(HeadsHandle* h, Ctx& c, int scalars_ready, bool dp) {
   const dsact_cnn_config& cf = h->cfg;
   const long long n_all = 2 * h->q.n + h->pi.n + 1;
   ApplyArgs a;
@@ -665,269 +659,24 @@ static void cnn_enqueue_apply(dsact_cnn_handle* h, Ctx& c, int scalars_ready, bo
   c.check();
 }
 
+static HeadsHandle* heads(dsact_handle* h) { return static_cast<HeadsHandle*>(h); }
+
 #include "v1_step.cuh"
 
-extern "C" {
-
-int dsact_cnn_query_layout(const dsact_cnn_config* cfg, dsact_layout* out) {
-  int rc = cnn_validate(cfg);
-  if (rc) return rc;
-  if (!out) return fail(DSACT_EINVAL, "null out");
-  dsact_cnn_handle h;
-  h.cfg = *cfg;
-  cnn_build_nets(&h);
-  h.layout();
-  const int ncrit = cfg->algo == 1 ? 1 : 2;   // DSAC_V1 has one critic
-  out->n_q = h.q.n; out->n_pi = h.pi.n;
-  out->n_params = ncrit * h.q.n + h.pi.n + 1;
-  out->n_targets = ncrit * h.q.n + h.pi.n;
-  out->workspace_bytes = h.total * (int64_t)sizeof(float);
-  out->state_floats = ST_FLOATS;
-  out->max_batch = cfg->max_batch;
-  return DSACT_OK;
-}
-
-int dsact_cnn_create(const dsact_cnn_config* cfg, int device, dsact_cnn_handle** out) {
-  int rc = cnn_validate(cfg);
-  if (rc) return rc;
-  if (!out) return fail(DSACT_EINVAL, "null out");
-  CUDA_TRY(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0) return fail(DSACT_EARCH, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
-  CUDA_TRY(cudaFuncSetAttribute(conv_dgrad8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CNN_DGRAD_SMEM));
-  dsact_cnn_handle* h = new dsact_cnn_handle();
-  h->cfg = *cfg;
-  h->device = device;
-  h->num_sms = prop.multiProcessorCount;
-  cnn_build_nets(h);
-  h->layout();
-  *out = h;
-  return DSACT_OK;
-}
-
-void dsact_cnn_destroy(dsact_cnn_handle* h) {
-  if (!h) return;
-  if (h->dp.buf) { cudaSetDevice(h->device); dp_peer_release(h->dp); }
-  delete h;
-}
-
-int dsact_cnn_bind(dsact_cnn_handle* h, const dsact_buffers* b) {
-  if (!h || !b) return fail(DSACT_EINVAL, "null argument");
-  if (!b->params || !b->targets || !b->grads || !b->adam_m || !b->adam_v || !b->act_high || !b->act_low || !b->state || !b->workspace)
-    return fail(DSACT_EINVAL, "null buffer pointer");
-  h->buf = *b;
-  h->bound = true;
-  h->dev_iter = -1;
-  return DSACT_OK;
-}
-
-int dsact_cnn_set_carry(dsact_cnn_handle* h, float m1, float m2, int64_t tq, int64_t tp, void* stream) {
-  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
-  CUDA_TRY(cudaSetDevice(h->device));
-  set_carry_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(h->buf.state, m1, m2, (int)tq, (int)tp);
-  CUDA_TRY(cudaGetLastError());
-  return DSACT_OK;
-}
-
-int dsact_cnn_seed(dsact_cnn_handle* h, uint64_t seed) {
-  if (!h) return fail(DSACT_EINVAL, "null handle");
-  h->seed = seed;
-  return DSACT_OK;
-}
-
-int dsact_cnn_read_stats(dsact_cnn_handle* h, int64_t global_batch, float* host_out, void* stream) {
-  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
-  if (!host_out || global_batch < 1) return fail(DSACT_EINVAL, "bad argument");
-  CUDA_TRY(cudaSetDevice(h->device));
-  // DSAC_V1 logs one entry of the logits row per sample (dsac_v1.py:142-143), DSAC-T the mean over all action dimensions
-  const double pol = h->cfg.algo == 1 ? (double)global_batch : (double)global_batch * h->cfg.act_dim;
-  finalize_stats_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(h->buf.state, (float)(1.0 / (double)global_batch), (float)(1.0 / pol));
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(host_out, h->buf.state + ST_STATS, DSACT_NUM_STATS * sizeof(float), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return DSACT_OK;
-}
-
-int dsact_cnn_replay_bind(dsact_cnn_handle* h, const dsact_replay* rb) {
-  if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
-  if (!rb->obs || !rb->obs2 || !rb->act || !rb->rew || !rb->done || !rb->logp || rb->capacity < 1) return fail(DSACT_EINVAL, "bad replay buffers");
-  h->rb = *rb;
-  h->rb_bound = true;
-  h->dev_rb_size = -1;
-  return DSACT_OK;
-}
-
-int dsact_cnn_replay_add(dsact_cnn_handle* h, const float* obs, const float* obs2, const float* act, const float* rew,
-                         const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
-  if (!h || !h->rb_bound) return fail(DSACT_ESTATE, "replay buffer not bound");
-  if (n < 0 || n > h->rb.capacity || ptr < 0 || ptr >= h->rb.capacity) return fail(DSACT_EINVAL, "bad n/ptr");
-  if (n == 0) return DSACT_OK;
-  if (!obs || !obs2 || !act || !rew || !done || !logp) return fail(DSACT_EINVAL, "null staging pointer");
-  CUDA_TRY(cudaSetDevice(h->device));
-  const int64_t first = (ptr + n <= h->rb.capacity) ? n : h->rb.capacity - ptr;
-  const int64_t O = (int64_t)h->cfg.channels * h->cfg.height * h->cfg.width, A = h->cfg.act_dim;
-  struct { float* dst; const float* src; int64_t w; } cols[6] = {
-      {h->rb.obs, obs, O}, {h->rb.obs2, obs2, O}, {h->rb.act, act, A}, {h->rb.rew, rew, 1}, {h->rb.done, done, 1}, {h->rb.logp, logp, 1}};
-  for (auto& c : cols) {
-    CUDA_TRY(cudaMemcpyAsync(c.dst + ptr * c.w, c.src, first * c.w * sizeof(float), cudaMemcpyDefault, (cudaStream_t)stream));
-    if (first < n)
-      CUDA_TRY(cudaMemcpyAsync(c.dst, c.src + first * c.w, (n - first) * c.w * sizeof(float), cudaMemcpyDefault, (cudaStream_t)stream));
-  }
-  return DSACT_OK;
-}
-
-int dsact_cnn_replay_sample(dsact_cnn_handle* h, int32_t batch, int64_t size, const int64_t* idx, dsact_batch* out, void* stream) {
-  if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
-  if (size < 1 || size > h->rb.capacity) return fail(DSACT_EINVAL, "size %lld outside [1, capacity]", (long long)size);
-  CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->dev_rb_size != size) { set_rb_size_kernel<<<1, 32, 0, s>>>(h->buf.state, size); CUDA_TRY(cudaGetLastError()); h->dev_rb_size = size; }
-  float* W = h->Wp();
-  const int O = h->cfg.channels * h->cfg.height * h->cfg.width, A = h->cfg.act_dim;
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = false;
-  int64_t* draw = idx ? nullptr : reinterpret_cast<int64_t*>(W + h->r_idx);
-  int blocks = (batch + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-  const ImgOut none{nullptr, 0, 1, 0};
-  launch_k(gather_kernel, blocks, 256, 0, c, (const float*)h->rb.obs, (const float*)h->rb.obs2, (const float*)h->rb.act, (const float*)h->rb.rew,
-           (const float*)h->rb.done, (const float*)h->rb.logp, idx, W + h->r_obs, W + h->r_obs2, W + h->r_act, W + h->r_rew, W + h->r_done,
-           W + h->r_logp, (int)batch, O, A, none, none, none, draw, (unsigned long long)h->seed, (const float*)h->buf.state, 1);
-  c.done();
-  if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
-  h->launches += c.launches;
-  if (out) {
-    out->obs = W + h->r_obs; out->act = W + h->r_act; out->rew = W + h->r_rew; out->obs2 = W + h->r_obs2; out->done = W + h->r_done;
-    out->logp = W + h->r_logp; out->batch = batch;
-  }
-  return DSACT_OK;
-}
-
-static int cnn_check_batch(const dsact_cnn_handle* h, const dsact_batch* batch) {
-  if (!h || !h->bound) return fail(DSACT_ESTATE, "dsact_cnn_bind has not been called");
-  if (!batch || !batch->obs || !batch->act || !batch->rew || !batch->obs2 || !batch->done) return fail(DSACT_EINVAL, "null batch pointer");
-  if (batch->batch < 1 || batch->batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch %d outside [1, max_batch=%d]", batch->batch, h->cfg.max_batch);
-  return DSACT_OK;
-}
-static int cnn_sync_iteration(dsact_cnn_handle* h, int64_t iteration, cudaStream_t s) {
-  if (iteration < 0 || iteration > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
-  if (h->dev_iter != iteration) { set_iter_kernel<<<1, 32, 0, s>>>(h->buf.state, (int)iteration); CUDA_TRY(cudaGetLastError()); }
-  return DSACT_OK;
-}
-// the split and data-parallel entry points implement DSAC_V2 (DSAC-T); DSAC_V1 (algo 1) has local steps only
-static int cnn_check_v2(const dsact_cnn_handle* h) {
-  if (!h) return fail(DSACT_EINVAL, "null handle");
-  if (h->cfg.algo != 0) return fail(DSACT_EINVAL, "DSAC_V1 handles (algo 1) have no split or data-parallel update");
-  return DSACT_OK;
-}
-static int cnn_finish(dsact_cnn_handle* h, Ctx& c) {
-  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
-  h->launches += c.launches;
-  return DSACT_OK;
-}
-
-int dsact_cnn_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration, void* stream) {
-  int rc = cnn_check_batch(h, batch);
-  if (rc || (rc = check_noise(noise))) return rc;
-  if (iteration < 0 || iteration > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
-  CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  if ((rc = cnn_sync_iteration(h, iteration, s))) return rc;
-  if (h->cfg.algo == 1) return cnn_step_v1(h, batch, noise, iteration, s);
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = false;
-  cnn_enqueue_phase1(h, *batch, noise, c);
-  cnn_enqueue_phase2(h, batch->batch, c);
+// dsact_step: phase 1, phase 2 and the update on its own rows, or the DSAC_V1 update
+static void cnn_enqueue_step(HeadsHandle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
+  if (h->v1) { cnn_enqueue_v1(h, &bt, noise, c); return; }
+  cnn_enqueue_phase1(h, bt, noise, c);
+  cnn_enqueue_phase2(h, bt.batch, c);
   cnn_enqueue_apply(h, c, 1, false);
-  if ((rc = cnn_finish(h, c))) return rc;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
 }
 
-int dsact_cnn_grad_phase1(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
-  int rc = cnn_check_v2(h);
-  if (rc || (rc = cnn_check_batch(h, batch)) || (rc = check_noise(noise))) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
-  c.pdl = false;
-  cnn_enqueue_phase1(h, *batch, noise, c);
-  return cnn_finish(h, c);
-}
-
-int dsact_cnn_grad_phase2(dsact_cnn_handle* h, int64_t global_batch, void* stream) {
-  int rc = cnn_check_v2(h);
-  if (rc) return rc;
-  if (!h->bound) return fail(DSACT_ESTATE, "not bound");
-  if (h->pending_batch < 1) return fail(DSACT_ESTATE, "dsact_cnn_grad_phase2 without a preceding dsact_cnn_grad_phase1");
-  if (global_batch < h->pending_batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, h->pending_batch);
-  CUDA_TRY(cudaSetDevice(h->device));
-  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
-  c.pdl = false;
-  cnn_enqueue_phase2(h, global_batch, c);
-  return cnn_finish(h, c);
-}
-
-int dsact_cnn_compute_grads(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
-  int rc = cnn_check_v2(h);
-  if (rc || (rc = cnn_check_batch(h, batch)) || (rc = check_noise(noise))) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
-  c.pdl = false;
-  cnn_enqueue_phase1(h, *batch, noise, c);
-  cnn_enqueue_phase2(h, batch->batch, c);
-  return cnn_finish(h, c);
-}
-
-int dsact_cnn_apply(dsact_cnn_handle* h, int64_t iteration, void* stream) {
-  int rc = cnn_check_v2(h);
-  if (rc) return rc;
-  if (!h->bound) return fail(DSACT_ESTATE, "not bound");
-  CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  if ((rc = cnn_sync_iteration(h, iteration, s))) return rc;
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = false;
-  cnn_enqueue_apply(h, c, 0, false);
-  if ((rc = cnn_finish(h, c))) return rc;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
-}
-
-// ---- data parallelism over peer memory (dp_peer.cuh; the same exchange buffer and kernels as dsact_dp_*) -------------
-int dsact_cnn_dp_export(dsact_cnn_handle* h, void* handle_out, int64_t* bytes_out) {
-  int rc = cnn_check_v2(h);
-  if (rc) return rc;
-  if (!handle_out) return fail(DSACT_EINVAL, "null argument");
-  return dp_peer_export(h->dp, h->device, 2 * h->q.n + h->pi.n + 1, handle_out, bytes_out);
-}
-
-int dsact_cnn_dp_connect(dsact_cnn_handle* h, int32_t rank, int32_t world, const void* handles) {
-  int rc = cnn_check_v2(h);
-  if (rc) return rc;
-  if (!handles) return fail(DSACT_EINVAL, "null argument");
-  if (!h->bound) return fail(DSACT_ESTATE, "dsact_cnn_bind has not been called");
-  if (!h->dp.buf) return fail(DSACT_ESTATE, "dsact_cnn_dp_export has not been called");
-  return dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
-}
-
-// One data-parallel update on this rank's shard, eager on the caller's stream: phase 1, critic-std sums exchanged,
-// phase 2 scaled by 1/global_batch, the local gradients into this rank's exchange block, logged sums exchanged (also the
-// "every block is complete" barrier), [reduce-scatter from 6 ranks up], Adam on the rank-ordered global sum.
-// Every rank must call it for the same iteration.
-int dsact_cnn_dp_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t global_batch, int64_t iteration,
-                      void* stream) {
-  int rc = cnn_check_v2(h);
-  if (rc || (rc = cnn_check_batch(h, batch)) || (rc = check_noise(noise))) return rc;
-  if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_cnn_dp_connect has not been called");
-  if (global_batch < batch->batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch->batch);
-  CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  if ((rc = cnn_sync_iteration(h, iteration, s))) return rc;
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = false;
+// One data-parallel update on this rank's shard (dsact_dp_step), eager on the caller's stream: phase 1, critic-std sums
+// exchanged, phase 2 scaled by 1/global_batch, the local gradients into this rank's exchange block, logged sums exchanged
+// (also the "every block is complete" barrier), [reduce-scatter from 6 ranks up], Adam on the rank-ordered global sum.
+static void cnn_enqueue_dp_step(HeadsHandle* h, const dsact_batch& bt, const dsact_noise* noise, int64_t global_batch, Ctx& c) {
   float* state = h->buf.state;
-  cnn_enqueue_phase1(h, *batch, noise, c);
+  cnn_enqueue_phase1(h, bt, noise, c);
   enqueue_dp_exchange(h->dp, state, 0, c);
   cnn_enqueue_phase2(h, global_batch, c);
   {   // phase 2 already wrote the log_alpha share: a plain copy of the flat gradients into this rank's block
@@ -942,8 +691,63 @@ int dsact_cnn_dp_step(dsact_cnn_handle* h, const dsact_batch* batch, const dsact
   enqueue_dp_exchange(h->dp, state, 1, c);
   if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, state, h->num_sms, c);
   cnn_enqueue_apply(h, c, 1, true);
-  if ((rc = cnn_finish(h, c))) return rc;
-  h->dev_iter = iteration + 1;
+}
+
+// dsact_replay_sample: ring rows idx[i] (NULL: drawn on the device and recorded in the arena) -> the arena minibatch
+static void cnn_enqueue_gather(HeadsHandle* h, int32_t batch, const int64_t* idx, Ctx& c) {
+  float* W = h->W();
+  int64_t* draw = idx ? nullptr : reinterpret_cast<int64_t*>(W + h->r_idx);
+  int blocks = (batch + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
+  const ImgOut none{nullptr, 0, 1, 0};
+  launch_k(gather_kernel, blocks, 256, 0, c, (const float*)h->rb.obs, (const float*)h->rb.obs2, (const float*)h->rb.act, (const float*)h->rb.rew,
+           (const float*)h->rb.done, (const float*)h->rb.logp, idx, W + h->r_obs, W + h->r_obs2, W + h->r_act, W + h->r_rew, W + h->r_done,
+           W + h->r_logp, (int)batch, (int)h->obs_elems, h->act_dim, none, none, none, draw, (unsigned long long)h->seed,
+           (const float*)h->buf.state, 1);
+  c.done();
+  if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
+}
+
+static dsact_batch cnn_arena_batch(const HeadsHandle* h, int32_t batch) {
+  float* W = h->W();
+  dsact_batch b;
+  b.obs = W + h->r_obs; b.act = W + h->r_act; b.rew = W + h->r_rew; b.obs2 = W + h->r_obs2; b.done = W + h->r_done;
+  b.logp = W + h->r_logp;
+  b.batch = batch;
+  return b;
+}
+
+extern "C" {
+
+int dsact_cnn_query_layout(const dsact_cnn_config* cfg, dsact_layout* out) {
+  int rc = cnn_validate(cfg);
+  if (rc) return rc;
+  if (!out) return fail(DSACT_EINVAL, "null out");
+  HeadsHandle h;
+  cnn_setup(&h, *cfg);
+  out->n_q = h.q.n; out->n_pi = h.pi.n;
+  out->n_params = h.n_params;
+  out->n_targets = h.n_params - 1;
+  out->workspace_bytes = h.total * (int64_t)sizeof(float);
+  out->state_floats = ST_FLOATS;
+  out->max_batch = cfg->max_batch;
+  out->off_idx = h.r_idx; out->off_eps1 = h.eps1; out->off_eps2 = h.eps2; out->off_z3 = h.z3; out->off_z4 = h.z4;
+  out->off_slabs = h.total; out->slab_floats = 0;
+  return DSACT_OK;
+}
+
+int dsact_cnn_create(const dsact_cnn_config* cfg, int device, dsact_handle** out) {
+  int rc = cnn_validate(cfg);
+  if (rc) return rc;
+  if (!out) return fail(DSACT_EINVAL, "null out");
+  CUDA_TRY(cudaSetDevice(device));
+  int num_sms = 0;
+  if ((rc = check_sm90(device, &num_sms))) return rc;
+  CUDA_TRY(cudaFuncSetAttribute(conv_dgrad8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CNN_DGRAD_SMEM));
+  HeadsHandle* h = new HeadsHandle();
+  h->device = device;
+  h->num_sms = num_sms;
+  cnn_setup(h, *cfg);
+  *out = h;
   return DSACT_OK;
 }
 
@@ -953,27 +757,25 @@ int dsact_cnn_test_conv(int32_t op, int32_t batch, int32_t cin, int32_t hin, int
   if (op < 0 || op > 2) return fail(DSACT_EINVAL, "op must be 0 (forward), 1 (weight gradient) or 2 (dgrad)");
   if (batch < 1 || cin < 1 || cout < 1 || k < 1 || stride < 1 || hin < k || win < k) return fail(DSACT_EINVAL, "bad layer shape");
   if (r < 0 || cob < 0 || slabs < 0 || channels < 0) return fail(DSACT_EINVAL, "negative kernel choice");
-  int dev = 0;
+  int dev = 0, num_sms = 0;
   CUDA_TRY(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 9 || prop.minor != 0) return fail(DSACT_EARCH, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major, prop.minor);
+  int rc = check_sm90(dev, &num_sms);
+  if (rc) return rc;
   CUDA_TRY(cudaFuncSetAttribute(conv_dgrad8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CNN_DGRAD_SMEM));
   ConvShape s;
   s.B = batch; s.Cin = cin; s.Hin = hin; s.Win = win; s.Cout = cout; s.K = k; s.S = stride;
   s.Hout = (hin - k) / stride + 1; s.Wout = (win - k) / stride + 1;
   ConvPick pk; pk.r = r; pk.cob = cob; pk.slabs = slabs; pk.channels = channels;
   Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
-  int rc;
   if (op == 0) {
     if (!x || !w || !b || !out) return fail(DSACT_EINVAL, "forward needs x, w, b, out");
-    rc = conv_layer_fwd(prop.multiProcessorCount, s, x, w, b, out, pk, c);
+    rc = conv_layer_fwd(num_sms, s, x, w, b, out, pk, c);
   } else if (op == 1) {
     if (!x || !dy || !dw || !db) return fail(DSACT_EINVAL, "weight gradient needs x, dy, dw, db");
-    rc = conv_layer_wgrad(prop.multiProcessorCount, s, dy, x, dw, db, pk, c);
+    rc = conv_layer_wgrad(num_sms, s, dy, x, dw, db, pk, c);
   } else {
     if (!x || !w || !dy || !out) return fail(DSACT_EINVAL, "dgrad needs x, w, dy, out");
-    rc = conv_layer_dgrad(prop.multiProcessorCount, s, dy, w, x, out, pk, c);
+    rc = conv_layer_dgrad(num_sms, s, dy, w, x, out, pk, c);
   }
   if (rc) return rc;
   c.check();

@@ -76,7 +76,7 @@ struct Arena {
   ImgSlot i_hQ[6][DSACT_MAX_HIDDEN], i_dzQ[6][DSACT_MAX_HIDDEN], i_dOut[6];
   ImgSlot i_wq[4][DSACT_MAX_HIDDEN + 1], i_wpi[2][DSACT_MAX_HIDDEN + 1];  // q1,q2,q1',q2' / pi,pi'
   int kpad_q0;        // column of the act block inside the Q layer-0 weight image
-  int64_t slabs;      // [nslabs][n_params] fp32 wgrad partials
+  int64_t slabs;      // [nslabs][n_params] fp32 wgrad partials, the arena's last region
   int nslabs;
   int64_t slab_stride;   // floats between slabs: n_params rounded up to 4 (float4 access to every slab)
   int64_t total;
@@ -120,6 +120,8 @@ struct Arena {
       nslabs = (int)(B / 256); if (nslabs > 4) nslabs = 4; if (nslabs < 1) nslabs = 1;
       slab_stride = (2 * q.n + pi.n + 1 + 3) / 4 * 4;
       slabs = take((int64_t)nslabs * slab_stride);
+    } else {
+      slabs = off;   // the (empty) last region
     }
     total = off;
   }
@@ -131,20 +133,37 @@ struct GraphKey {
 };
 struct GraphEntry { GraphKey key; cudaGraphExec_t exec; int launches; uint64_t stamp; };
 
+// The shell both engines share: device, bound buffers, generator seed, replay ring, peer exchange, what the last phase 1
+// ran on, launch counts, and the few sizes the shell's entry points check against.  `engine` says which of MlpHandle
+// (the wgmma / SIMT MLP engine, this file) and HeadsHandle (the head-wise fp32 engine, cnn_engine.cuh) it is.
+enum { ENGINE_MLP = 0, ENGINE_HEADS = 1 };
 struct dsact_handle {
+  int engine;
+  int device = 0, num_sms = 0;
+  int64_t obs_elems = 0;     // floats of one observation row
+  int act_dim = 0, max_batch = 0;
+  int64_t n_params = 0;      // flat parameter count (log_alpha included)
+  bool v1 = false;           // DSAC_V1: local steps only, its own policy-statistic denominator
+  dsact_buffers buf = {};
+  bool bound = false, rb_bound = false;
+  uint64_t seed = 0x5DEECE66Dull;
+  int64_t dev_iter = -1;     // what state[ST_ITER] will hold when the next enqueued work runs (-1 unknown)
+  int64_t dev_rb_size = -1;  // what state[ST_RB_SIZE] holds
+  dsact_replay rb = {};
+  DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
+  int32_t pending_batch = 0; // rows of the shard phase1 processed (phase2 must match)
+  dsact_batch pending = {};  // batch pointers of phase1
+  const float *pending_eps1 = nullptr, *pending_z3 = nullptr, *pending_z4 = nullptr;  // noise phase1 used (phase2 needs it again)
+  int64_t launches = 0;
+  int32_t last_launches = 0;
+  explicit dsact_handle(int e) : engine(e) {}
+  float* W() const { return reinterpret_cast<float*>(buf.workspace); }
+};
+
+struct MlpHandle : dsact_handle {
   dsact_config cfg;
-  int device, num_sms;
   Net q, pi;
   Arena ar;
-  dsact_buffers buf;
-  dsact_replay rb;
-  bool bound, rb_bound;
-  uint64_t seed;
-  int64_t dev_iter;          // what state[ST_ITER] will hold when the next enqueued work runs (-1 unknown)
-  int32_t pending_batch;     // rows of the shard phase1 processed (phase2 must match)
-  dsact_batch pending;       // batch pointers of phase1
-  const float *pending_eps1, *pending_z3, *pending_z4;  // noise phase1 used (phase2 needs it again)
-  int64_t dev_rb_size;       // what state[ST_RB_SIZE] holds
   bool join_pending = false; // a forked branch of the current enqueue has not been joined yet
   bool apply_early = false;  // phase 2 of the current enqueue already ran the critics' part of the update
   bool arena_imaged;         // the last dsact_replay_sample left bf16 images of obs/obs2/act beside the arena batch
@@ -153,7 +172,6 @@ struct dsact_handle {
   cudaEvent_t ev_fork, ev_join;
   cudaEvent_t ev_pro_fork, ev_pro_join;   // prologue branch (weight images, noise, clears) beside the replay gather
   cudaEvent_t ev_dp_fork, ev_dp_join;     // std-sum exchange of the data-parallel step beside the second forward chain
-  DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   // host-minibatch staging (dsact_stage_host): two device sets + a private copy stream
   float* stage_buf[2] = {nullptr, nullptr};
   int64_t stage_floats = 0;
@@ -164,9 +182,8 @@ struct dsact_handle {
   bool tc_attr_done = false, chain_attr_done = false;   // cudaFuncSetAttribute is per device: tracked per handle
   TcGroup tc_scratch;                                   // host-side lowering scratch of launch_tc (~5 KiB)
   std::vector<GraphEntry> graphs;
-  uint64_t stamp;
-  int64_t launches;
-  int32_t last_launches;
+  uint64_t stamp = 0;
+  MlpHandle() : dsact_handle(ENGINE_MLP) {}
   bool tc() const { return cfg.gemm_mode != DSACT_GEMM_FP32; }
   bool fused() const {  // layer-chain kernel: every layer must fit one 256-column wgmma accumulator / A operand
     if (!tc()) return false;
@@ -177,7 +194,6 @@ struct dsact_handle {
     return cfg.act_dim <= 256;
   }
   int passes() const { return cfg.gemm_mode == DSACT_GEMM_BF16X3 ? 3 : 1; }
-  float* W() const { return reinterpret_cast<float*>(buf.workspace); }
   Img img(const ImgSlot& s, int rows) const {  // image handle with the live row count
     Img i;
     if (s.off < 0) return i;
@@ -288,7 +304,7 @@ static void launch_simt(int num_sms, GemmGroup& g, int variant, Ctx& c) {
 // Lower the group onto wgmma: images instead of fp32 operands, TMA tensor maps, 64 x bn tiles.
 // `max_ctas` > 0: issue the group as several launches of at most that many CTAs (one CTA occupies an SM), which leaves
 // the remaining SMs to a concurrent branch of the step graph for the whole duration.
-static void launch_tc(dsact_handle* h, Group& G, int variant, Ctx& c, int max_ctas = 0) {
+static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas = 0) {
   TcGroup& t = h->tc_scratch;
   memset(&t, 0, sizeof(t));
   t.n = G.n;
@@ -395,7 +411,7 @@ static void launch_tc(dsact_handle* h, Group& G, int variant, Ctx& c, int max_ct
   }
 }
 
-static void launch_group(dsact_handle* h, Group& G, int variant, Ctx& c, int max_ctas = 0) {
+static void launch_group(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas = 0) {
   if (G.n == 0) return;
   double flops = 0.0;
   for (int i = 0; i < G.n; ++i) flops += 2.0 * G.prob(i).M * G.prob(i).N * ((double)G.prob(i).K[0] + G.prob(i).K[1]);
@@ -499,9 +515,9 @@ struct ImgBatch {
     j.seg_w[1] = w1; j.seg_src0[1] = w0; j.seg_dst0[1] = dst1;
     j.pitch = dst.pitch; j.fill_w = w1 > 0 ? dst1 + w1 : w0; j.plane = dst.plane;
   }
-  void reserve(const dsact_handle* h, Ctx& c, int jobs) { if (g.n + jobs > IMG_MAXJ) launch(h, c); }   // flush when full
+  void reserve(const MlpHandle* h, Ctx& c, int jobs) { if (g.n + jobs > IMG_MAXJ) launch(h, c); }   // flush when full
   // `pro` != null: the clears and the device noise ride in the same launch (step_prologue_kernel)
-  void launch(const dsact_handle* h, Ctx& c, PrologueArgs* pro = nullptr) {
+  void launch(const MlpHandle* h, Ctx& c, PrologueArgs* pro = nullptr) {
     if (overflow) { c.err = cudaErrorInvalidValue; return; }
     if (g.n == 0 && !pro) return;
     g.planes = h->passes() == 3 ? 2 : 1;
@@ -525,14 +541,14 @@ struct ImgBatch {
   }
 };
 
-static ImgOut img_out(const dsact_handle* h, const ImgSlot& s) {
+static ImgOut img_out(const MlpHandle* h, const ImgSlot& s) {
   ImgOut o;
   o.p = nullptr; o.pitch = 0; o.planes = h->passes() == 3 ? 2 : 1; o.plane = 0;
   if (h->tc() && s.off >= 0) { o.p = reinterpret_cast<__nv_bfloat16*>(h->W() + s.off); o.pitch = s.pitch; o.plane = s.plane; }
   return o;
 }
 
-static Wt weight(const dsact_handle* h, const Net& net, const float* base, int j, const ImgSlot& slot) {
+static Wt weight(const MlpHandle* h, const Net& net, const float* base, int j, const ImgSlot& slot) {
   Wt w;
   w.f = base + net.w[j];
   w.bias = base + net.b[j];
@@ -573,7 +589,7 @@ struct ChainBuild {
   }
 };
 
-static void launch_chain(dsact_handle* h, ChainBuild& cb, int cls, Ctx& c) {
+static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
   if (cb.g.n == 0) return;
   if (!cb.ok) { c.err = cudaErrorInvalidValue; return; }
   static unsigned long long* dbg = nullptr;
@@ -622,7 +638,7 @@ static void launch_chain(dsact_handle* h, ChainBuild& cb, int cls, Ctx& c) {
 }
 
 // forward chain of one pass: out = head(act(...act(in W_0^T + b_0)...))
-static ChainPass& chain_fwd_pass(ChainBuild& cb, const dsact_handle* h, const Net& net, const float* Wbase, const ImgSlot* wslots,
+static ChainPass& chain_fwd_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const float* Wbase, const ImgSlot* wslots,
                            const Img& in0, int k0, const Img& in1, int k1, int kB1, int B, int act,
                            const int64_t* zout_off, const ImgSlot* himg, float* out) {
   ChainPass& P = cb.begin(in0, in1, B);
@@ -647,7 +663,7 @@ static ChainPass& chain_fwd_pass(ChainBuild& cb, const dsact_handle* h, const Ne
 }
 
 // dgrad chain of one pass: dz_{j-1} = (dz_j W_j) (.) act'(z_{j-1}) for j = L..1 (+ dAct = dz_0 W_0[:, act columns])
-static ChainPass& chain_dgrad_pass(ChainBuild& cb, const dsact_handle* h, const Net& net, const ImgSlot* wslots, const Img& dout,
+static ChainPass& chain_dgrad_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const ImgSlot* wslots, const Img& dout,
                              int B, int act, const int64_t* zin_off, float* gbase /*bias grads of this net or null*/,
                              const ImgSlot* dzimg /*or null*/, float* dact_out, int act_col_img, int act_cols) {
   const Img none;
@@ -675,7 +691,7 @@ static ChainPass& chain_dgrad_pass(ChainBuild& cb, const dsact_handle* h, const 
 // ---- enqueue: pieces of one update ---------------------------------------------
 // Everything of a step that depends on neither the minibatch gather nor a forward pass: accumulator clears, the
 // gradient memset, the bf16 images of all weights (and of a caller-supplied batch), the device noise.
-static void enqueue_noise(dsact_handle* h, int B, Ctx& c) {
+static void enqueue_noise(MlpHandle* h, int B, Ctx& c) {
   const Arena& ar = h->ar;
   float* W = h->W();
   const int A = h->cfg.act_dim;
@@ -684,7 +700,7 @@ static void enqueue_noise(dsact_handle* h, int B, Ctx& c) {
   launch_k(noise_kernel, blocks, 256, 0, c, W + ar.eps1, W + ar.eps2, W + ar.z3, W + ar.z4, B, A, h->seed, h->buf.state);
   c.done();
 }
-static void enqueue_prologue(dsact_handle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged,
+static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged,
                              bool with_noise = true) {
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
@@ -749,7 +765,7 @@ static void enqueue_prologue(dsact_handle* h, const dsact_batch& bt, const dsact
 
 // In a captured step the prologue runs as its own branch next to whatever the main stream does first (the replay
 // gather); returns true if it was forked and must be joined (enqueue_phase1 does) before the first forward pass.
-static bool fork_prologue(dsact_handle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged) {
+static bool fork_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged) {
   if (!c.side) return false;
   cudaEventRecord(h->ev_pro_fork, c.s);
   cudaStreamWaitEvent(c.side, h->ev_pro_fork, 0);
@@ -788,7 +804,7 @@ static void enqueue_dp_exchange(const DpPeer& dp, float* state, int kind, Ctx& c
   launch_k(dp_exchange_kernel, 1, 32 * dp.comm.world, 0, c, dp.comm, state, kind, dp_timeout_ns());
   c.done();
 }
-static void enqueue_dp_exchange(dsact_handle* h, int kind, Ctx& c) { enqueue_dp_exchange(h->dp, h->buf.state, kind, c); }
+static void enqueue_dp_exchange(MlpHandle* h, int kind, Ctx& c) { enqueue_dp_exchange(h->dp, h->buf.state, kind, c); }
 
 // apply_kernel<2>'s view of the exchange: the reduced block in this rank's own memory once every rank's kind-2 flag is
 // here (two-shot), or every rank's block, summed in rank order (one-shot)
@@ -803,7 +819,7 @@ static void dp_apply_args(const DpPeer& dp, ApplyArgs& a) {
   }
 }
 
-// ---- exchange-buffer setup shared by dsact_dp_* and dsact_cnn_dp_* ----------------------------------------------
+// ---- exchange-buffer setup (dsact_dp_export / dsact_dp_connect, both engines) ---------------------------------------
 static int dp_peer_export(DpPeer& dp, int device, long long n_params, void* handle_out, int64_t* bytes_out) {
   CUDA_TRY(cudaSetDevice(device));
   dp.n_params = n_params;
@@ -858,7 +874,7 @@ static void dp_peer_release(DpPeer& dp) {
 // `dp_std_exchange`: the std sums are complete once sample_kernel has run, one whole forward chain before the loss needs
 // them: in a captured step their exchange (kernel + NVLink flag round trip + whatever the ranks are skewed by) runs as a
 // side branch under that chain.
-static void enqueue_phase1(dsact_handle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged = false,
+static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged = false,
                            bool prologue_forked = false, bool dp_std_exchange = false) {
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
@@ -984,10 +1000,10 @@ static void enqueue_phase1(dsact_handle* h, const dsact_batch& bt, const dsact_n
 }
 
 // the apply of a single-call step can fold the weight-gradient split slabs itself (apply_kernel<1>)
-static bool slabs_foldable(const dsact_handle* h) {
+static bool slabs_foldable(const MlpHandle* h) {
   return h->tc() && ((uintptr_t)(h->W() + h->ar.slabs) & 15) == 0 && ((uintptr_t)h->buf.grads & 15) == 0;
 }
-static TailArgs tail_args(const dsact_handle* h, int64_t global_batch, int rows) {
+static TailArgs tail_args(const MlpHandle* h, int64_t global_batch, int rows) {
   const Net &q = h->q, &pi = h->pi;
   TailArgs t;
   t.sc.tau_b = (float)h->cfg.tau_b; t.sc.alpha_fixed = (float)h->cfg.alpha_fixed;
@@ -996,13 +1012,13 @@ static TailArgs tail_args(const dsact_handle* h, int64_t global_batch, int rows)
   t.target_entropy = -(float)h->cfg.act_dim; t.rows = rows; t.enabled = 1;
   return t;
 }
-static void enqueue_apply(dsact_handle* h, Ctx& c, const TailArgs* tail, bool dp, int part);
+static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail, bool dp, int part);
 // `tail` == null (split API): the weight-gradient slabs are folded into the gradient buffer here and phase2_tail_kernel
 // closes the backward.  Otherwise (single-call steps) the kernels that follow do both: enqueue_apply (dp = false), or
 // dp_grad_fold into this rank's exchange block (dp = true).  Single-GPU fused steps also update the critics on the side
 // branch as soon as their weight gradients are complete, beside the policy backward; the caller's enqueue_apply then
 // does the rest.
-static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t global_batch, Ctx& c, const TailArgs* tail = nullptr,
+static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_batch, Ctx& c, const TailArgs* tail = nullptr,
                            bool dp = false) {
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
@@ -1158,7 +1174,7 @@ static void enqueue_phase2(dsact_handle* h, const dsact_batch& bt, int64_t globa
 // the weight-gradient split slabs.  `dp`: the gradients are the rank-ordered sum of the exchange blocks.
 // `part`: 0 = the whole flat buffer; 1 = the critics' span only, without closing the step (launched beside the policy
 // backward, see enqueue_phase2); 2 = everything after that span + the end-of-step bookkeeping
-static void enqueue_apply(dsact_handle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
+static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
   const dsact_config& cf = h->cfg;
   if (part == 0 && h->apply_early) { part = 2; h->apply_early = false; }   // phase 2 already updated the critics
   ApplyArgs a;
@@ -1195,7 +1211,7 @@ static void enqueue_apply(dsact_handle* h, Ctx& c, const TailArgs* tail = nullpt
 // One whole update of the single-call steps: phase 1, phase 2 over `global_batch` rows, then (dp) the logged-sum exchange
 // (also the "every rank's block is complete" barrier) and the reduce-scatter from 6 ranks up, then Adam / Polyak.
 // `dp`: the gradients and statistics are reduced over the peers (dsact_dp_connect) instead of locally.
-static void enqueue_update(dsact_handle* h, const dsact_batch& bt, const dsact_noise* nz, int64_t global_batch, bool dp,
+static void enqueue_update(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, int64_t global_batch, bool dp,
                            bool inputs_imaged, bool prologue_forked, Ctx& c) {
   enqueue_phase1(h, bt, nz, c, inputs_imaged, prologue_forked, dp);
   const TailArgs ta = tail_args(h, global_batch, bt.batch);
@@ -1208,7 +1224,7 @@ static void enqueue_update(dsact_handle* h, const dsact_batch& bt, const dsact_n
 }
 
 // `images_only`: the caller is a fused tensor-core step, which reads obs / obs2 / act through their bf16 images alone
-static void enqueue_gather(dsact_handle* h, int B, const int64_t* idx, Ctx& c, bool images_only = false) {
+static void enqueue_gather(MlpHandle* h, int B, const int64_t* idx, Ctx& c, bool images_only = false) {
   const Arena& ar = h->ar;
   float* W = h->W();
   // no index list: every warp of the gather draws its row's index itself (the sequence index_kernel defines) and records it
@@ -1225,22 +1241,26 @@ static void enqueue_gather(dsact_handle* h, int B, const int64_t* idx, Ctx& c, b
 // ---- graph cache -------------------------------------------------------------
 enum { K_STEP = 1, K_PHASE1 = 2, K_PHASE2 = 3, K_APPLY = 4, K_GRADS = 5, K_SAMPLE = 6, K_REPLAY_STEP = 7, K_DP_STEP = 8, K_DP_REPLAY_STEP = 9 };
 
-static void drop_graphs(dsact_handle* h) {
+static void drop_graphs(MlpHandle* h) {
   for (auto& e : h->graphs) cudaGraphExecDestroy(e.exec);
   h->graphs.clear();
 }
 
+// one eager enqueue on `s` and its launch bookkeeping (both engines)
 template <typename F>
-static int run(dsact_handle* h, cudaStream_t user, const GraphKey& key, F enqueue) {
-  if (!h->cfg.use_graph) {
-    Ctx c{user, 0, cudaSuccess};
-    c.pdl = h->tc();
-    enqueue(c);
-    if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
-    h->launches += c.launches;
-    h->last_launches = c.launches;
-    return DSACT_OK;
-  }
+static int run_eager(dsact_handle* h, cudaStream_t s, bool pdl, F enqueue) {
+  Ctx c{s, 0, cudaSuccess};
+  c.pdl = pdl;
+  enqueue(c);
+  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
+  h->launches += c.launches;
+  h->last_launches = c.launches;
+  return DSACT_OK;
+}
+
+template <typename F>
+static int run(MlpHandle* h, cudaStream_t user, const GraphKey& key, F enqueue) {
+  if (!h->cfg.use_graph) return run_eager(h, user, h->tc(), enqueue);
   GraphEntry* hit = nullptr;
   for (auto& e : h->graphs)
     if (e.key == key) { hit = &e; break; }
@@ -1287,27 +1307,47 @@ static GraphKey make_key(int kind, const dsact_batch* b, const dsact_noise* n, i
   return k;
 }
 
-static int check_batch(const dsact_handle* h, const dsact_batch* b) {
-  if (!h) return fail(DSACT_EINVAL, "null handle");
-  if (!h->bound) return fail(DSACT_ESTATE, "dsact_bind has not been called");
-  if (!b || !b->obs || !b->act || !b->rew || !b->obs2 || !b->done) return fail(DSACT_EINVAL, "null batch pointer");
-  if (b->batch < 1 || b->batch > h->cfg.max_batch)
-    return fail(DSACT_EINVAL, "batch %d outside [1, max_batch=%d]", b->batch, h->cfg.max_batch);
-  return DSACT_OK;
-}
-static int check_noise(const dsact_noise* n) {
-  if (n && (!n->eps1 || !n->eps2 || !n->z3 || !n->z4)) return fail(DSACT_EINVAL, "null noise pointer");
-  return DSACT_OK;
-}
-
 // true when `bt` is the arena minibatch that the preceding dsact_replay_sample gathered (images already there)
-static bool take_arena_images(dsact_handle* h, const dsact_batch& bt) {
+static bool take_arena_images(MlpHandle* h, const dsact_batch& bt) {
   const bool yes = h->tc() && h->arena_imaged && bt.obs == h->W() + h->ar.obs && bt.obs2 == h->W() + h->ar.obs2 &&
                    bt.act == h->W() + h->ar.act;
   // any other batch is imaged into the same shared slots by the call that asked: the arena's images are gone after it.
   // (The arena views handed out by dsact_replay_sample are read-only for the same reason: edits are not re-imaged.)
   if (!yes) h->arena_imaged = false;
   return yes;
+}
+
+static dsact_batch arena_batch(const MlpHandle* h, int32_t batch) {
+  float* W = h->W();
+  dsact_batch b;
+  b.obs = W + h->ar.obs; b.act = W + h->ar.act; b.rew = W + h->ar.rew; b.obs2 = W + h->ar.obs2; b.done = W + h->ar.done;
+  b.logp = W + h->ar.logp;
+  b.batch = batch;
+  return b;
+}
+
+static MlpHandle* mlp(dsact_handle* h) { return static_cast<MlpHandle*>(h); }
+
+// ---- checks and device-state syncs of the shell (both engines) ---------------------------------------------------
+static int check_batch(const dsact_handle* h, const dsact_batch* b) {
+  if (!h) return fail(DSACT_EINVAL, "null handle");
+  if (!h->bound) return fail(DSACT_ESTATE, "dsact_bind has not been called");
+  if (!b || !b->obs || !b->act || !b->rew || !b->obs2 || !b->done) return fail(DSACT_EINVAL, "null batch pointer");
+  if (b->batch < 1 || b->batch > h->max_batch)
+    return fail(DSACT_EINVAL, "batch %d outside [1, max_batch=%d]", b->batch, h->max_batch);
+  return DSACT_OK;
+}
+static int check_noise(const dsact_noise* n) {
+  if (n && (!n->eps1 || !n->eps2 || !n->z3 || !n->z4)) return fail(DSACT_EINVAL, "null noise pointer");
+  return DSACT_OK;
+}
+// the split and data-parallel entry points implement DSAC_V2 (DSAC-T); DSAC_V1 has local steps only
+static int check_v2(const dsact_handle* h) {
+  return h->v1 ? fail(DSACT_EINVAL, "DSAC_V1 handles (algo 1) have no split or data-parallel update") : DSACT_OK;
+}
+// host staging, the replay-fused steps, the profiler and the GEMM test hook exist on the MLP engine only
+static int check_mlp(const dsact_handle* h, const char* fn) {
+  return h && h->engine != ENGINE_MLP ? fail(DSACT_EINVAL, "%s: the head-wise engine does not implement this call", fn) : DSACT_OK;
 }
 
 static int sync_iteration(dsact_handle* h, int64_t iteration, cudaStream_t s) {
@@ -1319,6 +1359,28 @@ static int sync_iteration(dsact_handle* h, int64_t iteration, cudaStream_t s) {
   }
   return DSACT_OK;
 }
+
+static int sync_rb_size(dsact_handle* h, int64_t size, cudaStream_t s) {
+  if (size < 1 || size > h->rb.capacity) return fail(DSACT_EINVAL, "size %lld outside [1, capacity]", (long long)size);
+  if (h->dev_rb_size != size) {
+    set_rb_size_kernel<<<1, 32, 0, s>>>(h->buf.state, size);
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+    h->dev_rb_size = size;
+  }
+  return DSACT_OK;
+}
+
+// the SM count of `device`, which must be an sm_90 part
+static int check_sm90(int device, int* num_sms) {
+  cudaDeviceProp prop;
+  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9 || prop.minor != 0) return fail(DSACT_EARCH, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
+  *num_sms = prop.multiProcessorCount;
+  return DSACT_OK;
+}
+
+#include "cnn_engine.cuh"
 
 // ---- C ABI ---------------------------------------------------------------------
 extern "C" {
@@ -1358,6 +1420,8 @@ int dsact_query_layout(const dsact_config* cfg, dsact_layout* out) {
   out->workspace_bytes = ar.total * (int64_t)sizeof(float);
   out->state_floats = ST_FLOATS;
   out->max_batch = cfg->max_batch;
+  out->off_idx = ar.idx; out->off_eps1 = ar.eps1; out->off_eps2 = ar.eps2; out->off_z3 = ar.z3; out->off_z4 = ar.z4;
+  out->off_slabs = ar.slabs; out->slab_floats = ar.total - ar.slabs;
   return DSACT_OK;
 }
 
@@ -1366,23 +1430,18 @@ int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
   if (rc) return rc;
   if (!out) return fail(DSACT_EINVAL, "null out");
   CUDA_TRY(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0) return fail(DSACT_EARCH, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
-  dsact_handle* h = new dsact_handle();
+  int num_sms = 0;
+  if ((rc = check_sm90(device, &num_sms))) return rc;
+  MlpHandle* h = new MlpHandle();
   h->cfg = *cfg;
   h->device = device;
-  h->num_sms = prop.multiProcessorCount;
+  h->num_sms = num_sms;
   h->q.build(cfg->obs_dim + cfg->act_dim, cfg->hidden_q, cfg->n_hidden_q, 2);
   h->pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, 2 * cfg->act_dim);
   h->ar.build(*cfg, h->q, h->pi);
-  h->bound = h->rb_bound = false;
-  h->seed = 0x5DEECE66Dull;
-  h->dev_iter = -1;
-  h->dev_rb_size = -1;
-  h->pending_batch = 0;
+  h->obs_elems = cfg->obs_dim; h->act_dim = cfg->act_dim; h->max_batch = cfg->max_batch;
+  h->n_params = 2 * h->q.n + h->pi.n + 1;
   h->arena_imaged = false;
-  h->stamp = 0; h->launches = 0; h->last_launches = 0;
   cudaError_t e = cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming);
@@ -1396,9 +1455,12 @@ int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
   return DSACT_OK;
 }
 
-void dsact_destroy(dsact_handle* h) {
-  if (!h) return;
-  cudaSetDevice(h->device);
+void dsact_destroy(dsact_handle* hh) {
+  if (!hh) return;
+  cudaSetDevice(hh->device);
+  dp_peer_release(hh->dp);
+  if (hh->engine == ENGINE_HEADS) { delete heads(hh); return; }
+  MlpHandle* h = mlp(hh);
   drop_graphs(h);
   cudaStreamDestroy(h->cap_stream);
   cudaStreamDestroy(h->side_stream);
@@ -1408,7 +1470,6 @@ void dsact_destroy(dsact_handle* h) {
   cudaEventDestroy(h->ev_pro_join);
   cudaEventDestroy(h->ev_dp_fork);
   cudaEventDestroy(h->ev_dp_join);
-  dp_peer_release(h->dp);
   for (int t = 0; t < 2; ++t) {
     if (h->stage_buf[t]) cudaFree(h->stage_buf[t]);
     if (h->ev_stage_ready[t]) cudaEventDestroy(h->ev_stage_ready[t]);
@@ -1425,21 +1486,23 @@ int dsact_bind(dsact_handle* h, const dsact_buffers* b) {
   if ((reinterpret_cast<uintptr_t>(b->workspace) & 255) != 0) return fail(DSACT_EINVAL, "workspace must be 256-byte aligned");
   h->buf = *b;
   h->bound = true;
-  h->arena_imaged = false;
-  if (h->tc()) {  // bias regions of the wgrad slabs are never written by a kernel: they must read as zero
-    CUDA_TRY(cudaSetDevice(h->device));
-    CUDA_TRY(cudaMemset(h->W() + h->ar.slabs, 0, sizeof(float) * (size_t)h->ar.nslabs * h->ar.slab_stride));
-  }
   h->dev_iter = -1;
   h->dev_rb_size = -1;
-  drop_graphs(h);
+  if (h->engine != ENGINE_MLP) return DSACT_OK;
+  MlpHandle* m = mlp(h);
+  m->arena_imaged = false;
+  drop_graphs(m);
+  if (m->tc()) {  // bias regions of the wgrad slabs are never written by a kernel: they must read as zero
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaMemset(m->W() + m->ar.slabs, 0, sizeof(float) * (size_t)m->ar.nslabs * m->ar.slab_stride));
+  }
   return DSACT_OK;
 }
 
 int dsact_seed(dsact_handle* h, uint64_t seed) {
   if (!h) return fail(DSACT_EINVAL, "null handle");
   h->seed = seed;
-  drop_graphs(h);  // the seed is a baked kernel argument
+  if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));  // the seed is a baked kernel argument
   return DSACT_OK;
 }
 
@@ -1454,48 +1517,69 @@ int dsact_set_carry(dsact_handle* h, float m1, float m2, int64_t tq, int64_t tp,
 
 int dsact_grad_phase1(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
   int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise))) return rc;
+  if (rc || (rc = check_noise(noise)) || (rc = check_v2(h))) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
+  const cudaStream_t s = (cudaStream_t)stream;
   const dsact_batch bt = *batch;
   dsact_noise nz; const dsact_noise* np = nullptr;
   if (noise) { nz = *noise; np = &nz; }
-  const bool imaged = take_arena_images(h, bt);
-  rc = run(h, (cudaStream_t)stream, make_key(K_PHASE1, &bt, np, imaged ? 1 : 0), [&](Ctx& c) { enqueue_phase1(h, bt, np, c, imaged); });
+  if (h->engine == ENGINE_HEADS) {
+    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_phase1(heads(h), bt, np, c); });
+  } else {
+    MlpHandle* m = mlp(h);
+    const bool imaged = take_arena_images(m, bt);
+    rc = run(m, s, make_key(K_PHASE1, &bt, np, imaged ? 1 : 0), [&](Ctx& c) { enqueue_phase1(m, bt, np, c, imaged); });
+    if (rc == DSACT_OK) {  // (a replayed graph does not run enqueue_phase1, so record the noise pointers here as well)
+      m->pending_eps1 = np ? np->eps1 : m->W() + m->ar.eps1;
+      m->pending_z3 = np ? np->z3 : m->W() + m->ar.z3;
+      m->pending_z4 = np ? np->z4 : m->W() + m->ar.z4;
+    }
+  }
   if (rc) return rc;
   h->pending = bt;
   h->pending_batch = bt.batch;
-  // (a replayed graph does not run enqueue_phase1, so record the noise pointers here as well)
-  h->pending_eps1 = np ? np->eps1 : h->W() + h->ar.eps1;
-  h->pending_z3 = np ? np->z3 : h->W() + h->ar.z3;
-  h->pending_z4 = np ? np->z4 : h->W() + h->ar.z4;
   return DSACT_OK;
 }
 
 int dsact_grad_phase2(dsact_handle* h, int64_t global_batch, void* stream) {
   if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
+  int rc = check_v2(h);
+  if (rc) return rc;
   if (h->pending_batch < 1) return fail(DSACT_ESTATE, "dsact_grad_phase2 without a preceding dsact_grad_phase1");
   if (global_batch < h->pending_batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, h->pending_batch);
   CUDA_TRY(cudaSetDevice(h->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (h->engine == ENGINE_HEADS) return run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_phase2(heads(h), global_batch, c); });
+  MlpHandle* m = mlp(h);
   const dsact_batch bt = h->pending;
   dsact_noise nz{h->pending_eps1, nullptr, h->pending_z3, h->pending_z4};
   GraphKey key = make_key(K_PHASE2, &bt, &nz, global_batch);
-  return run(h, (cudaStream_t)stream, key, [&](Ctx& c) { enqueue_phase2(h, bt, global_batch, c); });
+  return run(m, s, key, [&](Ctx& c) { enqueue_phase2(m, bt, global_batch, c); });
 }
 
 int dsact_compute_grads(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
   int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise))) return rc;
+  if (rc || (rc = check_noise(noise)) || (rc = check_v2(h))) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
+  const cudaStream_t s = (cudaStream_t)stream;
   const dsact_batch bt = *batch;
   dsact_noise nz; const dsact_noise* np = nullptr;
   if (noise) { nz = *noise; np = &nz; }
-  const bool imaged = take_arena_images(h, bt);
-  GraphKey gkey = make_key(K_GRADS, &bt, np, bt.batch);
-  gkey.size = imaged ? 1 : 0;
-  rc = run(h, (cudaStream_t)stream, gkey, [&](Ctx& c) {
-    enqueue_phase1(h, bt, np, c, imaged);
-    enqueue_phase2(h, bt, bt.batch, c);
-  });
+  if (h->engine == ENGINE_HEADS) {
+    rc = run_eager(h, s, false, [&](Ctx& c) {
+      cnn_enqueue_phase1(heads(h), bt, np, c);
+      cnn_enqueue_phase2(heads(h), bt.batch, c);
+    });
+  } else {
+    MlpHandle* m = mlp(h);
+    const bool imaged = take_arena_images(m, bt);
+    GraphKey gkey = make_key(K_GRADS, &bt, np, bt.batch);
+    gkey.size = imaged ? 1 : 0;
+    rc = run(m, s, gkey, [&](Ctx& c) {
+      enqueue_phase1(m, bt, np, c, imaged);
+      enqueue_phase2(m, bt, bt.batch, c);
+    });
+  }
   if (rc) return rc;
   h->pending = bt; h->pending_batch = bt.batch;
   return DSACT_OK;
@@ -1503,10 +1587,13 @@ int dsact_compute_grads(dsact_handle* h, const dsact_batch* batch, const dsact_n
 
 int dsact_apply(dsact_handle* h, int64_t iteration, void* stream) {
   if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
-  CUDA_TRY(cudaSetDevice(h->device));
-  int rc = sync_iteration(h, iteration, (cudaStream_t)stream);
+  int rc = check_v2(h);
   if (rc) return rc;
-  rc = run(h, (cudaStream_t)stream, make_key(K_APPLY, nullptr, nullptr, 0), [&](Ctx& c) { enqueue_apply(h, c); });
+  CUDA_TRY(cudaSetDevice(h->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = sync_iteration(h, iteration, s))) return rc;
+  if (h->engine == ENGINE_HEADS) rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_apply(heads(h), c, 0, false); });
+  else rc = run(mlp(h), s, make_key(K_APPLY, nullptr, nullptr, 0), [&](Ctx& c) { enqueue_apply(mlp(h), c); });
   if (rc) return rc;
   h->dev_iter = iteration + 1;
   return DSACT_OK;
@@ -1516,15 +1603,21 @@ int dsact_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noi
   int rc = check_batch(h, batch);
   if (rc || (rc = check_noise(noise))) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
-  rc = sync_iteration(h, iteration, (cudaStream_t)stream);
+  const cudaStream_t s = (cudaStream_t)stream;
+  rc = sync_iteration(h, iteration, s);
   if (rc) return rc;
   const dsact_batch bt = *batch;
   dsact_noise nz; const dsact_noise* np = nullptr;
   if (noise) { nz = *noise; np = &nz; }
-  const bool imaged = take_arena_images(h, bt);
-  GraphKey skey = make_key(K_STEP, &bt, np, bt.batch);
-  skey.size = imaged ? 1 : 0;
-  rc = run(h, (cudaStream_t)stream, skey, [&](Ctx& c) { enqueue_update(h, bt, np, bt.batch, false, imaged, false, c); });
+  if (h->engine == ENGINE_HEADS) {
+    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_step(heads(h), bt, np, c); });
+  } else {
+    MlpHandle* m = mlp(h);
+    const bool imaged = take_arena_images(m, bt);
+    GraphKey skey = make_key(K_STEP, &bt, np, bt.batch);
+    skey.size = imaged ? 1 : 0;
+    rc = run(m, s, skey, [&](Ctx& c) { enqueue_update(m, bt, np, bt.batch, false, imaged, false, c); });
+  }
   if (rc) return rc;
   h->pending = bt; h->pending_batch = bt.batch;
   h->dev_iter = iteration + 1;
@@ -1532,10 +1625,11 @@ int dsact_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noi
 }
 
 // ---- host minibatches: staging on a private copy stream -------------------------------------------------------
-int dsact_stage_host(dsact_handle* h, const dsact_batch* host, dsact_batch* dev, void* stream) {
-  int rc = check_batch(h, host);
-  if (rc) return rc;
+int dsact_stage_host(dsact_handle* hh, const dsact_batch* host, dsact_batch* dev, void* stream) {
+  int rc = check_mlp(hh, "dsact_stage_host");
+  if (rc || (rc = check_batch(hh, host))) return rc;
   if (!dev) return fail(DSACT_EINVAL, "null out");
+  MlpHandle* h = mlp(hh);
   CUDA_TRY(cudaSetDevice(h->device));
   const int64_t O = h->cfg.obs_dim, A = h->cfg.act_dim, Bm = h->cfg.max_batch;
   const int64_t seg[5] = {round64(Bm * O), round64(Bm * A), round64(Bm), round64(Bm * O), round64(Bm)};   // obs act rew obs2 done
@@ -1567,8 +1661,11 @@ int dsact_stage_host(dsact_handle* h, const dsact_batch* host, dsact_batch* dev,
   return DSACT_OK;
 }
 
-int dsact_stage_release(dsact_handle* h, void* stream) {
-  if (!h) return fail(DSACT_EINVAL, "null handle");
+int dsact_stage_release(dsact_handle* hh, void* stream) {
+  if (!hh) return fail(DSACT_EINVAL, "null handle");
+  int rc = check_mlp(hh, "dsact_stage_release");
+  if (rc) return rc;
+  MlpHandle* h = mlp(hh);
   if (h->stage_held < 0) return DSACT_OK;
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaEventRecord(h->ev_stage_done[h->stage_held], (cudaStream_t)stream));
@@ -1578,8 +1675,10 @@ int dsact_stage_release(dsact_handle* h, void* stream) {
 }
 
 int dsact_step_host(dsact_handle* h, const dsact_batch* host, const dsact_noise* noise, int64_t iteration, void* stream) {
+  int rc = check_mlp(h, "dsact_step_host");
+  if (rc) return rc;
   dsact_batch dev;
-  int rc = dsact_stage_host(h, host, &dev, stream);
+  rc = dsact_stage_host(h, host, &dev, stream);
   if (rc) return rc;
   rc = dsact_step(h, &dev, noise, iteration, stream);
   const int rc2 = dsact_stage_release(h, stream);
@@ -1590,9 +1689,9 @@ int dsact_read_stats(dsact_handle* h, int64_t global_batch, float* host_out, voi
   if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
   if (!host_out || global_batch < 1) return fail(DSACT_EINVAL, "bad argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  const float invB = (float)(1.0 / (double)global_batch);
-  const float invBA = (float)(1.0 / ((double)global_batch * h->cfg.act_dim));
-  finalize_stats_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(h->buf.state, invB, invBA);
+  // DSAC_V1 logs one entry of the logits row per sample (dsac_v1.py:142-143), DSAC-T the mean over all action dimensions
+  const double pol = h->v1 ? (double)global_batch : (double)global_batch * h->act_dim;
+  finalize_stats_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(h->buf.state, (float)(1.0 / (double)global_batch), (float)(1.0 / pol));
   CUDA_TRY(cudaGetLastError());
   h->launches++;
   CUDA_TRY(cudaMemcpyAsync(host_out, h->buf.state + ST_STATS, DSACT_NUM_STATS * sizeof(float), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
@@ -1606,7 +1705,7 @@ int dsact_replay_bind(dsact_handle* h, const dsact_replay* rb) {
     return fail(DSACT_EINVAL, "bad replay buffers");
   h->rb = *rb;
   h->rb_bound = true;
-  drop_graphs(h);
+  if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
   return DSACT_OK;
 }
 
@@ -1618,7 +1717,7 @@ int dsact_replay_add(dsact_handle* h, const float* obs, const float* obs2, const
   if (!obs || !obs2 || !act || !rew || !done || !logp) return fail(DSACT_EINVAL, "null staging pointer");
   CUDA_TRY(cudaSetDevice(h->device));
   const int64_t first = (ptr + n <= h->rb.capacity) ? n : h->rb.capacity - ptr;
-  const int64_t O = h->cfg.obs_dim, A = h->cfg.act_dim;
+  const int64_t O = h->obs_elems, A = h->act_dim;
   struct { float* dst; const float* src; int64_t w; } cols[6] = {
       {h->rb.obs, obs, O}, {h->rb.obs2, obs2, O}, {h->rb.act, act, A}, {h->rb.rew, rew, 1}, {h->rb.done, done, 1}, {h->rb.logp, logp, 1}};
   for (auto& c : cols) {
@@ -1629,49 +1728,40 @@ int dsact_replay_add(dsact_handle* h, const float* obs, const float* obs2, const
   return DSACT_OK;
 }
 
-static int sync_rb_size(dsact_handle* h, int64_t size, cudaStream_t s) {
-  if (size < 1 || size > h->rb.capacity) return fail(DSACT_EINVAL, "size %lld outside [1, capacity]", (long long)size);
-  if (h->dev_rb_size != size) {
-    set_rb_size_kernel<<<1, 32, 0, s>>>(h->buf.state, size);
-    CUDA_TRY(cudaGetLastError());
-    h->launches++;
-    h->dev_rb_size = size;
-  }
-  return DSACT_OK;
-}
-
-static dsact_batch arena_batch(const dsact_handle* h, int32_t batch) {
-  float* W = h->W();
-  dsact_batch b;
-  b.obs = W + h->ar.obs; b.act = W + h->ar.act; b.rew = W + h->ar.rew; b.obs2 = W + h->ar.obs2; b.done = W + h->ar.done;
-  b.logp = W + h->ar.logp;
-  b.batch = batch;
-  return b;
-}
-
 int dsact_replay_sample(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, dsact_batch* out, void* stream) {
   if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
+  if (batch < 1 || batch > h->max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
   CUDA_TRY(cudaSetDevice(h->device));
-  int rc = sync_rb_size(h, size, (cudaStream_t)stream);
+  const cudaStream_t s = (cudaStream_t)stream;
+  int rc = sync_rb_size(h, size, s);
   if (rc) return rc;
+  if (h->engine == ENGINE_HEADS) {
+    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_gather(heads(h), batch, idx, c); });
+    if (rc) return rc;
+    if (out) *out = cnn_arena_batch(heads(h), batch);
+    return DSACT_OK;
+  }
+  MlpHandle* m = mlp(h);
   GraphKey key = make_key(K_SAMPLE, nullptr, nullptr, 0);
   key.batch = batch; key.idx = idx;
-  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) {
-    enqueue_gather(h, batch, idx, c);
-    if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
+  rc = run(m, s, key, [&](Ctx& c) {
+    enqueue_gather(m, batch, idx, c);
+    if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, m->buf.state); c.done(); }
   });
   if (rc) return rc;
-  h->arena_imaged = true;
-  if (out) *out = arena_batch(h, batch);
+  m->arena_imaged = true;
+  if (out) *out = arena_batch(m, batch);
   return DSACT_OK;
 }
 
-int dsact_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
+int dsact_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
                       int64_t iteration, void* stream) {
+  int rc = check_mlp(hh, "dsact_replay_step");
+  if (rc) return rc;
+  MlpHandle* h = mlp(hh);
   if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
   if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
-  int rc = check_noise(noise);
+  rc = check_noise(noise);
   if (rc) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
   if ((rc = sync_rb_size(h, size, (cudaStream_t)stream))) return rc;
@@ -1697,15 +1787,19 @@ int dsact_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_
 // ---- data parallelism over peer memory (dp_peer.cuh) ------------------------------------------------------------
 int dsact_dp_export(dsact_handle* h, void* handle_out, int64_t* bytes_out) {
   if (!h || !handle_out) return fail(DSACT_EINVAL, "null argument");
-  return dp_peer_export(h->dp, h->device, 2 * h->q.n + h->pi.n + 1, handle_out, bytes_out);
+  int rc = check_v2(h);
+  if (rc) return rc;
+  return dp_peer_export(h->dp, h->device, h->n_params, handle_out, bytes_out);
 }
 
 int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* handles) {
   if (!h || !handles) return fail(DSACT_EINVAL, "null argument");
   if (!h->bound) return fail(DSACT_ESTATE, "dsact_bind has not been called");
+  int rc = check_v2(h);
+  if (rc) return rc;
   if (!h->dp.buf) return fail(DSACT_ESTATE, "dsact_dp_export has not been called");
-  const int rc = dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
-  if (rc == DSACT_OK) drop_graphs(h);   // captured data-parallel steps hold the previous peer map
+  rc = dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
+  if (rc == DSACT_OK && h->engine == ENGINE_MLP) drop_graphs(mlp(h));   // captured data-parallel steps hold the previous peer map
   return rc;
 }
 
@@ -1714,31 +1808,40 @@ int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* h
 int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t global_batch, int64_t iteration,
                   void* stream) {
   int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise))) return rc;
+  if (rc || (rc = check_noise(noise)) || (rc = check_v2(h))) return rc;
   if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (global_batch < batch->batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch->batch);
   CUDA_TRY(cudaSetDevice(h->device));
-  if ((rc = sync_iteration(h, iteration, (cudaStream_t)stream))) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = sync_iteration(h, iteration, s))) return rc;
   const dsact_batch bt = *batch;
   dsact_noise nz; const dsact_noise* np = nullptr;
   if (noise) { nz = *noise; np = &nz; }
-  const bool imaged = take_arena_images(h, bt);
-  GraphKey key = make_key(K_DP_STEP, &bt, np, global_batch);
-  key.size = imaged ? 1 : 0;
-  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) { enqueue_update(h, bt, np, global_batch, true, imaged, false, c); });
+  if (h->engine == ENGINE_HEADS) {
+    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_dp_step(heads(h), bt, np, global_batch, c); });
+  } else {
+    MlpHandle* m = mlp(h);
+    const bool imaged = take_arena_images(m, bt);
+    GraphKey key = make_key(K_DP_STEP, &bt, np, global_batch);
+    key.size = imaged ? 1 : 0;
+    rc = run(m, s, key, [&](Ctx& c) { enqueue_update(m, bt, np, global_batch, true, imaged, false, c); });
+  }
   if (rc) return rc;
   h->pending = bt; h->pending_batch = bt.batch;
   h->dev_iter = iteration + 1;
   return DSACT_OK;
 }
 
-int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
+int dsact_dp_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
                          int64_t global_batch, int64_t iteration, void* stream) {
+  int rc = check_mlp(hh, "dsact_dp_replay_step");
+  if (rc) return rc;
+  MlpHandle* h = mlp(hh);
   if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
   if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
   if (global_batch < batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch);
-  int rc = check_noise(noise);
+  rc = check_noise(noise);
   if (rc) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
   if ((rc = sync_rb_size(h, size, (cudaStream_t)stream))) return rc;
@@ -1761,11 +1864,12 @@ int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int
   return DSACT_OK;
 }
 
-int dsact_profile_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration,
+int dsact_profile_step(dsact_handle* hh, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration,
                        void* stream, dsact_profile* out) {
-  int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise))) return rc;
+  int rc = check_mlp(hh, "dsact_profile_step");
+  if (rc || (rc = check_batch(hh, batch)) || (rc = check_noise(noise))) return rc;
   if (!out) return fail(DSACT_EINVAL, "null out");
+  MlpHandle* h = mlp(hh);
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
   rc = sync_iteration(h, iteration, s);
@@ -1807,9 +1911,12 @@ int dsact_profile_step(dsact_handle* h, const dsact_batch* batch, const dsact_no
 int64_t dsact_launch_count(const dsact_handle* h) { return h ? h->launches : 0; }
 int32_t dsact_last_call_launches(const dsact_handle* h) { return h ? h->last_launches : 0; }
 
-int dsact_test_gemm(dsact_handle* h, int32_t variant, const float* A, int32_t lda, const float* B, int32_t ldb,
+int dsact_test_gemm(dsact_handle* hh, int32_t variant, const float* A, int32_t lda, const float* B, int32_t ldb,
                     const float* bias, float* C, int32_t ldc, int32_t M, int32_t N, int32_t K, void* stream) {
-  if (!h) return fail(DSACT_EINVAL, "null handle");
+  if (!hh) return fail(DSACT_EINVAL, "null handle");
+  int rc = check_mlp(hh, "dsact_test_gemm");
+  if (rc) return rc;
+  MlpHandle* h = mlp(hh);
   if (variant < 0 || variant > 2 || M < 1 || N < 1 || K < 1) return fail(DSACT_EINVAL, "bad argument");
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
@@ -1864,5 +1971,3 @@ int dsact_test_gemm(dsact_handle* h, int32_t variant, const float* A, int32_t ld
 }
 
 }  // extern "C"
-
-#include "cnn_engine.cuh"

@@ -70,17 +70,15 @@ __global__ void loss_v1_kernel(const __grid_constant__ LossV1Args a) {
 
 // One DSAC_V1 update (local_update, dsac_v1.py:95-98).  `noise`: eps1, eps2 as for DSAC-T; z3 = the draw of the target
 // critic's sample (the reference's second of three z draws; the other two do not enter the arithmetic); z4 unused.
-static int cnn_step_v1(dsact_cnn_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration, cudaStream_t s) {
+static void cnn_enqueue_v1(HeadsHandle* h, const dsact_batch* batch, const dsact_noise* noise, Ctx& c) {
   const dsact_cnn_config& cf = h->cfg;
   const CnnGeom &q = h->q, &pi = h->pi;
   const int B = batch->batch, A = cf.act_dim;
-  float* W = h->Wp();
+  float* W = h->W();
   float* P = h->buf.params; float* T = h->buf.targets; float* G = h->buf.grads;
   float* Pq = P; float* Ppi = P + q.n;
   float* Tq = T; float* Tpi = T + q.n;
   float* Gq = G; float* Gpi = G + q.n;
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = false;
   const long long n_all = q.n + pi.n + 1;
   {
     int blocks = (int)((n_all / 4 + 255) / 256); if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms; if (blocks < 1) blocks = 1;
@@ -189,8 +187,11 @@ static int cnn_step_v1(dsact_cnn_handle* h, const dsact_batch* batch, const dsac
     }
     launch_simt(h->num_sms, gd, V_DGRAD, c); c.done();
   }
-  CUDA_TRY(cudaMemcpy2DAsync(W + h->dAct[0], sizeof(float) * A, W + h->dfa[0] + q.F, sizeof(float) * (q.F + A), sizeof(float) * A, B,
-                             cudaMemcpyDeviceToDevice, s));
+  {
+    const cudaError_t e = cudaMemcpy2DAsync(W + h->dAct[0], sizeof(float) * A, W + h->dfa[0] + q.F, sizeof(float) * (q.F + A),
+                                            sizeof(float) * A, B, cudaMemcpyDeviceToDevice, c.s);
+    if (e != cudaSuccess && c.err == cudaSuccess) c.err = e;
+  }
   {
     PolicyGradArgs a;
     a.logits = W + h->logitsP; a.eps = eps1; a.d_act1 = W + h->dAct[0]; a.d_act2 = W + h->dAct[1];
@@ -231,8 +232,5 @@ static int cnn_step_v1(dsact_cnn_handle* h, const dsact_batch* batch, const dsac
     int blocks = (int)(((n_all + 3) / 4 + 255) / 256); if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
     launch_k(apply_kernel<0>, blocks, 256, 0, c, a); c.done();
   }
-  if (c.err != cudaSuccess) return fail(DSACT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(c.err));
-  h->launches += c.launches;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  c.check();
 }

@@ -1,6 +1,6 @@
 """`dsac_v1` of the drop-in: `ApproxContainer` and `DSAC_V1` with the reference's names, kwargs and `tb_info` keys
 (reference dsac_v1.py:17-52, 56-273) — the older algorithm (one distributional critic, fixed TD bound; selectable with
-`--algorithm DSAC_V1`), backed by the head-wise fp32 engine of libdsact.so (`dsact_cnn_*` with `algo = 1`).
+`--algorithm DSAC_V1`), backed by the head-wise fp32 engine of libdsact.so (`dsact_cnn_create` with `algo = 1`).
 
 * `ApproxContainer`: `q`, `q_target`, `policy`, `policy_target` (the same `networks.mlp` / `networks.cnn` classes as
   DSAC-T) + `log_alpha`; on a CUDA device the parameters are views into the engine's flat buffers [q | policy | log_alpha].

@@ -138,7 +138,7 @@ def full_state_dict(networks) -> dict:
         "mean_std": [float(st[0]), float(st[1])],
         "adam_steps": [int(ints[8]), int(ints[9])],
         "rng_counter": int(ints[10]) & 0xFFFFFFFF,
-        "rng_seed": int(getattr(eng, "_seed", 0)),
+        "rng_seed": int(eng._seed),
     }
 
 

@@ -4,7 +4,7 @@ keeps the shipped schema (`policy.conv.0.weight`, `policy.mean.0.weight`, `q1.lo
 
 As in `networks.mlp`, these modules are containers + the plain-torch forward used by the CPU sampler and the evaluator;
 during training their parameters are views into the CUDA engine's flat buffers and the update runs in libdsact.so
-(`dsact_cnn_step`).  The reference's other classes of this file (DetermPolicy, ActionValue, the discrete variants) are
+(`dsact_step` on a head-wise handle).  The reference's other classes of this file (DetermPolicy, ActionValue, the discrete variants) are
 not on the DSAC-T path and are not mirrored.
 """
 __all__ = ["StochaPolicy", "ActionValueDistri", "CONV_TYPES"]

@@ -82,6 +82,9 @@ def _f32c(t: torch.Tensor, device) -> torch.Tensor:
 class Engine:
     """One handle bound to flat torch-owned buffers on one CUDA device."""
 
+    # the entry points that turn a configuration into its layout and a handle; every other call is shared by both engines
+    _query, _create = "dsact_query_layout", "dsact_create"
+
     def __init__(self, cfg: Config, device: torch.device, act_high: torch.Tensor, act_low: torch.Tensor, *,
                  workspace_fill: float = 0.0):
         """`workspace_fill`: the value the scratch workspace holds when it is bound.  No step depends on it: every region a
@@ -95,8 +98,8 @@ class Engine:
             raise _lib.DsactError(f"engine device must be CUDA, got {self.device}")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
-        self.layout = query_layout(cfg)
-        L = self.layout
+        self.layout = L = Layout()
+        check(getattr(self.lib, self._query)(C.byref(cfg), C.byref(L)))
         with torch.cuda.device(self.device):
             z = lambda n: torch.zeros(int(n), dtype=torch.float32, device=self.device)
             self.params, self.targets = z(L.n_params), z(L.n_targets)
@@ -107,12 +110,13 @@ class Engine:
             self.act_high = _f32c(torch.as_tensor(act_high).reshape(-1), self.device).clone()
             self.act_low = _f32c(torch.as_tensor(act_low).reshape(-1), self.device).clone()
             h = C.c_void_p()
-            check(self.lib.dsact_create(C.byref(cfg), self.device.index, C.byref(h)))
+            check(getattr(self.lib, self._create)(C.byref(cfg), self.device.index, C.byref(h)))
             self.h = h
             self._stats_host = torch.zeros(_lib.NUM_STATS, dtype=torch.float32).pin_memory()
             self._bind()
             check(self.lib.dsact_set_carry(self.h, -1.0, -1.0, 0, 0, self._stream()))
         self.replay = None
+        self.last_batch = 0
         self.dp_world = 0          # > 1 once dp_connect has mapped the peers
         self._seed = 0x5DEECE66D   # the library's default (csrc/engine.cu)
         self._staged = False
@@ -196,23 +200,14 @@ class Engine:
     def arena_views(self, batch: Optional[int] = None) -> Dict[str, torch.Tensor]:
         """Views of the arena slots the device generator writes, for the first `batch` rows (default max_batch): `idx`
         (int64 [B], the replay indices the last index-drawing gather recorded) and the noise `eps1`, `eps2` [B, A],
-        `z3`, `z4` [B] (device noise, or host noise staged there); and `slabs`, the one region dsact_bind initialises.
-        Offsets follow Arena::build (csrc/engine.cu)."""
-        O, A, r64 = self.cfg.obs_dim, self.cfg.act_dim, lambda n: (n + 63) // 64 * 64
-        mb = self.cfg.max_batch
-        B = mb if batch is None else int(batch)
-        off = 2 * r64(mb * O) + r64(mb * A) + 3 * r64(mb)  # obs obs2 act rew done logp
-        out = {"idx": self._ws_view[off:off + 2 * B].view(torch.int64)}
-        off += r64(2 * mb)
-        for name, n, shape in (("eps1", A, (B, A)), ("eps2", A, (B, A)), ("z3", 1, (B,)), ("z4", 1, (B,))):
-            out[name] = self._ws_view[off:off + B * n].view(shape)
-            off += r64(mb * n)
-        # the tensor-core modes' weight-gradient split slabs, the arena's last region: dsact_bind zeroes them, because
-        # their bias entries are read by the fold and never written by a kernel
-        end = int(self.layout.workspace_bytes) // 4
-        n = r64(min(max(mb // 256, 1), 4) * ((int(self.layout.n_params) + 3) // 4 * 4)) if self.cfg.gemm_mode else 0
-        out["slabs"] = self._ws_view[end - n:end]
-        return out
+        `z3`, `z4` [B] (device noise, or host noise staged there); and `slabs`, the one region dsact_bind initialises
+        (empty in fp32 mode and on the head-wise engine).  Offsets are the ones the library reports (dsact_layout)."""
+        L, A, v = self.layout, self.cfg.act_dim, self._ws_view
+        B = int(L.max_batch) if batch is None else int(batch)
+        return {"idx": v[L.off_idx:L.off_idx + 2 * B].view(torch.int64),
+                "eps1": v[L.off_eps1:L.off_eps1 + B * A].view(B, A), "eps2": v[L.off_eps2:L.off_eps2 + B * A].view(B, A),
+                "z3": v[L.off_z3:L.off_z3 + B], "z4": v[L.off_z4:L.off_z4 + B],
+                "slabs": v[L.off_slabs:L.off_slabs + L.slab_floats]}
 
     def _noise_slots(self, B):
         v = self.arena_views(B)
@@ -304,6 +299,8 @@ class Engine:
         return {k: float(out[i]) for i, k in enumerate(STAT_KEYS)}
 
     def set_carry(self, mean_std1=-1.0, mean_std2=-1.0, adam_steps_q=0, adam_steps_pi=0):
+        """The state one update carries to the next besides weights and Adam moments: the mean_std EMA pair (-1 = not
+        started; unused by DSAC_V1) and the Adam step counters of the critic and policy optimizers."""
         with torch.cuda.device(self.device):
             check(self.lib.dsact_set_carry(self.h, float(mean_std1), float(mean_std2), int(adam_steps_q),
                                            int(adam_steps_pi), self._stream()))
@@ -313,8 +310,13 @@ class Engine:
         check(self.lib.dsact_seed(self.h, self._seed))
 
     # ---- replay ring buffer -------------------------------------------------------
+    @property
+    def obs_elems(self) -> int:
+        """Floats of one observation (a replay row of obs / obs2)."""
+        return self.cfg.obs_dim
+
     def bind_replay(self, capacity: int):
-        O, A = self.cfg.obs_dim, self.cfg.act_dim
+        O, A = self.obs_elems, self.cfg.act_dim
         with torch.cuda.device(self.device):
             z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)
             self.replay = dict(obs=z(capacity, O), obs2=z(capacity, O), act=z(capacity, A), rew=z(capacity),
@@ -335,7 +337,7 @@ class Engine:
 
     def arena_batch(self, b: Batch) -> Dict[str, torch.Tensor]:
         """Torch views of the engine's gathered-minibatch arena (no copies)."""
-        O, A, B = self.cfg.obs_dim, self.cfg.act_dim, b.batch
+        O, A, B = self.obs_elems, self.cfg.act_dim, b.batch
         base = self._ws_view.data_ptr()
 
         def view(ptr, n, shape):
@@ -424,6 +426,7 @@ class Engine:
     def load_weights(self, weights: dict):
         """Fill params/targets from a dict keyed like the reference's state_dict."""
         schema, n = self._schema()
+        assert n == self.layout.n_targets, (n, self.layout.n_targets)
         with torch.no_grad():
             for key, tkey, off, cnt, shape in schema:
                 self.params[off:off + cnt].copy_(torch.as_tensor(weights[key]).reshape(-1))

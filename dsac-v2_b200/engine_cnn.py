@@ -1,6 +1,7 @@
-"""Python owner of one libdsact CNN handle (`dsact_cnn_*`, include/dsact.h): the DSAC-T update with the reference's CNN
-approximators (BASELINE config 5; reference networks/cnn.py).  Same division of labour as `engine.Engine`: torch owns the
-flat device buffers, every arithmetic step runs in the CUDA library; there is no CPU fallback.
+"""Python owner of one handle of libdsact's head-wise fp32 engine (`dsact_cnn_create`, include/dsact.h): the update with
+the reference's CNN approximators (BASELINE config 5; reference networks/cnn.py), the policy std types the MLP engine
+does not implement, and DSAC_V1.  Everything but the configuration, the state_dict schema and the image-shaped
+minibatches is `engine.Engine`'s: the same buffers, and the same dsact_* calls on the handle.
 """
 from __future__ import annotations
 
@@ -10,8 +11,8 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import Batch, Buffers, CnnConfig, Layout, Noise, Replay, check
-from .engine import STAT_KEYS
+from ._lib import Batch, CnnConfig, check
+from .engine import Engine
 
 
 def make_cnn_config(obs_shape: Sequence[int], act_dim: int, kernels: Sequence[int], channels: Sequence[int],
@@ -53,56 +54,16 @@ def make_heads_config(obs_dim: int, act_dim: int, hidden: Sequence[int], std_typ
                            pi_std={"mlp_separated": "head", "parameter": "row", "mlp_shared": "shared"}[std_type], **kw)
 
 
-class CnnEngine:
-    """One `dsact_cnn_handle` bound to flat torch-owned buffers on one CUDA device."""
+class CnnEngine(Engine):
+    """A head-wise engine handle bound to flat torch-owned buffers on one CUDA device.  Minibatches are copied to the
+    device by torch (image observations [B, C, H, W], host or device tensors); the MLP engine's host-staging path, its
+    replay-fused steps, `profile_step` and `test_gemm` raise `DsactError`."""
 
-    def __init__(self, cfg: CnnConfig, device, act_high, act_low, *, workspace_fill: float = 0.0):
-        """`workspace_fill`: the value the scratch workspace holds when it is bound (see `engine.Engine`)."""
-        if not torch.cuda.is_available():
-            raise _lib.DsactError("the DSAC-T update engine needs a CUDA device (sm_90a); there is no CPU fallback")
-        self.lib, self.cfg = _lib.load(), cfg
-        self.device = torch.device(device)
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
-        lay = Layout()
-        check(self.lib.dsact_cnn_query_layout(C.byref(cfg), C.byref(lay)))
-        self.layout = lay
-        with torch.cuda.device(self.device):
-            z = lambda n: torch.zeros(int(n), dtype=torch.float32, device=self.device)
-            self.params, self.targets = z(lay.n_params), z(lay.n_targets)
-            self.grads, self.adam_m, self.adam_v = z(lay.n_params), z(lay.n_params), z(lay.n_params)
-            self.state = z(lay.state_floats)
-            self.workspace = torch.full((int(lay.workspace_bytes) // 4 + 64,), float(workspace_fill), dtype=torch.float32,
-                                        device=self.device)
-            off = (-self.workspace.data_ptr() % 256) // 4
-            self._ws_view = self.workspace[off:]
-            self.act_high = torch.as_tensor(act_high, dtype=torch.float32).reshape(-1).to(self.device).clone()
-            self.act_low = torch.as_tensor(act_low, dtype=torch.float32).reshape(-1).to(self.device).clone()
-            h = C.c_void_p()
-            check(self.lib.dsact_cnn_create(C.byref(cfg), self.device.index, C.byref(h)))
-            self.h = h
-            b = Buffers(self.params.data_ptr(), self.targets.data_ptr(), self.grads.data_ptr(), self.adam_m.data_ptr(),
-                        self.adam_v.data_ptr(), self.act_high.data_ptr(), self.act_low.data_ptr(), self.state.data_ptr(),
-                        self._ws_view.data_ptr())
-            check(self.lib.dsact_cnn_bind(self.h, C.byref(b)))
-            check(self.lib.dsact_cnn_set_carry(self.h, -1.0, -1.0, 0, 0, self._stream()))
-            self._stats_host = torch.zeros(_lib.NUM_STATS, dtype=torch.float32).pin_memory()
-        self.last_batch = 0
-        self.dp_world = 0          # > 1 once dp_connect has mapped the peers
+    _query, _create = "dsact_cnn_query_layout", "dsact_cnn_create"
 
-    def _stream(self) -> int:
-        return torch.cuda.current_stream(self.device).cuda_stream
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.lib.dsact_cnn_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:   # noqa: BLE001
-            pass
+    @property
+    def obs_elems(self) -> int:
+        return self.cfg.channels * self.cfg.height * self.cfg.width
 
     # ---- flat layout in the reference's state_dict schema (include/dsact.h) --------------------------------------------
     def _schema(self):
@@ -147,184 +108,27 @@ class CnnEngine:
                     mlp(net, head, [feat + extra] + hidden + [width])
         return out, off
 
-    def load_weights(self, weights: dict):
-        schema, n = self._schema()
-        assert n == self.layout.n_targets, (n, self.layout.n_targets)
-        with torch.no_grad():
-            for key, tkey, off, cnt, shape in schema:
-                self.params[off:off + cnt].copy_(torch.as_tensor(weights[key]).reshape(-1))
-                self.targets[off:off + cnt].copy_(torch.as_tensor(weights.get(tkey, weights[key])).reshape(-1))
-            self.params[n] = float(weights.get("log_alpha", 1.0))
-
-    def export_weights(self, grads: bool = False) -> dict:
-        schema, n = self._schema()
-        src = (self.grads if grads else self.params).detach().cpu()
-        tgt = self.targets.detach().cpu()
-        out = {"log_alpha": src[n].clone()}
-        for key, tkey, off, cnt, shape in schema:
-            out[key] = src[off:off + cnt].view(shape).clone()
-            if not grads:
-                out[tkey] = tgt[off:off + cnt].view(shape).clone()
-        return out
-
-    # ---- the path -------------------------------------------------------------------------------------------------------
-    def _args(self, data: Dict[str, torch.Tensor], noise):
-        """ctypes batch / noise of a minibatch (image observations [B, C, H, W]); the device copies stay referenced until
-        the next call, which is after the kernels reading them were enqueued."""
+    def _batch(self, data: Dict[str, torch.Tensor]) -> Batch:
+        """ctypes batch of a minibatch; the device copies stay referenced until the next call, which is after the kernels
+        reading them were enqueued."""
         t = {k: data[k].to(device=self.device, dtype=torch.float32).contiguous() for k in ("obs", "act", "rew", "obs2", "done")}
         B = t["obs"].shape[0]
-        c = self.cfg
-        if t["obs"][0].numel() != self.obs_elems or t["obs2"].shape != t["obs"].shape or t["act"].shape != (B, c.act_dim):
+        if t["obs"][0].numel() != self.obs_elems or t["obs2"].shape != t["obs"].shape or t["act"].shape != (B, self.cfg.act_dim):
             raise ValueError("minibatch shapes do not match the configured observation / action shape")
-        b = Batch(t["obs"].data_ptr(), t["act"].data_ptr(), t["rew"].data_ptr(), t["obs2"].data_ptr(), t["done"].data_ptr(), B, None)
-        n = None
-        if noise is not None:
-            nz = [torch.as_tensor(x).to(device=self.device, dtype=torch.float32).contiguous() for x in noise]
-            n = C.byref(Noise(*(x.data_ptr() for x in nz)))
-            self._keep_noise = nz
         self._keep = t
-        return b, n
+        return Batch(t["obs"].data_ptr(), t["act"].data_ptr(), t["rew"].data_ptr(), t["obs2"].data_ptr(), t["done"].data_ptr(), B, None)
 
     def step(self, data: Dict[str, torch.Tensor], iteration: int, noise=None):
-        """DSAC_V2.local_update (reference dsac_v2.py:102-105) with image observations [B, C, H, W] on the device."""
+        """DSAC_V2.local_update (reference dsac_v2.py:102-105), or DSAC_V1's, on a host or device minibatch."""
         with torch.cuda.device(self.device):
-            b, n = self._args(data, noise)
-            check(self.lib.dsact_cnn_step(self.h, C.byref(b), n, int(iteration), self._stream()))
+            b = self._batch(data)
+            n, self._keep_noise = self._noise(noise, b.batch)
+            check(self.lib.dsact_step(self.h, C.byref(b), n, int(iteration), self._stream()))
         self.last_batch = b.batch
-
-    # ---- split form (get_remote_update_info / remote_update) and data parallelism: the signatures of engine.Engine ------
-    def compute_grads(self, data, noise=None):
-        with torch.cuda.device(self.device):
-            b, n = self._args(data, noise)
-            check(self.lib.dsact_cnn_compute_grads(self.h, C.byref(b), n, self._stream()))
-        self.last_batch = b.batch
-
-    def grad_phase1(self, data, noise=None):
-        with torch.cuda.device(self.device):
-            b, n = self._args(data, noise)
-            check(self.lib.dsact_cnn_grad_phase1(self.h, C.byref(b), n, self._stream()))
-        self.last_batch = b.batch
-
-    def grad_phase2(self, global_batch: int):
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_grad_phase2(self.h, int(global_batch), self._stream()))
-
-    def apply(self, iteration: int):
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_apply(self.h, int(iteration), self._stream()))
-
-    def dp_export(self) -> bytes:
-        """Allocate this rank's exchange buffer; its CUDA IPC handle (to be handed to every other rank)."""
-        buf = C.create_string_buffer(_lib.IPC_HANDLE_BYTES)
-        n = C.c_int64(0)
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_dp_export(self.h, buf, C.byref(n)))
-        return buf.raw
-
-    def dp_connect(self, rank: int, handles: Sequence[bytes]):
-        """Map every rank's exchange buffer (`handles` in rank order, one per rank including this one)."""
-        blob = b"".join(handles)
-        if len(blob) != _lib.IPC_HANDLE_BYTES * len(handles):
-            raise ValueError("malformed IPC handle list")
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_dp_connect(self.h, int(rank), len(handles), blob))
-        self.dp_world = len(handles)
-
-    def dp_step(self, data, iteration: int, global_batch: int, noise=None):
-        """dsact_cnn_step on this rank's shard with the exchanges done in-kernel over peer memory."""
-        with torch.cuda.device(self.device):
-            b, n = self._args(data, noise)
-            check(self.lib.dsact_cnn_dp_step(self.h, C.byref(b), n, int(global_batch), int(iteration), self._stream()))
-        self.last_batch = b.batch
-
-    # ---- device replay ring (flattened image rows) ---------------------------------------------------------------------
-    @property
-    def obs_elems(self) -> int:
-        return self.cfg.channels * self.cfg.height * self.cfg.width
-
-    def bind_replay(self, capacity: int):
-        O, A = self.obs_elems, self.cfg.act_dim
-        with torch.cuda.device(self.device):
-            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)
-            self.replay = dict(obs=z(capacity, O), obs2=z(capacity, O), act=z(capacity, A), rew=z(capacity), done=z(capacity), logp=z(capacity))
-            r = self.replay
-            rb = Replay(r["obs"].data_ptr(), r["obs2"].data_ptr(), r["act"].data_ptr(), r["rew"].data_ptr(), r["done"].data_ptr(),
-                        r["logp"].data_ptr(), int(capacity))
-            check(self.lib.dsact_cnn_replay_bind(self.h, C.byref(rb)))
-        self.capacity = int(capacity)
-
-    def replay_add(self, staging: Dict[str, torch.Tensor], n: int, ptr: int):
-        s = staging
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_replay_add(self.h, s["obs"].data_ptr(), s["obs2"].data_ptr(), s["act"].data_ptr(), s["rew"].data_ptr(),
-                                                s["done"].data_ptr(), s["logp"].data_ptr(), int(n), int(ptr), self._stream()))
 
     def replay_sample(self, batch: int, size: int, idx: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
-        out = Batch()
-        with torch.cuda.device(self.device):
-            if idx is not None:
-                idx = idx.to(device=self.device, dtype=torch.int64).contiguous()
-                self._keep_idx = idx
-            check(self.lib.dsact_cnn_replay_sample(self.h, int(batch), int(size), None if idx is None else idx.data_ptr(), C.byref(out),
-                                                   self._stream()))
-        base, c, B, A = self._ws_view.data_ptr(), self.cfg, int(batch), self.cfg.act_dim
-
-        def view(ptr, n, shape):
-            off = (ptr - base) // 4
-            return self._ws_view[off:off + n].view(shape)
-
-        img = (B, c.channels, c.height, c.width) if c.n_conv else (B, self.obs_elems)
-        return {"obs": view(out.obs, B * self.obs_elems, img), "obs2": view(out.obs2, B * self.obs_elems, img),
-                "act": view(out.act, B * A, (B, A)), "rew": view(out.rew, B, (B,)), "done": view(out.done, B, (B,)),
-                "logp": view(out.logp, B, (B,))}
-
-    def arena_views(self, batch: Optional[int] = None) -> Dict[str, torch.Tensor]:
-        """Views of the arena slots the device generator writes, for the first `batch` rows (default max_batch): `idx`
-        (int64 [B]) and `eps1`, `eps2` [B, A], `z3`, `z4` [B].  Offsets follow dsact_cnn_handle::layout
-        (csrc/cnn_engine.cuh), counted back from the end of the workspace: the replay minibatch and its indices come last,
-        and between them and the noise lie the critic outputs, the action gradients, the feature gradients and the two
-        conv-backward buffers."""
-        c, r64 = self.cfg, lambda n: (n + 63) // 64 * 64
-        mb, A, O = c.max_batch, c.act_dim, self.obs_elems
-        B = mb if batch is None else int(batch)
-        cin, hh, ww, big = c.channels, c.height, c.width, 0
-        for j in range(c.n_conv):
-            k, st = c.conv_kernel[j], c.conv_stride[j]
-            cin, hh, ww = c.conv_channels[j], (hh - k) // st + 1, (ww - k) // st + 1
-            big = max(big, cin * hh * ww)
-        F = cin * hh * ww
-        end = int(self.layout.workspace_bytes) // 4
-        idx = end - r64(2 * mb)
-        r_obs = idx - 3 * r64(mb) - r64(mb * A) - 2 * r64(mb * O)
-        z4 = r_obs - 2 * r64(mb * big) - 2 * r64(mb * (F + A)) - 3 * r64(mb * F) - 2 * r64(mb * A) - 12 * r64(2 * mb) - r64(mb)
-        z3 = z4 - r64(mb)
-        eps2 = z3 - r64(mb * A)
-        eps1 = eps2 - r64(mb * A)
-        v = self._ws_view
-        return {"idx": v[idx:idx + 2 * B].view(torch.int64), "eps1": v[eps1:eps1 + B * A].view(B, A),
-                "eps2": v[eps2:eps2 + B * A].view(B, A), "z3": v[z3:z3 + B], "z4": v[z4:z4 + B]}
-
-    def set_carry(self, mean_std1=-1.0, mean_std2=-1.0, adam_steps_q=0, adam_steps_pi=0):
-        """The state one update carries to the next besides weights and Adam moments: the mean_std EMA pair (-1 = not
-        started; unused by DSAC_V1) and the Adam step counters of the critic and policy optimizers."""
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_set_carry(self.h, float(mean_std1), float(mean_std2), int(adam_steps_q),
-                                               int(adam_steps_pi), self._stream()))
-
-    def seed(self, seed: int):
-        self._seed = int(seed) & (2 ** 64 - 1)
-        check(self.lib.dsact_cnn_seed(self.h, self._seed))
-
-    def read_stats_async(self, global_batch: Optional[int] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        out = self._stats_host if out is None else out
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_read_stats(self.h, int(global_batch or self.last_batch), out.data_ptr(), self._stream()))
+        out = super().replay_sample(batch, size, idx)
+        if self.cfg.n_conv:   # image observations
+            shape = (int(batch), self.cfg.channels, self.cfg.height, self.cfg.width)
+            out["obs"], out["obs2"] = out["obs"].view(shape), out["obs2"].view(shape)
         return out
-
-    def read_stats(self, global_batch: Optional[int] = None) -> Dict[str, float]:
-        with torch.cuda.device(self.device):
-            check(self.lib.dsact_cnn_read_stats(self.h, int(global_batch or self.last_batch), self._stats_host.data_ptr(), self._stream()))
-            torch.cuda.current_stream(self.device).synchronize()
-        if float(self._stats_host[14]) != 0.0:   # include/dsact.h: slot 14 = 1 + rank of a peer that never arrived (dp_step)
-            raise _lib.DsactError(f"data-parallel exchange timed out waiting for rank {int(self._stats_host[14]) - 1}")
-        return dict(zip(STAT_KEYS, self._stats_host.tolist()))

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define DSACT_ABI_VERSION 1
+#define DSACT_ABI_VERSION 2
 #define DSACT_MAX_HIDDEN 6
 #define DSACT_NUM_STATS 16
 
@@ -93,6 +93,11 @@ typedef struct dsact_layout {
   int64_t workspace_bytes; /* activation / scratch arena the caller must provide */
   int64_t state_floats; /* persistent device state (EMA, counters, accumulators, stats) */
   int64_t max_batch;
+  /* workspace slots, in floats from the workspace base: the replay indices the last index-drawing gather recorded
+   * (int64 [max_batch]); the noise eps1 / eps2 [max_batch, act_dim], z3 / z4 [max_batch] (device noise, or host noise a
+   * caller stages there); the weight-gradient split slabs of the tensor-core modes, the last region, `slab_floats` long
+   * (0 in fp32 mode and on the head-wise engine) and zeroed by dsact_bind */
+  int64_t off_idx, off_eps1, off_eps2, off_z3, off_z4, off_slabs, slab_floats;
 } dsact_layout;
 
 /* Device pointers of caller-owned tensors. */
@@ -214,17 +219,24 @@ int dsact_dp_step(dsact_handle *h, const dsact_batch *batch, const dsact_noise *
 int dsact_dp_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx, const dsact_noise *noise,
                          int64_t global_batch, int64_t iteration, void *stream);
 
-/* ---- CNN approximators (BASELINE config 5, reference networks/cnn.py:30-53,151-240,383-461) --------------------------------
- * The same update path when value_func_type / policy_func_type = "CNN": every network is a private conv encoder
- * (Conv2d + ReLU per layer, no padding) followed by two separate MLP heads `mean` and `log_std` on the flattened
- * feature (the critics append the action to it).  Flat layout per network, in state_dict order: conv.{0,2,..}.weight
- * [Cout,Cin,k,k] / .bias, mean.{0,2,..}.weight / .bias, log_std.{0,2,..}.weight / .bias; params = [q1|q2|policy|log_alpha].
- * fp32 direct convolutions + the fp32 grouped GEMMs for the heads, eager launches.
- * dsact_cnn_step = DSAC_V2.local_update(data, iteration) with data["obs"] / ["obs2"] of shape [B, C, H, W] (contiguous).
- * The same head-wise engine also carries the variants of the reference that keep network outputs in separate heads or
- * need another loss, all in fp32: no encoder (n_conv = 0: the observation vector feeds the heads), one two-output head per
- * critic (q_heads = 1, networks/mlp.py), the policy's std types (pi_std), the plain Gaussian action distribution
- * (act_dist) and DSAC_V1 (algo = 1: ONE critic, flat layout [q | policy | log_alpha], dsac_v1.py). */
+/* ---- head-wise fp32 engine: CNN approximators and the variants the MLP engine does not implement ---------------------
+ * CNN approximators (BASELINE config 5, reference networks/cnn.py:30-53,151-240,383-461), value_func_type /
+ * policy_func_type = "CNN": every network is a private conv encoder (Conv2d + ReLU per layer, no padding) followed by two
+ * separate MLP heads `mean` and `log_std` on the flattened feature (the critics append the action to it).  Flat layout per
+ * network, in state_dict order: conv.{0,2,..}.weight [Cout,Cin,k,k] / .bias, mean.{0,2,..}.weight / .bias,
+ * log_std.{0,2,..}.weight / .bias; params = [q1|q2|policy|log_alpha].  fp32 direct convolutions + the fp32 grouped GEMMs
+ * for the heads, eager launches.  data["obs"] / ["obs2"] are [B, C, H, W] (contiguous); replay rows are the flattened
+ * [C*H*W] images (fp32, like the reference's CarRacing data, env_gym/gym_carracing_data.py:19-21).
+ * The same engine also carries the variants of the reference that keep network outputs in separate heads or need another
+ * loss, all in fp32: no encoder (n_conv = 0: the observation vector feeds the heads), one two-output head per critic
+ * (q_heads = 1, networks/mlp.py), the policy's std types (pi_std), the plain Gaussian action distribution (act_dist) and
+ * DSAC_V1 (algo = 1: ONE critic, flat layout [q | policy | log_alpha], dsac_v1.py).
+ * dsact_cnn_create returns a dsact_handle that every dsact_* entry point above takes, with the same semantics, except:
+ *  - dsact_step_host, dsact_stage_host / _release, dsact_replay_step, dsact_dp_replay_step, dsact_profile_step and
+ *    dsact_test_gemm return DSACT_EINVAL (the MLP engine implements them);
+ *  - a DSAC_V1 handle (algo = 1) returns DSACT_EINVAL from the split and data-parallel calls (dsact_grad_phase1/2,
+ *    dsact_compute_grads, dsact_apply, dsact_dp_export / _connect / _step);
+ *  - phase 2's log_alpha gradient is this shard's additive share, and dsact_dp_step runs eagerly on `stream`. */
 #define DSACT_MAX_CONV 8
 typedef struct dsact_cnn_config {
   int32_t abi_version;
@@ -249,37 +261,8 @@ typedef struct dsact_cnn_config {
   double adam_beta1, adam_beta2, adam_eps;
   double td_bound;                   /* DSAC_V1 `TD_bound` (dsac_v1.py:79, default 20) */
 } dsact_cnn_config;
-typedef struct dsact_cnn_handle dsact_cnn_handle;
 int dsact_cnn_query_layout(const dsact_cnn_config *cfg, dsact_layout *out);
-int dsact_cnn_create(const dsact_cnn_config *cfg, int device, dsact_cnn_handle **out);
-void dsact_cnn_destroy(dsact_cnn_handle *h);
-int dsact_cnn_bind(dsact_cnn_handle *h, const dsact_buffers *bufs);
-int dsact_cnn_set_carry(dsact_cnn_handle *h, float mean_std1, float mean_std2, int64_t adam_steps_q, int64_t adam_steps_pi,
-                        void *stream);
-int dsact_cnn_seed(dsact_cnn_handle *h, uint64_t seed);
-int dsact_cnn_step(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, int64_t iteration, void *stream);
-int dsact_cnn_read_stats(dsact_cnn_handle *h, int64_t global_batch, float *host_out, void *stream);
-/* device replay ring for image transitions: rows of obs / obs2 are the flattened [C*H*W] images (fp32, like the
- * reference's CarRacing data, env_gym/gym_carracing_data.py:19-21); same semantics as dsact_replay_bind / _add / _sample */
-int dsact_cnn_replay_bind(dsact_cnn_handle *h, const dsact_replay *rb);
-int dsact_cnn_replay_add(dsact_cnn_handle *h, const float *obs, const float *obs2, const float *act, const float *rew,
-                         const float *done, const float *logp, int64_t n, int64_t ptr, void *stream);
-int dsact_cnn_replay_sample(dsact_cnn_handle *h, int32_t batch, int64_t size, const int64_t *idx, dsact_batch *out, void *stream);
-/* Split form and data-parallel replicas of the head-wise DSAC-T step, with the semantics of their MLP-engine namesakes:
- * dsact_cnn_grad_phase1 (forwards; local critic-std sums in state[DSACT_STATE_STDSUM..+1]), dsact_cnn_grad_phase2 (losses
- * and backward passes with means over `global_batch` >= the phase-1 batch; the log_alpha gradient is this shard's additive
- * share), dsact_cnn_compute_grads (= phase 1 + phase 2 on its own rows), dsact_cnn_apply (Adam / Polyak on whatever
- * `grads` holds; also on a handle that never ran phase 2).  dsact_cnn_dp_export / _connect / _step: the peer-memory
- * exchange of dsact_dp_* (same buffer layout, kernels, rank-ordered sums, timeout and tb_info slot 14), eager on
- * `stream`.  dsact_cnn_step = phase 1 + phase 2 + apply.  DSAC_V1 handles (algo = 1) return DSACT_EINVAL from all seven. */
-int dsact_cnn_grad_phase1(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, void *stream);
-int dsact_cnn_grad_phase2(dsact_cnn_handle *h, int64_t global_batch, void *stream);
-int dsact_cnn_compute_grads(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, void *stream);
-int dsact_cnn_apply(dsact_cnn_handle *h, int64_t iteration, void *stream);
-int dsact_cnn_dp_export(dsact_cnn_handle *h, void *handle_out, int64_t *bytes_out);
-int dsact_cnn_dp_connect(dsact_cnn_handle *h, int32_t rank, int32_t world, const void *handles);
-int dsact_cnn_dp_step(dsact_cnn_handle *h, const dsact_batch *batch, const dsact_noise *noise, int64_t global_batch,
-                      int64_t iteration, void *stream);
+int dsact_cnn_create(const dsact_cnn_config *cfg, int device, dsact_handle **out);
 
 /* introspection for tests/bench: number of kernel launches (graph nodes included)
  * submitted by this handle so far, and by the most recent entry-point call */

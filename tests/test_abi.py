@@ -28,6 +28,7 @@ def test_struct_sizes_match_header_layout():
     assert C.sizeof(_lib.Config) == 104 + 12 * 8
     assert C.sizeof(_lib.Batch) == 5 * 8 + 8 + 8
     assert C.sizeof(_lib.Buffers) == 9 * 8
+    assert C.sizeof(_lib.Layout) == 14 * 8
 
 
 @pytest.mark.parametrize("name", list(synth.CONFIGS))
@@ -73,17 +74,39 @@ def test_no_cpu_fallback():
         alg.local_update({"obs": torch.zeros(4, 5)}, 0)
 
 
-@pytest.mark.parametrize("variant", ["cnn_type2", "cnn_type1", "mlp_separated", "parameter", "v1_mlp"])
-def test_head_wise_layouts_match_the_dropin_modules(variant):
-    """The flat layout the head-wise engine reports (`dsact_cnn_query_layout`, no GPU needed) and the state_dict schema
-    `CnnEngine._schema` walks are those of the drop-in modules' own parameter order, for every variant it serves."""
+def _check_slots(lay, act_dim, slabs):
+    """The workspace slots the library reports: 64-float aligned, inside the workspace for max_batch rows, disjoint; the
+    weight-gradient slabs are the last region and are empty exactly when `slabs` is false."""
+    mb, end = int(lay.max_batch), int(lay.workspace_bytes) // 4
+    regions = [(lay.off_idx, 2 * mb), (lay.off_eps1, mb * act_dim), (lay.off_eps2, mb * act_dim), (lay.off_z3, mb),
+               (lay.off_z4, mb), (lay.off_slabs, lay.slab_floats)]
+    for off, n in regions:
+        assert off % 64 == 0 and 0 <= off and off + n <= end, (off, n, end)
+    spans = sorted(regions)
+    assert all(a + n <= b for (a, n), (b, _) in zip(spans, spans[1:])), spans
+    assert lay.off_slabs + lay.slab_floats == end and all(off + n <= lay.off_slabs for off, n in regions[:-1])
+    assert (lay.slab_floats > 0) == slabs
+
+
+@pytest.mark.parametrize("mode", list(_lib.GEMM_MODES))
+@pytest.mark.parametrize("name", list(synth.CONFIGS))
+def test_reported_workspace_slots(name, mode):
+    cfg = synth.CONFIGS[name]
+    for mb in (1, 256, 1000):
+        lay = query_layout(make_config(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"], cfg["hidden"], max_batch=mb, gemm_mode=mode))
+        _check_slots(lay, cfg["act_dim"], mode != "fp32")
+
+
+HEAD_WISE = ["cnn_type2", "cnn_type1", "mlp_separated", "parameter", "v1_mlp"]
+
+
+def _head_wise(variant):
+    """(drop-in ApproxContainer, dsact_cnn_config) of one head-wise variant at max_batch 4."""
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     sys.path[:0] = [os.path.join(root, "dsac-v2_b200", "dropin")]
     import dsac_v1
     import dsac_v2
-    from dsac_v2_b200.engine_cnn import CnnEngine
-    from dsac_v2_b200._lib import Layout
     if variant.startswith("cnn"):
         cfg = synth.CNN_CONFIGS["small_t1" if variant != "cnn_type2" else "carracing"]
         kw = synth.cnn_reference_kwargs(cfg, replay_batch_size=4)
@@ -96,7 +119,25 @@ def test_head_wise_layouts_match_the_dropin_modules(variant):
     if make is None:
         from dsac_v2_b200.engine_cnn import make_cnn_config, make_heads_config
         make = make_heads_config if net._heads_std else make_cnn_config
-    c = make(max_batch=4, **net._cfg_args)
+    return net, make(max_batch=4, **net._cfg_args)
+
+
+@pytest.mark.parametrize("variant", HEAD_WISE)
+def test_head_wise_workspace_slots(variant):
+    from dsac_v2_b200._lib import Layout
+    _, c = _head_wise(variant)
+    lay = Layout()
+    assert _lib.load().dsact_cnn_query_layout(C.byref(c), C.byref(lay)) == 0
+    _check_slots(lay, c.act_dim, False)
+
+
+@pytest.mark.parametrize("variant", HEAD_WISE)
+def test_head_wise_layouts_match_the_dropin_modules(variant):
+    """The flat layout the head-wise engine reports (`dsact_cnn_query_layout`, no GPU needed) and the state_dict schema
+    `CnnEngine._schema` walks are those of the drop-in modules' own parameter order, for every variant it serves."""
+    from dsac_v2_b200.engine_cnn import CnnEngine
+    from dsac_v2_b200._lib import Layout
+    net, c = _head_wise(variant)
     lay = Layout()
     assert _lib.load().dsact_cnn_query_layout(C.byref(c), C.byref(lay)) == 0
     train, targ = net._flat_groups()

@@ -1,4 +1,4 @@
-"""BASELINE config 5 (CNN encoder + DSAC-T heads, reference networks/cnn.py) through the C ABI (`dsact_cnn_*`):
+"""BASELINE config 5 (CNN encoder + DSAC-T heads, reference networks/cnn.py) through the C ABI (a `dsact_cnn_create` handle):
 the CUDA path against the golden produced by the unmodified reference (tests/golden/cnn_carracing_b4.npz) and against
 the pinned oracle on a second batch size, gradients included.  fp32 direct convolutions + fp32 GEMMs: tolerance 1e-4
 relative (north_star's gate); observed ~1e-6."""

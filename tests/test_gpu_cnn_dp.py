@@ -1,6 +1,6 @@
 """Data-parallel updates of the head-wise engine on 2 / 4 / 8 GPUs (ragged shards) == one GPU on the concatenated
 minibatch, for the CNN approximators (config `odd`) and the policy std types "mlp_separated" / "parameter", over both
-transports: "peer" (`dsact_cnn_dp_step`, exchanges inside the step's kernels over NVLink peer memory) and "nccl"
+transports: "peer" (`dsact_dp_step` on head-wise handles, exchanges inside the step's kernels over NVLink peer memory) and "nccl"
 (`dp.data_parallel_gradients`: torch.distributed all-reduces between the split-API calls).  Each spawn also runs
 `DSAC_V2(**cnn_reference_kwargs).local_update` under torch.distributed.  World sizes above the device count are skipped."""
 import os

@@ -1,7 +1,9 @@
-"""The split gradient API of the head-wise engine (`dsact_cnn_grad_phase1` / `_grad_phase2` / `_compute_grads` /
-`_apply`) on one GPU, for the CNN approximators and the policy std types "mlp_separated" / "parameter": gradients and
+"""The split gradient API on a head-wise handle (`dsact_grad_phase1` / `_grad_phase2` / `dsact_compute_grads` /
+`dsact_apply`) on one GPU, for the CNN approximators and the policy std types "mlp_separated" / "parameter": gradients and
 post-update state against the pinned oracle, and the drop-in's gradient-message seam (`DSAC_V2.get_remote_update_info` /
 `remote_update`, reference dsac_v2.py:107-138) against `local_update`."""
+import ctypes as C
+
 import numpy as np
 import pytest
 import torch
@@ -86,6 +88,17 @@ def test_split_api_argument_checks():
         eng.grad_phase2(7)
     with pytest.raises(_lib.DsactError, match="dp_connect"):
         eng.dp_step(b, 0, 8, n)
+    # the calls only the MLP engine implements refuse a head-wise handle with a message
+    lib, stream, hb = eng.lib, eng._stream(), eng._batch(b)
+    for rc in (lib.dsact_step_host(eng.h, C.byref(hb), None, 0, stream), lib.dsact_replay_step(eng.h, 8, 8, None, None, 0, stream),
+               lib.dsact_profile_step(eng.h, C.byref(hb), None, 0, stream, C.byref(_lib.Profile()))):
+        assert rc == -1 and b"head-wise" in lib.dsact_last_error()
+    with pytest.raises(_lib.DsactError, match="head-wise"):
+        eng.profile_step(b, 0, n)
+    assert eng._seed == 0x5DEECE66D   # unseeded: the library's default generator seed
+    before = eng.launch_count()
+    eng.step(b, 0, n)
+    assert eng.launch_count() > before and eng.last_call_launches() > 0
     eng.close()
     tiny = synth.CONFIGS["tiny"]
     lim = torch.full((tiny["act_dim"],), tiny["act_lim"])

@@ -1,5 +1,5 @@
 """The policy's other std types (reference networks/mlp.py:43-72: "mlp_separated" = two MLPs, "parameter" = mean MLP +
-learnable log_std row) through the C ABI: the head-wise fp32 engine (`dsact_cnn_*` with no encoder, one two-output head
+learnable log_std row) through the C ABI: the head-wise fp32 engine (`dsact_cnn_create` with no encoder, one two-output head
 per critic) against the goldens produced by the unmodified reference (tests/golden/tiny_std_*.npz), against the pinned
 oracle on a ragged batch with gradients, and through the drop-in `DSAC_V2` (state_dict schema, `local_update`)."""
 import ast

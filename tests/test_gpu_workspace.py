@@ -173,3 +173,13 @@ def test_headwise_poisoned_workspace_changes_nothing(kind, B):
             same(getattr(p, k), getattr(a, k), B, f"{k}, poison {poison}")
     for _, e, _ in results:
         e.close()
+
+
+def test_headwise_bind_rejects_an_unaligned_workspace():
+    import ctypes as C
+    from dsac_v2_b200 import _lib
+    _, e, _ = cnn_case("separated", 8, 0.0)
+    ptrs = [t.data_ptr() for t in (e.params, e.targets, e.grads, e.adam_m, e.adam_v, e.act_high, e.act_low, e.state)]
+    assert e.lib.dsact_bind(e.h, C.byref(_lib.Buffers(*ptrs, e._ws_view.data_ptr() + 4))) == -1
+    assert b"256-byte aligned" in e.lib.dsact_last_error()
+    e.close()
