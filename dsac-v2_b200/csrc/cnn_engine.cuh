@@ -1,17 +1,18 @@
 // DSAC-T update with the reference's CNN approximators (BASELINE config 5; reference networks/cnn.py:30-53 conv stack,
 // :151-240 StochaPolicy, :383-461 ActionValueDistri).  Included by engine.cu before its C ABI: it reuses the grouped fp32 GEMM
-// launcher, the loss / sample / policy-gradient kernels and apply_kernel of the MLP engine; what is new here is the conv
-// stack (conv.cuh) and the two-head wiring (separate `mean` and `log_std` MLPs per network, their outputs packed into the
-// [B,2] / [B,2A] arrays the loss kernels read, by strided GEMM outputs).
+// launcher and the step launches both engines share (noise, sample, loss, policy gradient, apply, gather); what is new here
+// is the conv stack (conv.cuh) and the two-head wiring (separate `mean` and `log_std` MLPs per network, their outputs
+// packed into the [B,2] / [B,2A] arrays the loss kernels read, by strided GEMM outputs).
 //
 // The same wiring without an encoder (n_conv = 0), with one two-output head per critic (q_heads = 1), with the policy as one
 // head / two heads / mean head + learnable log_std row (pi_std) serves the MLP approximators whose variants the wgmma
-// engine does not implement (policy std_type mlp_separated / parameter), and DSAC_V1 (v1_step.cuh).
+// engine does not implement (policy std_type mlp_separated / parameter).  DSAC_V1 (algo = 1) runs the same phases with
+// one critic instead of two (flat layout [q | policy | log_alpha]) and its own critic loss, loss_v1_kernel.
 //
-// One eager sequence of launches per step (no graph capture yet):
-//   conv forwards: pi(s), pi'(s'), Q1/Q2 features of s (shared by the (s,a) and (s,a~) passes), Q1'/Q2' features of s'
+// One eager sequence of launches per step (no graph capture yet), for critics k = 0 .. nq-1:
+//   conv forwards: pi(s), pi'(s'), Q_k features of s (shared by the (s,a) and (s,a~) passes), Q'_k features of s'
 //   heads: pi, pi' -> sample -> Q_k(s,a), Q'_k(s',a'), mean head of Q_k(s,a~) -> loss -> head backward (critics: both
-//   heads; actor path: mean head, input gradient only) -> policy_grad -> policy heads backward -> conv backward x3 -> Adam.
+//   heads; actor path: mean head, input gradient only) -> policy_grad -> policy heads backward -> conv backward -> Adam.
 #pragma once
 #include "conv.cuh"
 
@@ -78,17 +79,17 @@ struct CnnHeadBuf { int64_t z[DSACT_MAX_HIDDEN], h[DSACT_MAX_HIDDEN], dz[DSACT_M
 struct HeadsHandle : dsact_handle {
   dsact_cnn_config cfg;
   CnnGeom q, pi;
-  // arena (floats from the workspace base)
+  // arena (floats from the workspace base), besides the shell's slots
   int64_t convP[DSACT_MAX_CONV + 1], convT[DSACT_MAX_CONV + 1], convQ[4][DSACT_MAX_CONV + 1];   // activations 1..nconv
   CnnHeadBuf hb[14];   // 0,1 pi mean/ls; 2,3 pi'; 4..7 Q1,Q2 (s,a) mean/ls; 8..11 Q1',Q2'; 12,13 mean head of Q1,Q2 on (s,a~)
-  int64_t logitsP, logitsT, dlogits, new_act, act2, logp_new, logp2, eps1, eps2, z3, z4, outQ[6], dOut[6], dAct[2];
   int64_t dfeat[3], dfa[2];   // dL/dfeature of pi, Q1, Q2; dL/d(feature|act) scratch of the actor path
   int64_t ga, gb;             // conv-backward ping-pong buffers (largest activation)
-  int64_t r_obs, r_obs2, r_act, r_rew, r_done, r_logp, r_idx;   // gathered replay minibatch
   int64_t total;
   HeadsHandle() : dsact_handle(ENGINE_HEADS) {}
+  int nq() const { return v1 ? 1 : 2; }   // critics: DSAC_V1 has one
   void layout() {
     const int64_t B = cfg.max_batch, A = cfg.act_dim;
+    StepSlots& s = slot;
     int64_t off = 0;
     auto take = [&](int64_t n) { int64_t o = off; off += round64(n); return o; };
     auto conv_acts = [&](const CnnGeom& g, int64_t* a) { a[0] = -1; for (int j = 1; j <= g.nconv; ++j) a[j] = take(B * g.act_elems(j)); };
@@ -98,11 +99,11 @@ struct HeadsHandle : dsact_handle {
       const Net& net = p < 4 ? pi.head : q.head;
       for (int j = 0; j < net.L; ++j) { hb[p].z[j] = take(B * net.s[j + 1]); hb[p].h[j] = take(B * net.s[j + 1]); hb[p].dz[j] = take(B * net.s[j + 1]); }
     }
-    logitsP = take(B * 2 * A); logitsT = take(B * 2 * A); dlogits = take(B * 2 * A);
-    new_act = take(B * A); act2 = take(B * A); logp_new = take(B); logp2 = take(B);
-    eps1 = take(B * A); eps2 = take(B * A); z3 = take(B); z4 = take(B);
-    for (int p = 0; p < 6; ++p) { outQ[p] = take(B * 2); dOut[p] = take(B * 2); }
-    dAct[0] = take(B * A); dAct[1] = take(B * A);
+    s.logitsP = take(B * 2 * A); s.logitsT = take(B * 2 * A); s.dlogits = take(B * 2 * A);
+    s.new_act = take(B * A); s.act2 = take(B * A); s.logp_new = take(B); s.logp2 = take(B);
+    s.eps1 = take(B * A); s.eps2 = take(B * A); s.z3 = take(B); s.z4 = take(B);
+    for (int p = 0; p < 6; ++p) { s.outQ[p] = take(B * 2); s.dOut[p] = take(B * 2); }
+    s.dAct[0] = take(B * A); s.dAct[1] = take(B * A);
     dfeat[0] = take(B * pi.F); dfeat[1] = take(B * q.F); dfeat[2] = take(B * q.F);
     dfa[0] = take(B * (q.F + A)); dfa[1] = take(B * (q.F + A));
     int64_t big = 0;
@@ -110,7 +111,7 @@ struct HeadsHandle : dsact_handle {
     for (int j = 1; j <= pi.nconv; ++j) big = big > pi.act_elems(j) ? big : pi.act_elems(j);
     ga = take(B * big); gb = take(B * big);
     const int64_t O = (int64_t)cfg.channels * cfg.height * cfg.width;
-    r_obs = take(B * O); r_obs2 = take(B * O); r_act = take(B * A); r_rew = take(B); r_done = take(B); r_logp = take(B); r_idx = take(2 * B);
+    s.obs = take(B * O); s.obs2 = take(B * O); s.act = take(B * A); s.rew = take(B); s.done = take(B); s.logp = take(B); s.idx = take(2 * B);
     total = off;
   }
 };
@@ -121,6 +122,7 @@ struct HeadsHandle : dsact_handle {
 static void cnn_setup(HeadsHandle* h, const dsact_cnn_config& c) {
   const bool q1 = c.q_heads == 1, row = c.pi_std == 1, shared = c.pi_std == 2;
   h->cfg = c;
+  h->hyper = StepHyper::of(c);
   h->q.build(c, c.act_dim, q1 ? 2 : 1, q1 ? 1 : 2, false);
   h->pi.build(c, 0, shared ? 2 * c.act_dim : c.act_dim, (row || shared) ? 1 : 2, row);
   h->layout();
@@ -128,7 +130,7 @@ static void cnn_setup(HeadsHandle* h, const dsact_cnn_config& c) {
   h->act_dim = c.act_dim;
   h->max_batch = c.max_batch;
   h->v1 = c.algo == 1;
-  h->n_params = (h->v1 ? 1 : 2) * h->q.n + h->pi.n + 1;   // DSAC_V1 has one critic
+  h->n_params = h->nq() * h->q.n + h->pi.n + 1;
 }
 
 static int cnn_validate(const dsact_cnn_config* c) {
@@ -417,9 +419,10 @@ static void cnn_conv_backward(HeadsHandle* h, const CnnGeom& g, const float* par
   c.check();
 }
 
-// ---- the DSAC-T step in three phases --------------------------------------------------------------------------------
+// ---- the step in three phases ---------------------------------------------------------------------------------------
 // dsact_step runs them back to back on its own rows; the data-parallel step (dsact_dp_step) runs the critic-std
-// exchange between phases 1 and 2 and the gradient exchange between phase 2 and the update.
+// exchange between phases 1 and 2 and the gradient exchange between phase 2 and the update.  DSAC_V1 runs them with one
+// critic: every "for k < nq" loop below then stops after k = 0.
 struct CnnFeats { const float *P, *T, *Q[4]; };   // head inputs: pi(s), pi'(s'), Q1/Q2 features of s, Q1'/Q2' features of s'
 static CnnFeats cnn_feats(const HeadsHandle* h, const dsact_batch& bt) {
   // without a conv stack (the MLP approximators with separate heads) the feature is the observation itself
@@ -440,33 +443,23 @@ static CnnFeats cnn_feats(const HeadsHandle* h, const dsact_batch& bt) {
 // (s, a), sample_kernel (whose y = 1 half leaves the local critic-std sums in state[ST_STDSUM..+1]), the targets and the
 // mean heads of the critics on (s, a~)
 static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
-  const dsact_cnn_config& cf = h->cfg;
   const CnnGeom &q = h->q, &pi = h->pi;
-  const int B = bt.batch, A = cf.act_dim;
+  const StepSlots& s = h->slot;
+  const int B = bt.batch, A = h->act_dim, nq = h->nq();
   float* W = h->W();
-  float* P = h->buf.params; float* T = h->buf.targets; float* G = h->buf.grads;
-  float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
-  float* Tq[2] = {T, T + q.n}; float* Tpi = T + 2 * q.n;
-  const long long n_all = 2 * q.n + pi.n + 1;
-  {
-    int blocks = (int)((n_all / 4 + 255) / 256); if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(begin_step_kernel, blocks, 256, 0, c, h->buf.state, G, n_all); c.done();
-  }
-  const float *eps1, *eps2, *z3, *z4;
-  if (noise) { eps1 = noise->eps1; eps2 = noise->eps2; z3 = noise->z3; z4 = noise->z4; }
-  else {
-    const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
-    int blocks = (total / 2 + 255) / 256; if (blocks < 1) blocks = 1;
-    launch_k(noise_kernel, blocks, 256, 0, c, W + h->eps1, W + h->eps2, W + h->z3, W + h->z4, B, A, h->seed, (const float*)h->buf.state); c.done();
-    eps1 = W + h->eps1; eps2 = W + h->eps2; z3 = W + h->z3; z4 = W + h->z4;
-  }
+  float* P = h->buf.params; float* T = h->buf.targets;
+  float* Pq[2] = {P, P + q.n}; float* Ppi = P + nq * q.n;
+  float* Tq[2] = {T, T + q.n}; float* Tpi = T + nq * q.n;
+  enqueue_begin_step(h, c);
+  if (!noise) enqueue_noise(h, B, c);
+  const dsact_noise nz = step_noise(h, noise);
   h->pending = bt; h->pending_batch = B;
-  h->pending_eps1 = eps1; h->pending_z3 = z3; h->pending_z4 = z4;
+  h->pending_eps1 = nz.eps1; h->pending_z3 = nz.z3; h->pending_z4 = nz.z4;
 
   // ---- encoders: pi(s), pi'(s'), Q_k features of s, Q'_k features of s'
   cnn_conv_forward(h, pi, Ppi, bt.obs, h->convP, B, c);
   cnn_conv_forward(h, pi, Tpi, bt.obs2, h->convT, B, c);
-  for (int k = 0; k < 2; ++k) {
+  for (int k = 0; k < nq; ++k) {
     cnn_conv_forward(h, q, Pq[k], bt.obs, h->convQ[k], B, c);
     cnn_conv_forward(h, q, Tq[k], bt.obs2, h->convQ[2 + k], B, c);
   }
@@ -476,46 +469,33 @@ static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsac
   {
     std::vector<CnnHeadFwd> v;
     for (int hd = 0; hd < pi.nheads; ++hd) {
-      v.push_back({Ppi + pi.head_off[hd], f.P, pi.F, nullptr, 0, &h->hb[hd], true, W + h->logitsP + hd * A, 2 * A});
-      v.push_back({Tpi + pi.head_off[hd], f.T, pi.F, nullptr, 0, &h->hb[2 + hd], false, W + h->logitsT + hd * A, 2 * A});
+      v.push_back({Ppi + pi.head_off[hd], f.P, pi.F, nullptr, 0, &h->hb[hd], true, W + s.logitsP + hd * A, 2 * A});
+      v.push_back({Tpi + pi.head_off[hd], f.T, pi.F, nullptr, 0, &h->hb[2 + hd], false, W + s.logitsT + hd * A, 2 * A});
     }
     cnn_heads_forward(h, pi.head, v, B, c);
     if (pi.ls_row >= 0) {   // std_type "parameter": log_std columns = the learnable row
       int blocks = (B * A + 255) / 256; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + h->logitsP, 2 * A, A, (const float*)(Ppi + pi.ls_row), B, A); c.done();
-      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + h->logitsT, 2 * A, A, (const float*)(Tpi + pi.ls_row), B, A); c.done();
+      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + s.logitsP, 2 * A, A, (const float*)(Ppi + pi.ls_row), B, A); c.done();
+      launch_k(bcast_row_kernel, blocks, 256, 0, c, W + s.logitsT, 2 * A, A, (const float*)(Tpi + pi.ls_row), B, A); c.done();
     }
   }
   // ---- critics on (s, a): out = (mean, raw std) packed [B,2] (networks/cnn.py:454-461; softplus is applied by the loss kernels)
   {
     std::vector<CnnHeadFwd> v;
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < nq; ++k)
       for (int hd = 0; hd < q.nheads; ++hd)
-        v.push_back({Pq[k] + q.head_off[hd], f.Q[k], q.F, bt.act, A, &h->hb[4 + 2 * k + hd], true, W + h->outQ[k] + hd, 2});
+        v.push_back({Pq[k] + q.head_off[hd], f.Q[k], q.F, bt.act, A, &h->hb[4 + 2 * k + hd], true, W + s.outQ[k] + hd, 2});
     cnn_heads_forward(h, q.head, v, B, c);
   }
-  {
-    SampleArgs a;
-    a.logits[0] = W + h->logitsP; a.logits[1] = W + h->logitsT;
-    a.eps[0] = eps1; a.eps[1] = eps2;
-    a.act[0] = W + h->new_act; a.act[1] = W + h->act2;
-    a.logp[0] = W + h->logp_new; a.logp[1] = W + h->logp2;
-    a.hi = h->buf.act_high; a.lo = h->buf.act_low; a.state = h->buf.state;
-    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
-    a.img[0] = ImgOut{nullptr, 0, 1, 0}; a.img[1] = ImgOut{nullptr, 0, 1, 0};
-    a.out_q[0] = W + h->outQ[0]; a.out_q[1] = W + h->outQ[1];
-    a.advance_rng = noise ? 0 : 1;
-    int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-    launch_k(sample_kernel, dim3(blocks, 2), 256, 0, c, a); c.done();
-  }
+  enqueue_sample(h, B, nz.eps1, nz.eps2, !noise, NO_IMG, NO_IMG, c);
   // ---- targets on (s', a') and the mean heads of the critics on (s, a~)
   {
     std::vector<CnnHeadFwd> v;
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < nq; ++k)
       for (int hd = 0; hd < q.nheads; ++hd)
-        v.push_back({Tq[k] + q.head_off[hd], f.Q[2 + k], q.F, W + h->act2, A, &h->hb[8 + 2 * k + hd], false, W + h->outQ[2 + k] + hd, 2});
-    for (int k = 0; k < 2; ++k)
-      v.push_back({Pq[k] + q.head_off[0], f.Q[k], q.F, W + h->new_act, A, &h->hb[12 + k], true, W + h->outQ[4 + k], 2});
+        v.push_back({Tq[k] + q.head_off[hd], f.Q[2 + k], q.F, W + s.act2, A, &h->hb[8 + 2 * k + hd], false, W + s.outQ[2 + k] + hd, 2});
+    for (int k = 0; k < nq; ++k)
+      v.push_back({Pq[k] + q.head_off[0], f.Q[k], q.F, W + s.new_act, A, &h->hb[12 + k], true, W + s.outQ[4 + k], 2});
     cnn_heads_forward(h, q.head, v, B, c);
   }
   c.check();
@@ -527,59 +507,61 @@ static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsac
 static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
   const dsact_cnn_config& cf = h->cfg;
   const CnnGeom &q = h->q, &pi = h->pi;
+  const StepSlots& s = h->slot;
   const dsact_batch& bt = h->pending;
-  const int B = bt.batch, A = cf.act_dim;
+  const int B = bt.batch, A = h->act_dim, nq = h->nq();
   float* W = h->W();
   float* P = h->buf.params; float* G = h->buf.grads;
-  float* Pq[2] = {P, P + q.n}; float* Ppi = P + 2 * q.n;
-  float* Gq[2] = {G, G + q.n}; float* Gpi = G + 2 * q.n;
+  float* Pq[2] = {P, P + q.n}; float* Ppi = P + nq * q.n;
+  float* Gq[2] = {G, G + q.n}; float* Gpi = G + nq * q.n;
   const bool enc = pi.nconv > 0;
   const CnnFeats f = cnn_feats(h, bt);
 
   // ---- losses and head-output gradients
-  const float inv_gb = (float)(1.0 / (double)global_batch);
-  StepScalars sc;
-  sc.tau_b = (float)cf.tau_b; sc.alpha_fixed = (float)cf.alpha_fixed; sc.inv_global_batch = inv_gb;
-  sc.auto_alpha = cf.auto_alpha; sc.log_alpha = P + 2 * q.n + pi.n;
-  {
-    LossArgs a;
-    a.sc = sc;
-    a.rew = bt.rew; a.done = bt.done; a.z3 = h->pending_z3; a.z4 = h->pending_z4;
-    a.logp2 = W + h->logp2; a.logp_new = W + h->logp_new;
-    for (int k = 0; k < 2; ++k) {
-      a.out_q[k] = W + h->outQ[k]; a.out_qt[k] = W + h->outQ[2 + k]; a.out_qa[k] = W + h->outQ[4 + k];
-      a.d_out_q[k] = W + h->dOut[k]; a.d_out_qa[k] = W + h->dOut[4 + k];
-      a.gbias_q[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];          // output bias of the mean head
-      a.gbias_q_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
-      a.img_q[k] = ImgOut{nullptr, 0, 1, 0}; a.img_qa[k] = ImgOut{nullptr, 0, 1, 0};
-    }
-    a.state = h->buf.state; a.B = B; a.gamma = (float)cf.gamma; a.inv_global_batch = inv_gb;
+  const StepScalars sc = step_scalars(h, global_batch);
+  float* gbias[2], *gbias_raw[2];
+  for (int k = 0; k < 2; ++k) {
+    gbias[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];                                       // output bias of the mean head
+    gbias_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
+  }
+  if (h->v1) {
+    LossV1Args a;
+    a.rew = bt.rew; a.done = bt.done; a.z = h->pending_z3; a.logp2 = W + s.logp2; a.logp_new = W + s.logp_new;
+    a.out_q = W + s.outQ[0]; a.out_qt = W + s.outQ[2]; a.out_qa = W + s.outQ[4];
+    a.d_out_q = W + s.dOut[0]; a.d_out_qa = W + s.dOut[4];
+    a.gbias_q = gbias[0]; a.gbias_q_raw = gbias_raw[0];
+    a.state = h->buf.state; a.B = B; a.bound = cf.v1_bound; a.gamma = (float)cf.gamma; a.inv_global_batch = sc.inv_global_batch;
+    a.td_bound = (float)cf.td_bound; a.sc = sc;
     int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-    launch_k(loss_kernel, blocks, 64, 0, c, a); c.done();
+    launch_k(loss_v1_kernel, blocks, 64, 0, c, a); c.done();
+  } else {
+    const ImgOut none[2] = {NO_IMG, NO_IMG};
+    enqueue_loss(h, bt, sc, gbias, gbias_raw, none, none, c);
   }
   auto zero = [&](float* p, long long n) {
     int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
     launch_k(zero_kernel, blocks, 256, 0, c, p, n); c.done();
   };
-  zero(W + h->dfeat[0], (long long)B * pi.F);
-  zero(W + h->dfeat[1], (long long)B * q.F);
-  zero(W + h->dfeat[2], (long long)B * q.F);
-  zero(W + h->dfa[0], (long long)B * (q.F + A));
-  zero(W + h->dfa[1], (long long)B * (q.F + A));
+  if (enc) {   // feature gradients (read only by the encoders' backward)
+    zero(W + h->dfeat[0], (long long)B * pi.F);
+    for (int k = 0; k < nq; ++k) zero(W + h->dfeat[1 + k], (long long)B * q.F);
+  }
+  for (int k = 0; k < nq; ++k) zero(W + h->dfa[k], (long long)B * (q.F + A));
+  if (h->v1) zero(W + s.dAct[1], (long long)B * A);   // policy_grad_kernel adds the action gradients of two critics: the second is absent
   // ---- critic backward through both heads (feature gradient accumulated over the heads), actor path through the mean head
   {
     std::vector<CnnHeadBwd> v;
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < nq; ++k)
       for (int hd = 0; hd < q.nheads; ++hd)   // d(feature|act): only the feature part is used (replayed actions carry no gradient)
         v.push_back({Pq[k] + q.head_off[hd], Gq[k] + q.head_off[hd], f.Q[k], q.F, bt.act, A, &h->hb[4 + 2 * k + hd],
-                     W + h->dOut[k] + hd, 2, nullptr});
-    for (int k = 0; k < 2; ++k)
-      v.push_back({Pq[k] + q.head_off[0], nullptr, f.Q[k], q.F, W + h->new_act, A, &h->hb[12 + k], W + h->dOut[4 + k], 2, W + h->dfa[k]});
+                     W + s.dOut[k] + hd, 2, nullptr});
+    for (int k = 0; k < nq; ++k)
+      v.push_back({Pq[k] + q.head_off[0], nullptr, f.Q[k], q.F, W + s.new_act, A, &h->hb[12 + k], W + s.dOut[4 + k], 2, W + h->dfa[k]});
     cnn_heads_backward(h, q.head, v, B, c);
   }
   // feature gradients of the critics: the layer-0 input gradient of both heads, feature columns only.  The generic
   // backward above skipped it for the critic passes (din = null): do it here with the feature-width problem
-  for (int k = 0; k < 2 && enc; ++k) {
+  for (int k = 0; k < nq && enc; ++k) {
     GemmGroup gd;
     gd.n = 0;
     for (int hd = 0; hd < q.nheads; ++hd) {
@@ -593,79 +575,44 @@ static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
     launch_simt(h->num_sms, gd, V_DGRAD, c); c.done();
   }
   // dL/da~ through critic k = the action columns of dfa[k]: compact them for policy_grad_kernel
-  for (int k = 0; k < 2; ++k) {
-    const cudaError_t e = cudaMemcpy2DAsync(W + h->dAct[k], sizeof(float) * A, W + h->dfa[k] + q.F, sizeof(float) * (q.F + A),
+  for (int k = 0; k < nq; ++k) {
+    const cudaError_t e = cudaMemcpy2DAsync(W + s.dAct[k], sizeof(float) * A, W + h->dfa[k] + q.F, sizeof(float) * (q.F + A),
                                             sizeof(float) * A, B, cudaMemcpyDeviceToDevice, c.s);
     if (e != cudaSuccess && c.err == cudaSuccess) c.err = e;
   }
-  {
-    PolicyGradArgs a;
-    a.logits = W + h->logitsP; a.eps = h->pending_eps1; a.d_act1 = W + h->dAct[0]; a.d_act2 = W + h->dAct[1];
-    a.hi = h->buf.act_high; a.lo = h->buf.act_low;
-    a.d_logits = W + h->dlogits; a.state = h->buf.state;
-    a.gbias = Gpi + pi.head_off[0] + pi.head.b[pi.head.L];        // output bias of the mean head [A]
-    a.gbias_ls = pi.ls_row >= 0 ? Gpi + pi.ls_row : (pi.nheads == 2 ? Gpi + pi.head_off[1] + pi.head.b[pi.head.L] : nullptr);   // log_std head / row [A]
-    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
-    a.inv_global_batch = inv_gb;
-    a.img = ImgOut{nullptr, 0, 1, 0};
-    a.sc = sc;
-    int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(policy_grad_kernel, blocks, 256, sizeof(float) * 2 * A, c, a); c.done();
-  }
+  enqueue_policy_grad(h, B, sc, Gpi + pi.head_off[0] + pi.head.b[pi.head.L],   // output bias of the mean head [A]
+                      pi.ls_row >= 0 ? Gpi + pi.ls_row : (pi.nheads == 2 ? Gpi + pi.head_off[1] + pi.head.b[pi.head.L] : nullptr),   // log_std head / row [A]
+                      NO_IMG, c);
   {
     std::vector<CnnHeadBwd> v;
     for (int hd = 0; hd < pi.nheads; ++hd)
-      v.push_back({Ppi + pi.head_off[hd], Gpi + pi.head_off[hd], f.P, pi.F, nullptr, 0, &h->hb[hd], W + h->dlogits + hd * A, 2 * A,
+      v.push_back({Ppi + pi.head_off[hd], Gpi + pi.head_off[hd], f.P, pi.F, nullptr, 0, &h->hb[hd], W + s.dlogits + hd * A, 2 * A,
                    enc ? W + h->dfeat[0] : nullptr});
     cnn_heads_backward(h, pi.head, v, B, c);
   }
   // ---- encoders backward
   if (enc) {
     cnn_conv_backward(h, pi, Ppi, Gpi, bt.obs, h->convP, W + h->dfeat[0], B, c);
-    for (int k = 0; k < 2; ++k) cnn_conv_backward(h, q, Pq[k], Gq[k], bt.obs, h->convQ[k], W + h->dfeat[1 + k], B, c);
+    for (int k = 0; k < nq; ++k) cnn_conv_backward(h, q, Pq[k], Gq[k], bt.obs, h->convQ[k], W + h->dfeat[1 + k], B, c);
   }
 
   // ---- end of backward bookkeeping: log_alpha gradient (this shard's share), mean_std EMA commit, the Adam scalars
-  const AdamHyper hy{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-  launch_k(phase2_tail_kernel, 1, 32, 0, c, G + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, hy, 1); c.done();
+  launch_k(phase2_tail_kernel, 1, 32, 0, c, G + h->n_params - 1, h->buf.state, sc, -(float)A, B, adam_hyper(h), 1); c.done();
   c.check();
 }
 
-// Adam / Polyak on `grads` (dp = false), or on the rank-ordered sum of every rank's exchange block (dp = true).
+// Adam / Polyak on `grads` (dp = false), or on the rank-ordered sum of every rank's exchange block (dp = true).  The
+// critics' span is nq networks: DSAC_V1's q_optimizer also steps every iteration (dsac_v1.py:259).
 // scalars_ready: 1 = phase 2 of this step wrote the Adam scalars; 0 = apply_kernel forms them (a handle that only receives
 // gradients never runs phase 2)
 static void cnn_enqueue_apply(HeadsHandle* h, Ctx& c, int scalars_ready, bool dp) {
-  const dsact_cnn_config& cf = h->cfg;
-  const long long n_all = 2 * h->q.n + h->pi.n + 1;
-  ApplyArgs a;
-  memset(&a, 0, sizeof(a));
-  a.params = h->buf.params; a.targets = h->buf.targets; a.grads = h->buf.grads; a.m = h->buf.adam_m; a.v = h->buf.adam_v;
-  a.state = h->buf.state;
-  a.n_q2 = 2 * h->q.n; a.n_all = n_all;
-  a.delay_update = cf.delay_update; a.auto_alpha = cf.auto_alpha;
-  a.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2}; a.scalars_ready = scalars_ready;
-  a.eps = (float)cf.adam_eps; a.tau = (float)cf.tau;
-  a.omb1 = (float)(1.0 - cf.adam_beta1); a.b2f = (float)cf.adam_beta2; a.omb2 = (float)(1.0 - cf.adam_beta2);
-  a.g_lo = 0; a.g_hi = (n_all + 3) / 4; a.finish = 1;
-  int blocks = (int)(((n_all + 3) / 4 + 255) / 256); if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-  if (dp) {
-    a.dp_timeout_ns = dp_timeout_ns();
-    dp_apply_args(h->dp, a);
-    launch_k(apply_kernel<2>, blocks, 256, 0, c, a);
-  } else {
-    launch_k(apply_kernel<0>, blocks, 256, 0, c, a);
-  }
-  c.done();
-  c.check();
+  launch_apply(h, apply_args(h, h->nq() * h->q.n, scalars_ready, dp), c);
 }
 
 static HeadsHandle* heads(dsact_handle* h) { return static_cast<HeadsHandle*>(h); }
 
-#include "v1_step.cuh"
-
-// dsact_step: phase 1, phase 2 and the update on its own rows, or the DSAC_V1 update
+// dsact_step: phase 1, phase 2 and the update on its own rows
 static void cnn_enqueue_step(HeadsHandle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
-  if (h->v1) { cnn_enqueue_v1(h, &bt, noise, c); return; }
   cnn_enqueue_phase1(h, bt, noise, c);
   cnn_enqueue_phase2(h, bt.batch, c);
   cnn_enqueue_apply(h, c, 1, false);
@@ -680,7 +627,7 @@ static void cnn_enqueue_dp_step(HeadsHandle* h, const dsact_batch& bt, const dsa
   enqueue_dp_exchange(h->dp, state, 0, c);
   cnn_enqueue_phase2(h, global_batch, c);
   {   // phase 2 already wrote the log_alpha share: a plain copy of the flat gradients into this rank's block
-    const long long n = 2 * h->q.n + h->pi.n + 1;
+    const long long n = h->n_params;
     TailArgs none;
     memset(&none, 0, sizeof(none));
     int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
@@ -691,29 +638,6 @@ static void cnn_enqueue_dp_step(HeadsHandle* h, const dsact_batch& bt, const dsa
   enqueue_dp_exchange(h->dp, state, 1, c);
   if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, state, h->num_sms, c);
   cnn_enqueue_apply(h, c, 1, true);
-}
-
-// dsact_replay_sample: ring rows idx[i] (NULL: drawn on the device and recorded in the arena) -> the arena minibatch
-static void cnn_enqueue_gather(HeadsHandle* h, int32_t batch, const int64_t* idx, Ctx& c) {
-  float* W = h->W();
-  int64_t* draw = idx ? nullptr : reinterpret_cast<int64_t*>(W + h->r_idx);
-  int blocks = (batch + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-  const ImgOut none{nullptr, 0, 1, 0};
-  launch_k(gather_kernel, blocks, 256, 0, c, (const float*)h->rb.obs, (const float*)h->rb.obs2, (const float*)h->rb.act, (const float*)h->rb.rew,
-           (const float*)h->rb.done, (const float*)h->rb.logp, idx, W + h->r_obs, W + h->r_obs2, W + h->r_act, W + h->r_rew, W + h->r_done,
-           W + h->r_logp, (int)batch, (int)h->obs_elems, h->act_dim, none, none, none, draw, (unsigned long long)h->seed,
-           (const float*)h->buf.state, 1);
-  c.done();
-  if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-}
-
-static dsact_batch cnn_arena_batch(const HeadsHandle* h, int32_t batch) {
-  float* W = h->W();
-  dsact_batch b;
-  b.obs = W + h->r_obs; b.act = W + h->r_act; b.rew = W + h->r_rew; b.obs2 = W + h->r_obs2; b.done = W + h->r_done;
-  b.logp = W + h->r_logp;
-  b.batch = batch;
-  return b;
 }
 
 extern "C" {
@@ -730,7 +654,8 @@ int dsact_cnn_query_layout(const dsact_cnn_config* cfg, dsact_layout* out) {
   out->workspace_bytes = h.total * (int64_t)sizeof(float);
   out->state_floats = ST_FLOATS;
   out->max_batch = cfg->max_batch;
-  out->off_idx = h.r_idx; out->off_eps1 = h.eps1; out->off_eps2 = h.eps2; out->off_z3 = h.z3; out->off_z4 = h.z4;
+  const StepSlots& s = h.slot;
+  out->off_idx = s.idx; out->off_eps1 = s.eps1; out->off_eps2 = s.eps2; out->off_z3 = s.z3; out->off_z4 = s.z4;
   out->off_slabs = h.total; out->slab_floats = 0;
   return DSACT_OK;
 }

@@ -3,6 +3,11 @@
 // Orchestrates one `DSAC_V2.local_update` (reference dsac_v2.py:102-105,150-347) as a fixed sequence of
 // kernel launches on caller-owned flat fp32 buffers, optionally captured once into a CUDA graph and
 // replayed.  No CPU fallback: every entry point needs a CUDA device.
+//
+// Two engines sit behind one handle: the MLP engine of this file (wgmma / SIMT GEMMs) and the head-wise fp32 engine of
+// cnn_engine.cuh (CNN approximators, the policy's other std types, DSAC_V1).  This file holds the shell they share, the
+// launches of the step kernels they share (noise, begin_step, sample, loss, policy gradient, apply, gather) and the
+// C entry points, which dispatch once on the handle's engine.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -61,14 +66,31 @@ struct ImgSlot {
   int64_t plane = 0;
 };
 
-// activation arena, all offsets in floats from the workspace base
-struct Arena {
+// The arena slots both engines have and the step kernels they share read (floats from the workspace base).  Each engine
+// places them in its own arena order.
+struct StepSlots {
   int64_t obs, obs2, act, rew, done, logp, idx;    // gathered minibatch + int64 indices
   int64_t eps1, eps2, z3, z4;                      // device-generated noise
-  int64_t zP[DSACT_MAX_HIDDEN], hP[DSACT_MAX_HIDDEN], hT[DSACT_MAX_HIDDEN], logitsP, logitsT;
-  int64_t new_act, act2, logp_new, logp2;
-  int64_t zQ[6][DSACT_MAX_HIDDEN], hQ[6][DSACT_MAX_HIDDEN], outQ[6];
-  int64_t dOut[6], dzQ[6][DSACT_MAX_HIDDEN], dAct[2], dlogits, dzP[DSACT_MAX_HIDDEN];
+  int64_t logitsP, logitsT, dlogits;               // policy outputs (mean | log_std) of pi(s), pi'(s'); their gradient
+  int64_t new_act, act2, logp_new, logp2;          // a~ ~ pi(s), a' ~ pi'(s') and their log-probs
+  int64_t outQ[6], dOut[6], dAct[2];               // Q_k(s,a), Q'_k(s',a'), Q_k(s,a~) [B,2] and gradients; dL/da~ per critic
+};
+
+// The hyperparameters both configuration structs name alike
+struct StepHyper {
+  int auto_alpha, delay_update, act_dist;
+  double gamma, tau, tau_b, alpha_fixed, lr_q, lr_pi, lr_alpha, min_log_std, max_log_std, adam_beta1, adam_beta2, adam_eps;
+  template <typename Cfg> static StepHyper of(const Cfg& c) {
+    return StepHyper{c.auto_alpha, c.delay_update, c.act_dist, c.gamma, c.tau, c.tau_b, c.alpha_fixed, c.lr_q, c.lr_pi,
+                     c.lr_alpha, c.min_log_std, c.max_log_std, c.adam_beta1, c.adam_beta2, c.adam_eps};
+  }
+};
+
+// activation arena of the MLP engine, all offsets in floats from the workspace base
+struct Arena : StepSlots {
+  int64_t zP[DSACT_MAX_HIDDEN], hP[DSACT_MAX_HIDDEN], hT[DSACT_MAX_HIDDEN];
+  int64_t zQ[6][DSACT_MAX_HIDDEN], hQ[6][DSACT_MAX_HIDDEN];
+  int64_t dzQ[6][DSACT_MAX_HIDDEN], dzP[DSACT_MAX_HIDDEN];
   // ---- tensor-core modes: bf16 hi/lo images of every GEMM operand + wgrad split slabs
   bool tc;
   ImgSlot i_obs, i_obs2, i_act, i_new_act, i_act2, i_dlogits;
@@ -134,8 +156,9 @@ struct GraphKey {
 struct GraphEntry { GraphKey key; cudaGraphExec_t exec; int launches; uint64_t stamp; };
 
 // The shell both engines share: device, bound buffers, generator seed, replay ring, peer exchange, what the last phase 1
-// ran on, launch counts, and the few sizes the shell's entry points check against.  `engine` says which of MlpHandle
-// (the wgmma / SIMT MLP engine, this file) and HeadsHandle (the head-wise fp32 engine, cnn_engine.cuh) it is.
+// ran on, launch counts, the few sizes the shell's entry points check against, and the arena slots and hyperparameters
+// of the step kernels both engines launch.  `engine` says which of MlpHandle (the wgmma / SIMT MLP engine, this file)
+// and HeadsHandle (the head-wise fp32 engine, cnn_engine.cuh) it is.
 enum { ENGINE_MLP = 0, ENGINE_HEADS = 1 };
 struct dsact_handle {
   int engine;
@@ -143,7 +166,9 @@ struct dsact_handle {
   int64_t obs_elems = 0;     // floats of one observation row
   int act_dim = 0, max_batch = 0;
   int64_t n_params = 0;      // flat parameter count (log_alpha included)
-  bool v1 = false;           // DSAC_V1: local steps only, its own policy-statistic denominator
+  bool v1 = false;           // DSAC_V1: one critic, local steps only, its own policy-statistic denominator
+  StepSlots slot = {};
+  StepHyper hyper = {};
   dsact_buffers buf = {};
   bool bound = false, rb_bound = false;
   uint64_t seed = 0x5DEECE66Dull;
@@ -688,18 +713,199 @@ static ChainPass& chain_dgrad_pass(ChainBuild& cb, const MlpHandle* h, const Net
   return P;
 }
 
-// ---- enqueue: pieces of one update ---------------------------------------------
-// Everything of a step that depends on neither the minibatch gather nor a forward pass: accumulator clears, the
-// gradient memset, the bf16 images of all weights (and of a caller-supplied batch), the device noise.
-static void enqueue_noise(MlpHandle* h, int B, Ctx& c) {
-  const Arena& ar = h->ar;
-  float* W = h->W();
-  const int A = h->cfg.act_dim;
-  const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
-  int blocks = (total / 2 + 255) / 256; if (blocks < 1) blocks = 1;
-  launch_k(noise_kernel, blocks, 256, 0, c, W + ar.eps1, W + ar.eps2, W + ar.z3, W + ar.z4, B, A, h->seed, h->buf.state);
+static unsigned long long dp_timeout_ns() {
+  static const unsigned long long t =
+      (unsigned long long)(getenv("DSACT_DP_TIMEOUT_MS") ? atoll(getenv("DSACT_DP_TIMEOUT_MS")) : 10000) * 1000000ull;
+  return t;
+}
+// two-shot gradient exchange (dp_peer.cuh) from 6 ranks up, one-shot below (fewer barriers).  Replicas stay bit-identical
+// in both variants.
+static bool dp_two_shot(const DpPeer& dp) { return dp.comm.world >= 6; }
+
+// apply_kernel<2>'s view of the exchange: the reduced block in this rank's own memory once every rank's kind-2 flag is
+// here (two-shot), or every rank's block, summed in rank order (one-shot)
+static void dp_apply_args(const DpPeer& dp, ApplyArgs& a) {
+  if (dp_two_shot(dp)) {
+    a.dp_world = 1;
+    a.dp_grads[0] = dp.buf + DP_GRADS_OFF + dp.npad();
+    a.dp_own = dp.buf; a.dp_wait_world = dp.comm.world;
+  } else {
+    a.dp_world = dp.comm.world;
+    for (int r = 0; r < dp.comm.world; ++r) a.dp_grads[r] = dp.comm.peer[r] + DP_GRADS_OFF;
+  }
+}
+
+// ---- the step kernels both engines launch ---------------------------------------------------------------------------
+// They read the shell's arena slots and hyperparameters.  What only the MLP engine has (the bf16 images its tensor-core
+// GEMMs read) comes in as ImgOut arguments; the head-wise engine passes NO_IMG.
+static const ImgOut NO_IMG{nullptr, 0, 1, 0};
+
+static AdamHyper adam_hyper(const dsact_handle* h) {
+  const StepHyper& p = h->hyper;
+  return AdamHyper{p.lr_q, p.lr_pi, p.lr_alpha, p.adam_beta1, p.adam_beta2};
+}
+static StepScalars step_scalars(const dsact_handle* h, int64_t global_batch) {
+  StepScalars sc;
+  sc.tau_b = (float)h->hyper.tau_b; sc.alpha_fixed = (float)h->hyper.alpha_fixed;
+  sc.inv_global_batch = (float)(1.0 / (double)global_batch);
+  sc.auto_alpha = h->hyper.auto_alpha; sc.log_alpha = h->buf.params + h->n_params - 1;   // log_alpha is the last parameter
+  return sc;
+}
+// the caller's noise, or the arena's device-noise slots
+static dsact_noise step_noise(const dsact_handle* h, const dsact_noise* nz) {
+  const float* W = h->W();
+  return nz ? *nz : dsact_noise{W + h->slot.eps1, W + h->slot.eps2, W + h->slot.z3, W + h->slot.z4};
+}
+
+static int begin_step_blocks(const dsact_handle* h) {
+  int blocks = (int)((h->n_params / 4 + 255) / 256); if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms; if (blocks < 1) blocks = 1;
+  return blocks;
+}
+// accumulator clears and the flat gradient memset
+static void enqueue_begin_step(const dsact_handle* h, Ctx& c) {
+  launch_k(begin_step_kernel, begin_step_blocks(h), 256, 0, c, h->buf.state, h->buf.grads, (long long)h->n_params);
   c.done();
 }
+
+static int noise_blocks(int B, int A) {   // one thread per pair of draws
+  const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
+  const int blocks = (total / 2 + 255) / 256;
+  return blocks < 1 ? 1 : blocks;
+}
+// device noise into the arena; the counter it reads is stepped by sample_kernel, once every reader of this step has run
+static void enqueue_noise(const dsact_handle* h, int B, Ctx& c) {
+  const StepSlots& s = h->slot;
+  float* W = h->W();
+  launch_k(noise_kernel, noise_blocks(B, h->act_dim), 256, 0, c, W + s.eps1, W + s.eps2, W + s.z3, W + s.z4, B, h->act_dim, h->seed,
+           h->buf.state);
+  c.done();
+}
+
+// rsample of both policies (utils/act_distribution_cls.py:44-54); also sums the critics' std over the rows (DSAC_V1: of
+// its one critic, and its own logged policy statistics)
+static void enqueue_sample(const dsact_handle* h, int B, const float* eps1, const float* eps2, bool advance_rng,
+                           const ImgOut& img_new_act, const ImgOut& img_act2, Ctx& c) {
+  const StepSlots& s = h->slot;
+  const StepHyper& p = h->hyper;
+  float* W = h->W();
+  SampleArgs a;
+  a.logits[0] = W + s.logitsP; a.logits[1] = W + s.logitsT;
+  a.eps[0] = eps1; a.eps[1] = eps2;
+  a.act[0] = W + s.new_act; a.act[1] = W + s.act2;
+  a.logp[0] = W + s.logp_new; a.logp[1] = W + s.logp2;
+  a.hi = h->buf.act_high; a.lo = h->buf.act_low; a.state = h->buf.state;
+  a.B = B; a.A = h->act_dim; a.min_log_std = (float)p.min_log_std; a.max_log_std = (float)p.max_log_std; a.gauss = p.act_dist;
+  a.img[0] = img_new_act; a.img[1] = img_act2;
+  a.out_q[0] = W + s.outQ[0]; a.out_q[1] = W + s.outQ[h->v1 ? 0 : 1];
+  a.advance_rng = advance_rng ? 1 : 0;
+  a.v1_stats = h->v1 ? 1 : 0;
+  int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
+  launch_k(sample_kernel, dim3(blocks, 2), 256, 0, c, a);
+  c.done();
+}
+
+// the DSAC-T losses and the gradients of the critics' outputs.  gbias[k]: output-bias gradient of critic k's mean;
+// gbias_raw[k]: of its std output, or null for the element after gbias[k] (one two-output layer)
+static void enqueue_loss(const dsact_handle* h, const dsact_batch& bt, const StepScalars& sc, float* const gbias[2],
+                         float* const gbias_raw[2], const ImgOut img_q[2], const ImgOut img_qa[2], Ctx& c) {
+  const StepSlots& s = h->slot;
+  float* W = h->W();
+  const int B = bt.batch;
+  LossArgs a;
+  a.sc = sc;
+  a.rew = bt.rew; a.done = bt.done; a.z3 = h->pending_z3; a.z4 = h->pending_z4;
+  a.logp2 = W + s.logp2; a.logp_new = W + s.logp_new;
+  for (int k = 0; k < 2; ++k) {
+    a.out_q[k] = W + s.outQ[k]; a.out_qt[k] = W + s.outQ[2 + k]; a.out_qa[k] = W + s.outQ[4 + k];
+    a.d_out_q[k] = W + s.dOut[k]; a.d_out_qa[k] = W + s.dOut[4 + k];
+    a.gbias_q[k] = gbias[k]; a.gbias_q_raw[k] = gbias_raw[k];
+    a.img_q[k] = img_q[k]; a.img_qa[k] = img_qa[k];
+  }
+  a.state = h->buf.state; a.B = B; a.gamma = (float)h->hyper.gamma; a.inv_global_batch = sc.inv_global_batch;
+  int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;   // latency bound: spread over the SMs
+  launch_k(loss_kernel, blocks, 64, 0, c, a);
+  c.done();
+}
+
+// the actor loss's gradient w.r.t. the policy outputs of pi(s).  gbias: output-bias gradient of the mean (the whole
+// (mean | log_std) row when gbias_ls is null); gbias_ls: of a separate log_std head or row
+static void enqueue_policy_grad(const dsact_handle* h, int B, const StepScalars& sc, float* gbias, float* gbias_ls, const ImgOut& img,
+                                Ctx& c) {
+  const StepSlots& s = h->slot;
+  const StepHyper& p = h->hyper;
+  float* W = h->W();
+  const int A = h->act_dim;
+  PolicyGradArgs a;
+  a.logits = W + s.logitsP; a.eps = h->pending_eps1; a.d_act1 = W + s.dAct[0]; a.d_act2 = W + s.dAct[1];
+  a.hi = h->buf.act_high; a.lo = h->buf.act_low;
+  a.d_logits = W + s.dlogits; a.gbias = gbias; a.gbias_ls = gbias_ls; a.state = h->buf.state;
+  a.B = B; a.A = A; a.min_log_std = (float)p.min_log_std; a.max_log_std = (float)p.max_log_std; a.gauss = p.act_dist;
+  a.inv_global_batch = sc.inv_global_batch;
+  a.img = img;
+  a.sc = sc;
+  int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;   // a warp per row
+  launch_k(policy_grad_kernel, blocks, 256, sizeof(float) * 2 * A, c, a);
+  c.done();
+}
+
+// Adam / Polyak over the whole flat buffers, on `grads` or (dp) on the rank-ordered sum of every rank's exchange block.
+// n_q2: the critics' span (Adam every iteration).  scalars_ready: see ApplyArgs
+static ApplyArgs apply_args(const dsact_handle* h, int64_t n_q2, int scalars_ready, bool dp) {
+  const StepHyper& p = h->hyper;
+  ApplyArgs a;
+  memset(&a, 0, sizeof(a));
+  a.params = h->buf.params; a.targets = h->buf.targets; a.grads = h->buf.grads; a.m = h->buf.adam_m; a.v = h->buf.adam_v;
+  a.state = h->buf.state;
+  a.n_q2 = n_q2; a.n_all = h->n_params;
+  a.delay_update = p.delay_update; a.auto_alpha = p.auto_alpha;
+  a.hy = adam_hyper(h); a.scalars_ready = scalars_ready;
+  a.eps = (float)p.adam_eps; a.tau = (float)p.tau;
+  a.omb1 = (float)(1.0 - p.adam_beta1); a.b2f = (float)p.adam_beta2; a.omb2 = (float)(1.0 - p.adam_beta2);
+  a.dp_timeout_ns = dp_timeout_ns();
+  if (dp) dp_apply_args(h->dp, a);
+  a.g_lo = 0; a.g_hi = (a.n_all + 3) / 4; a.finish = 1;
+  return a;
+}
+static void launch_apply(const dsact_handle* h, const ApplyArgs& a, Ctx& c) {
+  int blocks = (int)((a.g_hi - a.g_lo + 255) / 256);   // one 4-element group per thread
+  if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
+  if (blocks < 1) blocks = 1;
+  // (its last block also advances the step counters)
+  if (a.dp_world > 0) launch_k(apply_kernel<2>, blocks, 256, 0, c, a);
+  else if (a.nslabs > 0) launch_k(apply_kernel<1>, blocks, 256, 0, c, a);
+  else launch_k(apply_kernel<0>, blocks, 256, 0, c, a);
+  c.done();
+  c.check();
+}
+
+// the replay gather: ring rows idx[i] (null: drawn on the device and recorded in the arena) -> the arena minibatch.
+// img: bf16 images of obs / obs2 / act to write as well; write_f32 = false leaves out their fp32 rows
+static void enqueue_gather(const dsact_handle* h, int B, const int64_t* idx, const ImgOut img[3], bool write_f32, Ctx& c) {
+  const StepSlots& s = h->slot;
+  float* W = h->W();
+  // no index list: every warp of the gather draws its row's index itself (the sequence index_kernel defines) and records it
+  int64_t* draw = idx ? nullptr : reinterpret_cast<int64_t*>(W + s.idx);
+  int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
+  launch_k(gather_kernel, blocks, 256, 0, c, h->rb.obs, h->rb.obs2, h->rb.act, h->rb.rew, h->rb.done, h->rb.logp, idx,
+           W + s.obs, W + s.obs2, W + s.act, W + s.rew, W + s.done, W + s.logp, B, (int)h->obs_elems, h->act_dim,
+           img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0);
+  c.done();
+  c.check();
+}
+
+static dsact_batch arena_batch(const dsact_handle* h, int32_t batch) {
+  const StepSlots& s = h->slot;
+  float* W = h->W();
+  dsact_batch b;
+  b.obs = W + s.obs; b.act = W + s.act; b.rew = W + s.rew; b.obs2 = W + s.obs2; b.done = W + s.done;
+  b.logp = W + s.logp;
+  b.batch = batch;
+  return b;
+}
+
+// ---- enqueue: pieces of one MLP update -------------------------------------------
+// Everything of a step that depends on neither the minibatch gather nor a forward pass: accumulator clears, the
+// gradient memset, the bf16 images of all weights (and of a caller-supplied batch), the device noise.
 static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged,
                              bool with_noise = true) {
   const dsact_config& cf = h->cfg;
@@ -713,10 +919,8 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
   const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2'
   const float* PIb[2] = {P + 2 * q.n, T + 2 * q.n};     // pi, pi'
 
-  const long long n_grads = 2 * q.n + pi.n + 1;
-  int zero_blocks = (int)((n_grads / 4 + 255) / 256); if (zero_blocks > 2 * h->num_sms) zero_blocks = 2 * h->num_sms; if (zero_blocks < 1) zero_blocks = 1;
   const bool want_noise = !nz && with_noise;
-  if (!tc) { launch_k(begin_step_kernel, zero_blocks, 256, 0, c, h->buf.state, h->buf.grads, n_grads); c.done(); }
+  if (!tc) enqueue_begin_step(h, c);
 
   if (tc) {  // refresh the weight images (the caller may have written params/targets through its views) + inputs; the clears
              // and the device noise ride in the same launch
@@ -746,19 +950,17 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
     }
     PrologueArgs pa;
     memset(&pa, 0, sizeof(pa));
-    pa.zero_blocks = zero_blocks;
-    pa.state = h->buf.state; pa.grads = h->buf.grads; pa.n_grads = n_grads;
-    pa.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
+    pa.zero_blocks = begin_step_blocks(h);
+    pa.state = h->buf.state; pa.grads = h->buf.grads; pa.n_grads = h->n_params;
+    pa.hy = adam_hyper(h);
     if (want_noise) {
-      const int total = (B * A + 1) / 2 * 2 + (B + 1) / 2 * 2;
-      pa.noise_blocks = (total / 2 + 255) / 256; if (pa.noise_blocks < 1) pa.noise_blocks = 1;
+      pa.noise_blocks = noise_blocks(B, A);
       pa.eps1 = W + ar.eps1; pa.eps2 = W + ar.eps2; pa.z3 = W + ar.z3; pa.z4 = W + ar.z4;
       pa.B = B; pa.A = A; pa.seed = h->seed;
     }
     ib.launch(h, c, &pa);
   }
 
-  // device noise; the counter it reads is stepped by sample_kernel, once every reader of this step has run
   if (want_noise && !tc) enqueue_noise(h, B, c);
   c.check();
 }
@@ -778,14 +980,6 @@ static bool fork_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise
   return true;
 }
 
-static unsigned long long dp_timeout_ns() {
-  static const unsigned long long t =
-      (unsigned long long)(getenv("DSACT_DP_TIMEOUT_MS") ? atoll(getenv("DSACT_DP_TIMEOUT_MS")) : 10000) * 1000000ull;
-  return t;
-}
-// two-shot gradient exchange (dp_peer.cuh) from 6 ranks up, one-shot below (fewer barriers).  Replicas stay bit-identical
-// in both variants.
-static bool dp_two_shot(const DpPeer& dp) { return dp.comm.world >= 6; }
 static void enqueue_dp_reduce_scatter(const DpPeer& dp, const float* state, int num_sms, Ctx& c) {
   const long long groups = dp.npad() / 4, per = (groups + dp.comm.world - 1) / dp.comm.world;
   DpSlice sl;
@@ -805,19 +999,6 @@ static void enqueue_dp_exchange(const DpPeer& dp, float* state, int kind, Ctx& c
   c.done();
 }
 static void enqueue_dp_exchange(MlpHandle* h, int kind, Ctx& c) { enqueue_dp_exchange(h->dp, h->buf.state, kind, c); }
-
-// apply_kernel<2>'s view of the exchange: the reduced block in this rank's own memory once every rank's kind-2 flag is
-// here (two-shot), or every rank's block, summed in rank order (one-shot)
-static void dp_apply_args(const DpPeer& dp, ApplyArgs& a) {
-  if (dp_two_shot(dp)) {
-    a.dp_world = 1;
-    a.dp_grads[0] = dp.buf + DP_GRADS_OFF + dp.npad();
-    a.dp_own = dp.buf; a.dp_wait_world = dp.comm.world;
-  } else {
-    a.dp_world = dp.comm.world;
-    for (int r = 0; r < dp.comm.world; ++r) a.dp_grads[r] = dp.comm.peer[r] + DP_GRADS_OFF;
-  }
-}
 
 // ---- exchange-buffer setup (dsact_dp_export / dsact_dp_connect, both engines) ---------------------------------------
 static int dp_peer_export(DpPeer& dp, int device, long long n_params, void* handle_out, int64_t* bytes_out) {
@@ -894,12 +1075,7 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
     enqueue_prologue(h, bt, nz, c, inputs_imaged);
   }
 
-  const float *eps1, *eps2, *z3, *z4;
-  if (nz) { eps1 = nz->eps1; eps2 = nz->eps2; z3 = nz->z3; z4 = nz->z4; }
-  else {
-    eps1 = W + ar.eps1; eps2 = W + ar.eps2; z3 = W + ar.z3; z4 = W + ar.z4;   // sample_kernel steps the counter
-  }
-
+  const dsact_noise noise = step_noise(h, nz);   // device noise: sample_kernel steps the counter
   const Ten t_obs = ten(bt.obs, ar.i_obs), t_obs2 = ten(bt.obs2, ar.i_obs2), t_act = ten(bt.act, ar.i_act);
   const Ten t_none;
 
@@ -937,21 +1113,7 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
     launch_group(h, G, V_FWD, c);
   }
 
-  // rsample of both policies (utils/act_distribution_cls.py:44-54)
-  {
-    SampleArgs a;
-    a.logits[0] = W + ar.logitsP; a.logits[1] = W + ar.logitsT;
-    a.eps[0] = eps1; a.eps[1] = eps2;
-    a.act[0] = W + ar.new_act; a.act[1] = W + ar.act2;
-    a.logp[0] = W + ar.logp_new; a.logp[1] = W + ar.logp2;
-    a.hi = h->buf.act_high; a.lo = h->buf.act_low; a.state = h->buf.state;
-    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
-    a.img[0] = img_out(h, ar.i_new_act); a.img[1] = img_out(h, ar.i_act2);
-    a.out_q[0] = W + ar.outQ[0]; a.out_q[1] = W + ar.outQ[1];
-    a.advance_rng = nz ? 0 : 1;
-    int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-    launch_k(sample_kernel, dim3(blocks, 2), 256, 0, c, a); c.done();
-  }
+  enqueue_sample(h, B, noise.eps1, noise.eps2, !nz, img_out(h, ar.i_new_act), img_out(h, ar.i_act2), c);
   bool dp_forked = false;
   if (dp_std_exchange) {
     if (c.side) {
@@ -995,7 +1157,7 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
   }
 
   if (dp_forked) cudaStreamWaitEvent(c.s, h->ev_dp_join, 0);
-  h->pending_eps1 = eps1; h->pending_z3 = z3; h->pending_z4 = z4;
+  h->pending_eps1 = noise.eps1; h->pending_z3 = noise.z3; h->pending_z4 = noise.z4;
   c.check();
 }
 
@@ -1004,11 +1166,8 @@ static bool slabs_foldable(const MlpHandle* h) {
   return h->tc() && ((uintptr_t)(h->W() + h->ar.slabs) & 15) == 0 && ((uintptr_t)h->buf.grads & 15) == 0;
 }
 static TailArgs tail_args(const MlpHandle* h, int64_t global_batch, int rows) {
-  const Net &q = h->q, &pi = h->pi;
   TailArgs t;
-  t.sc.tau_b = (float)h->cfg.tau_b; t.sc.alpha_fixed = (float)h->cfg.alpha_fixed;
-  t.sc.inv_global_batch = (float)(1.0 / (double)global_batch);
-  t.sc.auto_alpha = h->cfg.auto_alpha; t.sc.log_alpha = h->buf.params + 2 * q.n + pi.n;
+  t.sc = step_scalars(h, global_batch);
   t.target_entropy = -(float)h->cfg.act_dim; t.rows = rows; t.enabled = 1;
   return t;
 }
@@ -1030,29 +1189,16 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   float* G_ = h->buf.grads;
   const float *Pq[2] = {P, P + q.n}, *Ppi = P + 2 * q.n;
   float *Gq[2] = {G_, G_ + q.n}, *Gpi = G_ + 2 * q.n;
-  const float invB = (float)(1.0 / (double)global_batch);
   auto ten = [&](const float* f, const ImgSlot& s) { Ten t; t.f = const_cast<float*>(f); t.im = h->img(s, B); return t; };
   const ImgSlot none;
 
-  StepScalars sc;
-  sc.tau_b = (float)cf.tau_b; sc.alpha_fixed = (float)cf.alpha_fixed; sc.inv_global_batch = invB;
-  sc.auto_alpha = cf.auto_alpha; sc.log_alpha = P + 2 * q.n + pi.n;
+  const StepScalars sc = step_scalars(h, global_batch);
   {
-    LossArgs a;
-    a.sc = sc;
-    a.rew = bt.rew; a.done = bt.done;
-    a.z3 = h->pending_z3; a.z4 = h->pending_z4;
-    a.logp2 = W + ar.logp2; a.logp_new = W + ar.logp_new;
-    for (int k = 0; k < 2; ++k) {
-      a.out_q[k] = W + ar.outQ[k]; a.out_qt[k] = W + ar.outQ[2 + k]; a.out_qa[k] = W + ar.outQ[4 + k];
-      a.d_out_q[k] = W + ar.dOut[k]; a.d_out_qa[k] = W + ar.dOut[4 + k];
-      a.gbias_q[k] = Gq[k] + q.b[q.L];
-      a.gbias_q_raw[k] = nullptr;
-    }
-    a.state = h->buf.state; a.B = B; a.gamma = (float)cf.gamma; a.inv_global_batch = invB;
-    for (int k = 0; k < 2; ++k) { a.img_q[k] = img_out(h, ar.i_dOut[k]); a.img_qa[k] = img_out(h, ar.i_dOut[4 + k]); }
-    int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;   // latency bound: spread over the SMs
-    launch_k(loss_kernel, blocks, 64, 0, c, a); c.done();
+    float* const gbias[2] = {Gq[0] + q.b[q.L], Gq[1] + q.b[q.L]};
+    float* const gbias_raw[2] = {nullptr, nullptr};   // one two-output layer
+    const ImgOut img_q[2] = {img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[1])};
+    const ImgOut img_qa[2] = {img_out(h, ar.i_dOut[4]), img_out(h, ar.i_dOut[5])};
+    enqueue_loss(h, bt, sc, gbias, gbias_raw, img_q, img_qa, c);
   }
   const int passes[4] = {0, 1, 4, 5};
   const Ten t_obs = ten(bt.obs, ar.i_obs), t_act = ten(bt.act, ar.i_act);
@@ -1117,18 +1263,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
     h->join_pending = fused && c.side != nullptr;
   }
 
-  {
-    PolicyGradArgs a;
-    a.logits = W + ar.logitsP; a.eps = h->pending_eps1; a.d_act1 = W + ar.dAct[0]; a.d_act2 = W + ar.dAct[1];
-    a.hi = h->buf.act_high; a.lo = h->buf.act_low;
-    a.d_logits = W + ar.dlogits; a.gbias = Gpi + pi.b[pi.L]; a.gbias_ls = nullptr; a.state = h->buf.state;
-    a.B = B; a.A = A; a.min_log_std = (float)cf.min_log_std; a.max_log_std = (float)cf.max_log_std; a.gauss = cf.act_dist;
-    a.inv_global_batch = invB;
-    a.img = img_out(h, ar.i_dlogits);
-    a.sc = sc;
-    int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;   // a warp per row
-    launch_k(policy_grad_kernel, blocks, 256, sizeof(float) * 2 * A, c, a); c.done();
-  }
+  enqueue_policy_grad(h, B, sc, Gpi + pi.b[pi.L], nullptr, img_out(h, ar.i_dlogits), c);
 
   // wave D: policy backward
   Group gwp;
@@ -1156,8 +1291,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
     launch_k(grad_reduce_kernel, blocks, 256, 0, c, G_, W + ar.slabs, n, ar.nslabs, (long long)ar.slab_stride); c.done();
   }
   if (!tail) {
-    AdamHyper hy{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-    launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, hy, 0);
+    launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, adam_hyper(h), 0);
     c.done();
   }
   if (dp) {  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
@@ -1175,37 +1309,16 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
 // `part`: 0 = the whole flat buffer; 1 = the critics' span only, without closing the step (launched beside the policy
 // backward, see enqueue_phase2); 2 = everything after that span + the end-of-step bookkeeping
 static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
-  const dsact_config& cf = h->cfg;
   if (part == 0 && h->apply_early) { part = 2; h->apply_early = false; }   // phase 2 already updated the critics
-  ApplyArgs a;
-  a.params = h->buf.params; a.targets = h->buf.targets; a.grads = h->buf.grads; a.m = h->buf.adam_m; a.v = h->buf.adam_v;
-  a.state = h->buf.state;
-  a.n_q2 = 2 * h->q.n; a.n_all = 2 * h->q.n + h->pi.n + 1;
-  a.delay_update = cf.delay_update; a.auto_alpha = cf.auto_alpha;
-  a.hy = AdamHyper{cf.lr_q, cf.lr_pi, cf.lr_alpha, cf.adam_beta1, cf.adam_beta2};
-  memset(&a.tail, 0, sizeof(a.tail));
-  a.scalars_ready = 0;   // split API: formed here
-  if (tail) { a.tail = *tail; a.scalars_ready = 2; }   // single-call steps: precomputed by the previous apply / prologue if stamped
-  a.dp_world = 0;
-  a.dp_own = nullptr; a.dp_wait_world = 0; a.dp_timeout_ns = dp_timeout_ns();
-  for (int r = 0; r < 8; ++r) a.dp_grads[r] = nullptr;
-  if (dp) dp_apply_args(h->dp, a);
-  a.eps = (float)cf.adam_eps; a.tau = (float)cf.tau;
-  a.omb1 = (float)(1.0 - cf.adam_beta1); a.b2f = (float)cf.adam_beta2; a.omb2 = (float)(1.0 - cf.adam_beta2);
-  a.slabs = nullptr; a.nslabs = 0; a.slab_stride = 0;
+  // split API: the Adam scalars are formed here; single-call steps: precomputed by the previous apply / prologue if stamped
+  ApplyArgs a = apply_args(h, 2 * h->q.n, tail ? 2 : 0, dp);
+  if (tail) a.tail = *tail;
   if (tail && !dp && slabs_foldable(h)) { a.slabs = h->W() + h->ar.slabs; a.nslabs = h->ar.nslabs; a.slab_stride = h->ar.slab_stride; }
-  const int64_t g_all = (a.n_all + 3) / 4, g_q = a.n_q2 / 4;   // a group straddling the critic / policy boundary goes with part 2
-  a.g_lo = part == 2 ? g_q : 0; a.g_hi = part == 1 ? g_q : g_all; a.finish = part == 1 ? 0 : 1;
+  const int64_t g_q = a.n_q2 / 4;   // a group straddling the critic / policy boundary goes with part 2
+  if (part == 2) a.g_lo = g_q;
+  if (part == 1) { a.g_hi = g_q; a.finish = 0; }
   a.next_scalars = h->tc() ? 0 : 1;   // the tensor-core modes' prologue (step_prologue_kernel) forms them itself
-  int blocks = (int)((a.g_hi - a.g_lo + 255) / 256);   // one 4-element group per thread
-  if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-  if (blocks < 1) blocks = 1;
-  // (its last block also advances the step counters)
-  if (a.dp_world > 0) launch_k(apply_kernel<2>, blocks, 256, 0, c, a);
-  else if (a.nslabs > 0) launch_k(apply_kernel<1>, blocks, 256, 0, c, a);
-  else launch_k(apply_kernel<0>, blocks, 256, 0, c, a);
-  c.done();
-  c.check();
+  launch_apply(h, a, c);
 }
 
 // One whole update of the single-call steps: phase 1, phase 2 over `global_batch` rows, then (dp) the logged-sum exchange
@@ -1223,19 +1336,11 @@ static void enqueue_update(MlpHandle* h, const dsact_batch& bt, const dsact_nois
   enqueue_apply(h, c, &ta, dp);
 }
 
-// `images_only`: the caller is a fused tensor-core step, which reads obs / obs2 / act through their bf16 images alone
-static void enqueue_gather(MlpHandle* h, int B, const int64_t* idx, Ctx& c, bool images_only = false) {
-  const Arena& ar = h->ar;
-  float* W = h->W();
-  // no index list: every warp of the gather draws its row's index itself (the sequence index_kernel defines) and records it
-  int64_t* draw = idx ? nullptr : reinterpret_cast<int64_t*>(W + ar.idx);
-  int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-  launch_k(gather_kernel, blocks, 256, 0, c, h->rb.obs, h->rb.obs2, h->rb.act, h->rb.rew, h->rb.done, h->rb.logp, idx,
-                                          W + ar.obs, W + ar.obs2, W + ar.act, W + ar.rew, W + ar.done, W + ar.logp, B,
-                                          h->cfg.obs_dim, h->cfg.act_dim, img_out(h, ar.i_obs), img_out(h, ar.i_obs2), img_out(h, ar.i_act),
-                                          draw, (unsigned long long)h->seed, (const float*)h->buf.state, images_only ? 0 : 1);
-  c.done();
-  c.check();
+// the replay gather with the bf16 images of obs / obs2 / act.  `images_only`: the caller is a fused tensor-core step,
+// which reads them through their images alone
+static void enqueue_gather_imaged(MlpHandle* h, int B, const int64_t* idx, Ctx& c, bool images_only) {
+  const ImgOut img[3] = {img_out(h, h->ar.i_obs), img_out(h, h->ar.i_obs2), img_out(h, h->ar.i_act)};
+  enqueue_gather(h, B, idx, img, !images_only, c);
 }
 
 // ---- graph cache -------------------------------------------------------------
@@ -1315,15 +1420,6 @@ static bool take_arena_images(MlpHandle* h, const dsact_batch& bt) {
   // (The arena views handed out by dsact_replay_sample are read-only for the same reason: edits are not re-imaged.)
   if (!yes) h->arena_imaged = false;
   return yes;
-}
-
-static dsact_batch arena_batch(const MlpHandle* h, int32_t batch) {
-  float* W = h->W();
-  dsact_batch b;
-  b.obs = W + h->ar.obs; b.act = W + h->ar.act; b.rew = W + h->ar.rew; b.obs2 = W + h->ar.obs2; b.done = W + h->ar.done;
-  b.logp = W + h->ar.logp;
-  b.batch = batch;
-  return b;
 }
 
 static MlpHandle* mlp(dsact_handle* h) { return static_cast<MlpHandle*>(h); }
@@ -1439,6 +1535,8 @@ int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
   h->q.build(cfg->obs_dim + cfg->act_dim, cfg->hidden_q, cfg->n_hidden_q, 2);
   h->pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, 2 * cfg->act_dim);
   h->ar.build(*cfg, h->q, h->pi);
+  h->slot = h->ar;
+  h->hyper = StepHyper::of(*cfg);
   h->obs_elems = cfg->obs_dim; h->act_dim = cfg->act_dim; h->max_batch = cfg->max_batch;
   h->n_params = 2 * h->q.n + h->pi.n + 1;
   h->arena_imaged = false;
@@ -1530,9 +1628,8 @@ int dsact_grad_phase1(dsact_handle* h, const dsact_batch* batch, const dsact_noi
     const bool imaged = take_arena_images(m, bt);
     rc = run(m, s, make_key(K_PHASE1, &bt, np, imaged ? 1 : 0), [&](Ctx& c) { enqueue_phase1(m, bt, np, c, imaged); });
     if (rc == DSACT_OK) {  // (a replayed graph does not run enqueue_phase1, so record the noise pointers here as well)
-      m->pending_eps1 = np ? np->eps1 : m->W() + m->ar.eps1;
-      m->pending_z3 = np ? np->z3 : m->W() + m->ar.z3;
-      m->pending_z4 = np ? np->z4 : m->W() + m->ar.z4;
+      const dsact_noise n = step_noise(m, np);
+      m->pending_eps1 = n.eps1; m->pending_z3 = n.z3; m->pending_z4 = n.z4;
     }
   }
   if (rc) return rc;
@@ -1735,22 +1832,23 @@ int dsact_replay_sample(dsact_handle* h, int32_t batch, int64_t size, const int6
   const cudaStream_t s = (cudaStream_t)stream;
   int rc = sync_rb_size(h, size, s);
   if (rc) return rc;
+  ImgOut img[3] = {NO_IMG, NO_IMG, NO_IMG};
+  auto gather = [&](Ctx& c) {
+    enqueue_gather(h, batch, idx, img, true, c);
+    if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
+  };
   if (h->engine == ENGINE_HEADS) {
-    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_gather(heads(h), batch, idx, c); });
-    if (rc) return rc;
-    if (out) *out = cnn_arena_batch(heads(h), batch);
-    return DSACT_OK;
+    rc = run_eager(h, s, false, gather);
+  } else {
+    MlpHandle* m = mlp(h);
+    img[0] = img_out(m, m->ar.i_obs); img[1] = img_out(m, m->ar.i_obs2); img[2] = img_out(m, m->ar.i_act);
+    GraphKey key = make_key(K_SAMPLE, nullptr, nullptr, 0);
+    key.batch = batch; key.idx = idx;
+    rc = run(m, s, key, gather);
+    if (rc == DSACT_OK) m->arena_imaged = true;
   }
-  MlpHandle* m = mlp(h);
-  GraphKey key = make_key(K_SAMPLE, nullptr, nullptr, 0);
-  key.batch = batch; key.idx = idx;
-  rc = run(m, s, key, [&](Ctx& c) {
-    enqueue_gather(m, batch, idx, c);
-    if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, m->buf.state); c.done(); }
-  });
   if (rc) return rc;
-  m->arena_imaged = true;
-  if (out) *out = arena_batch(m, batch);
+  if (out) *out = arena_batch(h, batch);
   return DSACT_OK;
 }
 
@@ -1773,7 +1871,7 @@ int dsact_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const int64
   key.idx = idx;
   rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) {
     const bool forked = fork_prologue(h, bt, np, c, true);   // weight images, noise, clears: beside the gather
-    enqueue_gather(h, batch, idx, c, h->fused());
+    enqueue_gather_imaged(h, batch, idx, c, h->fused());
     if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
     enqueue_update(h, bt, np, batch, false, true, forked, c);  // device noise (np == null): phase1 advances the counter after the join
   });
@@ -1853,7 +1951,7 @@ int dsact_dp_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const in
   key.idx = idx;
   rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) {
     const bool forked = fork_prologue(h, bt, np, c, true);
-    enqueue_gather(h, batch, idx, c, h->fused());
+    enqueue_gather_imaged(h, batch, idx, c, h->fused());
     if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
     enqueue_update(h, bt, np, global_batch, true, true, forked, c);
   });

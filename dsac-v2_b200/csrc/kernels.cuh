@@ -1,6 +1,6 @@
 // Non-GEMM kernels of the DSAC-T update: tanh-Gaussian sampling, the fused
-// target/loss/gradient kernel, the policy-head gradient, Adam + Polyak, noise
-// and index generation, replay gather.  Formulas follow SURVEY.md Appendix A;
+// target/loss/gradient kernel (and DSAC_V1's), the policy-head gradient, Adam +
+// Polyak, noise and index generation, replay gather.  Formulas follow SURVEY.md Appendix A;
 // reference line numbers are given per kernel.
 #pragma once
 #include <cuda_bf16.h>
@@ -482,6 +482,68 @@ __global__ void loss_kernel(const __grid_constant__ LossArgs a) {
     atomicAdd(acc + ACC_LOGP, s[6]);
     atomicAdd(a.gbias_q[0], s[7]); atomicAdd(a.gbias_q_raw[0] ? a.gbias_q_raw[0] : a.gbias_q[0] + 1, s[8]);
     atomicAdd(a.gbias_q[1], s[9]); atomicAdd(a.gbias_q_raw[1] ? a.gbias_q_raw[1] : a.gbias_q[1] + 1, one[0]);
+  }
+}
+
+// The critic loss of DSAC_V1 (reference dsac_v1.py:56-273; SURVEY.md §8f rank 4), which has ONE distributional critic
+// and a fixed TD bound; it takes the place of loss_kernel in the head-wise engine's phase 2 (`dsact_cnn_config.algo = 1`).
+struct LossV1Args {
+  const float *rew, *done, *z, *logp2, *logp_new;
+  const float *out_q, *out_qt, *out_qa;   // Q(s,a), Q'(s',a'), Q(s,a~): [B,2] (mean, raw std)
+  float *d_out_q, *d_out_qa;              // dL/d(mean, raw std)
+  float *gbias_q, *gbias_q_raw;           // output-bias gradient (+=); raw: null = gbias_q + 1 (one two-output head)
+  float* state;
+  int B, bound;
+  float gamma, inv_global_batch, td_bound;
+  StepScalars sc;
+};
+
+// __compute_loss_q / __compute_target_q / __compute_loss_policy of dsac_v1.py:195-248, one thread per sample:
+//   target = r + (1-d) gamma (q' + clamp(z,-3,3) sigma' - alpha logp'),  target_b = q + clamp(target - q, -TD, TD)
+//   bound:  L = mean( -(target - q)/(sigma^2 + 0.1) q - ((q - target_b)^2 - sigma^2)/(sigma^3 + 0.1) sigma )   (coefficients detached)
+//   else:   L = mean( -log N(target; q, sigma) )
+//   actor:  L_pi = mean( alpha logp - q(s,a~) )
+__global__ void loss_v1_kernel(const __grid_constant__ LossV1Args a) {
+  pdl_sync();
+  __shared__ float red[6 * 32];
+  const float alpha = step_alpha(a.sc);
+  const float invB = a.inv_global_batch;
+  float s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // q, sigma, loss_pi, logp, gb_mean, gb_raw
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.B; i += gridDim.x * blockDim.x) {
+    const float qn = a.out_qt[2 * i], sn = softplus_f(a.out_qt[2 * i + 1]);
+    const float zc = fminf(fmaxf(a.z[i], -3.f), 3.f);
+    const float target = a.rew[i] + (1.f - a.done[i]) * a.gamma * ((qn + zc * sn) - alpha * a.logp2[i]);
+    const float q = a.out_q[2 * i], raw = a.out_q[2 * i + 1];
+    const float sd = softplus_f(raw);
+    float g_mean, g_sd;
+    if (a.bound) {
+      const float sdd = fmaxf(sd, 0.f);
+      const float tb = q + fminf(fmaxf(target - q, -a.td_bound), a.td_bound);
+      g_mean = -(target - q) / (sdd * sdd + 0.1f) * invB;
+      g_sd = -((q - tb) * (q - tb) - sdd * sdd) / (sdd * sdd * sdd + 0.1f) * invB;
+    } else {
+      const float d = target - q;
+      g_mean = -d / (sd * sd) * invB;
+      g_sd = (1.f / sd - d * d / (sd * sd * sd)) * invB;
+    }
+    const float dsoft = raw > 20.f ? 1.f : 1.f / (1.f + expf(-raw));
+    const float g_raw = g_sd * dsoft;
+    a.d_out_q[2 * i] = g_mean;
+    a.d_out_q[2 * i + 1] = g_raw;
+    const float lp = a.logp_new[i];
+    a.d_out_qa[2 * i] = -invB;
+    a.d_out_qa[2 * i + 1] = 0.f;
+    s[0] += q; s[1] += sd; s[2] += alpha * lp - a.out_qa[2 * i]; s[3] += lp; s[4] += g_mean; s[5] += g_raw;
+  }
+  block_sum<6>(s, red);
+  if (threadIdx.x == 0) {
+    float* acc = a.state + ST_ACC;
+    atomicAdd(acc + ACC_Q1, s[0]);
+    atomicAdd(acc + ACC_S1, s[1]);
+    atomicAdd(acc + ACC_LOSS_PI, s[2]);
+    atomicAdd(acc + ACC_LOGP, s[3]);
+    atomicAdd(a.gbias_q, s[4]);
+    atomicAdd(a.gbias_q_raw ? a.gbias_q_raw : a.gbias_q + 1, s[5]);
   }
 }
 
