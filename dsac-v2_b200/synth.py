@@ -27,6 +27,24 @@ CONFIGS = {
     "ragged": dict(obs_dim=11, act_dim=3, hidden=(40, 24, 72), act_lim=1.5),
 }
 
+# Critics and policy of different depths, widths and activations (`hidden_q` / `act_q` for the critics, `hidden_pi` /
+# `act_pi` for the policy), the way the reference's value_* / policy_* kwargs build them.  Kept out of CONFIGS, whose
+# entries size both networks from one `hidden`.  Widths that are multiples of 8 and at most 256 run the layer-chain kernel.
+ASYM_CONFIGS = {
+    # chain widths in all four 64-column blocks, off the 16- and 64-grids, an 8-wide bottleneck; obs_dim = 64 puts the
+    # critic's action segment at the start of a k-block; six critic layers, a one-layer policy
+    "asym": dict(obs_dim=64, act_dim=5, hidden_q=(152, 104, 8, 192, 256, 72), act_q="elu", hidden_pi=(136,), act_pi="tanh",
+                 act_lim=1.0),
+    # the policy deeper than the critics; its 2A = 192 output and a 96-column action segment over two k-blocks
+    "deep_pi": dict(obs_dim=13, act_dim=96, hidden_q=(200,), act_q="selu", hidden_pi=(256, 24, 128, 200, 64, 248),
+                    act_pi="gelu", act_lim=1.0),
+    # widths the chain kernel does not take: the per-layer path, with pi.L > q.L and with q.L > pi.L
+    "layered_pi": dict(obs_dim=7, act_dim=3, hidden_q=(300, 40), act_q="relu", hidden_pi=(48, 48, 48, 48), act_pi="sigmoid",
+                       act_lim=1.0),
+    "layered_q": dict(obs_dim=9, act_dim=2, hidden_q=(45, 40, 40, 40, 40, 40), act_q="tanh", hidden_pi=(520,), act_pi="gelu",
+                      act_lim=1.0),
+}
+
 # BASELINE.json config 5 (gym_carracingraw, SURVEY.md §8f rank 1): conv encoder `type_2` + separate mean / log_std
 # heads (csrc/cnn_engine.cuh; oracle/dsact_oracle.py:OracleDSACTCNN, tests/golden/cnn_carracing_b4.npz).
 CNN_CONFIGS = {
@@ -62,10 +80,28 @@ def _rng(*key) -> np.random.Generator:
     return np.random.default_rng([int(k) for k in key])
 
 
-def net_shapes(obs_dim, act_dim, hidden):
-    """(q_sizes, pi_sizes) layer-size lists, reference networks/mlp.py:58,116."""
-    q = [obs_dim + act_dim] + list(hidden) + [2]
-    pi = [obs_dim] + list(hidden) + [2 * act_dim]
+def mlp_config(name: str) -> dict:
+    """A named MLP configuration of CONFIGS or ASYM_CONFIGS."""
+    return CONFIGS[name] if name in CONFIGS else ASYM_CONFIGS[name]
+
+
+def hidden_sizes(cfg: dict) -> tuple:
+    """(hidden_q, hidden_pi): the critics' and the policy's hidden widths of a CONFIGS or ASYM_CONFIGS entry."""
+    if "hidden" in cfg:
+        return tuple(cfg["hidden"]), tuple(cfg["hidden"])
+    return tuple(cfg["hidden_q"]), tuple(cfg["hidden_pi"])
+
+
+def activations(cfg: dict) -> tuple:
+    """(act_q, act_pi): the critics' and the policy's hidden activations (the reference's default GELU unless given)."""
+    return cfg.get("act_q", "gelu"), cfg.get("act_pi", "gelu")
+
+
+def net_shapes(obs_dim, act_dim, hidden_q, hidden_pi=None):
+    """(q_sizes, pi_sizes) layer-size lists, reference networks/mlp.py:58,116; the policy takes the critics' hidden
+    widths unless `hidden_pi` is given."""
+    q = [obs_dim + act_dim] + list(hidden_q) + [2]
+    pi = [obs_dim] + list(hidden_q if hidden_pi is None else hidden_pi) + [2 * act_dim]
     return q, pi
 
 
@@ -75,7 +111,7 @@ def make_weights(cfg: dict, seed: int = 0) -> dict:
     U(-1/sqrt(fan_in), 1/sqrt(fan_in)) like nn.Linear's default init; keys use
     the reference's schema (`q1.q.{0,2,..}.weight`, `policy.policy.{0,2,..}.bias`).
     """
-    q_sizes, pi_sizes = net_shapes(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"])
+    q_sizes, pi_sizes = net_shapes(cfg["obs_dim"], cfg["act_dim"], *hidden_sizes(cfg))
     out = {}
     for n, (name, inner, sizes) in enumerate(
         (("q1", "q", q_sizes), ("q2", "q", q_sizes), ("policy", "policy", pi_sizes))
@@ -122,6 +158,8 @@ def reference_kwargs(cfg: dict, **over) -> dict:
     """The kwargs dict the reference threads through DSAC_V2 / ApproxContainer
     (what example_train/main.py + utils/init_args.py would have produced)."""
     lim = np.full(cfg["act_dim"], cfg["act_lim"], dtype=np.float32)
+    hidden_q, hidden_pi = hidden_sizes(cfg)
+    act_q, act_pi = activations(cfg)
     kw = dict(
         algorithm="DSAC_V2",
         obsv_dim=cfg["obs_dim"],
@@ -131,14 +169,14 @@ def reference_kwargs(cfg: dict, **over) -> dict:
         action_low_limit=-lim,
         value_func_name="ActionValueDistri",
         value_func_type="MLP",
-        value_hidden_sizes=list(cfg["hidden"]),
-        value_hidden_activation="gelu",
+        value_hidden_sizes=list(hidden_q),
+        value_hidden_activation=act_q,
         value_output_activation="linear",
         policy_func_name="StochaPolicy",
         policy_func_type="MLP",
         policy_act_distribution="TanhGaussDistribution",
-        policy_hidden_sizes=list(cfg["hidden"]),
-        policy_hidden_activation="gelu",
+        policy_hidden_sizes=list(hidden_pi),
+        policy_hidden_activation=act_pi,
         policy_output_activation="linear",
         cnn_shared=False,
     )

@@ -91,10 +91,13 @@ class OracleDSACT:
                  delay_update=2, auto_alpha=True, alpha=0.2, value_learning_rate=1e-4,
                  policy_learning_rate=1e-4, alpha_learning_rate=3e-4,
                  policy_min_log_std=-20.0, policy_max_log_std=0.5, hidden_activation="gelu",
+                 value_hidden_activation=None, policy_hidden_activation=None,
                  policy_act_distribution="TanhGaussDistribution", dtype=torch.float32, **_ignored):
         self.O, self.A = int(obs_dim), int(act_dim)
         self.dtype = dtype
-        self.act = hidden_activation
+        # critics / policy: the reference's value_* / policy_* kwargs, else `hidden_activation` for both networks
+        self.act_q = value_hidden_activation or hidden_activation
+        self.act_pi = policy_hidden_activation or hidden_activation
         assert policy_act_distribution in ("TanhGaussDistribution", "GaussDistribution")
         self.gauss_only = policy_act_distribution == "GaussDistribution"   # utils/act_distribution_cls.py:82-116
         self.gamma, self.tau = float(gamma), float(tau)
@@ -155,13 +158,13 @@ class OracleDSACT:
     # ---- network pieces -------------------------------------------------
     def policy_logits(self, layers, obs):
         """StochaPolicy.forward, std_type='mlp_shared' (networks/mlp.py:85-100)."""
-        out = mlp_forward(layers, obs, self.act)
+        out = mlp_forward(layers, obs, self.act_pi)
         mean, log_std = torch.chunk(out, 2, dim=-1)
         return mean, torch.clamp(log_std, self.min_log_std, self.max_log_std).exp()
 
     def q_dist(self, layers, obs, act):
         """ActionValueDistri.forward (networks/mlp.py:122-127): mean, softplus(std)."""
-        out = mlp_forward(layers, torch.cat([obs, act], dim=-1), self.act)
+        out = mlp_forward(layers, torch.cat([obs, act], dim=-1), self.act_q)
         return out[..., 0], F.softplus(out[..., 1])
 
     def tanh_gauss_rsample(self, mean, std, eps):
@@ -355,7 +358,7 @@ class OracleDSACTStd(OracleDSACT):
             while f"{name}.{2 * j}.weight" in w:
                 ls += [w[f"{name}.{2 * j}.weight"], w[f"{name}.{2 * j}.bias"]]
                 j += 1
-            return mlp_forward(ls, obs, self.act)
+            return mlp_forward(ls, obs, self.act_pi)
 
         mean = head("mean")
         log_std = head("log_std") if self.std_type == "mlp_separated" else w["log_std"] + torch.zeros_like(mean)
@@ -417,24 +420,25 @@ class OracleDSACTCNN(OracleDSACT):
             j += 1
         return x.reshape(x.shape[0], -1)     # img.view(img.size(0), -1), networks/cnn.py:234-235
 
-    def _head(self, w, head, x):
+    def _head(self, w, head, x, act):
         layers, j = [], 0
         while f"{head}.{2 * j}.weight" in w:
             layers += [w[f"{head}.{2 * j}.weight"], w[f"{head}.{2 * j}.bias"]]
             j += 1
-        return mlp_forward(layers, x, self.act)
+        return mlp_forward(layers, x, act)
 
     def policy_logits(self, layers, obs):
         """StochaPolicy.forward (networks/cnn.py:233-240): mean head, exp(clamp(log_std head))."""
         w = dict(zip(self.names["policy"], layers))
         f = self._features(w, obs)
-        return self._head(w, "mean", f), torch.clamp(self._head(w, "log_std", f), self.min_log_std, self.max_log_std).exp()
+        return self._head(w, "mean", f, self.act_pi), \
+            torch.clamp(self._head(w, "log_std", f, self.act_pi), self.min_log_std, self.max_log_std).exp()
 
     def q_dist(self, layers, obs, act):
         """ActionValueDistri.forward (networks/cnn.py:454-461): heads on cat(feature, act); softplus on the std head."""
         w = dict(zip(self.names["q1"], layers))
         f = torch.cat([self._features(w, obs), act], dim=-1)
-        return self._head(w, "mean", f)[..., 0], F.softplus(self._head(w, "log_std", f)[..., 0])
+        return self._head(w, "mean", f, self.act_q)[..., 0], F.softplus(self._head(w, "log_std", f, self.act_q)[..., 0])
 
     def state_dict(self):
         out = {"log_alpha": self.log_alpha.detach()}
@@ -470,10 +474,15 @@ def cnn_from_config(cfg: dict, weights: dict, **hyper) -> OracleDSACTCNN:
 
 
 def from_config(cfg: dict, weights: dict, **hyper) -> OracleDSACT:
-    """Build from a `synth.CONFIGS` entry (+ `synth.HYPER`-style overrides)."""
+    """Build from a `synth.CONFIGS` or `synth.ASYM_CONFIGS` entry (+ `synth.HYPER`-style overrides).  The networks'
+    activations are the config's unless the overrides name `hidden_activation` (both networks) or the reference's
+    `value_hidden_activation` / `policy_hidden_activation`."""
+    from dsac_v2_b200.synth import activations, hidden_sizes
     lim = [cfg["act_lim"]] * cfg["act_dim"]
-    return OracleDSACT(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"], cfg["hidden"], lim,
-                       [-x for x in lim], weights, **hyper)
+    if "hidden_activation" not in hyper:
+        act_q, act_pi = activations(cfg)
+        hyper = dict(dict(value_hidden_activation=act_q, policy_hidden_activation=act_pi), **hyper)
+    return OracleDSACT(cfg["obs_dim"], cfg["act_dim"], *hidden_sizes(cfg), lim, [-x for x in lim], weights, **hyper)
 
 
 # ---- DSAC_V1 (reference dsac_v1.py; SURVEY.md §8f rank 4): one critic, fixed TD bound ---------------------------------

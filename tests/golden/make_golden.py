@@ -63,6 +63,10 @@ CASES = [
     (f"{cfg}_{act}", cfg, batch, 10, (10,), {"value_hidden_activation": act, "policy_hidden_activation": act})
     for cfg, batch, act in (("tiny", 16, "relu"), ("tiny", 33, "tanh"), ("ragged", 19, "elu"), ("ragged", 37, "selu"),
                             ("tiny", 8, "sigmoid"))
+] + [
+    # critics and policy of different depths, widths and activations (synth.ASYM_CONFIGS): two row tiles of 64, the last
+    # ragged; the full state only for the smallest
+    (f"{cfg}_b70", cfg, 70, 10, (1,) if cfg == "layered_q" else (), {}) for cfg in synth.ASYM_CONFIGS
 ]
 
 V1_TB_KEYS = ["DSAC/critic_avg_q-RL iter", "DSAC/critic_avg_std-RL iter", "Loss/Actor loss-RL iter", "DSAC/policy_mean-RL iter",
@@ -127,7 +131,7 @@ def digest(t) -> np.ndarray:
 
 def run_case(name, cfg_name, batch, steps, snaps, over):
     cnn = cfg_name in synth.CNN_CONFIGS   # BASELINE config 5: conv encoder + separate heads (networks/cnn.py)
-    cfg = synth.CNN_CONFIGS[cfg_name] if cnn else synth.CONFIGS[cfg_name]
+    cfg = synth.CNN_CONFIGS[cfg_name] if cnn else synth.mlp_config(cfg_name)
     torch.manual_seed(0)
     v1 = over.get("algorithm") == "DSAC_V1"
     tb_keys = V1_TB_KEYS if v1 else TB_KEYS

@@ -31,12 +31,15 @@ def test_struct_sizes_match_header_layout():
     assert C.sizeof(_lib.Layout) == 14 * 8
 
 
-@pytest.mark.parametrize("name", list(synth.CONFIGS))
+MLP_CONFIGS = list(synth.CONFIGS) + list(synth.ASYM_CONFIGS)
+
+
+@pytest.mark.parametrize("name", MLP_CONFIGS)
 def test_layout_matches_network_shapes(name):
-    cfg = synth.CONFIGS[name]
-    q, pi = synth.net_shapes(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"])
+    cfg = synth.mlp_config(name)
+    q, pi = synth.net_shapes(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg))
     count = lambda s: sum(s[j] * s[j + 1] + s[j + 1] for j in range(len(s) - 1))
-    lay = query_layout(make_config(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"], cfg["hidden"], max_batch=256))
+    lay = query_layout(make_config(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), max_batch=256))
     assert lay.n_q == count(q) and lay.n_pi == count(pi)
     assert lay.n_params == 2 * count(q) + count(pi) + 1
     assert lay.n_targets == lay.n_params - 1
@@ -89,11 +92,11 @@ def _check_slots(lay, act_dim, slabs):
 
 
 @pytest.mark.parametrize("mode", list(_lib.GEMM_MODES))
-@pytest.mark.parametrize("name", list(synth.CONFIGS))
+@pytest.mark.parametrize("name", MLP_CONFIGS)
 def test_reported_workspace_slots(name, mode):
-    cfg = synth.CONFIGS[name]
+    cfg = synth.mlp_config(name)
     for mb in (1, 256, 1000):
-        lay = query_layout(make_config(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"], cfg["hidden"], max_batch=mb, gemm_mode=mode))
+        lay = query_layout(make_config(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), max_batch=mb, gemm_mode=mode))
         _check_slots(lay, cfg["act_dim"], mode != "fp32")
 
 

@@ -25,9 +25,20 @@ def build_alg(cfg, batch, **over):
 def test_local_update_same_seed_as_reference_rng_order():
     """dsact_noise='reference': the 8 normal draws come from torch's CPU generator in the reference's
     order (SURVEY Appendix B), so an oracle consuming the same stream must agree step for step."""
+    check_local_update_against_oracle(synth.CONFIGS["halfcheetah"], 64)
+
+
+@pytest.mark.parametrize("name,gemm", [("asym", "bf16x3"), ("layered_pi", "fp32")])
+def test_local_update_with_different_critic_and_policy_networks(name, gemm):
+    """value_hidden_sizes / value_hidden_activation differ from the policy_* ones: the fused layer chain (asym) and the
+    per-layer path (layered_pi) against the oracle of the same configuration.  layered_pi runs in fp32: its ReLU critic
+    has weight-gradient entries near zero, whose first Adam steps (about lr * sign) bf16x3 rounding can flip."""
+    check_local_update_against_oracle(synth.ASYM_CONFIGS[name], 70, dsact_gemm=gemm)
+
+
+def check_local_update_against_oracle(cfg, B, **over):
     from oracle.dsact_oracle import TB_KEYS, from_config
-    cfg, B = synth.CONFIGS["halfcheetah"], 64
-    alg, _ = build_alg(cfg, B, dsact_noise="reference")
+    alg, _ = build_alg(cfg, B, dsact_noise="reference", **over)
     alg.networks.cuda()
     orc = from_config(cfg, synth.make_weights(cfg), **synth.HYPER)
     A = cfg["act_dim"]

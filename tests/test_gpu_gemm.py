@@ -21,7 +21,9 @@ def eng(request):
 
 
 SHAPES = [(1, 1, 1), (16, 32, 7), (37, 40, 14), (64, 64, 64), (100, 34, 256), (256, 256, 376), (300, 2, 256),
-          (1000, 256, 17), (4096, 256, 256), (129, 257, 31)]
+          (1000, 256, 17), (4096, 256, 256), (129, 257, 31),
+          # N or K in 129..192: the three-block (192-column) accumulator of the tensor-core kernels
+          (70, 150, 129), (200, 192, 160), (64, 129, 192)]
 
 
 def _ref(a, b):

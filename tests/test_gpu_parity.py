@@ -19,7 +19,7 @@ RTOL = 1e-4
 def load(golden_dir, name):
     z = np.load(os.path.join(golden_dir, name + ".npz"))
     cfg_name, batch, steps, over = z["meta"]
-    return z, synth.CONFIGS[str(cfg_name)], int(batch), int(steps), dict(ast.literal_eval(str(over)))
+    return z, synth.mlp_config(str(cfg_name)), int(batch), int(steps), dict(ast.literal_eval(str(over)))
 
 
 def make_engine(cfg, batch, over=None, **kw):
@@ -28,10 +28,10 @@ def make_engine(cfg, batch, over=None, **kw):
     hyper.update(over or {})
     if "policy_act_distribution" in hyper:   # golden of the plain Gaussian action distribution
         kw.setdefault("act_dist", hyper.pop("policy_act_distribution"))
-    if "value_hidden_activation" in hyper:   # goldens of the reference's other activations
-        kw.setdefault("act_q", hyper.pop("value_hidden_activation"))
-        kw.setdefault("act_pi", hyper.pop("policy_hidden_activation"))
-    c = make_config(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"], cfg["hidden"], max_batch=batch,
+    act_q, act_pi = synth.activations(cfg)   # goldens of the reference's other activations override the config's
+    kw.setdefault("act_q", hyper.pop("value_hidden_activation", act_q))
+    kw.setdefault("act_pi", hyper.pop("policy_hidden_activation", act_pi))
+    c = make_config(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), max_batch=batch,
                     gamma=hyper["gamma"], tau=hyper["tau"], tau_b=hyper.get("tau_b"), delay_update=hyper["delay_update"],
                     auto_alpha=hyper["auto_alpha"], alpha=hyper["alpha"], lr_q=hyper["value_learning_rate"],
                     lr_pi=hyper["policy_learning_rate"], lr_alpha=hyper["alpha_learning_rate"],
@@ -54,8 +54,10 @@ def stats_vec(eng):
     return np.array([s[k] for k in STAT_KEYS])
 
 
+# critics and policy of different depths, widths and activations (synth.ASYM_CONFIGS)
+ASYM_CASES = ["asym_b70", "deep_pi_b70", "layered_pi_b70", "layered_q_b70"]
 CASES = ["tiny_b16", "ragged_b37", "tiny_fixed_alpha", "pendulum_b256", "halfcheetah_b512", "humanoid_b256",
-         "humanoid_b4096", "tiny_relu", "tiny_tanh", "ragged_elu", "ragged_selu", "tiny_sigmoid", "tiny_gauss"]
+         "humanoid_b4096", "tiny_relu", "tiny_tanh", "ragged_elu", "ragged_selu", "tiny_sigmoid", "tiny_gauss"] + ASYM_CASES
 
 
 @pytest.mark.parametrize("use_graph", [False, True])
@@ -164,7 +166,7 @@ def test_device_noise_statistics():
 # ---- tensor-core (wgmma) paths -------------------------------------------------------------------------------------
 TC_CASES = ["tiny_b16", "ragged_b37", "halfcheetah_b512", "humanoid_b256", "humanoid_b4096",
             # the generic-activation branch of the fused chain epilogue (GELU and ReLU have their own)
-            "tiny_relu", "tiny_tanh", "ragged_elu", "ragged_selu", "tiny_sigmoid", "tiny_gauss"]
+            "tiny_relu", "tiny_tanh", "ragged_elu", "ragged_selu", "tiny_sigmoid", "tiny_gauss"] + ASYM_CASES
 
 
 @pytest.mark.parametrize("name", TC_CASES)

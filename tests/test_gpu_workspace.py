@@ -15,7 +15,9 @@ pytestmark = pytest.mark.gpu
 
 POISONS = [float("nan"), 1e30, -1e30]
 SHAPES = {"tiny": (synth.CONFIGS["tiny"], 16), "ragged": (synth.CONFIGS["ragged"], 37),
-          "humanoid": (synth.CONFIGS["humanoid"], 100), "wide": (WIDE, 40)}
+          "humanoid": (synth.CONFIGS["humanoid"], 100), "wide": (WIDE, 40),
+          # critics and policy of different shapes: arena slots sized from the wrong network read unwritten memory
+          "asym": (synth.ASYM_CONFIGS["asym"], 70), "layered_q": (synth.ASYM_CONFIGS["layered_q"], 70)}
 STATE = ("params", "targets", "adam_m", "adam_v")
 
 

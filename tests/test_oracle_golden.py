@@ -17,14 +17,16 @@ CASES = ["tiny_b16", "ragged_b37", "tiny_fixed_alpha", "pendulum_b256", "halfche
          # the policy's other std types (oracle-level groundwork for SURVEY.md 8f rank 4)
          "tiny_std_separated", "tiny_std_parameter",
          # CNN approximators (BASELINE config 5; oracle-level groundwork for SURVEY.md 8f rank 1)
-         "cnn_carracing_b4", "cnn_type1_b5", "v1_tiny_b16", "v1_ragged_tight", "v1_tiny_nll"]
+         "cnn_carracing_b4", "cnn_type1_b5", "v1_tiny_b16", "v1_ragged_tight", "v1_tiny_nll",
+         # critics and policy of different depths, widths and activations (synth.ASYM_CONFIGS)
+         "asym_b70", "deep_pi_b70", "layered_pi_b70", "layered_q_b70"]
 MAX_STEPS = {"humanoid_b256": 100, "pendulum_b256": 100}
 
 
 def load(golden_dir, name):
     z = np.load(os.path.join(golden_dir, name + ".npz"))
     cfg_name, batch, steps, over = z["meta"]
-    cfg = synth.CNN_CONFIGS[str(cfg_name)] if str(cfg_name) in synth.CNN_CONFIGS else synth.CONFIGS[str(cfg_name)]
+    cfg = synth.CNN_CONFIGS[str(cfg_name)] if str(cfg_name) in synth.CNN_CONFIGS else synth.mlp_config(str(cfg_name))
     return z, cfg, int(batch), int(steps), dict(ast.literal_eval(str(over)))
 
 
@@ -38,18 +40,16 @@ def test_oracle_matches_reference(golden_dir, name):
     hyper = dict(synth.HYPER)
     hyper.update(over)
     hyper.pop("algorithm", None)
-    act = hyper.pop("value_hidden_activation", "gelu")
-    assert hyper.pop("policy_hidden_activation", act) == act
     cnn = "conv_type" in cfg
     std_type = hyper.pop("policy_std_type", "mlp_shared")
     if v1:
-        orc = v1_from_config(cfg, synth.make_weights_v1(cfg), hidden_activation=act, **hyper)
+        orc = v1_from_config(cfg, synth.make_weights_v1(cfg), **hyper)
     elif std_type != "mlp_shared":
-        orc = std_from_config(cfg, synth.make_weights_std(cfg, std_type), std_type, hidden_activation=act, **hyper)
+        orc = std_from_config(cfg, synth.make_weights_std(cfg, std_type), std_type, **hyper)
     elif cnn:
-        orc = cnn_from_config(cfg, synth.make_cnn_weights(cfg), hidden_activation=act, **hyper)
+        orc = cnn_from_config(cfg, synth.make_cnn_weights(cfg), **hyper)
     else:
-        orc = from_config(cfg, synth.make_weights(cfg), hidden_activation=act, **hyper)
+        orc = from_config(cfg, synth.make_weights(cfg), **hyper)
     make_batch = synth.make_cnn_batch if cnn else synth.make_batch
     names = [str(n) for n in z["param_names"]]
     trainable = [str(n) for n in z["trainable_names"]]
