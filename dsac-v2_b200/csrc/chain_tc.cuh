@@ -8,12 +8,16 @@
 // 128-byte-swizzled K-major layout wgmma reads, into the operand buffer, so hidden activations never leave the SM
 // unless the backward pass needs them (act' for the dgrad chain, images for wgrad).
 // The weight tiles of layer j+1 are prefetched by the TMA warp while the epilogue of layer j runs.  The MMAs of a k-block
-// issue back to back and one k-block stays in flight while the next is issued; the layer width (64, 128, 192 or 256) is
-// a compile-time parameter of each layer's body, dispatched once per layer.
+// issue back to back and one k-block stays in flight while the next is issued; each warpgroup's share of the layer width
+// (64 or 128 columns) is a compile-time parameter of its layer body, dispatched once per layer.
 //
 // Shared memory: [ B ring: stages x planes x stage_b ][ operand buffer: planes x 4 k-blocks x 8 KiB (layer 0: its A
 // ring) ][ 16-float scratch row per MMA thread ][ barriers ].
-// Roles: warps 0..3 the MMA warpgroup (wgmma, accumulator in registers, epilogue), warp 4 TMA producer.
+// Roles: warps 0..7 two MMA warpgroups (wgmma, accumulator in registers, epilogue), warp 8 TMA producer (warps 9..11
+// only complete its warpgroup, see CH_MMA_REGS).  Of a layer's nb = ceil(bn / 64) column blocks, warpgroup 0 takes the
+// first ceil(nb / 2) and warpgroup 1 the rest (256 = 128 + 128, 192 = 128 + 64, 64 = 64 + 0): both read the same A
+// operand and their own columns of the same B stage.  The epilogue is bound by instruction issue and latency, so two
+// warps per scheduler with half the values each finish it sooner than one warp with all of them.
 #pragma once
 #include "gemm_tc.cuh"
 
@@ -23,6 +27,19 @@ constexpr int CH_MAX_LAYERS = DSACT_MAX_HIDDEN + 1;
 constexpr int CH_MAX_PASSES = 4;
 constexpr int CH_KB_MAX = 4;                              // 256 columns of operand = 4 k-blocks of 64
 constexpr int CH_OPND_PLANE = CH_KB_MAX * TC_STAGE_A;     // 32 KiB
+constexpr int CH_MMA_THREADS = 2 * TC_MMA_THREADS;        // two MMA / epilogue warpgroups
+constexpr int CH_THREADS = CH_MMA_THREADS + TC_MMA_THREADS;   // + the producer warpgroup (warp 8 issues the TMA)
+constexpr int CH_SCRATCH = CH_MMA_THREADS * 16 * 4;       // per-thread 16-float rows for the generic activations
+// Registers per thread after the role split (setmaxnreg works on whole warpgroups, hence a whole producer warpgroup).
+// At launch 384 threads get 168 each (each SM sub-partition holds one warp of each warpgroup: 3 x 168 <= 512); the
+// epilogue of a 128-column accumulator spills at 168, so the producer gives its registers to the MMA warpgroups:
+// 40 + 232 + 232 = 504.
+constexpr int CH_PRODUCER_REGS = 40;
+constexpr int CH_MMA_REGS = 232;
+// Groups of 16 epilogue values whose global inputs (act' or bias) are loaded ahead of the one being computed; the first
+// CH_PF are loaded before the layer's MMAs retire.  3 of the 4 groups of a 128-column accumulator: with all 4 in flight
+// the bf16x3 kernels spill at 232 registers, with 3 none of the kernels spills.
+constexpr int CH_PF = 3;
 
 struct ChainLayer {
   CUtensorMap mapB;          // weight image; forward: K-major (box = bn rows), dgrad: MN-major (box = 64 x 64)
@@ -53,20 +70,30 @@ struct ChainGroup {
 };
 
 inline int chain_smem_bytes(int stages, int planes, int stage_b) {
-  return stages * planes * stage_b + planes * CH_OPND_PLANE + TC_SCRATCH + 2 * stages * 8 + 1024;
+  return stages * planes * stage_b + planes * CH_OPND_PLANE + CH_SCRATCH + 2 * stages * 8 + 1024;
 }
 
-// One layer on the MMA warpgroup, 64 x (64 NB) outputs: the MMAs with one k-block in flight (the ring slot of k-block kb is
-// released once kb + 1 has been issued and kb has retired), the epilogue on the accumulator registers, and the next
-// layer's A operand.  (stage, phase) is the consumer's position in the B ring, carried from layer to layer.
+// Both MMA warpgroups: the operand buffer is read by all of them and rewritten between layers.
+__device__ __forceinline__ void ch_bar() { asm volatile("bar.sync 1, %0;" ::"n"(CH_MMA_THREADS) : "memory"); }
+
+// One layer on one MMA warpgroup, 64 x (64 NB) outputs from column n0: the loads of the epilogue's global inputs, the MMAs
+// with one k-block in flight (the ring slot of k-block kb is released once kb + 1 has been issued and kb has retired), the
+// epilogue on the accumulator registers, and this warpgroup's columns of the next layer's A operand.  (stage, phase) is
+// the consumer's position in the B ring, carried from layer to layer.
 template <bool PLANES2, bool B_MN, int NB>
-__device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass& P, int j, uint8_t* ringB, uint8_t* opnd,
-                                            float* row, int stages, int stage_b, uint64_t* full, uint64_t* empty, int m0,
-                                            int& stage, uint32_t& phase) {
+__device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass& P, int j, int n0, uint8_t* ringB,
+                                            uint8_t* opnd, float* row, int stages, int stage_b, uint64_t* full,
+                                            uint64_t* empty, int m0, int& stage, uint32_t& phase) {
   constexpr int planes = PLANES2 ? 2 : 1;
   const ChainLayer& Lj = P.L[j];
-  const int lane = threadIdx.x & 31, r_lo = (threadIdx.x >> 5) * 16 + (lane >> 2);   // this thread's rows r_lo, r_lo + 8
+  const int lane = threadIdx.x & 31;
+  const int r_lo = ((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16 + (lane >> 2);   // this thread's rows r_lo, r_lo + 8
   const int nkb = Lj.kblocks[0] + Lj.kblocks[1];
+  EpiArgs E;
+  E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.N; E.ldz = Lj.N;
+  E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
+  E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
+  float in[2 * NB][16];   // act'(z) (dgrad) or the bias (forward) of this thread's values
   float acc[128];
 #pragma unroll
   for (int i = 0; i < 32 * NB; ++i) acc[i] = 0.f;
@@ -74,7 +101,8 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
   for (int kb = 0; kb < nkb; ++kb) {
     mbar_wait(&full[stage], phase);
     if (j == 0 && kb == 0 && threadIdx.x == 0) TC_STAMP(2);
-    const uint32_t sB = smem_u32(ringB + (size_t)stage * planes * stage_b);
+    // this warpgroup's columns of the stage: K-major rows of 128 B, MN-major 64-column boxes of 8 KiB (1024-byte aligned)
+    const uint32_t sB = smem_u32(ringB + (size_t)stage * planes * stage_b) + (uint32_t)(B_MN ? n0 / 64 * 8192 : n0 * 128);
     // layer 0: the ring slot of this stage; later layers: k-block kb of the operand buffer
     const uint32_t sA = smem_u32(opnd) + (uint32_t)(j == 0 ? stage * planes * TC_STAGE_A : kb * TC_STAGE_A);
     const uint32_t a_plane = j == 0 ? TC_STAGE_A : CH_OPND_PLANE;
@@ -96,22 +124,30 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
     prev = stage;
     if (++stage == stages) { stage = 0; phase ^= 1; }
   }
+  // The first groups' inputs load under the last k-block's MMAs, so their latency is off the epilogue's path.
+#pragma unroll
+  for (int q = 0; q < CH_PF && q < 2 * NB; ++q) epi_in(in[q], E, m0, n0, q);
   wg_wait<0>();
   if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
   if (threadIdx.x == 0) TC_STAMP(8 + 3 * j);   // MMAs of layer j retired
-  EpiArgs E;
-  E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.N; E.ldz = Lj.N;
-  E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
-  E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
-  epi_frag<PLANES2, NB>(acc, E, m0, 0, row);
+#pragma unroll
+  for (int q = 0; q < 2 * NB; ++q) {
+    if (q + CH_PF < 2 * NB) epi_in(in[q + CH_PF], E, m0, n0, q + CH_PF);
+    float v[16];
+#pragma unroll
+    for (int t = 0; t < 16; ++t) v[t] = acc[16 * q + t];
+    epi_group<PLANES2>(v, in[q], E, m0, n0, q, row);
+#pragma unroll
+    for (int t = 0; t < 16; ++t) acc[16 * q + t] = v[t];
+  }
   if (threadIdx.x == 0) TC_STAMP(9 + 3 * j);
   if (j + 1 < P.n_layers) {
     // next layer's A operand: bf16 hi/lo pairs at (row, column) of the swizzled K-major k-block tiles
-    // (16-byte chunk index ^= row & 7).  Every warp's MMAs of this layer have retired before anyone overwrites.
-    wg_bar();
+    // (16-byte chunk index ^= row & 7).  Both warpgroups' MMAs of this layer have retired before anyone overwrites.
+    ch_bar();
 #pragma unroll
     for (int i = 0; i < 8 * NB; ++i) {
-      const int c = 8 * i + 2 * (lane & 3), cc = c & 63;
+      const int c = n0 + 8 * i + 2 * (lane & 3), cc = c & 63;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r_lo + 8 * h;
@@ -123,24 +159,38 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
       }
     }
     fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads
-    wg_bar();
+    ch_bar();
   }
   if (threadIdx.x == 0) TC_STAMP(10 + 3 * j);
 }
 
+// A warpgroup with no columns in layer j (a layer of 64 columns) still consumes the layer's ring slots, so that the ring
+// protocol does not depend on the layer width, and meets the other warpgroup at the operand barriers.
+__device__ __forceinline__ void chain_idle(const ChainPass& P, int j, int stages, uint64_t* full, uint64_t* empty, int& stage,
+                                           uint32_t& phase) {
+  const int nkb = P.L[j].kblocks[0] + P.L[j].kblocks[1];
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait(&full[stage], phase);
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[stage]);
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+  if (j + 1 < P.n_layers) { ch_bar(); ch_bar(); }
+}
+
 // B_MN: the weight tiles are MN-major (dgrad chains); forward chains read them K-major.
 template <bool PLANES2, bool B_MN>
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_constant__ ChainGroup g, int stages, int stage_b) {
+__global__ void __launch_bounds__(CH_THREADS, 1) tc_chain_kernel(const __grid_constant__ ChainGroup g, int stages, int stage_b) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // keeps the shared address space (LDS/STS)
   constexpr int planes = PLANES2 ? 2 : 1;
   uint8_t* ringB = smem;
   uint8_t* opnd = smem + (size_t)stages * planes * stage_b;   // stages * planes <= 4 * planes: layer 0's A ring fits
   float* scratch = reinterpret_cast<float*>(opnd + planes * CH_OPND_PLANE);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(scratch) + TC_SCRATCH);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(scratch) + CH_SCRATCH);
   uint64_t* full = bars;               // [stages] TMA -> MMA
-  uint64_t* empty = bars + stages;     // [stages] MMA -> TMA (one arrival per MMA warp)
+  uint64_t* empty = bars + stages;     // [stages] MMA -> TMA (one arrival per MMA warp of both warpgroups)
 
+  constexpr int PRODUCER = CH_MMA_THREADS / 32;   // warp 8
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) TC_STAMP(0);
 
@@ -153,10 +203,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_co
   const int nl = P.n_layers;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], TC_MMA_THREADS / 32); }
+    for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CH_MMA_THREADS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {   // descriptor prefetch: every tensor map this CTA will use (kernel parameters: no dependency on the
+  if (warp == PRODUCER) {   // descriptor prefetch: every tensor map this CTA will use (kernel parameters: no dependency on the
                      // preceding kernel)
     for (int i = lane; i < 2 + nl; i += 32) {
       const CUtensorMap* m = nullptr;
@@ -171,9 +221,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_co
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (threadIdx.x == 0) TC_STAMP(1);
 
-  if (warp == 4) {
+  if (threadIdx.x >= CH_MMA_THREADS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(CH_PRODUCER_REGS));
     // ===== TMA producer: runs ahead of the epilogues, bounded only by free ring slots =====
-    if (lane == 0) {
+    if (warp == PRODUCER && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int j = 0; j < nl; ++j) {
@@ -203,22 +254,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_chain_kernel(const __grid_co
       }
     }
   } else {
-    // ===== MMA warpgroup: per layer the MMAs, then the epilogue on the accumulator registers, which also writes the
-    // next layer's operand; the tile width is dispatched once per layer =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CH_MMA_REGS));
+    // ===== MMA warpgroups: per layer the MMAs, then the epilogue on the accumulator registers, which also writes the
+    // next layer's operand; each warpgroup's share of the columns is dispatched once per layer =====
     float* row = scratch + threadIdx.x * 16;
+    const int wg = threadIdx.x / TC_MMA_THREADS;
     int stage = 0;
     uint32_t phase = 0;
     for (int j = 0; j < nl; ++j) {
-      switch ((P.L[j].bn + 63) / 64) {
-        case 1: chain_layer<PLANES2, B_MN, 1>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
-        case 2: chain_layer<PLANES2, B_MN, 2>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
-        case 3: chain_layer<PLANES2, B_MN, 3>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
-        default: chain_layer<PLANES2, B_MN, 4>(g, P, j, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
+      const int nb = (P.L[j].bn + 63) / 64, nb0 = (nb + 1) / 2;
+      const int n0 = wg == 0 ? 0 : 64 * nb0;
+      switch (wg == 0 ? nb0 : nb - nb0) {
+        case 0: chain_idle(P, j, stages, full, empty, stage, phase); break;
+        case 1: chain_layer<PLANES2, B_MN, 1>(g, P, j, n0, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
+        default: chain_layer<PLANES2, B_MN, 2>(g, P, j, n0, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
       }
     }
   }
 
-  if (lane == 0 && warp < 4) { if (g.dbg) atomicMax(&g.dbg[(size_t)blockIdx.x * TC_DBG_SLOTS + 5], gtime()); }
+  if (lane == 0 && warp < PRODUCER) { if (g.dbg) atomicMax(&g.dbg[(size_t)blockIdx.x * TC_DBG_SLOTS + 5], gtime()); }
   __syncthreads();
   if (threadIdx.x == 0) TC_STAMP(6);
 }

@@ -632,11 +632,11 @@ static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
     h->chain_attr_done = true;
   }
   if (planes == 2) {
-    if (cb.b_mn) launch_k(tc_chain_kernel<true, true>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
-    else launch_k(tc_chain_kernel<true, false>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+    if (cb.b_mn) launch_k(tc_chain_kernel<true, true>, cb.grid, CH_THREADS, smem, c, cb.g, stages, cb.stage_b);
+    else launch_k(tc_chain_kernel<true, false>, cb.grid, CH_THREADS, smem, c, cb.g, stages, cb.stage_b);
   } else {
-    if (cb.b_mn) launch_k(tc_chain_kernel<false, true>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
-    else launch_k(tc_chain_kernel<false, false>, cb.grid, TC_THREADS, smem, c, cb.g, stages, cb.stage_b);
+    if (cb.b_mn) launch_k(tc_chain_kernel<false, true>, cb.grid, CH_THREADS, smem, c, cb.g, stages, cb.stage_b);
+    else launch_k(tc_chain_kernel<false, false>, cb.grid, CH_THREADS, smem, c, cb.g, stages, cb.stage_b);
   }
   c.done(cls, cb.flops);
   c.check();

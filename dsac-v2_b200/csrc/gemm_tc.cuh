@@ -273,78 +273,151 @@ struct EpiArgs {
   long long img_plane;
 };
 
+// Predicated read-only loads (0 where `pred` is false), kept by the compiler where they are written: it would otherwise
+// hoist every load of an epilogue (__ldg reads invariant memory) to the top, where the results wait in registers through
+// the arithmetic of the groups before them, and a branch per load leaves a merge of values to allocate per load.
+__device__ __forceinline__ float ldg_if(const float* p, bool pred) {
+  float v = 0.f;
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p ld.global.nc.f32 %0, [%1];\n\t}"
+               : "+f"(v) : "l"(p), "r"((int)pred));
+  return v;
+}
+__device__ __forceinline__ float2 ldg2_if(const float* p, bool pred) {
+  float2 v = make_float2(0.f, 0.f);
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p ld.global.nc.v2.f32 {%0, %1}, [%2];\n\t}"
+               : "+f"(v.x), "+f"(v.y) : "l"(p), "r"((int)pred));
+  return v;
+}
+
+// Columns (c, c + 1) of one row, c even; columns >= n are not touched (loads return 0).  `pair`: the row pitch is even and
+// the base 8-byte aligned, so the two columns are one 8-byte access (the last column of an odd n a 4-byte one).
+__device__ __forceinline__ void ld_pair(const float* p, int c, int n, bool pair, float& a, float& b) {
+  if (pair) {
+    const float2 x = ldg2_if(p + c, c + 1 < n);
+    const float s = ldg_if(p + c, c + 1 == n);
+    a = c + 1 < n ? x.x : s;
+    b = x.y;
+  } else {
+    a = ldg_if(p + c, c < n);
+    b = ldg_if(p + c + 1, c + 1 < n);
+  }
+}
+__device__ __forceinline__ void st_pair(float* p, int c, int n, bool pair, float a, float b) {
+  if (pair && c + 1 < n) {
+    *reinterpret_cast<float2*>(p + c) = make_float2(a, b);
+  } else {
+    if (c < n) p[c] = a;
+    if (c + 1 < n) p[c + 1] = b;
+  }
+}
+__device__ __forceinline__ bool pairs_ok(const float* p, int ld) { return ((ld | (int)(reinterpret_cast<uintptr_t>(p) >> 2)) & 1) == 0; }
+
 // Epilogue of the warpgroup's 64 x (64 NB) accumulator, element (0, 0) = output (m0, n0), straight from the wgmma
 // fragment: acc[16 g + t] sits in row ra (t & 2 == 0) or ra + 8, column n0 + 32 g + 8 (t >> 2) + 2 (lane & 3) + (t & 1).
-// Columns >= N leave as zeros (they are the next layer's K padding and the image padding).  On return acc holds the
-// result.  `row`: this thread's 16-float shared-memory row (generic activations).
-template <bool PLANES2, int NB>
-__device__ __forceinline__ void epi_frag(float (&acc)[128], const EpiArgs& E, int m0, int n0, float* row) {
-  const int wl = threadIdx.x & (TC_MMA_THREADS - 1), lane = threadIdx.x & 31;
-  const int ra = m0 + (wl >> 5) * 16 + (lane >> 2);
-  const bool ok0 = ra < E.M, ok1 = ra + 8 < E.M;
-  const int cq = n0 + 2 * (lane & 3);
-  const int img_w = (E.N + 7) / 8 * 8;
-#pragma unroll
-  for (int g = 0; g < 2 * NB; ++g) {
-    float v[16], d[16];
-#pragma unroll
-    for (int t = 0; t < 16; ++t) v[t] = acc[16 * g + t];
+// Group g (16 values) is split into the loads of its global inputs (epi_in) and the arithmetic and stores (epi_group),
+// so that a caller can issue the loads early.
 #define COL(t) (cq + 32 * g + 8 * ((t) >> 2) + ((t) & 1))
 #define ROW(t) (ra + (((t) & 2) ? 8 : 0))
 #define ROW_OK(t) (((t) & 2) ? ok1 : ok0)
-    if (E.epi == EPI_STORE || E.epi == EPI_BIAS_ACT) {
-      if (E.bias) {
+#define EPI_FRAG_COORDS                                                         \
+  const int lane = threadIdx.x & 31;                                            \
+  const int ra = m0 + (((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16) + (lane >> 2); \
+  const bool ok0 = ra < E.M, ok1 = ra + 8 < E.M;                                \
+  const int cq = n0 + 2 * (lane & 3);
+
+// The global inputs of group g: x[t] = act'(z) of value t (EPI_DACT), or x[2 (t >> 2) + (t & 1)] = the bias of value t's
+// column (EPI_STORE / EPI_BIAS_ACT with a bias).
+__device__ __forceinline__ void epi_in(float (&x)[16], const EpiArgs& E, int m0, int n0, int g) {
+  EPI_FRAG_COORDS
+  // one loop body per access width, so that `pair` is a constant inside it
+#define EPI_IN_ZIN(pair) \
+  _Pragma("unroll") for (int t = 0; t < 16; t += 2) ld_pair(E.Zin + (size_t)ROW(t) * E.ldz, COL(t), ROW_OK(t) ? E.N : 0, pair, x[t], x[t + 1]);
+#define EPI_IN_BIAS(pair) \
+  _Pragma("unroll") for (int t = 0; t < 16; t += 4) ld_pair(E.bias, COL(t), E.N, pair, x[t / 2], x[t / 2 + 1]);
+  if (E.epi == EPI_DACT) {
+    if (pairs_ok(E.Zin, E.ldz)) { EPI_IN_ZIN(true) } else { EPI_IN_ZIN(false) }
+  } else if ((E.epi == EPI_STORE || E.epi == EPI_BIAS_ACT) && E.bias) {
+    if (pairs_ok(E.bias, 0)) { EPI_IN_BIAS(true) } else { EPI_IN_BIAS(false) }
+  }
+#undef EPI_IN_ZIN
+#undef EPI_IN_BIAS
+}
+
+// Arithmetic and stores of group g: v = the accumulator values on entry, the result on return.  Columns >= N leave as
+// zeros (they are the next layer's K padding and the image padding).  `row`: this thread's 16-float shared-memory row
+// (generic activations).
+template <bool PLANES2>
+__device__ __forceinline__ void epi_group(float (&v)[16], const float (&x)[16], const EpiArgs& E, int m0, int n0, int g,
+                                          float* row) {
+  EPI_FRAG_COORDS
+  const int img_w = (E.N + 7) / 8 * 8;
+  float d[16];
+  if (E.epi == EPI_STORE || E.epi == EPI_BIAS_ACT) {
+    if (E.bias) {
 #pragma unroll
-        for (int t = 0; t < 16; ++t) v[t] += COL(t) < E.N ? __ldg(E.bias + COL(t)) : 0.f;
+      for (int t = 0; t < 16; ++t) v[t] += x[2 * (t >> 2) + (t & 1)];
+    }
+    if (E.epi == EPI_BIAS_ACT) {
+      if (E.Zout) {
+        act_fwdN<true, 16>(v, d, E.act, row);
+        const bool pair = pairs_ok(E.Zout, E.ldc);
+#pragma unroll
+        for (int t = 0; t < 16; t += 2) st_pair(E.Zout + (size_t)ROW(t) * E.ldc, COL(t), ROW_OK(t) ? E.N : 0, pair, d[t], d[t + 1]);
+      } else {
+        act_fwdN<false, 16>(v, d, E.act, row);
       }
-      if (E.epi == EPI_BIAS_ACT) {
-        if (E.Zout) {
-          act_fwdN<true, 16>(v, d, E.act, row);
+    }
+  } else if (E.epi == EPI_DACT) {
 #pragma unroll
-          for (int t = 0; t < 16; ++t)
-            if (ROW_OK(t) && COL(t) < E.N) E.Zout[(size_t)ROW(t) * E.ldc + COL(t)] = d[t];
-        } else {
-          act_fwdN<false, 16>(v, d, E.act, row);
+    for (int t = 0; t < 16; ++t) v[t] *= x[t];
+    if (E.colsum) {  // bias gradient: both rows of the thread, then the eight lanes that share its columns
+#pragma unroll
+      for (int t = 0; t < 16; t += 4)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float s = v[t + e] + v[t + 2 + e];
+          s += __shfl_xor_sync(0xffffffffu, s, 4);
+          s += __shfl_xor_sync(0xffffffffu, s, 8);
+          s += __shfl_xor_sync(0xffffffffu, s, 16);
+          if (lane < 4 && COL(t + e) < E.N) atomicAdd(E.colsum + COL(t + e), s);
         }
-      }
-    } else if (E.epi == EPI_DACT) {
-#pragma unroll
-      for (int t = 0; t < 16; ++t) v[t] *= (ROW_OK(t) && COL(t) < E.N) ? __ldg(E.Zin + (size_t)ROW(t) * E.ldz + COL(t)) : 0.f;
-      if (E.colsum) {  // bias gradient: both rows of the thread, then the eight lanes that share its columns
-#pragma unroll
-        for (int t = 0; t < 16; t += 4)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float s = v[t + e] + v[t + 2 + e];
-            s += __shfl_xor_sync(0xffffffffu, s, 4);
-            s += __shfl_xor_sync(0xffffffffu, s, 8);
-            s += __shfl_xor_sync(0xffffffffu, s, 16);
-            if (lane < 4 && COL(t + e) < E.N) atomicAdd(E.colsum + COL(t + e), s);
-          }
-      }
     }
+  }
 #pragma unroll
-    for (int t = 0; t < 16; ++t) v[t] = COL(t) < E.N ? v[t] : 0.f;
-    if (E.C) {
+  for (int t = 0; t < 16; ++t) v[t] = COL(t) < E.N ? v[t] : 0.f;
+  if (E.C) {   // scalar: head outputs have odd widths (e.g. the action columns)
 #pragma unroll
-      for (int t = 0; t < 16; ++t)
-        if (ROW_OK(t) && COL(t) < E.N) E.C[(size_t)ROW(t) * E.ldc + COL(t)] = v[t];
-    }
-    if (E.img) {  // packed bf16 pairs (pitch % 8 == 0, even column): one 4-byte store per plane
+    for (int t = 0; t < 16; ++t)
+      if (ROW_OK(t) && COL(t) < E.N) E.C[(size_t)ROW(t) * E.ldc + COL(t)] = v[t];
+  }
+  if (E.img) {  // packed bf16 pairs (pitch % 8 == 0, even column): one 4-byte store per plane
 #pragma unroll
-      for (int t = 0; t < 16; t += 2) {
-        if (ROW_OK(t) && COL(t) < img_w) {
-          uint32_t whi, wlo;
-          split_pack2(v[t], v[t + 1], whi, wlo);
-          __nv_bfloat16* hp = E.img + (size_t)ROW(t) * E.img_pitch + COL(t);
-          *reinterpret_cast<uint32_t*>(hp) = whi;
-          if (PLANES2) *reinterpret_cast<uint32_t*>(hp + E.img_plane) = wlo;
-        }
+    for (int t = 0; t < 16; t += 2) {
+      if (ROW_OK(t) && COL(t) < img_w) {
+        uint32_t whi, wlo;
+        split_pack2(v[t], v[t + 1], whi, wlo);
+        __nv_bfloat16* hp = E.img + (size_t)ROW(t) * E.img_pitch + COL(t);
+        *reinterpret_cast<uint32_t*>(hp) = whi;
+        if (PLANES2) *reinterpret_cast<uint32_t*>(hp + E.img_plane) = wlo;
       }
     }
+  }
+}
 #undef COL
 #undef ROW
 #undef ROW_OK
+#undef EPI_FRAG_COORDS
+
+// The whole epilogue, group by group (loads, then arithmetic).  On return acc holds the result.
+template <bool PLANES2, int NB>
+__device__ __forceinline__ void epi_frag(float (&acc)[128], const EpiArgs& E, int m0, int n0, float* row) {
+#pragma unroll
+  for (int g = 0; g < 2 * NB; ++g) {
+    float x[16], v[16];
+    epi_in(x, E, m0, n0, g);
+#pragma unroll
+    for (int t = 0; t < 16; ++t) v[t] = acc[16 * g + t];
+    epi_group<PLANES2>(v, x, E, m0, n0, g, row);
 #pragma unroll
     for (int t = 0; t < 16; ++t) acc[16 * g + t] = v[t];
   }
