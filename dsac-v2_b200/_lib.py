@@ -60,6 +60,11 @@ class CnnConfig(C.Structure):
     ]
 
 
+class V1Options(C.Structure):
+    """dsact_v1_options: DSAC_V1's two settings on the MLP engine (dsact_v1_create)."""
+    _fields_ = [("abi_version", C.c_int32), ("bound", C.c_int32), ("td_bound", C.c_double)]
+
+
 class Layout(C.Structure):
     _fields_ = [("n_q", C.c_int64), ("n_pi", C.c_int64), ("n_params", C.c_int64), ("n_targets", C.c_int64),
                 ("workspace_bytes", C.c_int64), ("state_floats", C.c_int64), ("max_batch", C.c_int64),
@@ -124,6 +129,8 @@ SYMBOLS = {
     "dsact_dp_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_dp_replay_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_int64, C.c_int64,
                                        C.c_void_p]),
+    "dsact_v1_query_layout": (C.c_int, [C.POINTER(Config), C.POINTER(V1Options), C.POINTER(Layout)]),
+    "dsact_v1_create": (C.c_int, [C.POINTER(Config), C.POINTER(V1Options), C.c_int, C.POINTER(C.c_void_p)]),
     "dsact_cnn_query_layout": (C.c_int, [C.POINTER(CnnConfig), C.POINTER(Layout)]),
     "dsact_cnn_create": (C.c_int, [C.POINTER(CnnConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "dsact_profile_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_void_p, C.POINTER(Profile)]),

@@ -130,6 +130,7 @@ static void cnn_setup(HeadsHandle* h, const dsact_cnn_config& c) {
   h->act_dim = c.act_dim;
   h->max_batch = c.max_batch;
   h->v1 = c.algo == 1;
+  h->v1_bound = c.v1_bound; h->td_bound = c.td_bound;
   h->n_params = h->nq() * h->q.n + h->pi.n + 1;
 }
 
@@ -505,7 +506,6 @@ static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsac
 // mean is a sum over these rows times 1/global_batch; phase2_tail_kernel keeps rows = B (this shard), so that the log_alpha
 // gradient it writes is this rank's additive share -(sum_local logp + B * H) / global_batch (see tail_grad_log_alpha).
 static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
-  const dsact_cnn_config& cf = h->cfg;
   const CnnGeom &q = h->q, &pi = h->pi;
   const StepSlots& s = h->slot;
   const dsact_batch& bt = h->pending;
@@ -525,15 +525,7 @@ static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
     gbias_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
   }
   if (h->v1) {
-    LossV1Args a;
-    a.rew = bt.rew; a.done = bt.done; a.z = h->pending_z3; a.logp2 = W + s.logp2; a.logp_new = W + s.logp_new;
-    a.out_q = W + s.outQ[0]; a.out_qt = W + s.outQ[2]; a.out_qa = W + s.outQ[4];
-    a.d_out_q = W + s.dOut[0]; a.d_out_qa = W + s.dOut[4];
-    a.gbias_q = gbias[0]; a.gbias_q_raw = gbias_raw[0];
-    a.state = h->buf.state; a.B = B; a.bound = cf.v1_bound; a.gamma = (float)cf.gamma; a.inv_global_batch = sc.inv_global_batch;
-    a.td_bound = (float)cf.td_bound; a.sc = sc;
-    int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-    launch_k(loss_v1_kernel, blocks, 64, 0, c, a); c.done();
+    enqueue_loss_v1(h, bt, sc, gbias[0], gbias_raw[0], NO_IMG, NO_IMG, c);
   } else {
     const ImgOut none[2] = {NO_IMG, NO_IMG};
     enqueue_loss(h, bt, sc, gbias, gbias_raw, none, none, c);

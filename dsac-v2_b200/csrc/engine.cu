@@ -14,6 +14,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
+
 #include <vector>
 
 #include "../../include/dsact.h"
@@ -74,6 +76,7 @@ struct StepSlots {
   int64_t logitsP, logitsT, dlogits;               // policy outputs (mean | log_std) of pi(s), pi'(s'); their gradient
   int64_t new_act, act2, logp_new, logp2;          // a~ ~ pi(s), a' ~ pi'(s') and their log-probs
   int64_t outQ[6], dOut[6], dAct[2];               // Q_k(s,a), Q'_k(s',a'), Q_k(s,a~) [B,2] and gradients; dL/da~ per critic
+                                                   // (pass p belongs to critic p & 1; -1: a slot of a critic the handle lacks)
 };
 
 // The hyperparameters both configuration structs name alike
@@ -96,13 +99,14 @@ struct Arena : StepSlots {
   ImgSlot i_obs, i_obs2, i_act, i_new_act, i_act2, i_dlogits;
   ImgSlot i_hP[DSACT_MAX_HIDDEN], i_hT[DSACT_MAX_HIDDEN], i_dzP[DSACT_MAX_HIDDEN];
   ImgSlot i_hQ[6][DSACT_MAX_HIDDEN], i_dzQ[6][DSACT_MAX_HIDDEN], i_dOut[6];
-  ImgSlot i_wq[4][DSACT_MAX_HIDDEN + 1], i_wpi[2][DSACT_MAX_HIDDEN + 1];  // q1,q2,q1',q2' / pi,pi'
+  ImgSlot i_wq[4][DSACT_MAX_HIDDEN + 1], i_wpi[2][DSACT_MAX_HIDDEN + 1];  // q1,q2,q1',q2' (DSAC_V1: q, -, q', -) / pi,pi'
   int kpad_q0;        // column of the act block inside the Q layer-0 weight image
   int64_t slabs;      // [nslabs][n_params] fp32 wgrad partials, the arena's last region
   int nslabs;
   int64_t slab_stride;   // floats between slabs: n_params rounded up to 4 (float4 access to every slab)
   int64_t total;
-  void build(const dsact_config& c, const Net& q, const Net& pi) {
+  // nq critics (DSAC-T 2, DSAC_V1 1): the passes and weight images of critic 1 exist only with two
+  void build(const dsact_config& c, const Net& q, const Net& pi, int nq = 2) {
     int64_t B = c.max_batch, O = c.obs_dim, A = c.act_dim, off = 0;
     auto take = [&](int64_t n) { int64_t o = off; off += round64(n); return o; };
     auto img = [&](int rows, int width) {
@@ -118,10 +122,12 @@ struct Arena : StepSlots {
     logitsP = take(B * 2 * A); logitsT = take(B * 2 * A); dlogits = take(B * 2 * A);
     new_act = take(B * A); act2 = take(B * A); logp_new = take(B); logp2 = take(B);
     for (int p = 0; p < 6; ++p) {
+      outQ[p] = dOut[p] = -1;
+      if ((p & 1) >= nq) continue;
       for (int j = 0; j < q.L; ++j) { zQ[p][j] = take(B * q.s[j + 1]); hQ[p][j] = take(B * q.s[j + 1]); dzQ[p][j] = take(B * q.s[j + 1]); }
       outQ[p] = take(B * 2); dOut[p] = take(B * 2);
     }
-    dAct[0] = take(B * A); dAct[1] = take(B * A);
+    dAct[0] = take(B * A); dAct[1] = nq == 2 ? take(B * A) : -1;
     tc = c.gemm_mode != DSACT_GEMM_FP32;
     nslabs = 0; slabs = 0; slab_stride = 0; kpad_q0 = (int)((O + 63) / 64 * 64);
     if (tc) {
@@ -130,17 +136,18 @@ struct Arena : StepSlots {
       i_dlogits = img(Bi, 2 * (int)A);
       for (int j = 0; j < pi.L; ++j) { i_hP[j] = img(Bi, pi.s[j + 1]); i_hT[j] = img(Bi, pi.s[j + 1]); i_dzP[j] = img(Bi, pi.s[j + 1]); }
       for (int p = 0; p < 6; ++p) {
+        if ((p & 1) >= nq) continue;
         for (int j = 0; j < q.L; ++j) { i_hQ[p][j] = img(Bi, q.s[j + 1]); i_dzQ[p][j] = img(Bi, q.s[j + 1]); }
         i_dOut[p] = img(Bi, 2);
       }
       for (int n = 0; n < 4; ++n)
-        for (int j = 0; j <= q.L; ++j) i_wq[n][j] = img(q.s[j + 1], j == 0 ? kpad_q0 + (int)A : q.s[j]);
+        for (int j = 0; j <= q.L && (n & 1) < nq; ++j) i_wq[n][j] = img(q.s[j + 1], j == 0 ? kpad_q0 + (int)A : q.s[j]);
       for (int n = 0; n < 2; ++n)
         for (int j = 0; j <= pi.L; ++j) i_wpi[n][j] = img(pi.s[j + 1], pi.s[j]);
       // batch split of the weight-gradient GEMMs: at most 4 slabs of >= 256 rows (more slabs mean more partial tiles to
       // write and to fold in apply)
       nslabs = (int)(B / 256); if (nslabs > 4) nslabs = 4; if (nslabs < 1) nslabs = 1;
-      slab_stride = (2 * q.n + pi.n + 1 + 3) / 4 * 4;
+      slab_stride = (nq * q.n + pi.n + 1 + 3) / 4 * 4;
       slabs = take((int64_t)nslabs * slab_stride);
     } else {
       slabs = off;   // the (empty) last region
@@ -167,6 +174,8 @@ struct dsact_handle {
   int act_dim = 0, max_batch = 0;
   int64_t n_params = 0;      // flat parameter count (log_alpha included)
   bool v1 = false;           // DSAC_V1: one critic, local steps only, its own policy-statistic denominator
+  int v1_bound = 1;          // DSAC_V1's critic loss: 1 bounded (dsac_v1.py:219-229), 0 Gaussian NLL (:231)
+  double td_bound = 20.0;    // DSAC_V1's TD bound (dsac_v1.py:79)
   StepSlots slot = {};
   StepHyper hyper = {};
   dsact_buffers buf = {};
@@ -209,6 +218,7 @@ struct MlpHandle : dsact_handle {
   std::vector<GraphEntry> graphs;
   uint64_t stamp = 0;
   MlpHandle() : dsact_handle(ENGINE_MLP) {}
+  int nq() const { return v1 ? 1 : 2; }   // critics: DSAC_V1 has one (flat layout [q | policy | log_alpha])
   bool tc() const { return cfg.gemm_mode != DSACT_GEMM_FP32; }
   bool fused() const {  // layer-chain kernel: every layer must fit one 256-column wgmma accumulator / A operand
     if (!tc()) return false;
@@ -827,6 +837,26 @@ static void enqueue_loss(const dsact_handle* h, const dsact_batch& bt, const Ste
   c.done();
 }
 
+// DSAC_V1's losses (one critic, fixed TD bound) and the gradients of the critic's outputs.  gbias: output-bias gradient of
+// the mean; gbias_raw: of the std output, or null for the element after gbias
+static void enqueue_loss_v1(const dsact_handle* h, const dsact_batch& bt, const StepScalars& sc, float* gbias, float* gbias_raw,
+                            const ImgOut& img_q, const ImgOut& img_qa, Ctx& c) {
+  const StepSlots& s = h->slot;
+  float* W = h->W();
+  const int B = bt.batch;
+  LossV1Args a;
+  a.rew = bt.rew; a.done = bt.done; a.z = h->pending_z3; a.logp2 = W + s.logp2; a.logp_new = W + s.logp_new;
+  a.out_q = W + s.outQ[0]; a.out_qt = W + s.outQ[2]; a.out_qa = W + s.outQ[4];
+  a.d_out_q = W + s.dOut[0]; a.d_out_qa = W + s.dOut[4];
+  a.gbias_q = gbias; a.gbias_q_raw = gbias_raw;
+  a.state = h->buf.state; a.B = B; a.bound = h->v1_bound; a.gamma = (float)h->hyper.gamma; a.inv_global_batch = sc.inv_global_batch;
+  a.td_bound = (float)h->td_bound; a.sc = sc;
+  a.img_q = img_q; a.img_qa = img_qa;
+  int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
+  launch_k(loss_v1_kernel, blocks, 64, 0, c, a);
+  c.done();
+}
+
 // the actor loss's gradient w.r.t. the policy outputs of pi(s).  gbias: output-bias gradient of the mean (the whole
 // (mean | log_std) row when gbias_ls is null); gbias_ls: of a separate log_std head or row
 static void enqueue_policy_grad(const dsact_handle* h, int B, const StepScalars& sc, float* gbias, float* gbias_ls, const ImgOut& img,
@@ -836,7 +866,8 @@ static void enqueue_policy_grad(const dsact_handle* h, int B, const StepScalars&
   float* W = h->W();
   const int A = h->act_dim;
   PolicyGradArgs a;
-  a.logits = W + s.logitsP; a.eps = h->pending_eps1; a.d_act1 = W + s.dAct[0]; a.d_act2 = W + s.dAct[1];
+  const bool one_critic = s.dAct[1] < 0;   // DSAC_V1 on the MLP engine: no second action-gradient slot
+  a.logits = W + s.logitsP; a.eps = h->pending_eps1; a.d_act1 = W + s.dAct[0]; a.d_act2 = one_critic ? nullptr : W + s.dAct[1];
   a.hi = h->buf.act_high; a.lo = h->buf.act_low;
   a.d_logits = W + s.dlogits; a.gbias = gbias; a.gbias_ls = gbias_ls; a.state = h->buf.state;
   a.B = B; a.A = A; a.min_log_std = (float)p.min_log_std; a.max_log_std = (float)p.max_log_std; a.gauss = p.act_dist;
@@ -844,7 +875,7 @@ static void enqueue_policy_grad(const dsact_handle* h, int B, const StepScalars&
   a.img = img;
   a.sc = sc;
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;   // a warp per row
-  launch_k(policy_grad_kernel, blocks, 256, sizeof(float) * 2 * A, c, a);
+  launch_k(one_critic ? policy_grad_kernel<1> : policy_grad_kernel<2>, blocks, 256, sizeof(float) * 2 * A, c, a);
   c.done();
 }
 
@@ -916,8 +947,9 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
   const bool tc = h->tc();
   float* P = h->buf.params;
   float* T = h->buf.targets;
-  const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2'
-  const float* PIb[2] = {P + 2 * q.n, T + 2 * q.n};     // pi, pi'
+  const int nq = h->nq();
+  const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2' (DSAC_V1: q, -, q', -)
+  const float* PIb[2] = {P + nq * q.n, T + nq * q.n};   // pi, pi'
 
   const bool want_noise = !nz && with_noise;
   if (!tc) enqueue_begin_step(h, c);
@@ -925,7 +957,7 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
   if (tc) {  // refresh the weight images (the caller may have written params/targets through its views) + inputs; the clears
              // and the device noise ride in the same launch
     ImgBatch ib;
-    for (int n = 0; n < 2; ++n)
+    for (int n = 0; n < nq; ++n)
       for (int j = 0; j <= q.L; ++j) {
         ib.reserve(h, c, 1);
         const Img im = h->img(ar.i_wq[n][j], q.s[j + 1]);
@@ -935,7 +967,7 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
     ib.reserve(h, c, pi.L + 2);
     for (int j = 0; j <= pi.L; ++j) ib.add(PIb[0] + pi.w[j], pi.s[j], h->img(ar.i_wpi[0][j], pi.s[j + 1]), pi.s[j + 1], pi.s[j]);
     if (!inputs_imaged) ib.add(bt.obs, O, h->img(ar.i_obs, B), B, O);
-    for (int n = 2; n < 4; ++n)
+    for (int n = 2; n < 2 + nq; ++n)
       for (int j = 0; j <= q.L; ++j) {
         ib.reserve(h, c, 1);
         const Img im = h->img(ar.i_wq[n][j], q.s[j + 1]);
@@ -1061,11 +1093,11 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
   float* W = h->W();
-  const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim;
+  const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim, nq = h->nq();
   float* P = h->buf.params;
   float* T = h->buf.targets;
-  const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2'
-  const float* PIb[2] = {P + 2 * q.n, T + 2 * q.n};     // pi, pi'
+  const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2' (DSAC_V1: q, -, q', -)
+  const float* PIb[2] = {P + nq * q.n, T + nq * q.n};   // pi, pi'
   auto ten = [&](const float* f, const ImgSlot& s) { Ten t; t.f = const_cast<float*>(f); t.im = h->img(s, B); return t; };
   const ImgSlot none;
 
@@ -1085,11 +1117,11 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
     ChainBuild cb(h->passes());
     chain_fwd_pass(cb, h, pi, PIb[0], ar.i_wpi[0], t_obs.im, O, i_none, 0, 0, B, cf.act_pi, ar.zP, ar.i_hP, W + ar.logitsP);
     chain_fwd_pass(cb, h, pi, PIb[1], ar.i_wpi[1], t_obs2.im, O, i_none, 0, 0, B, cf.act_pi, nullptr, nullptr, W + ar.logitsT);
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < nq; ++k)
       chain_fwd_pass(cb, h, q, Qb[k], ar.i_wq[k], t_obs.im, O, t_act.im, A, ar.kpad_q0, B, cf.act_q, ar.zQ[k], ar.i_hQ[k], W + ar.outQ[k]);
     launch_chain(h, cb, CLS_GEMM_FWD, c);
   }
-  // wave A: pi(obs), pi'(obs2), Q1(s,a), Q2(s,a), layer by layer
+  // wave A: pi(obs), pi'(obs2), Q1(s,a), Q2(s,a) (DSAC_V1: Q(s,a)), layer by layer
   const int depth = fused ? 0 : (pi.L > q.L ? pi.L : q.L) + 1;
   for (int j = 0; j < depth; ++j) {
     Group G;
@@ -1102,7 +1134,7 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
       add_fwd(G, pi, j, weight(h, pi, PIb[1], j, ar.i_wpi[1][j]), inT, pi.s[j], t_none, 0, 0, outT, nullptr, B, cf.act_pi);
     }
     if (j <= q.L) {
-      for (int k = 0; k < 2; ++k) {
+      for (int k = 0; k < nq; ++k) {
         const Ten out = j == q.L ? ten(W + ar.outQ[k], none) : ten(W + ar.hQ[k][j], ar.i_hQ[k][j]);
         float* z = j == q.L ? nullptr : W + ar.zQ[k][j];
         const Wt w = weight(h, q, Qb[k], j, ar.i_wq[k][j]);
@@ -1131,13 +1163,13 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
     }
   }
 
-  // wave B: Q1', Q2' on (s', a') and Q1, Q2 on (s, a~)
+  // wave B: Q1', Q2' on (s', a') and Q1, Q2 on (s, a~) (DSAC_V1: Q', Q)
   const Ten t_new_act = ten(W + ar.new_act, ar.i_new_act), t_act2 = ten(W + ar.act2, ar.i_act2);
   if (fused) {
     ChainBuild cb(h->passes());
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < nq; ++k)
       chain_fwd_pass(cb, h, q, Qb[2 + k], ar.i_wq[2 + k], t_obs2.im, O, t_act2.im, A, ar.kpad_q0, B, cf.act_q, nullptr, nullptr, W + ar.outQ[2 + k]);
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < nq; ++k)
       chain_fwd_pass(cb, h, q, Qb[k], ar.i_wq[k], t_obs.im, O, t_new_act.im, A, ar.kpad_q0, B, cf.act_q, ar.zQ[4 + k], nullptr, W + ar.outQ[4 + k]);
     launch_chain(h, cb, CLS_GEMM_FWD, c);
   }
@@ -1145,6 +1177,7 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
     Group G;
     for (int p = 2; p < 6; ++p) {
       const int k = p & 1;
+      if (k >= nq) continue;
       const bool tgt = p < 4;
       const int wn = tgt ? 2 + k : k;
       const Ten out = j == q.L ? ten(W + ar.outQ[p], none) : ten(W + ar.hQ[p][j], ar.i_hQ[p][j]);
@@ -1183,24 +1216,30 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
   float* W = h->W();
-  const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim;
+  const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim, nq = h->nq();
   const bool tc = h->tc();
   float* P = h->buf.params;
   float* G_ = h->buf.grads;
-  const float *Pq[2] = {P, P + q.n}, *Ppi = P + 2 * q.n;
-  float *Gq[2] = {G_, G_ + q.n}, *Gpi = G_ + 2 * q.n;
+  const float *Pq[2] = {P, P + q.n}, *Ppi = P + nq * q.n;
+  float *Gq[2] = {G_, G_ + q.n}, *Gpi = G_ + nq * q.n;
+  const long long n_flat = nq * q.n + pi.n + 1;
   auto ten = [&](const float* f, const ImgSlot& s) { Ten t; t.f = const_cast<float*>(f); t.im = h->img(s, B); return t; };
   const ImgSlot none;
 
   const StepScalars sc = step_scalars(h, global_batch);
-  {
+  if (h->v1) {
+    enqueue_loss_v1(h, bt, sc, Gq[0] + q.b[q.L], nullptr, img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[4]), c);
+  } else {
     float* const gbias[2] = {Gq[0] + q.b[q.L], Gq[1] + q.b[q.L]};
     float* const gbias_raw[2] = {nullptr, nullptr};   // one two-output layer
     const ImgOut img_q[2] = {img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[1])};
     const ImgOut img_qa[2] = {img_out(h, ar.i_dOut[4]), img_out(h, ar.i_dOut[5])};
     enqueue_loss(h, bt, sc, gbias, gbias_raw, img_q, img_qa, c);
   }
-  const int passes[4] = {0, 1, 4, 5};
+  // critic passes with a backward: Q_k(s,a) (dgrad + wgrad) and Q_k(s,a~) (dgrad only); DSAC_V1: Q(s,a), Q(s,a~)
+  const int passes[4] = {0, 1, 4, 5}, v1_passes[2] = {0, 4};
+  const int* bwd = h->v1 ? v1_passes : passes;
+  const int n_bwd = 2 * nq;
   const Ten t_obs = ten(bt.obs, ar.i_obs), t_act = ten(bt.act, ar.i_act);
 
   // wave C: critic passes 0,1 (dgrad + wgrad) and actor passes 4,5 (dgrad only), top layer down.
@@ -1210,8 +1249,8 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const bool fused = h->fused();
   if (fused) {  // dgrad as one chain launch: dz stays on chip between layers
     ChainBuild cb(h->passes());
-    for (int pp = 0; pp < 4; ++pp) {
-      const int p = passes[pp], k = p & 1;
+    for (int pp = 0; pp < n_bwd; ++pp) {
+      const int p = bwd[pp], k = p & 1;
       chain_dgrad_pass(cb, h, q, ar.i_wq[k], h->img(ar.i_dOut[p], B), B, cf.act_q, ar.zQ[p], p < 2 ? Gq[k] : nullptr,
                        p < 2 ? ar.i_dzQ[p] : nullptr, p < 2 ? nullptr : W + ar.dAct[k], ar.kpad_q0, A);
     }
@@ -1219,8 +1258,8 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   }
   for (int j = q.L; j >= 1; --j) {
     Group gd;
-    for (int pp = 0; pp < 4; ++pp) {
-      const int p = passes[pp], k = p & 1;
+    for (int pp = 0; pp < n_bwd; ++pp) {
+      const int p = bwd[pp], k = p & 1;
       const Ten dY = j == q.L ? ten(W + ar.dOut[p], ar.i_dOut[p]) : ten(W + ar.dzQ[p][j], ar.i_dzQ[p][j]);
       float* gb = p < 2 ? Gq[k] + q.b[j - 1] : nullptr;
       add_dgrad(gd, q, j, weight(h, q, Pq[k], j, ar.i_wq[k][j]), 0, 0, q.s[j], dY, ten(W + ar.dzQ[p][j - 1], ar.i_dzQ[p][j - 1]),
@@ -1232,7 +1271,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   }
   {
     Group gd;
-    for (int k = 0; k < 2; ++k) {
+    for (int k = 0; k < nq; ++k) {
       const Ten dz0 = ten(W + ar.dzQ[k][0], ar.i_dzQ[k][0]);
       add_wgrad(gw, q, 0, Gq[k] + q.w[0], 0, O, dz0, t_obs, B);
       add_wgrad(gw, q, 0, Gq[k] + q.w[0], O, A, dz0, t_act, B);
@@ -1249,7 +1288,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
       const int chain_ctas = (B + TC_BM - 1) / TC_BM;
       const int cap = h->num_sms - chain_ctas;
       launch_group(h, gw, V_WGRAD, cs, cap >= h->num_sms / 2 ? cap : 0);
-      if (tail && !dp && slabs_foldable(h)) {   // Adam + Polyak of both critics beside the policy backward: every critic gradient is final here
+      if (tail && !dp && slabs_foldable(h)) {   // Adam + Polyak of the critics beside the policy backward: every critic gradient is final here
         enqueue_apply(h, cs, tail, false, 1);
         h->apply_early = true;
       }
@@ -1286,16 +1325,16 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
 
   if (h->join_pending) { cudaStreamWaitEvent(c.s, h->ev_join, 0); h->join_pending = false; }
   if (tc && !dp && !(tail && slabs_foldable(h))) {  // fold the weight-gradient split slabs into the flat gradient buffer
-    const long long n = 2 * q.n + pi.n + 1;
+    const long long n = n_flat;
     int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
     launch_k(grad_reduce_kernel, blocks, 256, 0, c, G_, W + ar.slabs, n, ar.nslabs, (long long)ar.slab_stride); c.done();
   }
   if (!tail) {
-    launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + 2 * q.n + pi.n, h->buf.state, sc, -(float)cf.act_dim, B, adam_hyper(h), 0);
+    launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + n_flat - 1, h->buf.state, sc, -(float)cf.act_dim, B, adam_hyper(h), 0);
     c.done();
   }
   if (dp) {  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
-    const long long n = 2 * q.n + pi.n + 1;
+    const long long n = n_flat;
     int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
     launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF, (const float*)G_, (const float*)(tc ? W + ar.slabs : G_), n,
              tc ? ar.nslabs : 0, (long long)(tc ? ar.slab_stride : 4), (const float*)h->buf.state, *tail);
@@ -1311,7 +1350,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
 static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
   if (part == 0 && h->apply_early) { part = 2; h->apply_early = false; }   // phase 2 already updated the critics
   // split API: the Adam scalars are formed here; single-call steps: precomputed by the previous apply / prologue if stamped
-  ApplyArgs a = apply_args(h, 2 * h->q.n, tail ? 2 : 0, dp);
+  ApplyArgs a = apply_args(h, h->nq() * h->q.n, tail ? 2 : 0, dp);
   if (tail) a.tail = *tail;
   if (tail && !dp && slabs_foldable(h)) { a.slabs = h->W() + h->ar.slabs; a.nslabs = h->ar.nslabs; a.slab_stride = h->ar.slab_stride; }
   const int64_t g_q = a.n_q2 / 4;   // a group straddling the critic / policy boundary goes with part 2
@@ -1439,7 +1478,7 @@ static int check_noise(const dsact_noise* n) {
 }
 // the split and data-parallel entry points implement DSAC_V2 (DSAC-T); DSAC_V1 has local steps only
 static int check_v2(const dsact_handle* h) {
-  return h->v1 ? fail(DSACT_EINVAL, "DSAC_V1 handles (algo 1) have no split or data-parallel update") : DSACT_OK;
+  return h->v1 ? fail(DSACT_EINVAL, "DSAC_V1 handles have no split or data-parallel update") : DSACT_OK;
 }
 // host staging, the replay-fused steps, the profiler and the GEMM test hook exist on the MLP engine only
 static int check_mlp(const dsact_handle* h, const char* fn) {
@@ -1501,18 +1540,25 @@ static int validate(const dsact_config* c) {
   return DSACT_OK;
 }
 
-int dsact_query_layout(const dsact_config* cfg, dsact_layout* out) {
-  int rc = validate(cfg);
-  if (rc) return rc;
+static int validate_v1(const dsact_v1_options* v) {
+  if (!v) return fail(DSACT_EINVAL, "null DSAC_V1 options");
+  if (v->abi_version != DSACT_ABI_VERSION) return fail(DSACT_EINVAL, "dsact_v1_options.abi_version %d != %d", v->abi_version, DSACT_ABI_VERSION);
+  if (v->bound != 0 && v->bound != 1) return fail(DSACT_EINVAL, "DSAC_V1 bound must be 0 (Gaussian NLL) or 1 (bounded loss), got %d", v->bound);
+  if (!(v->td_bound > 0.0) || !std::isfinite(v->td_bound)) return fail(DSACT_EINVAL, "DSAC_V1 TD_bound must be finite and > 0, got %g", v->td_bound);
+  return DSACT_OK;
+}
+
+// the layout of an MLP-engine handle with nq critics (DSAC-T 2, DSAC_V1 1)
+static int mlp_query_layout(const dsact_config* cfg, int nq, dsact_layout* out) {
   if (!out) return fail(DSACT_EINVAL, "null out");
   Net q, pi;
   q.build(cfg->obs_dim + cfg->act_dim, cfg->hidden_q, cfg->n_hidden_q, 2);
   pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, 2 * cfg->act_dim);
   Arena ar;
-  ar.build(*cfg, q, pi);
+  ar.build(*cfg, q, pi, nq);
   out->n_q = q.n; out->n_pi = pi.n;
-  out->n_params = 2 * q.n + pi.n + 1;
-  out->n_targets = 2 * q.n + pi.n;
+  out->n_params = nq * q.n + pi.n + 1;
+  out->n_targets = nq * q.n + pi.n;
   out->workspace_bytes = ar.total * (int64_t)sizeof(float);
   out->state_floats = ST_FLOATS;
   out->max_batch = cfg->max_batch;
@@ -1521,24 +1567,36 @@ int dsact_query_layout(const dsact_config* cfg, dsact_layout* out) {
   return DSACT_OK;
 }
 
-int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
+int dsact_query_layout(const dsact_config* cfg, dsact_layout* out) {
   int rc = validate(cfg);
-  if (rc) return rc;
+  return rc ? rc : mlp_query_layout(cfg, 2, out);
+}
+
+int dsact_v1_query_layout(const dsact_config* cfg, const dsact_v1_options* v1, dsact_layout* out) {
+  int rc = validate(cfg);
+  if (rc || (rc = validate_v1(v1))) return rc;
+  return mlp_query_layout(cfg, 1, out);
+}
+
+// an MLP-engine handle: DSAC-T (v1 == null) or DSAC_V1
+static int mlp_create(const dsact_config* cfg, const dsact_v1_options* v1, int device, dsact_handle** out) {
   if (!out) return fail(DSACT_EINVAL, "null out");
   CUDA_TRY(cudaSetDevice(device));
   int num_sms = 0;
-  if ((rc = check_sm90(device, &num_sms))) return rc;
+  int rc = check_sm90(device, &num_sms);
+  if (rc) return rc;
   MlpHandle* h = new MlpHandle();
   h->cfg = *cfg;
   h->device = device;
   h->num_sms = num_sms;
+  if (v1) { h->v1 = true; h->v1_bound = v1->bound; h->td_bound = v1->td_bound; }
   h->q.build(cfg->obs_dim + cfg->act_dim, cfg->hidden_q, cfg->n_hidden_q, 2);
   h->pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, 2 * cfg->act_dim);
-  h->ar.build(*cfg, h->q, h->pi);
+  h->ar.build(*cfg, h->q, h->pi, h->nq());
   h->slot = h->ar;
   h->hyper = StepHyper::of(*cfg);
   h->obs_elems = cfg->obs_dim; h->act_dim = cfg->act_dim; h->max_batch = cfg->max_batch;
-  h->n_params = 2 * h->q.n + h->pi.n + 1;
+  h->n_params = h->nq() * h->q.n + h->pi.n + 1;
   h->arena_imaged = false;
   cudaError_t e = cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking);
@@ -1551,6 +1609,17 @@ int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
   if (e != cudaSuccess) { delete h; return fail(DSACT_ECUDA, "cudaStreamCreate failed: %s", cudaGetErrorString(e)); }
   *out = h;
   return DSACT_OK;
+}
+
+int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
+  int rc = validate(cfg);
+  return rc ? rc : mlp_create(cfg, nullptr, device, out);
+}
+
+int dsact_v1_create(const dsact_config* cfg, const dsact_v1_options* v1, int device, dsact_handle** out) {
+  int rc = validate(cfg);
+  if (rc || (rc = validate_v1(v1))) return rc;
+  return mlp_create(cfg, v1, device, out);
 }
 
 void dsact_destroy(dsact_handle* hh) {
@@ -1936,6 +2005,7 @@ int dsact_dp_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const in
   if (rc) return rc;
   MlpHandle* h = mlp(hh);
   if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
+  if ((rc = check_v2(h))) return rc;
   if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
   if (global_batch < batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch);

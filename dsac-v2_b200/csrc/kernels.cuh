@@ -496,6 +496,7 @@ struct LossV1Args {
   int B, bound;
   float gamma, inv_global_batch, td_bound;
   StepScalars sc;
+  ImgOut img_q, img_qa;                   // bf16 images of d_out_q / d_out_qa (the MLP engine's dgrad chain reads them)
 };
 
 // __compute_loss_q / __compute_target_q / __compute_loss_policy of dsac_v1.py:195-248, one thread per sample:
@@ -530,9 +531,11 @@ __global__ void loss_v1_kernel(const __grid_constant__ LossV1Args a) {
     const float g_raw = g_sd * dsoft;
     a.d_out_q[2 * i] = g_mean;
     a.d_out_q[2 * i + 1] = g_raw;
+    img_put(a.img_q, i, 0, g_mean); img_put(a.img_q, i, 1, g_raw);
     const float lp = a.logp_new[i];
     a.d_out_qa[2 * i] = -invB;
     a.d_out_qa[2 * i + 1] = 0.f;
+    img_put(a.img_qa, i, 0, -invB); img_put(a.img_qa, i, 1, 0.f);
     s[0] += q; s[1] += sd; s[2] += alpha * lp - a.out_qa[2 * i]; s[3] += lp; s[4] += g_mean; s[5] += g_raw;
   }
   block_sum<6>(s, red);
@@ -551,7 +554,7 @@ __global__ void loss_v1_kernel(const __grid_constant__ LossV1Args a) {
 // a~ = scale*tanh(u)+shift, u = mean + std*eps, and log-prob (SURVEY Appendix A step 1 and 7).
 // Also accumulates the output-layer bias gradient.  One warp per row.
 struct PolicyGradArgs {
-  const float *logits, *eps, *d_act1, *d_act2;  // d_act_k: dL/da~ through critic k  [B,A]
+  const float *logits, *eps, *d_act1, *d_act2;  // d_act_k: dL/da~ through critic k  [B,A] (d_act2 unused with one critic)
   const float *hi, *lo;
   float* d_logits;   // [B,2A]
   float* gbias;      // [2A] (+=), or [A] for the mean half when gbias_ls is given
@@ -563,7 +566,9 @@ struct PolicyGradArgs {
   StepScalars sc;
   int gauss;         // 1: GaussDistribution (a~ = u, log-prob of the Normal only)
 };
-// d(actor loss)/d(mean_j, log_std_j) of one row (chain rule through a~ = scale tanh(u) + shift and the log-prob)
+// d(actor loss)/d(mean_j, log_std_j) of one row (chain rule through a~ = scale tanh(u) + shift and the log-prob).
+// NQ: critics whose action gradients add up (DSAC-T 2, DSAC_V1 on the MLP engine 1)
+template <int NQ>
 __device__ __forceinline__ void pgrad_elem(const PolicyGradArgs& a, int row, int j, float coef, float& gu, float& gls) {
   const int A = a.A;
   const float scale = 0.5f * (a.hi[j] - a.lo[j]);
@@ -572,7 +577,7 @@ __device__ __forceinline__ void pgrad_elem(const PolicyGradArgs& a, int row, int
   const bool inside = ls >= a.min_log_std && ls <= a.max_log_std;
   const float sd = expf(fminf(fmaxf(ls, a.min_log_std), a.max_log_std));
   const float e = a.eps[(size_t)row * A + j];
-  const float da = a.d_act1[(size_t)row * A + j] + a.d_act2[(size_t)row * A + j];
+  const float da = NQ == 2 ? a.d_act1[(size_t)row * A + j] + a.d_act2[(size_t)row * A + j] : a.d_act1[(size_t)row * A + j];
   if (a.gauss) {   // a~ = u; d logp / d mean = 0, d logp / d sd = -1/sd
     gu = da;
     gls = inside ? (gu * e - coef / sd) * sd : 0.f;
@@ -584,6 +589,7 @@ __device__ __forceinline__ void pgrad_elem(const PolicyGradArgs& a, int row, int
   const float gsd = gu * e - coef / sd;
   gls = inside ? gsd * sd : 0.f;
 }
+template <int NQ>
 __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
   pdl_sync();
   extern __shared__ float gb[];   // [2A] block-local bias-gradient sums
@@ -597,7 +603,7 @@ __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
     float gb_mean = 0.f, gb_ls = 0.f;
     for (int row = blockIdx.x * wpb + warp; j < A && row < a.B; row += gridDim.x * wpb) {
       float gu, gls;
-      pgrad_elem(a, row, j, coef, gu, gls);
+      pgrad_elem<NQ>(a, row, j, coef, gu, gls);
       a.d_logits[(size_t)row * 2 * A + j] = gu;
       a.d_logits[(size_t)row * 2 * A + A + j] = gls;
       img_put(a.img, row, j, gu);

@@ -1,6 +1,7 @@
 """`dsac_v1` of the drop-in: `ApproxContainer` and `DSAC_V1` with the reference's names, kwargs and `tb_info` keys
 (reference dsac_v1.py:17-52, 56-273) — the older algorithm (one distributional critic, fixed TD bound; selectable with
-`--algorithm DSAC_V1`), backed by the head-wise fp32 engine of libdsact.so (`dsact_cnn_create` with `algo = 1`).
+`--algorithm DSAC_V1`), backed by libdsact.so: by default the head-wise fp32 engine (`dsact_cnn_create` with `algo = 1`);
+with `dsact_gemm` the MLP engine (`dsact_v1_create`: wgmma layer chains or fp32 SIMT GEMMs, captured steps).
 
 * `ApproxContainer`: `q`, `q_target`, `policy`, `policy_target` (the same `networks.mlp` / `networks.cnn` classes as
   DSAC-T) + `log_alpha`; on a CUDA device the parameters are views into the engine's flat buffers [q | policy | log_alpha].
@@ -14,6 +15,10 @@
 
 Extra kwargs: `dsact_noise` = "device" (default) | "reference" (draw eps1, eps2 and the three z's of one update from torch's
 CPU generator in the reference's order), `dsact_max_batch`, `seed`.
+`dsact_gemm` = "fp32" | "bf16x3" | "bf16" (as in `dsac_v2`) selects the MLP engine in that arithmetic, and `dsact_graph`
+(default True) its captured steps.  It takes MLP approximators with the policy std_type "mlp_shared" (critic and policy may
+then differ in hidden_sizes and activation); any other approximator raises NotImplementedError with `dsact_gemm`.  Without
+`dsact_gemm` every configuration runs on the head-wise fp32 engine.
 """
 __all__ = ["ApproxContainer", "DSAC_V1"]
 
@@ -32,6 +37,7 @@ from dsact_host import load_full_state_dict as _load_full_state
 from dsact_host import net_kwargs
 
 from dsac_v2_b200 import _lib
+from dsac_v2_b200.engine import Engine, make_config, make_v1_options
 from dsac_v2_b200.engine_cnn import CnnEngine, make_cnn_config, make_heads_config
 
 # where the engine's 16-slot statistics carry DSAC_V1's tb_info (dsac_v1.py:172-181)
@@ -65,6 +71,30 @@ class ApproxContainer(nn.Module):
             raise NotImplementedError("the CUDA engine implements linear output activations")
         if pi_args["action_distribution_cls"].__name__ not in _lib.ACT_DISTS:
             raise NotImplementedError("the CUDA engine implements TanhGaussDistribution and GaussDistribution")
+        self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
+        self._engine = None
+        self._user_seed = kwargs.get("seed", None)
+        self._attachments = []
+        self._register_state_dict_hook(_detach_state_dict)
+        self._gemm = kwargs.get("dsact_gemm", None)
+        if self._gemm is not None:   # the MLP engine (dsact_v1_create)
+            if cnn or pi_args["std_type"] != "mlp_shared":
+                raise NotImplementedError(
+                    "dsact_gemm: DSAC_V1 runs on the MLP engine with MLP approximators and the policy std_type 'mlp_shared' "
+                    "(TanhGaussDistribution or GaussDistribution) only; drop dsact_gemm for the head-wise fp32 engine")
+            if self._gemm not in _lib.GEMM_MODES:
+                raise ValueError(f"dsact_gemm must be one of {sorted(_lib.GEMM_MODES)}, got {self._gemm!r}")
+            self._cfg_args = dict(
+                obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"], hidden_q=q_args["hidden_sizes"],
+                hidden_pi=pi_args["hidden_sizes"], act_q=q_args["hidden_activation"], act_pi=pi_args["hidden_activation"],
+                gemm_mode=self._gemm, use_graph=kwargs.get("dsact_graph", True), gamma=kwargs.get("gamma", 0.99),
+                tau=kwargs.get("tau", 0.005), delay_update=kwargs.get("delay_update", 2), auto_alpha=kwargs.get("auto_alpha", True),
+                alpha=kwargs.get("alpha", 0.2), lr_q=kwargs["value_learning_rate"], lr_pi=kwargs["policy_learning_rate"],
+                lr_alpha=kwargs["alpha_learning_rate"], min_log_std=pi_args["min_log_std"], max_log_std=pi_args["max_log_std"],
+                act_dist=pi_args["action_distribution_cls"].__name__)
+            self._v1 = make_v1_options(kwargs.get("bound", True), kwargs.get("TD_bound", 20))
+            self._make = make_config
+            return
         if q_args["hidden_activation"] != pi_args["hidden_activation"]:
             raise NotImplementedError("the head-wise engine takes one hidden activation for critic and policy")
         common = dict(gamma=kwargs.get("gamma", 0.99), tau=kwargs.get("tau", 0.005), delay_update=kwargs.get("delay_update", 2),
@@ -86,11 +116,6 @@ class ApproxContainer(nn.Module):
             self._make = make_heads_config
             self._cfg_args = dict(obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"], hidden=q_args["hidden_sizes"],
                                   std_type=pi_args["std_type"], **common)
-        self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
-        self._engine = None
-        self._user_seed = kwargs.get("seed", None)
-        self._attachments = []
-        self._register_state_dict_hook(_detach_state_dict)
 
     def create_action_distributions(self, logits):
         return self.policy.get_act_dist(logits)
@@ -112,7 +137,8 @@ class ApproxContainer(nn.Module):
             self._engine = eng = None
         if eng is None:
             cfg = self._make(max_batch=self._max_batch, **self._cfg_args)
-            eng = self._engine = CnnEngine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim)
+            lim = (self.policy.act_high_lim, self.policy.act_low_lim)
+            eng = self._engine = CnnEngine(cfg, device, *lim) if self._gemm is None else Engine(cfg, device, *lim, v1=self._v1)
             eng.seed(0x5DEECE66D if self._user_seed is None else int(self._user_seed))
         train, targ = self._flat_groups()
         with torch.no_grad():
@@ -127,7 +153,7 @@ class ApproxContainer(nn.Module):
                     off += n
                 assert off == flat.numel(), "flat layout does not match the module"
 
-    def engine(self, batch: int = 0) -> CnnEngine:
+    def engine(self, batch: int = 0) -> Engine:
         if self.log_alpha.device.type != "cuda" or self._engine is None:
             raise _lib.DsactError(
                 "DSAC_V1's update path runs only on the CUDA engine (libdsact.so, sm_90a); "

@@ -12,7 +12,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import Batch, Buffers, Config, Layout, Noise, Replay, check
+from ._lib import Batch, Buffers, Config, Layout, Noise, Replay, V1Options, check
 
 STAT_KEYS = [
     "DSAC2/critic_avg_q1-RL iter",
@@ -63,9 +63,20 @@ def make_config(obs_dim: int, act_dim: int, hidden_q: Sequence[int], hidden_pi: 
     return c
 
 
-def query_layout(cfg: Config) -> Layout:
+def make_v1_options(bound: bool = True, td_bound: float = 20.0) -> V1Options:
+    """DSAC_V1's settings (reference dsac_v1.py:79-80) for an MLP-engine handle: `bound` selects the bounded critic loss
+    (else the Gaussian NLL), `td_bound` is `TD_bound`."""
+    v = V1Options()
+    v.abi_version, v.bound, v.td_bound = _lib.ABI_VERSION, int(bool(bound)), float(td_bound)
+    return v
+
+
+def query_layout(cfg: Config, v1: Optional[V1Options] = None) -> Layout:
     out = Layout()
-    check(_lib.load().dsact_query_layout(C.byref(cfg), C.byref(out)))
+    if v1 is None:
+        check(_lib.load().dsact_query_layout(C.byref(cfg), C.byref(out)))
+    else:
+        check(_lib.load().dsact_v1_query_layout(C.byref(cfg), C.byref(v1), C.byref(out)))
     return out
 
 
@@ -86,9 +97,11 @@ class Engine:
     _query, _create = "dsact_query_layout", "dsact_create"
 
     def __init__(self, cfg: Config, device: torch.device, act_high: torch.Tensor, act_low: torch.Tensor, *,
-                 workspace_fill: float = 0.0):
+                 workspace_fill: float = 0.0, v1: Optional[V1Options] = None):
         """`workspace_fill`: the value the scratch workspace holds when it is bound.  No step depends on it: every region a
-        step reads is written first by that step, or by dsact_bind (arena_views()["slabs"])."""
+        step reads is written first by that step, or by dsact_bind (arena_views()["slabs"]).
+        `v1` (`make_v1_options`): a DSAC_V1 handle of the MLP engine (dsact_v1_create): one critic, flat layout
+        [q | policy | log_alpha], the reference's `dsac_v1.ApproxContainer` names."""
         if not torch.cuda.is_available():
             raise _lib.DsactError("the DSAC-T update engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
@@ -98,8 +111,12 @@ class Engine:
             raise _lib.DsactError(f"engine device must be CUDA, got {self.device}")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
+        self.v1 = v1
         self.layout = L = Layout()
-        check(getattr(self.lib, self._query)(C.byref(cfg), C.byref(L)))
+        if v1 is None:
+            check(getattr(self.lib, self._query)(C.byref(cfg), C.byref(L)))
+        else:
+            check(self.lib.dsact_v1_query_layout(C.byref(cfg), C.byref(v1), C.byref(L)))
         with torch.cuda.device(self.device):
             z = lambda n: torch.zeros(int(n), dtype=torch.float32, device=self.device)
             self.params, self.targets = z(L.n_params), z(L.n_targets)
@@ -110,7 +127,10 @@ class Engine:
             self.act_high = _f32c(torch.as_tensor(act_high).reshape(-1), self.device).clone()
             self.act_low = _f32c(torch.as_tensor(act_low).reshape(-1), self.device).clone()
             h = C.c_void_p()
-            check(getattr(self.lib, self._create)(C.byref(cfg), self.device.index, C.byref(h)))
+            if v1 is None:
+                check(getattr(self.lib, self._create)(C.byref(cfg), self.device.index, C.byref(h)))
+            else:
+                check(self.lib.dsact_v1_create(C.byref(cfg), C.byref(v1), self.device.index, C.byref(h)))
             self.h = h
             self._stats_host = torch.zeros(_lib.NUM_STATS, dtype=torch.float32).pin_memory()
             self._bind()
@@ -408,12 +428,14 @@ class Engine:
 
     # ---- weights in the reference's state_dict schema -----------------------------------
     def _schema(self):
-        """[(key, flat name, offset, shape)] for every tensor of the flat layout (include/dsact.h)."""
+        """[(key, flat name, offset, shape)] for every tensor of the flat layout (include/dsact.h).  DSAC_V1 handles walk
+        the one critic `q` (dsac_v1.ApproxContainer) instead of `q1`, `q2`."""
         c = self.cfg
         q_sizes = [c.obs_dim + c.act_dim] + [c.hidden_q[j] for j in range(c.n_hidden_q)] + [2]
         pi_sizes = [c.obs_dim] + [c.hidden_pi[j] for j in range(c.n_hidden_pi)] + [2 * c.act_dim]
         out, off = [], 0
-        for net, inner, sizes in (("q1", "q", q_sizes), ("q2", "q", q_sizes), ("policy", "policy", pi_sizes)):
+        critics = ("q",) if getattr(self, "v1", None) is not None else ("q1", "q2")
+        for net, inner, sizes in tuple((n, "q", q_sizes) for n in critics) + (("policy", "policy", pi_sizes),):
             for j in range(len(sizes) - 1):
                 for leaf, shape in (("weight", (sizes[j + 1], sizes[j])), ("bias", (sizes[j + 1],))):
                     n = 1

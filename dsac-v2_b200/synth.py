@@ -45,6 +45,12 @@ ASYM_CONFIGS = {
                       act_lim=1.0),
 }
 
+# The reference's DSAC_V1 MLP example (example_train/dsacv1_mlp_hopper_offserial.py): Hopper's observation and action
+# sizes, 256x3 GELU critic and policy.  Kept out of CONFIGS, whose entries the DSAC-T tests walk.
+EXAMPLE_CONFIGS = {
+    "hopper": dict(obs_dim=11, act_dim=3, hidden=(256, 256, 256), act_lim=1.0),
+}
+
 # BASELINE.json config 5 (gym_carracingraw, SURVEY.md §8f rank 1): conv encoder `type_2` + separate mean / log_std
 # heads (csrc/cnn_engine.cuh; oracle/dsact_oracle.py:OracleDSACTCNN, tests/golden/cnn_carracing_b4.npz).
 CNN_CONFIGS = {
@@ -81,8 +87,10 @@ def _rng(*key) -> np.random.Generator:
 
 
 def mlp_config(name: str) -> dict:
-    """A named MLP configuration of CONFIGS or ASYM_CONFIGS."""
-    return CONFIGS[name] if name in CONFIGS else ASYM_CONFIGS[name]
+    """A named MLP configuration of CONFIGS, ASYM_CONFIGS or EXAMPLE_CONFIGS."""
+    if name in CONFIGS:
+        return CONFIGS[name]
+    return ASYM_CONFIGS[name] if name in ASYM_CONFIGS else EXAMPLE_CONFIGS[name]
 
 
 def hidden_sizes(cfg: dict) -> tuple:

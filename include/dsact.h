@@ -219,6 +219,24 @@ int dsact_dp_step(dsact_handle *h, const dsact_batch *batch, const dsact_noise *
 int dsact_dp_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx, const dsact_noise *noise,
                          int64_t global_batch, int64_t iteration, void *stream);
 
+/* ---- DSAC_V1 on the MLP engine ---------------------------------------------------------------------------------------
+ * DSAC_V1 (reference dsac_v1.py:56-273: ONE distributional critic, fixed TD bound) with MLP approximators and the policy's
+ * "mlp_shared" std type, on the tensor-core / SIMT engine of dsact_create: the same dsact_config, in which critic and policy
+ * may differ in depth, width and activation, in all three gemm_modes, with use_graph on or off, plus the two settings
+ * DSAC-T lacks.
+ * Flat layout: params = [ q | policy | log_alpha ], targets = [ q_target | policy_target ] (n_params = n_q + n_pi + 1,
+ * n_targets = n_q + n_pi).  The handle takes dsact_step, dsact_step_host, dsact_stage_host / _release, dsact_replay_*,
+ * dsact_read_stats (DSAC_V1's tb_info in slots 0, 2, 6, 8, 9, 10, 11) and dsact_profile_step with the semantics they
+ * have for a DSAC-T handle; the split and data-parallel calls (dsact_grad_phase1/2, dsact_compute_grads, dsact_apply,
+ * dsact_dp_*) return DSACT_EINVAL. */
+typedef struct dsact_v1_options {
+  int32_t abi_version;   /* = DSACT_ABI_VERSION */
+  int32_t bound;         /* dsac_v1.py `bound` (:80): 1 = bounded loss (:219-229), 0 = Gaussian NLL (:231) */
+  double td_bound;       /* dsac_v1.py `TD_bound` (:79, default 20): finite, > 0 */
+} dsact_v1_options;
+int dsact_v1_query_layout(const dsact_config *cfg, const dsact_v1_options *v1, dsact_layout *out);
+int dsact_v1_create(const dsact_config *cfg, const dsact_v1_options *v1, int device, dsact_handle **out);
+
 /* ---- head-wise fp32 engine: CNN approximators and the variants the MLP engine does not implement ---------------------
  * CNN approximators (BASELINE config 5, reference networks/cnn.py:30-53,151-240,383-461), value_func_type /
  * policy_func_type = "CNN": every network is a private conv encoder (Conv2d + ReLU per layer, no padding) followed by two
@@ -230,7 +248,9 @@ int dsact_dp_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int
  * The same engine also carries the variants of the reference that keep network outputs in separate heads or need another
  * loss, all in fp32: no encoder (n_conv = 0: the observation vector feeds the heads), one two-output head per critic
  * (q_heads = 1, networks/mlp.py), the policy's std types (pi_std), the plain Gaussian action distribution (act_dist) and
- * DSAC_V1 (algo = 1: ONE critic, flat layout [q | policy | log_alpha], dsac_v1.py).
+ * DSAC_V1 (algo = 1: ONE critic, flat layout [q | policy | log_alpha], dsac_v1.py).  DSAC_V1 with MLP approximators and
+ * the "mlp_shared" policy also runs on the MLP engine (dsact_v1_create above), with its tensor-core modes, captured steps,
+ * host staging and replay-fused steps.
  * dsact_cnn_create returns a dsact_handle that every dsact_* entry point above takes, with the same semantics, except:
  *  - dsact_step_host, dsact_stage_host / _release, dsact_replay_step, dsact_dp_replay_step, dsact_profile_step and
  *    dsact_test_gemm return DSACT_EINVAL (the MLP engine implements them);
