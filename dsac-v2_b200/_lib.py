@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DSACT_LIB: kernel-development aid (A/B of two builds on one GPU box); the product is libdsact.so beside this file
 LIB_PATH = os.environ.get("DSACT_LIB") or os.path.join(_HERE, "libdsact.so")
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 MAX_HIDDEN = 6
 NUM_STATS = 16
 
@@ -98,6 +98,21 @@ class Replay(C.Structure):
                 ("capacity", C.c_int64)]
 
 
+class TestLayer(C.Structure):
+    """dsact_test_layer: one problem of a dsact_test_gemm group."""
+    _fields_ = [("M", C.c_int32), ("N", C.c_int32), ("K0", C.c_int32), ("K1", C.c_int32), ("kB1", C.c_int32),
+                ("A0", _fp), ("A1", _fp), ("B", _fp), ("lda0", C.c_int32), ("lda1", C.c_int32), ("ldb", C.c_int32),
+                ("epi", C.c_int32), ("act", C.c_int32), ("bias", _fp), ("Zout", _fp), ("Zin", _fp), ("ldz", C.c_int32),
+                ("colsum", _fp), ("C", _fp), ("ldc", C.c_int32), ("img", _fp), ("img_pitch", C.c_int32),
+                ("img_plane", C.c_int64)]
+
+
+class TestChainPass(C.Structure):
+    """dsact_test_chain_pass: one pass of a dsact_test_chain launch."""
+    _fields_ = [("M", C.c_int32), ("x0", _fp), ("x1", _fp), ("Zout", _fp * MAX_HIDDEN), ("Zin", _fp * MAX_HIDDEN),
+                ("img", _fp * MAX_HIDDEN), ("colsum", _fp * MAX_HIDDEN), ("out", _fp)]
+
+
 # every symbol include/dsact.h declares: (restype, argtypes)
 IPC_HANDLE_BYTES = 64   # DSACT_IPC_HANDLE_BYTES
 DP_MAX_RANKS = 8        # DSACT_DP_MAX_RANKS
@@ -137,8 +152,9 @@ SYMBOLS = {
     "dsact_launch_count": (C.c_int64, [C.c_void_p]),
     "dsact_last_call_launches": (C.c_int32, [C.c_void_p]),
     "dsact_cnn_test_conv": (C.c_int, [C.c_int32] * 8 + [C.c_void_p] * 7 + [C.c_int32] * 4 + [C.c_void_p]),
-    "dsact_test_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
-                                  C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "dsact_test_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TestLayer), C.c_int32, C.c_int32, C.c_void_p]),
+    "dsact_test_chain": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32,
+                                   C.c_int32, C.c_void_p, C.POINTER(TestChainPass), C.c_int32, C.c_void_p]),
 }
 
 _lib = None

@@ -293,6 +293,7 @@ struct Group {
   const GemmProb& prob(int i) const { return i < MAXG ? g.p[i] : more[i - MAXG]; }
   float* wg_slab = nullptr;   // wgrad split slabs (default: the arena's, addressed like the gradient buffer)
   long long wg_stride = 0;
+  long long wg_off[TC_MAXG] = {};   // with wg_slab: where problem i's partial tiles start inside each slab
   int wg_nslabs = 0;
   Group() { g.n = 0; }
   void push(const GemmProb& p, const TcExtra& e) { x[n] = e; prob(n) = p; ++n; g.n = n < MAXG ? n : MAXG; }
@@ -376,7 +377,7 @@ static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas 
     p.epi = s.epi; p.act = s.act;
     if (variant == V_WGRAD) {  // fixed slab count: empty splits store zeros so that the reduction is always valid
       p.epi = EPI_PARTIAL;
-      if (G.wg_slab) { p.ksplit = G.wg_nslabs; p.C = G.wg_slab; p.split_stride = G.wg_stride; }
+      if (G.wg_slab) { p.ksplit = G.wg_nslabs; p.C = G.wg_slab + G.wg_off[i]; p.split_stride = G.wg_stride; }
       else {
         p.ksplit = h->ar.nslabs;
         p.C = h->W() + h->ar.slabs + (s.C - h->buf.grads);
@@ -672,55 +673,78 @@ static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
   }
 }
 
+// Where one pass of a chain reads and writes, resolved to pointers and images: per layer j the weight image, and per hidden
+// layer j the act'(z_j) store / load (null: none), the image of its output (p null: none) and, in dgrad, its bias
+// gradient (null: none).
+struct ChainIo {
+  Img w[DSACT_MAX_HIDDEN + 1];
+  float* z[DSACT_MAX_HIDDEN] = {};
+  Img img[DSACT_MAX_HIDDEN];
+  float* colsum[DSACT_MAX_HIDDEN] = {};
+};
+
 // forward chain of one pass: out = head(act(...act(in W_0^T + b_0)...))
-static ChainPass& chain_fwd_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const float* Wbase, const ImgSlot* wslots,
-                           const Img& in0, int k0, const Img& in1, int k1, int kB1, int B, int act,
-                           const int64_t* zout_off, const ImgSlot* himg, float* out) {
+static ChainPass& chain_fwd_layers(ChainBuild& cb, const Net& net, const float* Wbase, const ChainIo& io, const Img& in0, int k0,
+                                   const Img& in1, int k1, int kB1, int B, int act, float* out) {
   ChainPass& P = cb.begin(in0, in1, B);
-  float* W = h->W();
   for (int j = 0; j <= net.L; ++j) {
-    const Img wim = h->img(wslots[j], net.s[j + 1]);
-    ChainLayer& L = j == 0 ? cb.layer(P, wim, false, net.s[1], k0, k1, kB1) : cb.layer(P, wim, false, net.s[j + 1], net.s[j], 0, 0);
+    ChainLayer& L = j == 0 ? cb.layer(P, io.w[0], false, net.s[1], k0, k1, kB1) : cb.layer(P, io.w[j], false, net.s[j + 1], net.s[j], 0, 0);
     const bool last = j == net.L;
     L.epi = last ? EPI_STORE : EPI_BIAS_ACT;
     L.act = act;
     L.bias = Wbase + net.b[j];
     if (last) L.C = out;
     else {
-      if (zout_off) L.Zout = W + zout_off[j];
-      if (himg) {
-        const Img im = h->img(himg[j], B);
-        L.img = im.p; L.img_pitch = im.pitch; L.img_plane = im.plane;
-      }
+      L.Zout = io.z[j];
+      L.img = io.img[j].p; L.img_pitch = io.img[j].pitch; L.img_plane = io.img[j].plane;
     }
   }
   return P;
 }
 
 // dgrad chain of one pass: dz_{j-1} = (dz_j W_j) (.) act'(z_{j-1}) for j = L..1 (+ dAct = dz_0 W_0[:, act columns])
-static ChainPass& chain_dgrad_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const ImgSlot* wslots, const Img& dout,
-                             int B, int act, const int64_t* zin_off, float* gbase /*bias grads of this net or null*/,
-                             const ImgSlot* dzimg /*or null*/, float* dact_out, int act_col_img, int act_cols) {
+static ChainPass& chain_dgrad_layers(ChainBuild& cb, const Net& net, const ChainIo& io, const Img& dout, int B, int act,
+                                     float* dact_out, int act_col_img, int act_cols) {
   const Img none;
   ChainPass& P = cb.begin(dout, none, B);
-  float* W = h->W();
   for (int j = net.L; j >= 1; --j) {
-    const Img wim = h->img(wslots[j], net.s[j + 1]);   // rows = reduction (outputs of layer j), width = inputs
-    ChainLayer& L = cb.layer(P, wim, true, net.s[j], net.s[j + 1], 0, 0);
+    ChainLayer& L = cb.layer(P, io.w[j], true, net.s[j], net.s[j + 1], 0, 0);   // image rows = reduction, width = inputs
     L.epi = EPI_DACT; L.act = act;
-    L.Zin = W + zin_off[j - 1];
-    L.colsum = gbase ? gbase + net.b[j - 1] : nullptr;
-    if (dzimg) {
-      const Img im = h->img(dzimg[j - 1], B);
-      L.img = im.p; L.img_pitch = im.pitch; L.img_plane = im.plane;
-    }
+    L.Zin = io.z[j - 1];
+    L.colsum = io.colsum[j - 1];
+    L.img = io.img[j - 1].p; L.img_pitch = io.img[j - 1].pitch; L.img_plane = io.img[j - 1].plane;
   }
   if (dact_out) {
-    const Img wim = h->img(wslots[0], net.s[1]).cols(act_col_img, act_cols);
-    ChainLayer& L = cb.layer(P, wim, true, act_cols, net.s[1], 0, 0);
+    ChainLayer& L = cb.layer(P, io.w[0].cols(act_col_img, act_cols), true, act_cols, net.s[1], 0, 0);
     L.epi = EPI_STORE; L.C = dact_out;
   }
   return P;
+}
+
+// The step's passes: arena slots resolved to the pointers and images above
+static ChainIo chain_io(const MlpHandle* h, const Net& net, const ImgSlot* wslots, int B, const int64_t* z_off, const ImgSlot* himg) {
+  ChainIo io;
+  float* W = h->W();
+  for (int j = 0; j <= net.L; ++j) io.w[j] = h->img(wslots[j], net.s[j + 1]);
+  for (int j = 0; j < net.L; ++j) {
+    if (z_off) io.z[j] = W + z_off[j];
+    if (himg) io.img[j] = h->img(himg[j], B);
+  }
+  return io;
+}
+
+static ChainPass& chain_fwd_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const float* Wbase, const ImgSlot* wslots,
+                           const Img& in0, int k0, const Img& in1, int k1, int kB1, int B, int act,
+                           const int64_t* zout_off, const ImgSlot* himg, float* out) {
+  return chain_fwd_layers(cb, net, Wbase, chain_io(h, net, wslots, B, zout_off, himg), in0, k0, in1, k1, kB1, B, act, out);
+}
+
+static ChainPass& chain_dgrad_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const ImgSlot* wslots, const Img& dout,
+                             int B, int act, const int64_t* zin_off, float* gbase /*bias grads of this net or null*/,
+                             const ImgSlot* dzimg /*or null*/, float* dact_out, int act_col_img, int act_cols) {
+  ChainIo io = chain_io(h, net, wslots, B, zin_off, dzimg);
+  for (int j = 0; j < net.L && gbase; ++j) io.colsum[j] = gbase + net.b[j];
+  return chain_dgrad_layers(cb, net, io, dout, B, act, dact_out, act_col_img, act_cols);
 }
 
 static unsigned long long dp_timeout_ns() {
@@ -2079,63 +2103,182 @@ int dsact_profile_step(dsact_handle* hh, const dsact_batch* batch, const dsact_n
 int64_t dsact_launch_count(const dsact_handle* h) { return h ? h->launches : 0; }
 int32_t dsact_last_call_launches(const dsact_handle* h) { return h ? h->last_launches : 0; }
 
-int dsact_test_gemm(dsact_handle* hh, int32_t variant, const float* A, int32_t lda, const float* B, int32_t ldb,
-                    const float* bias, float* C, int32_t ldc, int32_t M, int32_t N, int32_t K, void* stream) {
+// Scratch of the test hooks: one cudaMalloc per image or slab region, freed when the hook returns (after its stream has
+// been synchronised).
+struct HookScratch {
+  std::vector<void*> mem;
+  cudaError_t err = cudaSuccess;
+  void* get(size_t bytes) {
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, bytes);
+    if (e != cudaSuccess) { if (err == cudaSuccess) err = e; return nullptr; }
+    mem.push_back(p);
+    return p;
+  }
+  Img img(int rows, int width) {   // the arena's image geometry
+    Img i;
+    i.rows = rows; i.width = width; i.pitch = (width + 7) / 8 * 8; i.plane = round64((int64_t)rows * i.pitch);
+    i.p = static_cast<__nv_bfloat16*>(get((size_t)i.plane * 4));
+    return i;
+  }
+  ~HookScratch() { for (void* p : mem) cudaFree(p); }
+};
+
+static int finish_hook(MlpHandle* h, Ctx& c, const HookScratch& mem) {
+  const cudaError_t e = cudaStreamSynchronize(c.s);
+  const cudaError_t err = mem.err != cudaSuccess ? mem.err : (c.err != cudaSuccess ? c.err : e);
+  if (err != cudaSuccess) return fail(DSACT_ECUDA, "launch failed: %s", cudaGetErrorString(err));
+  h->launches += c.launches;
+  return DSACT_OK;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+int dsact_test_gemm(dsact_handle* hh, int32_t variant, const dsact_test_layer* probs, int32_t n, int32_t max_ctas, void* stream) {
   if (!hh) return fail(DSACT_EINVAL, "null handle");
   int rc = check_mlp(hh, "dsact_test_gemm");
   if (rc) return rc;
   MlpHandle* h = mlp(hh);
-  if (variant < 0 || variant > 2 || M < 1 || N < 1 || K < 1) return fail(DSACT_EINVAL, "bad argument");
+  if (variant < 0 || variant > 2 || !probs || n < 1 || n > TC_MAXG || max_ctas < 0) return fail(DSACT_EINVAL, "bad argument");
+  const bool tc = h->tc();
+  for (int i = 0; i < n; ++i) {
+    const dsact_test_layer& t = probs[i];
+    const int epi_ok = variant == V_FWD ? EPI_BIAS_ACT : (variant == V_DGRAD ? EPI_DACT : EPI_STORE);
+    if (t.M < 1 || t.N < 1 || t.K0 < 1 || t.K1 < 0 || !t.A0 || !t.B || (!t.C && !t.img) || t.act < 0 || t.act > ACT_SELU ||
+        (t.epi != EPI_STORE && t.epi != epi_ok))
+      return fail(DSACT_EINVAL, "problem %d: bad argument", i);
+    if (t.K1 > 0 && (variant != V_FWD || !t.A1 || t.kB1 < t.K0 || t.kB1 % 8))
+      return fail(DSACT_EINVAL, "problem %d: a second K segment needs the forward variant, A1 and kB1 >= K0, kB1 %% 8 == 0", i);
+    if (t.epi == EPI_DACT && !t.Zin) return fail(DSACT_EINVAL, "problem %d: the derivative epilogue needs Zin", i);
+    if (t.img && (!tc || variant == V_WGRAD || t.img_pitch < (t.N + 7) / 8 * 8 || t.img_pitch % 8 || t.img_plane < (int64_t)t.M * t.img_pitch))
+      return fail(DSACT_EINVAL, "problem %d: bad output image", i);
+    if (tc && variant == V_WGRAD && (t.ldc != t.N || !aligned16(t.C)))
+      return fail(DSACT_EINVAL, "problem %d: the tensor-core weight gradient needs a contiguous, 16-byte aligned C", i);
+  }
   CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = tc;
+  HookScratch mem;
+  ImgBatch ibt;
   Group G;
-  GemmProb p = prob_zero();
-  p.A[0] = A; p.lda[0] = lda; p.B[0] = B; p.ldb[0] = ldb; p.K[0] = K;
-  p.M = M; p.N = N; p.C = C; p.ldc = ldc; p.bias = variant == V_FWD ? bias : nullptr;
-  p.epi = variant == V_WGRAD ? EPI_ATOMIC : EPI_STORE;
-  G.push(p, TcExtra());
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = h->tc();
-  void* scratch = nullptr;
-  if (h->tc()) {  // test hook only: scratch images (and slabs) come from cudaMalloc, not from the caller
-    if (variant == V_WGRAD && ldc != N) return fail(DSACT_EINVAL, "tc wgrad test needs contiguous C");
-    const int a_rows = variant == V_WGRAD ? K : M, a_w = variant == V_WGRAD ? M : K;
-    const int b_rows = variant == V_FWD ? N : K, b_w = variant == V_FWD ? K : N;
-    auto mk = [&](int rows, int w, size_t& off) {
-      Img i; i.rows = rows; i.width = w; i.pitch = (w + 7) / 8 * 8; i.plane = round64((int64_t)rows * i.pitch);
-      off = (off + 255) / 256 * 256; size_t o = off; off += (size_t)i.plane * 4; i.p = reinterpret_cast<__nv_bfloat16*>(o);
-      return i;
-    };
-    size_t off = 0;
-    Img ia = mk(a_rows, a_w, off), ib = mk(b_rows, b_w, off);
-    const int nslabs = 4;
-    off = (off + 255) / 256 * 256;
-    const size_t slab_off = off;
-    if (variant == V_WGRAD) off += sizeof(float) * (size_t)nslabs * M * N;
-    CUDA_TRY(cudaMalloc(&scratch, off + 256));
-    ia.p = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<uintptr_t>(scratch) + reinterpret_cast<uintptr_t>(ia.p));
-    ib.p = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<uintptr_t>(scratch) + reinterpret_cast<uintptr_t>(ib.p));
-    ImgBatch ibt;
-    ibt.add(A, lda, ia, a_rows, a_w);
-    ibt.add(B, ldb, ib, b_rows, b_w);
+  long long slab_floats = 0;
+  for (int i = 0; i < n; ++i) {
+    const dsact_test_layer& t = probs[i];
+    GemmProb p = prob_zero();
+    TcExtra x;
+    p.A[0] = t.A0; p.lda[0] = t.lda0; p.K[0] = t.K0;
+    p.B[0] = t.B; p.ldb[0] = t.ldb;
+    if (t.K1 > 0) { p.A[1] = t.A1; p.lda[1] = t.lda1; p.K[1] = t.K1; p.B[1] = t.B + t.K0; p.ldb[1] = t.ldb; x.kB0[1] = t.kB1; }
+    p.M = t.M; p.N = t.N; p.C = t.C; p.ldc = t.ldc;
+    p.epi = variant == V_WGRAD ? EPI_ATOMIC : t.epi; p.act = t.act;
+    if (variant != V_WGRAD) { p.bias = t.bias; p.Zout = t.Zout; p.Zin = t.Zin; p.ldz = t.ldz; p.colsum = t.colsum; }
+    if (tc) {   // images as the step forms them: operands by image_kernel, the B segments at their image columns
+      const int a_rows = variant == V_WGRAD ? t.K0 : t.M, a_w = variant == V_WGRAD ? t.M : t.K0;
+      ibt.reserve(h, c, 3);
+      x.a[0] = mem.img(a_rows, a_w);
+      ibt.add(t.A0, t.lda0, x.a[0], a_rows, a_w);
+      if (t.K1 > 0) { x.a[1] = mem.img(t.M, t.K1); ibt.add(t.A1, t.lda1, x.a[1], t.M, t.K1); }
+      if (variant == V_FWD) {
+        x.b = mem.img(t.N, t.K1 > 0 ? t.kB1 + t.K1 : t.K0);
+        ibt.add(t.B, t.ldb, x.b, t.N, t.K0, t.K1, t.kB1);
+      } else {
+        x.b = mem.img(t.K0, t.N);
+        ibt.add(t.B, t.ldb, x.b, t.K0, t.N);
+      }
+      if (t.img) {
+        x.out.p = static_cast<__nv_bfloat16*>(t.img); x.out.rows = t.M; x.out.width = t.N;
+        x.out.pitch = t.img_pitch; x.out.plane = t.img_plane;
+      }
+      G.wg_off[i] = slab_floats;
+      if (variant == V_WGRAD) slab_floats += ((long long)t.M * t.N + 3) / 4 * 4;
+    }
+    G.push(p, x);
+  }
+  const int nslabs = 4;
+  if (tc) {
     ibt.launch(h, c);
-    G.x[0].a[0] = ia; G.x[0].b = ib;
     if (variant == V_WGRAD) {
-      G.wg_slab = reinterpret_cast<float*>(reinterpret_cast<uintptr_t>(scratch) + slab_off);
-      G.wg_stride = (long long)M * N; G.wg_nslabs = nslabs;
+      G.wg_slab = static_cast<float*>(mem.get(sizeof(float) * (size_t)nslabs * slab_floats));
+      G.wg_stride = slab_floats; G.wg_nslabs = nslabs;
     }
   }
-  launch_group(h, G, variant, c);
-  if (h->tc() && variant == V_WGRAD && c.err == cudaSuccess) {
-    grad_reduce_kernel<<<64, 256, 0, s>>>(C, G.wg_slab, (long long)M * N, G.wg_nslabs, (long long)M * N);
-    c.done();
+  if (mem.err == cudaSuccess) launch_group(h, G, variant, c, max_ctas);
+  if (tc && variant == V_WGRAD && c.err == cudaSuccess && mem.err == cudaSuccess) {
+    for (int i = 0; i < n; ++i) {
+      grad_reduce_kernel<<<64, 256, 0, c.s>>>(probs[i].C, G.wg_slab + G.wg_off[i], (long long)probs[i].M * probs[i].N, nslabs,
+                                               G.wg_stride);
+      c.done();
+    }
+    c.check();
   }
-  cudaError_t e = cudaSuccess;
-  if (scratch) { e = cudaStreamSynchronize(s); cudaFree(scratch); }
-  if (c.err != cudaSuccess || e != cudaSuccess)
-    return fail(DSACT_ECUDA, "launch failed: %s", cudaGetErrorString(c.err != cudaSuccess ? c.err : e));
-  h->launches += c.launches;
-  return DSACT_OK;
+  return finish_hook(h, c, mem);
+}
+
+int dsact_test_chain(dsact_handle* hh, int32_t dgrad, int32_t L, const int32_t* sizes, int32_t K0, int32_t K1, int32_t kB1,
+                     int32_t act, const float* params, const dsact_test_chain_pass* passes, int32_t n_passes, void* stream) {
+  if (!hh) return fail(DSACT_EINVAL, "null handle");
+  int rc = check_mlp(hh, "dsact_test_chain");
+  if (rc) return rc;
+  MlpHandle* h = mlp(hh);
+  if (!h->tc()) return fail(DSACT_EINVAL, "dsact_test_chain: the layer-chain kernel runs in the tensor-core modes only");
+  if (!sizes || !params || !passes || L < 0 || L > DSACT_MAX_HIDDEN || n_passes < 1 || n_passes > CH_MAX_PASSES ||
+      act < 0 || act > ACT_SELU || (dgrad != 0 && dgrad != 1) || (dgrad && L < 1))
+    return fail(DSACT_EINVAL, "bad argument");
+  for (int j = 0; j <= L + 1; ++j)
+    if (sizes[j] < 1 || (j > 0 && sizes[j] > 256) || (j > 0 && j <= L && sizes[j] % 8))
+      return fail(DSACT_EINVAL, "sizes[%d] = %d: widths are >= 1, layer outputs <= 256, hidden widths multiples of 8", j, sizes[j]);
+  if (K0 < 1 || K1 < 0 || K0 + K1 != sizes[0] || (K1 > 0 && (kB1 < K0 || kB1 % 8)))
+    return fail(DSACT_EINVAL, "layer-0 segments: K0 + K1 == sizes[0], kB1 >= K0, kB1 %% 8 == 0");
+  for (int i = 0; i < n_passes; ++i) {
+    const dsact_test_chain_pass& q = passes[i];
+    if (q.M < 1 || !q.x0 || (!dgrad && (!q.out || (K1 > 0 && !q.x1))) || (dgrad && q.out && K1 == 0))
+      return fail(DSACT_EINVAL, "pass %d: bad argument", i);
+    for (int j = 0; j < L && dgrad; ++j)
+      if (!q.Zin[j]) return fail(DSACT_EINVAL, "pass %d: Zin[%d] is null", i, j);
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  HookScratch mem;
+  ImgBatch ibt;
+  Net net;
+  net.build(sizes[0], sizes + 1, L, sizes[L + 1]);
+  ChainIo io;
+  for (int j = 0; j <= L; ++j) {   // weight images: layer 0's second segment at column kB1, as the critics' in the step
+    io.w[j] = mem.img(sizes[j + 1], j == 0 && K1 > 0 ? kB1 + K1 : sizes[j]);
+    ibt.reserve(h, c, 1);
+    if (j == 0) ibt.add(params + net.w[0], sizes[0], io.w[0], sizes[1], K0, K1, kB1);
+    else ibt.add(params + net.w[j], sizes[j], io.w[j], sizes[j + 1], sizes[j]);
+  }
+  ChainBuild cb(h->passes());
+  for (int i = 0; i < n_passes; ++i) {
+    const dsact_test_chain_pass& q = passes[i];
+    ChainIo pio = io;
+    for (int j = 0; j < L; ++j) {
+      pio.z[j] = dgrad ? const_cast<float*>(q.Zin[j]) : q.Zout[j];
+      pio.colsum[j] = dgrad ? q.colsum[j] : nullptr;
+      if (q.img[j]) {
+        Img& o = pio.img[j];
+        o.p = static_cast<__nv_bfloat16*>(q.img[j]); o.rows = q.M; o.width = sizes[j + 1];
+        o.pitch = (sizes[j + 1] + 7) / 8 * 8; o.plane = (long long)o.pitch * q.M;
+      }
+    }
+    const int w0 = dgrad ? sizes[L + 1] : K0;
+    ibt.reserve(h, c, 2);
+    const Img in0 = mem.img(q.M, w0);
+    ibt.add(q.x0, w0, in0, q.M, w0);
+    if (dgrad) {
+      chain_dgrad_layers(cb, net, pio, in0, q.M, act, q.out, kB1, K1);
+    } else {
+      Img in1;
+      if (K1 > 0) { in1 = mem.img(q.M, K1); ibt.add(q.x1, K1, in1, q.M, K1); }
+      chain_fwd_layers(cb, net, params, pio, in0, K0, in1, K1, kB1, q.M, act, q.out);
+    }
+  }
+  if (mem.err == cudaSuccess) {
+    ibt.launch(h, c);
+    launch_chain(h, cb, dgrad ? CLS_GEMM_DGRAD : CLS_GEMM_FWD, c);
+  }
+  return finish_hook(h, c, mem);
 }
 
 }  // extern "C"

@@ -475,6 +475,39 @@ class Engine:
 
     def test_gemm(self, variant: int, A: torch.Tensor, B: torch.Tensor, bias: Optional[torch.Tensor], C_out: torch.Tensor,
                   M: int, N: int, K: int):
+        """One plain problem (store epilogue) of `test_layers`."""
+        self.test_layers(variant, [dict(M=M, N=N, K0=K, A0=A, B=B, bias=bias, C=C_out)])
+
+    def test_layers(self, variant: int, probs, max_ctas: int = 0):
+        """dsact_test_gemm: one group of problems, each a dict of dsact_test_layer fields with tensors for the pointers
+        (leading dimensions default to the tensors' row strides; `img` is a [2, M, pitch] bf16 tensor)."""
+        arr = (_lib.TestLayer * len(probs))()
+        for t, p in zip(arr, probs):
+            for k, v in p.items():
+                if k == "img":
+                    t.img, t.img_pitch, t.img_plane = v.data_ptr(), v.stride(1), v.stride(0)
+                elif isinstance(v, torch.Tensor):
+                    setattr(t, k, v.data_ptr())
+                    ld = {"A0": "lda0", "A1": "lda1", "B": "ldb", "Zin": "ldz", "C": "ldc"}.get(k)
+                    if ld and ld not in p:
+                        setattr(t, ld, v.stride(0))
+                elif v is not None:
+                    setattr(t, k, v)
         with torch.cuda.device(self.device):
-            check(self.lib.dsact_test_gemm(self.h, variant, A.data_ptr(), A.stride(0), B.data_ptr(), B.stride(0),
-                                           _ptr(bias), C_out.data_ptr(), C_out.stride(0), M, N, K, self._stream()))
+            check(self.lib.dsact_test_gemm(self.h, variant, arr, len(probs), max_ctas, self._stream()))
+
+    def test_chain(self, dgrad: bool, sizes, K0: int, K1: int, kB1: int, act: int, params: torch.Tensor, passes):
+        """dsact_test_chain: one launch of the layer-chain kernel; `passes` are dicts of dsact_test_chain_pass fields
+        (Zout / Zin / img / colsum: lists per hidden layer, entries may be None; `img` entries [2, M, pitch] bf16)."""
+        arr = (_lib.TestChainPass * len(passes))()
+        for t, p in zip(arr, passes):
+            t.M = p["M"]
+            for k in ("x0", "x1", "out"):
+                setattr(t, k, _ptr(p.get(k)))
+            for k in ("Zout", "Zin", "img", "colsum"):
+                for j, v in enumerate(p.get(k) or []):
+                    getattr(t, k)[j] = _ptr(v)
+        sz = (C.c_int32 * len(sizes))(*sizes)
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_test_chain(self.h, int(dgrad), len(sizes) - 2, sz, K0, K1, kB1, act, params.data_ptr(), arr,
+                                            len(passes), self._stream()))

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define DSACT_ABI_VERSION 2
+#define DSACT_ABI_VERSION 3
 #define DSACT_MAX_HIDDEN 6
 #define DSACT_NUM_STATS 16
 
@@ -253,7 +253,7 @@ int dsact_v1_create(const dsact_config *cfg, const dsact_v1_options *v1, int dev
  * host staging and replay-fused steps.
  * dsact_cnn_create returns a dsact_handle that every dsact_* entry point above takes, with the same semantics, except:
  *  - dsact_step_host, dsact_stage_host / _release, dsact_replay_step, dsact_dp_replay_step, dsact_profile_step and
- *    dsact_test_gemm return DSACT_EINVAL (the MLP engine implements them);
+ *    dsact_test_gemm / dsact_test_chain return DSACT_EINVAL (the MLP engine implements them);
  *  - a DSAC_V1 handle (algo = 1) returns DSACT_EINVAL from the split and data-parallel calls (dsact_grad_phase1/2,
  *    dsact_compute_grads, dsact_apply, dsact_dp_export / _connect / _step);
  *  - phase 2's log_alpha gradient is this shard's additive share, and dsact_dp_step runs eagerly on `stream`. */
@@ -300,12 +300,59 @@ typedef struct dsact_profile {
 int dsact_profile_step(dsact_handle *h, const dsact_batch *batch, const dsact_noise *noise, int64_t iteration,
                        void *stream, dsact_profile *out);
 
-/* raw dense-layer entry for unit tests of the GEMM kernels, in the handle's gemm_mode:
- *  variant 0 (forward): C[M,N]  = A[M,K] * B[N,K]^T (+ bias[N])
- *  variant 1 (dgrad)  : C[M,N]  = A[M,K] * B[K,N]
- *  variant 2 (wgrad)  : C[M,N] += A[K,M]^T * B[K,N]   (split-K, atomic accumulate) */
-int dsact_test_gemm(dsact_handle *h, int32_t variant, const float *A, int32_t lda, const float *B, int32_t ldb,
-                    const float *bias, float *C, int32_t ldc, int32_t M, int32_t N, int32_t K, void *stream);
+/* Test hooks of the dense-layer kernels, in the handle's gemm_mode, on caller buffers (scratch images and weight-gradient
+ * slabs come from cudaMalloc; the call synchronises `stream`).
+ *
+ * dsact_test_gemm: one group of problems of one variant, lowered and launched as a step lowers and launches its GEMM
+ * groups (up to 16 problems; in fp32 mode a group of more than 8 is issued as two launches).
+ *  variant 0 (forward): C[M,N]  = epi(A0[M,K0] * B[N,K0]^T + A1[M,K1] * B[N,K0:K0+K1]^T)
+ *  variant 1 (dgrad)  : C[M,N]  = epi(A0[M,K0] * B[K0,N])
+ *  variant 2 (wgrad)  : C[M,N] += A0[K0,M]^T * B[K0,N]   (batch split into slabs, summed into C)
+ * epi (forward / dgrad): 0 store (+ bias[N]); 1 (forward) y = act(z), z = the product + bias, with Zout[M,ldc] (optional) = z (fp32
+ * mode) or act'(z) (tensor-core modes); 2 (dgrad) y = the product * act'(z) with act'(z) from Zin[M,ldz] (tensor-core
+ * modes; fp32 mode: z, the derivative taken in the epilogue), colsum[N] += column sums of y.
+ * kB1: column of the second segment inside B's image (K0 rounded up to 64 in the step).  img (tensor-core modes): the bf16
+ * hi/lo image of y ([M, img_pitch] per plane, planes img_plane elements apart, img_pitch % 8 == 0) is also stored; with
+ * epi 1 or 2 C is then not written.  max_ctas > 0: issue the group in launches of at most that many CTAs. */
+typedef struct dsact_test_layer {
+  int32_t M, N, K0, K1, kB1;
+  const float *A0, *A1, *B;
+  int32_t lda0, lda1, ldb;
+  int32_t epi, act;
+  const float *bias;
+  float *Zout;
+  const float *Zin;
+  int32_t ldz;
+  float *colsum;
+  float *C;
+  int32_t ldc;
+  void *img;            /* bf16 */
+  int32_t img_pitch;
+  int64_t img_plane;
+} dsact_test_layer;
+int dsact_test_gemm(dsact_handle *h, int32_t variant, const dsact_test_layer *probs, int32_t n, int32_t max_ctas, void *stream);
+
+/* dsact_test_chain (tensor-core modes): one launch of the fused layer-chain kernel with 1-4 passes of one MLP, built by
+ * the step's own chain code.  sizes[0..L+1]: input, L hidden widths, output; params: the flat fp32 [W_0 | b_0 | ... |
+ * W_L | b_L] (W_j [sizes[j+1], sizes[j]]); act: hidden activation.  Layer 0 reads cat(x0[M,K0], x1[M,K1]) (K0 + K1 =
+ * sizes[0]) with the x1 block at column kB1 of W_0's image.
+ *  dgrad 0 (forward): out[M, sizes[L+1]] = the MLP's output; per hidden layer j (0-based), optional Zout[j] [M, sizes[j+1]]
+ *                     = act'(z_j) and img[j] = the bf16 image of act(z_j).
+ *  dgrad 1          : x0 = dOut[M, sizes[L+1]]; dz_j = (dz_{j+1} W_{j+1}) * act'(z_j) with Zin[j] = act'(z_j) [M, sizes[j+1]];
+ *                     optional img[j] = the image of dz_j, colsum[j] += column sums of dz_j; out (optional) = dz_0 W_0
+ *                     restricted to the x1 columns, [M, K1].
+ * Images: pitch = sizes[j+1] rounded up to 8, planes pitch * M elements apart. */
+typedef struct dsact_test_chain_pass {
+  int32_t M;
+  const float *x0, *x1;
+  float *Zout[DSACT_MAX_HIDDEN];
+  const float *Zin[DSACT_MAX_HIDDEN];
+  void *img[DSACT_MAX_HIDDEN];
+  float *colsum[DSACT_MAX_HIDDEN];
+  float *out;
+} dsact_test_chain_pass;
+int dsact_test_chain(dsact_handle *h, int32_t dgrad, int32_t L, const int32_t *sizes, int32_t K0, int32_t K1, int32_t kB1,
+                     int32_t act, const float *params, const dsact_test_chain_pass *passes, int32_t n_passes, void *stream);
 
 /* Test hook of the head-wise engine's convolution kernels: one layer (NCHW, square k x k window, stride, no padding) on
  * caller buffers, enqueued on `stream` of the current device.
