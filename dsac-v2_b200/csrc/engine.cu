@@ -584,14 +584,6 @@ static ImgOut img_out(const MlpHandle* h, const ImgSlot& s) {
   return o;
 }
 
-static Wt weight(const MlpHandle* h, const Net& net, const float* base, int j, const ImgSlot& slot) {
-  Wt w;
-  w.f = base + net.w[j];
-  w.bias = base + net.b[j];
-  w.im = h->img(slot, net.s[j + 1]);
-  return w;
-}
-
 
 // ---- layer-chain launches (tensor-core modes) -------------------------------------------------------
 struct ChainBuild {
@@ -721,11 +713,107 @@ static ChainPass& chain_dgrad_layers(ChainBuild& cb, const Net& net, const Chain
   return P;
 }
 
-// The step's passes: arena slots resolved to the pointers and images above
-static ChainIo chain_io(const MlpHandle* h, const Net& net, const ImgSlot* wslots, int B, const int64_t* z_off, const ImgSlot* himg) {
+// ---- the network passes of a step and their two lowerings ----------------------------------------------------------
+// A network instance of the step (q_k and q'_k for k < nq, pi, pi'): its fp32 parameters (in params; in targets for q'_k
+// and pi'), gradients (null: a target network), the weight-image slot of every layer and the hidden activation
+struct NetInst { const Net* net; const float* P; float* G; const ImgSlot* wimg; int act; };
+struct NetInsts { NetInst q[2], qt[2], pi, pit; };
+
+static NetInsts net_insts(const MlpHandle* h) {
+  const Net &q = h->q, &pi = h->pi;
+  const int nq = h->nq();
+  float *P = h->buf.params, *T = h->buf.targets, *G = h->buf.grads;   // flat layout [q_0 .. q_{nq-1} | pi | log_alpha]
+  NetInsts I = {};
+  for (int k = 0; k < nq; ++k) {
+    I.q[k] = NetInst{&q, P + k * q.n, G + k * q.n, h->ar.i_wq[k], h->cfg.act_q};
+    I.qt[k] = NetInst{&q, T + k * q.n, nullptr, h->ar.i_wq[2 + k], h->cfg.act_q};
+  }
+  I.pi = NetInst{&pi, P + nq * q.n, G + nq * q.n, h->ar.i_wpi[0], h->cfg.act_pi};
+  I.pit = NetInst{&pi, T + nq * q.n, nullptr, h->ar.i_wpi[1], h->cfg.act_pi};
+  return I;
+}
+
+// A forward pass.  Layer 0 reads in0 (k0 columns) and, for a critic, the action segment in1 (k1 columns, at column kB1 of
+// the weight image).  Per hidden layer j, act'(z_j) goes to slot z[j] (z null: nowhere) and the activation to slots hf[j]
+// (fp32) / hi[j] (image); a layer chain writes the activations only if they must outlive the pass (`keep`: the weight
+// gradients read them).
+struct FwdPass {
+  NetInst n;
+  Ten in0, in1;
+  int k0, k1, kB1;
+  const int64_t *z, *hf;
+  const ImgSlot* hi;
+  bool keep;
+  float* out;
+};
+
+// The backward of forward pass f: dL/d(output) in slots dout / dout_img, dL/dz_j in slots dz[j] / dz_img[j].  `grads`: it
+// adds the bias gradients and, from f's layer inputs, the weight gradients of f's network (a layer chain writes the dz
+// images only then).  dact != null: dL/d(f's action segment) goes there.
+struct BwdPass {
+  FwdPass f;
+  int64_t dout;
+  ImgSlot dout_img;
+  const int64_t* dz;
+  const ImgSlot* dz_img;
+  bool grads;
+  float* dact;
+};
+
+// The passes of one step in launch order.  Wave A: pi(s), pi'(s'), Q_k(s,a); wave B (it reads a~ ~ pi(s), a' ~ pi'(s')):
+// Q'_k(s',a'), Q_k(s,a~); the critics' backward: Q_k(s,a) with gradients, Q_k(s,a~) with dL/da~; the policy's: pi(s).
+struct StepPasses {
+  NetInsts I;
+  FwdPass a[4], b[4];
+  BwdPass q[4], pi;
+  int na = 0, nb = 0, nqb = 0;
+};
+
+static Ten ten(const MlpHandle* h, const float* f, const ImgSlot& s, int B) { return Ten{const_cast<float*>(f), h->img(s, B)}; }
+static Wt weight(const MlpHandle* h, const NetInst& n, int j) {   // layer j of instance n
+  return Wt{n.P + n.net->w[j], n.P + n.net->b[j], h->img(n.wimg[j], n.net->s[j + 1])};
+}
+
+static StepPasses step_passes(const MlpHandle* h, const dsact_batch& bt) {
+  const Arena& ar = h->ar;
+  float* W = h->W();
+  const int B = bt.batch, O = h->cfg.obs_dim, A = h->cfg.act_dim;
+  StepPasses s;
+  s.I = net_insts(h);
+  const Ten obs = ten(h, bt.obs, ar.i_obs, B), obs2 = ten(h, bt.obs2, ar.i_obs2, B), act = ten(h, bt.act, ar.i_act, B);
+  const Ten new_act = ten(h, W + ar.new_act, ar.i_new_act, B), act2 = ten(h, W + ar.act2, ar.i_act2, B);
+  // the arena holds critic pass Q_k(s,a) at slot k, Q'_k(s',a') at 2 + k and Q_k(s,a~) at 4 + k
+  auto critic = [&](const NetInst& n, int p, const Ten& in, const Ten& a, bool store_z, bool keep) {
+    return FwdPass{n, in, a, O, A, ar.kpad_q0, store_z ? ar.zQ[p] : nullptr, ar.hQ[p], ar.i_hQ[p], keep, W + ar.outQ[p]};
+  };
+  auto critic_bwd = [&](const FwdPass& f, int p, bool grads, float* dact) {
+    return BwdPass{f, ar.dOut[p], ar.i_dOut[p], ar.dzQ[p], ar.i_dzQ[p], grads, dact};
+  };
+  const FwdPass pi{s.I.pi, obs, Ten(), O, 0, 0, ar.zP, ar.hP, ar.i_hP, true, W + ar.logitsP};
+  s.a[s.na++] = pi;
+  s.a[s.na++] = FwdPass{s.I.pit, obs2, Ten(), O, 0, 0, nullptr, ar.hT, ar.i_hT, false, W + ar.logitsT};
+  s.pi = BwdPass{pi, ar.dlogits, ar.i_dlogits, ar.dzP, ar.i_dzP, true, nullptr};
+  const int nq = h->nq();
+  for (int k = 0; k < nq; ++k) {
+    const FwdPass f = critic(s.I.q[k], k, obs, act, true, true);
+    s.a[s.na++] = f;
+    s.q[s.nqb++] = critic_bwd(f, k, true, nullptr);
+  }
+  for (int k = 0; k < nq; ++k) s.b[s.nb++] = critic(s.I.qt[k], 2 + k, obs2, act2, false, false);
+  for (int k = 0; k < nq; ++k) {
+    const FwdPass f = critic(s.I.q[k], 4 + k, obs, new_act, true, false);
+    s.b[s.nb++] = f;
+    s.q[s.nqb++] = critic_bwd(f, 4 + k, false, W + ar.dAct[k]);
+  }
+  return s;
+}
+
+// a pass's weight images and, per hidden layer, its act'(z) slot and output image (null slots: none)
+static ChainIo chain_io(const MlpHandle* h, const NetInst& n, int B, const int64_t* z_off, const ImgSlot* himg) {
   ChainIo io;
   float* W = h->W();
-  for (int j = 0; j <= net.L; ++j) io.w[j] = h->img(wslots[j], net.s[j + 1]);
+  const Net& net = *n.net;
+  for (int j = 0; j <= net.L; ++j) io.w[j] = h->img(n.wimg[j], net.s[j + 1]);
   for (int j = 0; j < net.L; ++j) {
     if (z_off) io.z[j] = W + z_off[j];
     if (himg) io.img[j] = h->img(himg[j], B);
@@ -733,18 +821,104 @@ static ChainIo chain_io(const MlpHandle* h, const Net& net, const ImgSlot* wslot
   return io;
 }
 
-static ChainPass& chain_fwd_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const float* Wbase, const ImgSlot* wslots,
-                           const Img& in0, int k0, const Img& in1, int k1, int kB1, int B, int act,
-                           const int64_t* zout_off, const ImgSlot* himg, float* out) {
-  return chain_fwd_layers(cb, net, Wbase, chain_io(h, net, wslots, B, zout_off, himg), in0, k0, in1, k1, kB1, B, act, out);
+// One wave of forward passes: one layer-chain launch (each CTA runs a 64-row block through every layer of its pass), or
+// one GEMM group per layer depth
+static void enqueue_fwd(MlpHandle* h, const FwdPass* ps, int n, int B, Ctx& c) {
+  float* W = h->W();
+  if (h->fused()) {
+    ChainBuild cb(h->passes());
+    for (int i = 0; i < n; ++i) {
+      const FwdPass& p = ps[i];
+      chain_fwd_layers(cb, *p.n.net, p.n.P, chain_io(h, p.n, B, p.z, p.keep ? p.hi : nullptr), p.in0.im, p.k0, p.in1.im, p.k1,
+                       p.kB1, B, p.n.act, p.out);
+    }
+    launch_chain(h, cb, CLS_GEMM_FWD, c);
+    return;
+  }
+  for (int j = 0; j <= DSACT_MAX_HIDDEN; ++j) {
+    Group G;
+    for (int i = 0; i < n; ++i) {
+      const FwdPass& p = ps[i];
+      const Net& net = *p.n.net;
+      if (j > net.L) continue;
+      const bool last = j == net.L;
+      const Ten out = last ? Ten{p.out} : ten(h, W + p.hf[j], p.hi[j], B);
+      float* z = last || !p.z ? nullptr : W + p.z[j];
+      const Wt w = weight(h, p.n, j);
+      if (j == 0) add_fwd(G, net, 0, w, p.in0, p.k0, p.in1, p.k1, p.kB1, out, z, B, p.n.act);
+      else add_fwd(G, net, j, w, ten(h, W + p.hf[j - 1], p.hi[j - 1], B), net.s[j], Ten(), 0, 0, out, z, B, p.n.act);
+    }
+    launch_group(h, G, V_FWD, c);
+  }
 }
 
-static ChainPass& chain_dgrad_pass(ChainBuild& cb, const MlpHandle* h, const Net& net, const ImgSlot* wslots, const Img& dout,
-                             int B, int act, const int64_t* zin_off, float* gbase /*bias grads of this net or null*/,
-                             const ImgSlot* dzimg /*or null*/, float* dact_out, int act_col_img, int act_cols) {
-  ChainIo io = chain_io(h, net, wslots, B, zin_off, dzimg);
-  for (int j = 0; j < net.L && gbase; ++j) io.colsum[j] = gbase + net.b[j];
-  return chain_dgrad_layers(cb, net, io, dout, B, act, dact_out, act_col_img, act_cols);
+// dL/d(output of layer j) of a backward pass
+static Ten bwd_dy(const MlpHandle* h, const BwdPass& p, int j, int B) {
+  return j == p.f.n.net->L ? ten(h, h->W() + p.dout, p.dout_img, B) : ten(h, h->W() + p.dz[j], p.dz_img[j], B);
+}
+
+// The dgrad of a list of backward passes, top layer down: one layer-chain launch (dz stays on chip between layers), or one
+// GEMM group per layer.  Returns true for the chain.  The chain also computes dL/d(action); the per-layer lowering leaves
+// those problems in `act_cols` for the caller to launch.
+static bool enqueue_dgrad(MlpHandle* h, const BwdPass* ps, int n, int B, Ctx& c, Group& act_cols) {
+  float* W = h->W();
+  if (h->fused()) {
+    ChainBuild cb(h->passes());
+    for (int i = 0; i < n; ++i) {
+      const BwdPass& p = ps[i];
+      const NetInst& ni = p.f.n;
+      ChainIo io = chain_io(h, ni, B, p.f.z, p.grads ? p.dz_img : nullptr);
+      for (int j = 0; j < ni.net->L && p.grads; ++j) io.colsum[j] = ni.G + ni.net->b[j];
+      chain_dgrad_layers(cb, *ni.net, io, h->img(p.dout_img, B), B, ni.act, p.dact, p.f.kB1, p.f.k1);
+    }
+    launch_chain(h, cb, CLS_GEMM_DGRAD, c);
+    return true;
+  }
+  for (int j = DSACT_MAX_HIDDEN; j >= 0; --j) {
+    Group gd;   // (stays empty at j = 0)
+    for (int i = 0; i < n; ++i) {
+      const BwdPass& p = ps[i];
+      const NetInst& ni = p.f.n;
+      const Net& net = *ni.net;
+      if (j > net.L) continue;
+      const Wt w = weight(h, ni, j);
+      if (j > 0)
+        add_dgrad(gd, net, j, w, 0, 0, net.s[j], bwd_dy(h, p, j, B), ten(h, W + p.dz[j - 1], p.dz_img[j - 1], B), W + p.f.z[j - 1],
+                  p.grads ? ni.G + net.b[j - 1] : nullptr, B, ni.act);
+      else if (p.dact)
+        add_dgrad(act_cols, net, 0, w, p.f.k0, p.f.kB1, p.f.k1, bwd_dy(h, p, 0, B), Ten{p.dact}, nullptr, nullptr, B, 0);
+    }
+    launch_group(h, gd, V_DGRAD, c);
+  }
+  return false;
+}
+
+// The weight-gradient problems of the backward passes with `grads`, layers top down (layer 0: one per input segment)
+static void add_wgrads(Group& gw, const MlpHandle* h, const BwdPass* ps, int n, int B) {
+  for (int j = DSACT_MAX_HIDDEN; j >= 0; --j)
+    for (int i = 0; i < n; ++i) {
+      const BwdPass& p = ps[i];
+      const Net& net = *p.f.n.net;
+      if (!p.grads || j > net.L) continue;
+      float* g = p.f.n.G + net.w[j];
+      const Ten dy = bwd_dy(h, p, j, B);
+      if (j > 0) add_wgrad(gw, net, j, g, 0, net.s[j], dy, ten(h, h->W() + p.f.hf[j - 1], p.f.hi[j - 1], B), B);
+      else add_wgrad(gw, net, 0, g, 0, p.f.k0, dy, p.f.in0, B);
+      if (j == 0 && p.f.k1 > 0) add_wgrad(gw, net, 0, g, p.f.k0, p.f.k1, dy, p.f.in1, B);
+    }
+}
+
+// `branch` on the side stream, after all that c.s holds so far; the caller joins it by waiting on `join`
+template <typename F>
+static void fork_branch(Ctx& c, cudaEvent_t fork, cudaEvent_t join, F branch) {
+  cudaEventRecord(fork, c.s);
+  cudaStreamWaitEvent(c.side, fork, 0);
+  Ctx cs{c.side, 0, cudaSuccess};
+  cs.pdl = c.pdl;
+  branch(cs);
+  cudaEventRecord(join, c.side);
+  c.launches += cs.launches;
+  if (cs.err != cudaSuccess && c.err == cudaSuccess) c.err = cs.err;
 }
 
 static unsigned long long dp_timeout_ns() {
@@ -961,45 +1135,39 @@ static dsact_batch arena_batch(const dsact_handle* h, int32_t batch) {
 // ---- enqueue: pieces of one MLP update -------------------------------------------
 // Everything of a step that depends on neither the minibatch gather nor a forward pass: accumulator clears, the
 // gradient memset, the bf16 images of all weights (and of a caller-supplied batch), the device noise.
-static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged,
-                             bool with_noise = true) {
+static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged) {
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
   float* W = h->W();
   const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim;
   const bool tc = h->tc();
-  float* P = h->buf.params;
-  float* T = h->buf.targets;
   const int nq = h->nq();
-  const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2' (DSAC_V1: q, -, q', -)
-  const float* PIb[2] = {P + nq * q.n, T + nq * q.n};   // pi, pi'
+  const NetInsts I = net_insts(h);
 
-  const bool want_noise = !nz && with_noise;
+  const bool want_noise = !nz;
   if (!tc) enqueue_begin_step(h, c);
 
   if (tc) {  // refresh the weight images (the caller may have written params/targets through its views) + inputs; the clears
              // and the device noise ride in the same launch
     ImgBatch ib;
-    for (int n = 0; n < nq; ++n)
-      for (int j = 0; j <= q.L; ++j) {
+    // one job per layer (a critic's layer 0: its obs and act columns, the act block at column kpad_q0 of the image)
+    auto add_weights = [&](const NetInst& n) {
+      const Net& net = *n.net;
+      for (int j = 0; j <= net.L; ++j) {
         ib.reserve(h, c, 1);
-        const Img im = h->img(ar.i_wq[n][j], q.s[j + 1]);
-        if (j == 0) ib.add(Qb[n] + q.w[0], O + A, im, q.s[1], O, A, ar.kpad_q0);
-        else ib.add(Qb[n] + q.w[j], q.s[j], im, q.s[j + 1], q.s[j]);
+        const Img im = h->img(n.wimg[j], net.s[j + 1]);
+        if (j == 0 && &net == &q) ib.add(n.P + q.w[0], O + A, im, q.s[1], O, A, ar.kpad_q0);
+        else ib.add(n.P + net.w[j], net.s[j], im, net.s[j + 1], net.s[j]);
       }
+    };
+    for (int k = 0; k < nq; ++k) add_weights(I.q[k]);
     ib.reserve(h, c, pi.L + 2);
-    for (int j = 0; j <= pi.L; ++j) ib.add(PIb[0] + pi.w[j], pi.s[j], h->img(ar.i_wpi[0][j], pi.s[j + 1]), pi.s[j + 1], pi.s[j]);
+    add_weights(I.pi);
     if (!inputs_imaged) ib.add(bt.obs, O, h->img(ar.i_obs, B), B, O);
-    for (int n = 2; n < 2 + nq; ++n)
-      for (int j = 0; j <= q.L; ++j) {
-        ib.reserve(h, c, 1);
-        const Img im = h->img(ar.i_wq[n][j], q.s[j + 1]);
-        if (j == 0) ib.add(Qb[n] + q.w[0], O + A, im, q.s[1], O, A, ar.kpad_q0);
-        else ib.add(Qb[n] + q.w[j], q.s[j], im, q.s[j + 1], q.s[j]);
-      }
+    for (int k = 0; k < nq; ++k) add_weights(I.qt[k]);
     ib.reserve(h, c, pi.L + 3);
-    for (int j = 0; j <= pi.L; ++j) ib.add(PIb[1] + pi.w[j], pi.s[j], h->img(ar.i_wpi[1][j], pi.s[j + 1]), pi.s[j + 1], pi.s[j]);
+    add_weights(I.pit);
     if (!inputs_imaged) {
       ib.add(bt.obs2, O, h->img(ar.i_obs2, B), B, O);
       ib.add(bt.act, A, h->img(ar.i_act, B), B, A);
@@ -1025,14 +1193,7 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
 // gather); returns true if it was forked and must be joined (enqueue_phase1 does) before the first forward pass.
 static bool fork_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged) {
   if (!c.side) return false;
-  cudaEventRecord(h->ev_pro_fork, c.s);
-  cudaStreamWaitEvent(c.side, h->ev_pro_fork, 0);
-  Ctx cs{c.side, 0, cudaSuccess};
-  cs.pdl = c.pdl;
-  enqueue_prologue(h, bt, nz, cs, inputs_imaged, true);
-  cudaEventRecord(h->ev_pro_join, c.side);
-  c.launches += cs.launches;
-  if (cs.err != cudaSuccess && c.err == cudaSuccess) c.err = cs.err;
+  fork_branch(c, h->ev_pro_fork, h->ev_pro_join, [&](Ctx& cs) { enqueue_prologue(h, bt, nz, cs, inputs_imaged); });
   return true;
 }
 
@@ -1113,18 +1274,7 @@ static void dp_peer_release(DpPeer& dp) {
 // side branch under that chain.
 static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged = false,
                            bool prologue_forked = false, bool dp_std_exchange = false) {
-  const dsact_config& cf = h->cfg;
-  const Net &q = h->q, &pi = h->pi;
-  const Arena& ar = h->ar;
-  float* W = h->W();
-  const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim, nq = h->nq();
-  float* P = h->buf.params;
-  float* T = h->buf.targets;
-  const float* Qb[4] = {P, P + q.n, T, T + q.n};        // q1, q2, q1', q2' (DSAC_V1: q, -, q', -)
-  const float* PIb[2] = {P + nq * q.n, T + nq * q.n};   // pi, pi'
-  auto ten = [&](const float* f, const ImgSlot& s) { Ten t; t.f = const_cast<float*>(f); t.im = h->img(s, B); return t; };
-  const ImgSlot none;
-
+  const int B = bt.batch;
   if (prologue_forked) {
     cudaStreamWaitEvent(c.s, h->ev_pro_join, 0);
   } else {
@@ -1132,87 +1282,13 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
   }
 
   const dsact_noise noise = step_noise(h, nz);   // device noise: sample_kernel steps the counter
-  const Ten t_obs = ten(bt.obs, ar.i_obs), t_obs2 = ten(bt.obs2, ar.i_obs2), t_act = ten(bt.act, ar.i_act);
-  const Ten t_none;
-
-  const bool fused = h->fused();
-  const Img i_none;
-  if (fused) {  // wave A as ONE launch: each CTA runs a 64-row block through every layer of its pass
-    ChainBuild cb(h->passes());
-    chain_fwd_pass(cb, h, pi, PIb[0], ar.i_wpi[0], t_obs.im, O, i_none, 0, 0, B, cf.act_pi, ar.zP, ar.i_hP, W + ar.logitsP);
-    chain_fwd_pass(cb, h, pi, PIb[1], ar.i_wpi[1], t_obs2.im, O, i_none, 0, 0, B, cf.act_pi, nullptr, nullptr, W + ar.logitsT);
-    for (int k = 0; k < nq; ++k)
-      chain_fwd_pass(cb, h, q, Qb[k], ar.i_wq[k], t_obs.im, O, t_act.im, A, ar.kpad_q0, B, cf.act_q, ar.zQ[k], ar.i_hQ[k], W + ar.outQ[k]);
-    launch_chain(h, cb, CLS_GEMM_FWD, c);
-  }
-  // wave A: pi(obs), pi'(obs2), Q1(s,a), Q2(s,a) (DSAC_V1: Q(s,a)), layer by layer
-  const int depth = fused ? 0 : (pi.L > q.L ? pi.L : q.L) + 1;
-  for (int j = 0; j < depth; ++j) {
-    Group G;
-    if (j <= pi.L) {
-      const Ten inP = j == 0 ? t_obs : ten(W + ar.hP[j - 1], ar.i_hP[j - 1]);
-      const Ten inT = j == 0 ? t_obs2 : ten(W + ar.hT[j - 1], ar.i_hT[j - 1]);
-      const Ten outP = j == pi.L ? ten(W + ar.logitsP, none) : ten(W + ar.hP[j], ar.i_hP[j]);
-      const Ten outT = j == pi.L ? ten(W + ar.logitsT, none) : ten(W + ar.hT[j], ar.i_hT[j]);
-      add_fwd(G, pi, j, weight(h, pi, PIb[0], j, ar.i_wpi[0][j]), inP, pi.s[j], t_none, 0, 0, outP, j == pi.L ? nullptr : W + ar.zP[j], B, cf.act_pi);
-      add_fwd(G, pi, j, weight(h, pi, PIb[1], j, ar.i_wpi[1][j]), inT, pi.s[j], t_none, 0, 0, outT, nullptr, B, cf.act_pi);
-    }
-    if (j <= q.L) {
-      for (int k = 0; k < nq; ++k) {
-        const Ten out = j == q.L ? ten(W + ar.outQ[k], none) : ten(W + ar.hQ[k][j], ar.i_hQ[k][j]);
-        float* z = j == q.L ? nullptr : W + ar.zQ[k][j];
-        const Wt w = weight(h, q, Qb[k], j, ar.i_wq[k][j]);
-        if (j == 0) add_fwd(G, q, 0, w, t_obs, O, t_act, A, ar.kpad_q0, out, z, B, cf.act_q);
-        else add_fwd(G, q, j, w, ten(W + ar.hQ[k][j - 1], ar.i_hQ[k][j - 1]), q.s[j], t_none, 0, 0, out, z, B, cf.act_q);
-      }
-    }
-    launch_group(h, G, V_FWD, c);
-  }
-
-  enqueue_sample(h, B, noise.eps1, noise.eps2, !nz, img_out(h, ar.i_new_act), img_out(h, ar.i_act2), c);
-  bool dp_forked = false;
-  if (dp_std_exchange) {
-    if (c.side) {
-      cudaEventRecord(h->ev_dp_fork, c.s);
-      cudaStreamWaitEvent(c.side, h->ev_dp_fork, 0);
-      Ctx cs{c.side, 0, cudaSuccess};
-      cs.pdl = c.pdl;
-      enqueue_dp_exchange(h, 0, cs);
-      cudaEventRecord(h->ev_dp_join, c.side);
-      c.launches += cs.launches;
-      if (cs.err != cudaSuccess && c.err == cudaSuccess) c.err = cs.err;
-      dp_forked = true;
-    } else {
-      enqueue_dp_exchange(h, 0, c);
-    }
-  }
-
-  // wave B: Q1', Q2' on (s', a') and Q1, Q2 on (s, a~) (DSAC_V1: Q', Q)
-  const Ten t_new_act = ten(W + ar.new_act, ar.i_new_act), t_act2 = ten(W + ar.act2, ar.i_act2);
-  if (fused) {
-    ChainBuild cb(h->passes());
-    for (int k = 0; k < nq; ++k)
-      chain_fwd_pass(cb, h, q, Qb[2 + k], ar.i_wq[2 + k], t_obs2.im, O, t_act2.im, A, ar.kpad_q0, B, cf.act_q, nullptr, nullptr, W + ar.outQ[2 + k]);
-    for (int k = 0; k < nq; ++k)
-      chain_fwd_pass(cb, h, q, Qb[k], ar.i_wq[k], t_obs.im, O, t_new_act.im, A, ar.kpad_q0, B, cf.act_q, ar.zQ[4 + k], nullptr, W + ar.outQ[4 + k]);
-    launch_chain(h, cb, CLS_GEMM_FWD, c);
-  }
-  for (int j = 0; j <= (fused ? -1 : q.L); ++j) {
-    Group G;
-    for (int p = 2; p < 6; ++p) {
-      const int k = p & 1;
-      if (k >= nq) continue;
-      const bool tgt = p < 4;
-      const int wn = tgt ? 2 + k : k;
-      const Ten out = j == q.L ? ten(W + ar.outQ[p], none) : ten(W + ar.hQ[p][j], ar.i_hQ[p][j]);
-      float* z = (j == q.L || tgt) ? nullptr : W + ar.zQ[p][j];
-      const Wt w = weight(h, q, Qb[wn], j, ar.i_wq[wn][j]);
-      if (j == 0) add_fwd(G, q, 0, w, tgt ? t_obs2 : t_obs, O, tgt ? t_act2 : t_new_act, A, ar.kpad_q0, out, z, B, cf.act_q);
-      else add_fwd(G, q, j, w, ten(W + ar.hQ[p][j - 1], ar.i_hQ[p][j - 1]), q.s[j], t_none, 0, 0, out, z, B, cf.act_q);
-    }
-    launch_group(h, G, V_FWD, c);
-  }
-
+  const StepPasses sp = step_passes(h, bt);
+  enqueue_fwd(h, sp.a, sp.na, B, c);
+  enqueue_sample(h, B, noise.eps1, noise.eps2, !nz, img_out(h, h->ar.i_new_act), img_out(h, h->ar.i_act2), c);
+  const bool dp_forked = dp_std_exchange && c.side != nullptr;
+  if (dp_forked) fork_branch(c, h->ev_dp_fork, h->ev_dp_join, [&](Ctx& cs) { enqueue_dp_exchange(h, 0, cs); });
+  else if (dp_std_exchange) enqueue_dp_exchange(h, 0, c);
+  enqueue_fwd(h, sp.b, sp.nb, B, c);
   if (dp_forked) cudaStreamWaitEvent(c.s, h->ev_dp_join, 0);
   h->pending_eps1 = noise.eps1; h->pending_z3 = noise.z3; h->pending_z4 = noise.z4;
   c.check();
@@ -1240,74 +1316,31 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
   float* W = h->W();
-  const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim, nq = h->nq();
+  const int B = bt.batch;
   const bool tc = h->tc();
-  float* P = h->buf.params;
   float* G_ = h->buf.grads;
-  const float *Pq[2] = {P, P + q.n}, *Ppi = P + nq * q.n;
-  float *Gq[2] = {G_, G_ + q.n}, *Gpi = G_ + nq * q.n;
-  const long long n_flat = nq * q.n + pi.n + 1;
-  auto ten = [&](const float* f, const ImgSlot& s) { Ten t; t.f = const_cast<float*>(f); t.im = h->img(s, B); return t; };
-  const ImgSlot none;
+  const long long n_flat = h->nq() * q.n + pi.n + 1;
+  const StepPasses sp = step_passes(h, bt);
+  const NetInsts& I = sp.I;
 
   const StepScalars sc = step_scalars(h, global_batch);
   if (h->v1) {
-    enqueue_loss_v1(h, bt, sc, Gq[0] + q.b[q.L], nullptr, img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[4]), c);
+    enqueue_loss_v1(h, bt, sc, I.q[0].G + q.b[q.L], nullptr, img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[4]), c);
   } else {
-    float* const gbias[2] = {Gq[0] + q.b[q.L], Gq[1] + q.b[q.L]};
+    float* const gbias[2] = {I.q[0].G + q.b[q.L], I.q[1].G + q.b[q.L]};
     float* const gbias_raw[2] = {nullptr, nullptr};   // one two-output layer
     const ImgOut img_q[2] = {img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[1])};
     const ImgOut img_qa[2] = {img_out(h, ar.i_dOut[4]), img_out(h, ar.i_dOut[5])};
     enqueue_loss(h, bt, sc, gbias, gbias_raw, img_q, img_qa, c);
   }
-  // critic passes with a backward: Q_k(s,a) (dgrad + wgrad) and Q_k(s,a~) (dgrad only); DSAC_V1: Q(s,a), Q(s,a~)
-  const int passes[4] = {0, 1, 4, 5}, v1_passes[2] = {0, 4};
-  const int* bwd = h->v1 ? v1_passes : passes;
-  const int n_bwd = 2 * nq;
-  const Ten t_obs = ten(bt.obs, ar.i_obs), t_act = ten(bt.act, ar.i_act);
-
-  // wave C: critic passes 0,1 (dgrad + wgrad) and actor passes 4,5 (dgrad only), top layer down.
-  // The freeze trick of the reference (dsac_v2.py:166-181) makes the two backward passes independent: one 4-pass dgrad
-  // chain, then the critics' weight gradients as a side branch beside the policy backward.
-  Group gw;  // every weight-gradient problem of the two critics
-  const bool fused = h->fused();
-  if (fused) {  // dgrad as one chain launch: dz stays on chip between layers
-    ChainBuild cb(h->passes());
-    for (int pp = 0; pp < n_bwd; ++pp) {
-      const int p = bwd[pp], k = p & 1;
-      chain_dgrad_pass(cb, h, q, ar.i_wq[k], h->img(ar.i_dOut[p], B), B, cf.act_q, ar.zQ[p], p < 2 ? Gq[k] : nullptr,
-                       p < 2 ? ar.i_dzQ[p] : nullptr, p < 2 ? nullptr : W + ar.dAct[k], ar.kpad_q0, A);
-    }
-    launch_chain(h, cb, CLS_GEMM_DGRAD, c);
-  }
-  for (int j = q.L; j >= 1; --j) {
-    Group gd;
-    for (int pp = 0; pp < n_bwd; ++pp) {
-      const int p = bwd[pp], k = p & 1;
-      const Ten dY = j == q.L ? ten(W + ar.dOut[p], ar.i_dOut[p]) : ten(W + ar.dzQ[p][j], ar.i_dzQ[p][j]);
-      float* gb = p < 2 ? Gq[k] + q.b[j - 1] : nullptr;
-      add_dgrad(gd, q, j, weight(h, q, Pq[k], j, ar.i_wq[k][j]), 0, 0, q.s[j], dY, ten(W + ar.dzQ[p][j - 1], ar.i_dzQ[p][j - 1]),
-                W + ar.zQ[p][j - 1], gb, B, cf.act_q);
-      if (fused) gd.n = gd.g.n = 0;  // done by the chain launch; only the weight-gradient problems are collected here
-      if (p < 2) add_wgrad(gw, q, j, Gq[k] + q.w[j], 0, q.s[j], dY, ten(W + ar.hQ[p][j - 1], ar.i_hQ[p][j - 1]), B);
-    }
-    launch_group(h, gd, V_DGRAD, c);
-  }
-  {
-    Group gd;
-    for (int k = 0; k < nq; ++k) {
-      const Ten dz0 = ten(W + ar.dzQ[k][0], ar.i_dzQ[k][0]);
-      add_wgrad(gw, q, 0, Gq[k] + q.w[0], 0, O, dz0, t_obs, B);
-      add_wgrad(gw, q, 0, Gq[k] + q.w[0], O, A, dz0, t_act, B);
-      if (!fused)
-        add_dgrad(gd, q, 0, weight(h, q, Pq[k], 0, ar.i_wq[k][0]), O, ar.kpad_q0, A, ten(W + ar.dzQ[4 + k][0], ar.i_dzQ[4 + k][0]),
-                  ten(W + ar.dAct[k], none), nullptr, nullptr, B, 0);
-    }
-    if (fused && c.side != nullptr) {   // the critics' weight gradients beside the policy backward
-      cudaEventRecord(h->ev_fork, c.s);
-      cudaStreamWaitEvent(c.side, h->ev_fork, 0);
-      Ctx cs{c.side, 0, cudaSuccess};
-      cs.pdl = c.pdl;
+  // The freeze trick of the reference (dsac_v2.py:166-181) makes the critics' and the policy's backward independent: the
+  // critics' dgrad, then, beside a policy backward chain, their weight gradients as a side branch.
+  Group gw, ga;   // the critics' weight gradients; the per-layer lowering's dL/da~
+  const bool chained = enqueue_dgrad(h, sp.q, sp.nqb, B, c, ga);
+  add_wgrads(gw, h, sp.q, sp.nqb, B);
+  const bool forked = chained && c.side != nullptr;
+  if (forked) {
+    fork_branch(c, h->ev_fork, h->ev_join, [&](Ctx& cs) {
       // the policy backward chain needs ceil(B/64) whole SMs: keep them free of weight-gradient CTAs
       const int chain_ctas = (B + TC_BM - 1) / TC_BM;
       const int cap = h->num_sms - chain_ctas;
@@ -1316,35 +1349,17 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
         enqueue_apply(h, cs, tail, false, 1);
         h->apply_early = true;
       }
-      cudaEventRecord(h->ev_join, c.side);
-      c.launches += cs.launches;
-      if (cs.err != cudaSuccess && c.err == cudaSuccess) c.err = cs.err;
-    } else {
-      launch_group(h, gw, V_WGRAD, c);
-    }
-    launch_group(h, gd, V_DGRAD, c);
-    h->join_pending = fused && c.side != nullptr;
+    });
+  } else {
+    launch_group(h, gw, V_WGRAD, c);
   }
+  launch_group(h, ga, V_DGRAD, c);
+  h->join_pending = forked;
 
-  enqueue_policy_grad(h, B, sc, Gpi + pi.b[pi.L], nullptr, img_out(h, ar.i_dlogits), c);
-
-  // wave D: policy backward
-  Group gwp;
-  if (fused) {
-    ChainBuild cb(h->passes());
-    chain_dgrad_pass(cb, h, pi, ar.i_wpi[0], h->img(ar.i_dlogits, B), B, cf.act_pi, ar.zP, Gpi, ar.i_dzP, nullptr, 0, 0);
-    launch_chain(h, cb, CLS_GEMM_DGRAD, c);
-  }
-  for (int j = pi.L; j >= 0; --j) {
-    const Ten dY = j == pi.L ? ten(W + ar.dlogits, ar.i_dlogits) : ten(W + ar.dzP[j], ar.i_dzP[j]);
-    add_wgrad(gwp, pi, j, Gpi + pi.w[j], 0, pi.s[j], dY, j == 0 ? t_obs : ten(W + ar.hP[j - 1], ar.i_hP[j - 1]), B);
-    if (j >= 1 && !fused) {
-      Group gd;
-      add_dgrad(gd, pi, j, weight(h, pi, Ppi, j, ar.i_wpi[0][j]), 0, 0, pi.s[j], dY, ten(W + ar.dzP[j - 1], ar.i_dzP[j - 1]),
-                W + ar.zP[j - 1], Gpi + pi.b[j - 1], B, cf.act_pi);
-      launch_group(h, gd, V_DGRAD, c);
-    }
-  }
+  enqueue_policy_grad(h, B, sc, I.pi.G + pi.b[pi.L], nullptr, img_out(h, ar.i_dlogits), c);
+  Group gwp, no_act;   // (the policy pass has no action segment)
+  enqueue_dgrad(h, &sp.pi, 1, B, c, no_act);
+  add_wgrads(gwp, h, &sp.pi, 1, B);
   launch_group(h, gwp, V_WGRAD, c);
 
   if (h->join_pending) { cudaStreamWaitEvent(c.s, h->ev_join, 0); h->join_pending = false; }
