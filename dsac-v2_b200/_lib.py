@@ -139,6 +139,8 @@ SYMBOLS = {
     "dsact_replay_add": (C.c_int, [C.c_void_p] + [C.c_void_p] * 6 + [C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_replay_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Batch), C.c_void_p]),
     "dsact_replay_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_int64, C.c_void_p]),
+    "dsact_replay_steps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_void_p,
+                                     C.c_int64, C.c_void_p]),
     "dsact_dp_export": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "dsact_dp_connect": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "dsact_dp_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_int64, C.c_void_p]),

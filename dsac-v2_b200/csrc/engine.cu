@@ -158,6 +158,7 @@ struct Arena : StepSlots {
 
 struct GraphKey {
   int kind; const void* p[9]; int32_t batch; int64_t gb; int64_t size; const void* idx;
+  int64_t n_steps; const void* out;   // dsact_replay_steps: updates per call, per-update statistics rows
   bool operator==(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) == 0; }
 };
 struct GraphEntry { GraphKey key; cudaGraphExec_t exec; int launches; uint64_t stamp; };
@@ -213,6 +214,16 @@ struct MlpHandle : dsact_handle {
   cudaEvent_t ev_stage_ready[2] = {nullptr, nullptr}, ev_stage_done[2] = {nullptr, nullptr};
   bool stage_done_valid[2] = {false, false};
   int stage_turn = 0, stage_held = -1;
+  // second minibatch input set of dsact_replay_steps (library-owned, allocated on its first call for max_batch rows):
+  // consecutive updates of one call alternate between the arena's set (0) and this one (1), so that the gather of update
+  // k + 1 runs beside update k's backward.  Offsets in floats from in2: fp32 obs / obs2 / act / rew / done / logp, and
+  // (tensor-core modes) the bf16 images of obs / obs2 / act.
+  float* in2 = nullptr;
+  int64_t in2_obs = 0, in2_obs2 = 0, in2_act = 0, in2_rew = 0, in2_done = 0, in2_logp = 0;
+  ImgSlot in2_img[3];
+  int in_set = 0;            // the input set the passes being enqueued read
+  cudaStream_t gather_stream = nullptr;   // the next update's gather, forked beside a captured update's backward
+  cudaEvent_t ev_gather_fork = nullptr, ev_gather_join = nullptr;
   bool tc_attr_done = false, chain_attr_done = false;   // cudaFuncSetAttribute is per device: tracked per handle
   TcGroup tc_scratch;                                   // host-side lowering scratch of launch_tc (~5 KiB)
   std::vector<GraphEntry> graphs;
@@ -233,6 +244,16 @@ struct MlpHandle : dsact_handle {
     Img i;
     if (s.off < 0) return i;
     i.p = reinterpret_cast<__nv_bfloat16*>(W() + s.off);
+    i.rows = rows; i.width = s.width; i.pitch = s.pitch; i.plane = s.plane;
+    return i;
+  }
+  // image of input `which` (0 obs, 1 obs2, 2 act) of input set `set`
+  Img input_img(int set, int which, int rows) const {
+    if (set == 0) return img(which == 0 ? ar.i_obs : which == 1 ? ar.i_obs2 : ar.i_act, rows);
+    Img i;
+    const ImgSlot& s = in2_img[which];
+    if (s.off < 0) return i;
+    i.p = reinterpret_cast<__nv_bfloat16*>(in2 + s.off);
     i.rows = rows; i.width = s.width; i.pitch = s.pitch; i.plane = s.plane;
     return i;
   }
@@ -583,6 +604,11 @@ static ImgOut img_out(const MlpHandle* h, const ImgSlot& s) {
   if (h->tc() && s.off >= 0) { o.p = reinterpret_cast<__nv_bfloat16*>(h->W() + s.off); o.pitch = s.pitch; o.plane = s.plane; }
   return o;
 }
+static ImgOut img_out_of(const MlpHandle* h, const Img& i) {
+  ImgOut o;
+  o.p = i.p; o.pitch = i.p ? i.pitch : 0; o.planes = h->passes() == 3 ? 2 : 1; o.plane = i.p ? i.plane : 0;
+  return o;
+}
 
 
 // ---- layer-chain launches (tensor-core modes) -------------------------------------------------------
@@ -780,7 +806,9 @@ static StepPasses step_passes(const MlpHandle* h, const dsact_batch& bt) {
   const int B = bt.batch, O = h->cfg.obs_dim, A = h->cfg.act_dim;
   StepPasses s;
   s.I = net_insts(h);
-  const Ten obs = ten(h, bt.obs, ar.i_obs, B), obs2 = ten(h, bt.obs2, ar.i_obs2, B), act = ten(h, bt.act, ar.i_act, B);
+  const int in = h->in_set;
+  const Ten obs{const_cast<float*>(bt.obs), h->input_img(in, 0, B)}, obs2{const_cast<float*>(bt.obs2), h->input_img(in, 1, B)};
+  const Ten act{const_cast<float*>(bt.act), h->input_img(in, 2, B)};
   const Ten new_act = ten(h, W + ar.new_act, ar.i_new_act, B), act2 = ten(h, W + ar.act2, ar.i_act2, B);
   // the arena holds critic pass Q_k(s,a) at slot k, Q'_k(s',a') at 2 + k and Q_k(s,a~) at 4 + k
   auto critic = [&](const NetInst& n, int p, const Ten& in, const Ten& a, bool store_z, bool keep) {
@@ -908,15 +936,16 @@ static void add_wgrads(Group& gw, const MlpHandle* h, const BwdPass* ps, int n, 
     }
 }
 
-// `branch` on the side stream, after all that c.s holds so far; the caller joins it by waiting on `join`
+// `branch` on the side stream (or on `on`), after all that c.s holds so far; the caller joins it by waiting on `join`
 template <typename F>
-static void fork_branch(Ctx& c, cudaEvent_t fork, cudaEvent_t join, F branch) {
+static void fork_branch(Ctx& c, cudaEvent_t fork, cudaEvent_t join, F branch, cudaStream_t on = nullptr) {
+  if (!on) on = c.side;
   cudaEventRecord(fork, c.s);
-  cudaStreamWaitEvent(c.side, fork, 0);
-  Ctx cs{c.side, 0, cudaSuccess};
+  cudaStreamWaitEvent(on, fork, 0);
+  Ctx cs{on, 0, cudaSuccess};
   cs.pdl = c.pdl;
   branch(cs);
-  cudaEventRecord(join, c.side);
+  cudaEventRecord(join, on);
   c.launches += cs.launches;
   if (cs.err != cudaSuccess && c.err == cudaSuccess) c.err = cs.err;
 }
@@ -1107,16 +1136,23 @@ static void launch_apply(const dsact_handle* h, const ApplyArgs& a, Ctx& c) {
   c.check();
 }
 
-// the replay gather: ring rows idx[i] (null: drawn on the device and recorded in the arena) -> the arena minibatch.
-// img: bf16 images of obs / obs2 / act to write as well; write_f32 = false leaves out their fp32 rows
-static void enqueue_gather(const dsact_handle* h, int B, const int64_t* idx, const ImgOut img[3], bool write_f32, Ctx& c) {
+// the replay gather: ring rows idx[i] (null: drawn on the device and recorded in the arena) -> the arena minibatch (or
+// the fp32 rows of `dst`).  img: bf16 images of obs / obs2 / act to write as well; write_f32 = false leaves out their
+// fp32 rows
+static void enqueue_gather(const dsact_handle* h, int B, const int64_t* idx, const ImgOut img[3], bool write_f32, Ctx& c,
+                           const dsact_batch* dst = nullptr) {
   const StepSlots& s = h->slot;
   float* W = h->W();
   // no index list: every warp of the gather draws its row's index itself (the sequence index_kernel defines) and records it
   int64_t* draw = idx ? nullptr : reinterpret_cast<int64_t*>(W + s.idx);
+  float* d[6] = {W + s.obs, W + s.obs2, W + s.act, W + s.rew, W + s.done, W + s.logp};
+  if (dst) {
+    const float* o[6] = {dst->obs, dst->obs2, dst->act, dst->rew, dst->done, dst->logp};
+    for (int i = 0; i < 6; ++i) d[i] = const_cast<float*>(o[i]);
+  }
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
   launch_k(gather_kernel, blocks, 256, 0, c, h->rb.obs, h->rb.obs2, h->rb.act, h->rb.rew, h->rb.done, h->rb.logp, idx,
-           W + s.obs, W + s.obs2, W + s.act, W + s.rew, W + s.done, W + s.logp, B, (int)h->obs_elems, h->act_dim,
+           d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
            img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0);
   c.done();
   c.check();
@@ -1271,13 +1307,13 @@ static void dp_peer_release(DpPeer& dp) {
 
 // `dp_std_exchange`: the std sums are complete once sample_kernel has run, one whole forward chain before the loss needs
 // them: in a captured step their exchange (kernel + NVLink flag round trip + whatever the ranks are skewed by) runs as a
-// side branch under that chain.
+// side branch under that chain.  `prologue_done`: the caller has enqueued the prologue on c.s already.
 static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged = false,
-                           bool prologue_forked = false, bool dp_std_exchange = false) {
+                           bool prologue_forked = false, bool dp_std_exchange = false, bool prologue_done = false) {
   const int B = bt.batch;
   if (prologue_forked) {
     cudaStreamWaitEvent(c.s, h->ev_pro_join, 0);
-  } else {
+  } else if (!prologue_done) {
     enqueue_prologue(h, bt, nz, c, inputs_imaged);
   }
 
@@ -1421,8 +1457,115 @@ static void enqueue_gather_imaged(MlpHandle* h, int B, const int64_t* idx, Ctx& 
   enqueue_gather(h, B, idx, img, !images_only, c);
 }
 
+// ---- n replay-fed updates in one submission (dsact_replay_steps) ----------------------------------------------------
+// the minibatch of input set `set` (0: the arena's, 1: the library-owned second set)
+static dsact_batch input_batch(const MlpHandle* h, int set, int32_t batch) {
+  if (set == 0) return arena_batch(h, batch);
+  const float* b = h->in2;
+  dsact_batch o;
+  o.obs = b + h->in2_obs; o.obs2 = b + h->in2_obs2; o.act = b + h->in2_act; o.rew = b + h->in2_rew; o.done = b + h->in2_done;
+  o.logp = b + h->in2_logp; o.batch = batch;
+  return o;
+}
+
+// allocate the second input set on the first call, laid out like the arena's (Arena::build)
+static int ensure_input_set2(MlpHandle* h) {
+  if (h->in2) return DSACT_OK;
+  const int64_t B = h->cfg.max_batch, O = h->cfg.obs_dim, A = h->cfg.act_dim;
+  int64_t off = 0;
+  auto take = [&](int64_t n) { int64_t o = off; off += round64(n); return o; };
+  h->in2_obs = take(B * O); h->in2_obs2 = take(B * O); h->in2_act = take(B * A);
+  h->in2_rew = take(B); h->in2_done = take(B); h->in2_logp = take(B);
+  const int widths[3] = {(int)O, (int)O, (int)A};
+  for (int i = 0; i < 3; ++i) {
+    ImgSlot& s = h->in2_img[i];
+    if (!h->tc()) { s = ImgSlot(); continue; }
+    s.rows = (int)B; s.width = widths[i]; s.pitch = (widths[i] + 7) / 8 * 8;
+    s.plane = round64(B * s.pitch);
+    s.off = take(s.plane);   // 2 planes of bf16 = plane floats
+  }
+  CUDA_TRY(cudaMalloc(&h->in2, sizeof(float) * (size_t)off));
+  CUDA_TRY(cudaMemset(h->in2, 0, sizeof(float) * (size_t)off));
+  CUDA_TRY(cudaStreamCreateWithFlags(&h->gather_stream, cudaStreamNonBlocking));
+  CUDA_TRY(cudaEventCreateWithFlags(&h->ev_gather_fork, cudaEventDisableTiming));
+  CUDA_TRY(cudaEventCreateWithFlags(&h->ev_gather_join, cudaEventDisableTiming));
+  return DSACT_OK;
+}
+
+// tb_info denominators (dsact_read_stats): DSAC_V1 logs one entry of the logits row per sample (dsac_v1.py:142-143),
+// DSAC-T the mean over all action dimensions
+static void stats_scales(const dsact_handle* h, int64_t global_batch, float* inv_batch, float* inv_policy) {
+  const double pol = h->v1 ? (double)global_batch : (double)global_batch * h->act_dim;
+  *inv_batch = (float)(1.0 / (double)global_batch);
+  *inv_policy = (float)(1.0 / pol);
+}
+
+// Updates k = 0 .. n-1, each one dsact_replay_step on its slice of idx / noise.  Update k reads input set k & 1; the gather
+// of update k + 1 into the other set needs only the generator counter update k's sample_kernel leaves, so it is forked
+// (captured: onto its own stream) once update k's forward passes are enqueued and runs beside update k's backward; the
+// set it overwrites was last read by update k - 1.  The prologue of update k + 1 (weight images, noise, clears, Adam
+// scalars) reads what update k's apply writes and follows it on the main stream with programmatic dependent launch.
+// stats_out: row k = update k's finalised tb_info, written before update k + 1 clears the accumulators.
+static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx, const dsact_noise* np, float* stats_out, Ctx& c) {
+  const int64_t A = h->cfg.act_dim;
+  const bool fused = h->fused();
+  const bool fork = c.side != nullptr;
+  auto noise_of = [&](int k) {
+    return dsact_noise{np->eps1 + (size_t)k * B * A, np->eps2 + (size_t)k * B * A, np->z3 + (size_t)k * B, np->z4 + (size_t)k * B};
+  };
+  auto idx_of = [&](int k) { return idx ? idx + (size_t)k * B : nullptr; };
+  // gather of update k into input set k & 1 (+ the counter step a drawn-index, caller-noise update takes after it)
+  auto gather = [&](int k, Ctx& cg) {
+    const int set = k & 1;
+    const dsact_batch dst = input_batch(h, set, B);
+    const ImgOut img[3] = {img_out_of(h, h->input_img(set, 0, B)), img_out_of(h, h->input_img(set, 1, B)),
+                           img_out_of(h, h->input_img(set, 2, B))};
+    enqueue_gather(h, B, idx_of(k), img, !fused, cg, &dst);
+    if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, cg, h->buf.state); cg.done(); }
+  };
+  float inv_b, inv_pol;
+  stats_scales(h, B, &inv_b, &inv_pol);
+  bool gather_forked = false;
+  for (int k = 0; k < n; ++k) {
+    const int set = k & 1;
+    h->in_set = set;
+    const dsact_batch bt = input_batch(h, set, B);
+    dsact_noise nk;
+    const dsact_noise* npk = nullptr;
+    if (np) { nk = noise_of(k); npk = &nk; }
+    if (k == 0) {   // as dsact_replay_step: the prologue beside the gather
+      const bool forked = fork_prologue(h, bt, npk, c, true);
+      gather(0, c);
+      enqueue_phase1(h, bt, npk, c, true, forked);
+    } else {
+      enqueue_prologue(h, bt, npk, c, true);
+      if (gather_forked) cudaStreamWaitEvent(c.s, h->ev_gather_join, 0);
+      enqueue_phase1(h, bt, npk, c, true, false, false, true);
+    }
+    gather_forked = false;
+    if (k + 1 < n) {
+      if (fork) {
+        fork_branch(c, h->ev_gather_fork, h->ev_gather_join, [&](Ctx& cg) { gather(k + 1, cg); }, h->gather_stream);
+        gather_forked = true;
+      } else {
+        gather(k + 1, c);
+      }
+    }
+    const TailArgs ta = tail_args(h, B, B);
+    enqueue_phase2(h, bt, B, c, &ta, false);
+    enqueue_apply(h, c, &ta, false);
+    if (stats_out) {
+      launch_k(finalize_stats_kernel, 1, 32, 0, c, h->buf.state, inv_b, inv_pol, stats_out + (size_t)k * DSACT_NUM_STATS);
+      c.done();
+    }
+  }
+  h->in_set = 0;
+  c.check();
+}
+
 // ---- graph cache -------------------------------------------------------------
-enum { K_STEP = 1, K_PHASE1 = 2, K_PHASE2 = 3, K_APPLY = 4, K_GRADS = 5, K_SAMPLE = 6, K_REPLAY_STEP = 7, K_DP_STEP = 8, K_DP_REPLAY_STEP = 9 };
+enum { K_STEP = 1, K_PHASE1 = 2, K_PHASE2 = 3, K_APPLY = 4, K_GRADS = 5, K_SAMPLE = 6, K_REPLAY_STEP = 7, K_DP_STEP = 8, K_DP_REPLAY_STEP = 9,
+       K_REPLAY_STEPS = 10 };
 
 static void drop_graphs(MlpHandle* h) {
   for (auto& e : h->graphs) cudaGraphExecDestroy(e.exec);
@@ -1682,6 +1825,10 @@ void dsact_destroy(dsact_handle* hh) {
     if (h->ev_stage_done[t]) cudaEventDestroy(h->ev_stage_done[t]);
   }
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
+  if (h->in2) cudaFree(h->in2);
+  if (h->gather_stream) cudaStreamDestroy(h->gather_stream);
+  if (h->ev_gather_fork) cudaEventDestroy(h->ev_gather_fork);
+  if (h->ev_gather_join) cudaEventDestroy(h->ev_gather_join);
   delete h;
 }
 
@@ -1894,9 +2041,9 @@ int dsact_read_stats(dsact_handle* h, int64_t global_batch, float* host_out, voi
   if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
   if (!host_out || global_batch < 1) return fail(DSACT_EINVAL, "bad argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  // DSAC_V1 logs one entry of the logits row per sample (dsac_v1.py:142-143), DSAC-T the mean over all action dimensions
-  const double pol = h->v1 ? (double)global_batch : (double)global_batch * h->act_dim;
-  finalize_stats_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(h->buf.state, (float)(1.0 / (double)global_batch), (float)(1.0 / pol));
+  float inv_b, inv_pol;
+  stats_scales(h, global_batch, &inv_b, &inv_pol);
+  finalize_stats_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(h->buf.state, inv_b, inv_pol, nullptr);
   CUDA_TRY(cudaGetLastError());
   h->launches++;
   CUDA_TRY(cudaMemcpyAsync(host_out, h->buf.state + ST_STATS, DSACT_NUM_STATS * sizeof(float), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
@@ -1987,6 +2134,34 @@ int dsact_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const int64
   h->pending = bt; h->pending_batch = batch;
   h->arena_imaged = false;   // the arena's images (and, in the fused modes, only they) now belong to this step's gather
   h->dev_iter = iteration + 1;
+  return DSACT_OK;
+}
+
+int dsact_replay_steps(dsact_handle* hh, int32_t n_steps, int32_t batch, int64_t size, const int64_t* idx,
+                       const dsact_noise* noise, float* stats_out, int64_t iteration, void* stream) {
+  int rc = check_mlp(hh, "dsact_replay_steps");
+  if (rc) return rc;
+  MlpHandle* h = mlp(hh);
+  if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
+  if (n_steps < 1 || n_steps > DSACT_MAX_REPLAY_STEPS) return fail(DSACT_EINVAL, "n_steps %d outside [1, %d]", n_steps, DSACT_MAX_REPLAY_STEPS);
+  if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
+  if (iteration + n_steps - 1 > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
+  rc = check_noise(noise);
+  if (rc) return rc;
+  CUDA_TRY(cudaSetDevice(h->device));
+  if ((rc = ensure_input_set2(h))) return rc;
+  if ((rc = sync_rb_size(h, size, (cudaStream_t)stream))) return rc;
+  if ((rc = sync_iteration(h, iteration, (cudaStream_t)stream))) return rc;
+  dsact_noise nz; const dsact_noise* np = nullptr;
+  if (noise) { nz = *noise; np = &nz; }
+  const dsact_batch bt = arena_batch(h, batch);
+  GraphKey key = make_key(K_REPLAY_STEPS, &bt, np, batch);
+  key.idx = idx; key.n_steps = n_steps; key.out = stats_out;
+  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) { enqueue_replay_steps(h, n_steps, batch, idx, np, stats_out, c); });
+  if (rc) return rc;
+  h->pending = input_batch(h, (n_steps - 1) & 1, batch); h->pending_batch = batch;
+  h->arena_imaged = false;
+  h->dev_iter = iteration + n_steps;
   return DSACT_OK;
 }
 

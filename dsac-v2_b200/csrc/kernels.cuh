@@ -890,12 +890,13 @@ __global__ void phase2_tail_kernel(float* __restrict__ grad_log_alpha, float* __
   else if (t == 2) state[ST_ALPHA_USED] = val;
 }
 
-// tb_info (dsac_v2.py:188-202) from the accumulators.
-__global__ void finalize_stats_kernel(float* __restrict__ state, float inv_global_batch, float inv_policy_elems) {
+// tb_info (dsac_v2.py:188-202) from the accumulators, into `out` (16 floats; null: the state's ST_STATS slots).
+__global__ void finalize_stats_kernel(float* __restrict__ state, float inv_global_batch, float inv_policy_elems,
+                                      float* __restrict__ out) {
   pdl_sync();
   if (threadIdx.x != 0) return;
   const float* acc = state + ST_ACC;
-  float* o = state + ST_STATS;
+  float* o = out ? out : state + ST_STATS;
   o[0] = acc[ACC_Q1] * inv_global_batch;
   o[1] = acc[ACC_Q2] * inv_global_batch;
   o[2] = acc[ACC_S1] * inv_global_batch;

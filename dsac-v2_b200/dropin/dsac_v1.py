@@ -35,6 +35,7 @@ from dsact_host import TB_TAGS as tb_tags
 from dsact_host import full_state_dict as _full_state
 from dsact_host import load_full_state_dict as _load_full_state
 from dsact_host import net_kwargs
+from dsact_host import replay_updates_on_engine
 
 from dsac_v2_b200 import _lib
 from dsac_v2_b200.engine import Engine, make_config, make_v1_options
@@ -211,6 +212,16 @@ class DSAC_V1:
         tb = {k: vals[i] for k, i in _V1_KEYS}
         tb[tb_tags["alg_time"]] = (time.time() - t0) * 1000
         return tb
+
+    def replay_updates(self, buffer, batch_size: int, iteration: int, n: int) -> list:
+        """n rounds of `local_update(buffer.sample_batch(batch_size), iteration + k)`, k = 0 .. n-1, as ONE engine call
+        (Engine.replay_steps) on the MLP engine: the same host draws in the same order, the same results.  Returns the n
+        tb_info mappings, fetched with one copy of the [n, 16] block on first access.  The head-wise engine takes the n
+        rounds one by one."""
+        eng = self.networks.engine(batch_size)
+        if self.networks._gemm is None:
+            return [self.local_update(buffer.sample_batch(batch_size), iteration + k) for k in range(n)]
+        return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, _V1_KEYS)
 
     # ---- full training state (the reference saves weights only, training/trainer.py:137-152) ----
     def full_state_dict(self) -> dict:

@@ -32,6 +32,7 @@ import networks.cnn as _cnn
 import networks.mlp as _mlp
 from dsact_host import TB_TAGS as tb_tags
 from dsact_host import full_state_dict as _full_state
+from dsact_host import replay_updates_on_engine
 from dsact_host import load_full_state_dict as _load_full_state
 from dsact_host import net_kwargs
 
@@ -347,6 +348,18 @@ class DSAC_V2:
         gb = self._gradients(data, eng)
         eng.apply(iteration)
         return self._stats(eng, gb, t0)
+
+    def replay_updates(self, buffer, batch_size: int, iteration: int, n: int) -> list:
+        """n rounds of `local_update(buffer.sample_batch(batch_size), iteration + k)`, k = 0 .. n-1, as ONE engine call
+        (Engine.replay_steps) where the engine has one: the same host draws in the same order (numpy indices, torch CPU
+        noise), the same results.  Device draws take one generator counter per update (as replay_step), not two as a
+        sample_batch + local_update round does: same distribution, other numbers.  Returns the n tb_info mappings; their values are fetched with one copy of the [n, 16]
+        block on first access.  The head-wise engine and data-parallel runs take the n rounds one by one."""
+        eng = self.networks.engine(batch_size)
+        _, world = self._world()
+        if self.networks._cnn or world > 1:
+            return [self.local_update(buffer.sample_batch(batch_size), iteration + k) for k in range(n)]
+        return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, list(zip(STAT_KEYS, range(14))))
 
     def get_remote_update_info(self, data: Dict, iteration: int) -> Tuple[dict, dict]:
         t0 = time.time()

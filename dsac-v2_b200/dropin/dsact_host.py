@@ -8,6 +8,8 @@ from __future__ import annotations
 import math
 import os
 import sys
+import time
+from collections.abc import Mapping
 
 import numpy as np
 import torch
@@ -185,3 +187,73 @@ def net_kwargs(kind: str, kwargs: dict) -> dict:
         act_low_lim=np.array(kwargs["action_low_limit"], dtype=np.float32),
         action_distribution_cls=cls,
     )
+
+
+# ---- n replay-fed updates per call (DSAC_V2.replay_updates / DSAC_V1.replay_updates) --------------------------------
+def host_draws(buffer, batch: int, n: int, noise_fn):
+    """The host draws of n rounds of `buffer.sample_batch(batch)` + `local_update`, in that order: per round the replay
+    indices (numpy's global generator, index_source "numpy"; else None) then the update's noise (`noise_fn(batch)`, torch's
+    CPU generator; None for device noise).  Returns (idx [n, batch] or None, (eps1, eps2, z3, z4) stacked over rounds or
+    None)."""
+    idx, noise = [], []
+    for _ in range(n):
+        idx.append(buffer.sample_indices(batch))
+        noise.append(noise_fn(batch))
+    idx = None if idx[0] is None else torch.stack([torch.as_tensor(i) for i in idx])
+    noise = None if noise[0] is None else tuple(torch.stack([z[j] for z in noise]) for j in range(4))
+    return idx, noise
+
+
+class LazyStatsRow(Mapping):
+    """tb_info of update k of a replay_updates call: the [n, 16] statistics block is copied to pinned host memory once
+    (asynchronously, at the call) and read on the first access to any of its rows.  `keys`: (tag, column) pairs."""
+
+    class Block:
+        def __init__(self, dev_stats: torch.Tensor):
+            self.host = torch.empty(dev_stats.shape, dtype=torch.float32).pin_memory()
+            self.host.copy_(dev_stats, non_blocking=True)
+            self.event = torch.cuda.Event()
+            self.event.record(torch.cuda.current_stream(dev_stats.device))
+            self.rows = None
+
+        def get(self):
+            if self.rows is None:
+                self.event.synchronize()
+                self.rows = self.host.tolist()
+            return self.rows
+
+    def __init__(self, block: "LazyStatsRow.Block", k: int, keys, alg_ms: float):
+        self._block, self._k, self._keys, self._alg_ms, self._vals = block, k, keys, alg_ms, None
+
+    def _materialise(self) -> dict:
+        if self._vals is None:
+            row = self._block.get()[self._k]
+            vals = {tag: row[c] for tag, c in self._keys}
+            vals[TB_TAGS["alg_time"]] = self._alg_ms
+            self._vals, self._block = vals, None
+        return self._vals
+
+    def __getitem__(self, k):
+        return self._materialise()[k]
+
+    def __iter__(self):
+        return iter(self._materialise())
+
+    def __len__(self):
+        return len(self._keys) + 1
+
+
+def replay_updates_on_engine(eng, buffer, batch: int, iteration: int, n: int, noise_fn, keys) -> list:
+    """replay_updates on the MLP engine: the host draws of n rounds, one Engine.replay_steps call, one lazy tb_info
+    mapping per update (`keys`: (tag, column of the 16 statistics) pairs)."""
+    t0 = time.time()
+    if buffer.engine is not eng:
+        raise ValueError("the replay buffer is not attached to this algorithm's engine")
+    if buffer.size == 0:
+        raise ValueError("cannot sample from an empty replay buffer")
+    buffer.flush()
+    idx, noise = host_draws(buffer, batch, n, noise_fn)
+    stats = eng.replay_steps(n, batch, buffer.size, iteration, idx=idx, noise=noise)
+    block = LazyStatsRow.Block(stats)
+    alg_ms = (time.time() - t0) * 1000 / n
+    return [LazyStatsRow(block, k, keys, alg_ms) for k in range(n)]

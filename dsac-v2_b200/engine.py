@@ -386,6 +386,52 @@ class Engine:
             check(self.lib.dsact_replay_step(self.h, int(batch), int(size), _ptr(idx), n, int(iteration), self._stream()))
         self.last_batch = int(batch)
 
+    def _steps_buffer(self, name: str, src: torch.Tensor, dtype) -> torch.Tensor:
+        """`src` as a contiguous device tensor.  Host data is staged into a buffer kept per name and shape, so that a
+        repeated call hands the library the same pointers (they are part of the captured graph's key)."""
+        if src.device == self.device and src.dtype == dtype and src.is_contiguous():
+            return src
+        if src.device.type != "cpu":
+            return src.to(device=self.device, dtype=dtype).contiguous()
+        bufs = self.__dict__.setdefault("_steps_bufs", {})
+        key = (name, tuple(src.shape))
+        if key not in bufs:
+            bufs[key] = torch.empty(src.shape, dtype=dtype, device=self.device)
+        buf = bufs[key]
+        buf.copy_(src.to(dtype).contiguous(), non_blocking=True)
+        return buf
+
+    def replay_steps(self, n: int, batch: int, size: int, iteration: int, idx: Optional[torch.Tensor] = None, noise=None,
+                     stats: bool = True) -> Optional[torch.Tensor]:
+        """n replay_step calls in one submission (dsact_replay_steps): updates for iterations iteration .. iteration+n-1.
+        `idx`: None (device draws) or int64 [n, batch]; `noise`: None or (eps1, eps2 [n, batch, A], z3, z4 [n, batch]).
+        Returns the [n, 16] device tensor of per-update tb_info rows (valid until the next call with the same n), or None
+        with stats=False."""
+        n, B, A = int(n), int(batch), self.cfg.act_dim
+        with torch.cuda.device(self.device):
+            if idx is not None:
+                idx = self._steps_buffer("idx", torch.as_tensor(idx), torch.int64)
+                if idx.shape != (n, B):
+                    raise ValueError(f"idx must be [n, batch] = [{n}, {B}], got {tuple(idx.shape)}")
+            nz = None
+            if noise is not None:
+                shapes = ((n, B, A), (n, B, A), (n, B), (n, B))
+                ts = [self._steps_buffer(k, torch.as_tensor(x).reshape(s), torch.float32)
+                      for k, x, s in zip(("eps1", "eps2", "z3", "z4"), noise, shapes)]
+                nz = C.byref(Noise(*(t.data_ptr() for t in ts)))
+                self._keep_noise = ts
+            out = None
+            if stats:
+                outs = self.__dict__.setdefault("_steps_stats", {})
+                if n not in outs:
+                    outs[n] = torch.zeros(n, _lib.NUM_STATS, dtype=torch.float32, device=self.device)
+                out = outs[n]
+            self._keep_idx = idx
+            check(self.lib.dsact_replay_steps(self.h, n, B, int(size), _ptr(idx), nz, _ptr(out), int(iteration),
+                                              self._stream()))
+        self.last_batch = B
+        return out
+
     # ---- data-parallel replicas over NVLink peer memory (include/dsact.h) ---------------------
     def dp_export(self) -> bytes:
         """Allocate this rank's exchange buffer; its CUDA IPC handle (to be handed to every other rank)."""

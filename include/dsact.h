@@ -197,6 +197,20 @@ int dsact_replay_sample(dsact_handle *h, int32_t batch, int64_t size, const int6
 /* sample_batch + local_update in one submission (no host round trip in between) */
 int dsact_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx,
                       const dsact_noise *noise, int64_t iteration, void *stream);
+/* n_steps consecutive dsact_replay_step calls in one submission (one graph launch with use_graph): updates for iterations
+ * iteration .. iteration+n_steps-1, each drawing from the ring of `size` rows, with the same generator counters, delayed-
+ * update phases and resulting device state as the n single calls (the off_idx slot holds the last update's indices,
+ * dsact_read_stats returns the last update's statistics).  The gather of update k+1 runs beside update k's backward, into
+ * a second minibatch input set the library allocates on the first call (for max_batch rows; freed by dsact_destroy).
+ *   idx:       NULL (each update draws its own indices on the device) or device int64 [n_steps, batch].
+ *   noise:     NULL (device draws) or arrays with a leading n_steps dimension: eps1/eps2 [n_steps, batch, act_dim],
+ *              z3/z4 [n_steps, batch].
+ *   stats_out: NULL or device float [n_steps, DSACT_NUM_STATS]. Row k holds update k's finalised tb_info over `batch`
+ *              rows: the 16 floats dsact_read_stats(h, batch, ...) would return after the k-th single call.
+ * MLP-engine handles only (DSAC-T and DSAC_V1); 1 <= n_steps <= DSACT_MAX_REPLAY_STEPS. */
+#define DSACT_MAX_REPLAY_STEPS 64
+int dsact_replay_steps(dsact_handle *h, int32_t n_steps, int32_t batch, int64_t size, const int64_t *idx,
+                       const dsact_noise *noise, float *stats_out, int64_t iteration, void *stream);
 
 /* ---- data-parallel replicas over NVLink peer memory (one process per GPU) ---------------------------------------
  * Replaces, for the same path, what `dsac-v2_b200/dp.py` does with three graph launches and four NCCL all-reduces
