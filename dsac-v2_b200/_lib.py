@@ -113,6 +113,19 @@ class TestChainPass(C.Structure):
                 ("img", _fp * MAX_HIDDEN), ("colsum", _fp * MAX_HIDDEN), ("out", _fp)]
 
 
+TEST_KERNELS = {"sample": 0, "loss": 1, "policy_grad": 2, "stats": 3}   # DSACT_TEST_*
+
+
+class TestRowIo(C.Structure):
+    """dsact_test_row_io: the per-row arrays of one dsact_test_rows launch."""
+    _fields_ = [("kernel", C.c_int32), ("batch", C.c_int32), ("global_batch", C.c_int64), ("max_blocks", C.c_int32),
+                ("advance_rng", C.c_int32), ("logits", _fp * 2), ("eps", _fp * 2), ("act", _fp * 2), ("logp", _fp * 2),
+                ("rew", _fp), ("done", _fp), ("z3", _fp), ("z4", _fp), ("out_q", _fp * 6), ("d_out_q", _fp * 2),
+                ("d_out_qa", _fp * 2), ("d_act", _fp * 2), ("d_logits", _fp), ("gbias_q", _fp * 2), ("gbias_q_raw", _fp * 2),
+                ("gbias_pi", _fp), ("gbias_ls", _fp), ("img_act", _fp * 2), ("img_q", _fp * 2), ("img_qa", _fp * 2),
+                ("img_dlogits", _fp), ("stats_out", _fp)]
+
+
 # every symbol include/dsact.h declares: (restype, argtypes)
 IPC_HANDLE_BYTES = 64   # DSACT_IPC_HANDLE_BYTES
 DP_MAX_RANKS = 8        # DSACT_DP_MAX_RANKS
@@ -157,6 +170,8 @@ SYMBOLS = {
     "dsact_test_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TestLayer), C.c_int32, C.c_int32, C.c_void_p]),
     "dsact_test_chain": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_void_p, C.POINTER(TestChainPass), C.c_int32, C.c_void_p]),
+    "dsact_test_rows": (C.c_int, [C.c_void_p, C.POINTER(TestRowIo), C.c_void_p]),
+    "dsact_test_apply": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]),
 }
 
 _lib = None

@@ -488,7 +488,7 @@ static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsac
         v.push_back({Pq[k] + q.head_off[hd], f.Q[k], q.F, bt.act, A, &h->hb[4 + 2 * k + hd], true, W + s.outQ[k] + hd, 2});
     cnn_heads_forward(h, q.head, v, B, c);
   }
-  enqueue_sample(h, B, nz.eps1, nz.eps2, !noise, NO_IMG, NO_IMG, c);
+  enqueue_sample(h, step_rows(h, bt, nz), B, !noise, c);
   // ---- targets on (s', a') and the mean heads of the critics on (s, a~)
   {
     std::vector<CnnHeadFwd> v;
@@ -519,17 +519,15 @@ static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
 
   // ---- losses and head-output gradients
   const StepScalars sc = step_scalars(h, global_batch);
-  float* gbias[2], *gbias_raw[2];
+  RowIo io = step_rows(h, bt, dsact_noise{h->pending_eps1, nullptr, h->pending_z3, h->pending_z4});
   for (int k = 0; k < 2; ++k) {
-    gbias[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];                                       // output bias of the mean head
-    gbias_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
+    io.gbias_q[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];                                       // output bias of the mean head
+    io.gbias_q_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
   }
-  if (h->v1) {
-    enqueue_loss_v1(h, bt, sc, gbias[0], gbias_raw[0], NO_IMG, NO_IMG, c);
-  } else {
-    const ImgOut none[2] = {NO_IMG, NO_IMG};
-    enqueue_loss(h, bt, sc, gbias, gbias_raw, none, none, c);
-  }
+  io.gbias_pi = Gpi + pi.head_off[0] + pi.head.b[pi.head.L];   // output bias of the mean head [A]
+  io.gbias_ls = pi.ls_row >= 0 ? Gpi + pi.ls_row : (pi.nheads == 2 ? Gpi + pi.head_off[1] + pi.head.b[pi.head.L] : nullptr);   // log_std head / row [A]
+  if (h->v1) enqueue_loss_v1(h, io, B, sc, c);
+  else enqueue_loss(h, io, B, sc, c);
   auto zero = [&](float* p, long long n) {
     int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
     launch_k(zero_kernel, blocks, 256, 0, c, p, n); c.done();
@@ -572,9 +570,7 @@ static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
                                             sizeof(float) * A, B, cudaMemcpyDeviceToDevice, c.s);
     if (e != cudaSuccess && c.err == cudaSuccess) c.err = e;
   }
-  enqueue_policy_grad(h, B, sc, Gpi + pi.head_off[0] + pi.head.b[pi.head.L],   // output bias of the mean head [A]
-                      pi.ls_row >= 0 ? Gpi + pi.ls_row : (pi.nheads == 2 ? Gpi + pi.head_off[1] + pi.head.b[pi.head.L] : nullptr),   // log_std head / row [A]
-                      NO_IMG, c);
+  enqueue_policy_grad(h, io, B, sc, c);
   {
     std::vector<CnnHeadBwd> v;
     for (int hd = 0; hd < pi.nheads; ++hd)

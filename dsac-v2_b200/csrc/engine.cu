@@ -1018,91 +1018,113 @@ static void enqueue_noise(const dsact_handle* h, int B, Ctx& c) {
   c.done();
 }
 
+// The per-row arrays the sampling, loss and policy-gradient kernels read and write, and where they add their output-bias
+// gradients.  The steps fill it from the arena slots (step_rows); dsact_test_rows from caller buffers.  Indices follow
+// StepSlots: out_q[p] is pass p (Q_k(s,a) = k, Q'_k(s',a') = 2 + k, Q_k(s,a~) = 4 + k; DSAC_V1: k = 0 only).
+struct RowIo {
+  const float *logits[2], *eps[2];   // pi(s), pi'(s') outputs (mean | log_std) [B,2A]; their noise [B,A]
+  float *act[2], *logp[2];           // a~, a' [B,A]; logp_new, logp2 [B] (written by sample, read by the losses)
+  const float *rew, *done, *z3, *z4;
+  const float* out_q[6];             // [B,2] (mean, raw std)
+  float *d_out_q[2], *d_out_qa[2];   // dL/d(mean, raw std) of Q_k(s,a) and of Q_k(s,a~)
+  const float* d_act[2];             // dL/da~ through critic k [B,A]; d_act[1] null: one critic (policy_grad_kernel<1>)
+  float* d_logits;                   // [B,2A]
+  // output-bias gradients (+=): gbias_q[k] critic k's mean; gbias_q_raw[k] its std output, or null for the element after
+  // gbias_q[k] (one two-output layer); gbias_pi the policy's mean (the whole (mean | log_std) row when gbias_ls is null)
+  float *gbias_q[2], *gbias_q_raw[2], *gbias_pi, *gbias_ls;
+  ImgOut img_act[2], img_q[2], img_qa[2], img_dlogits;   // bf16 images (NO_IMG: none)
+};
+// the step's row arrays: the arena slots, the minibatch `bt` and the noise `nz`; no bias-gradient targets and no images
+static RowIo step_rows(const dsact_handle* h, const dsact_batch& bt, const dsact_noise& nz) {
+  const StepSlots& s = h->slot;
+  float* W = h->W();
+  RowIo io;
+  memset(&io, 0, sizeof(io));
+  io.logits[0] = W + s.logitsP; io.logits[1] = W + s.logitsT;
+  io.eps[0] = nz.eps1; io.eps[1] = nz.eps2;
+  io.act[0] = W + s.new_act; io.act[1] = W + s.act2;
+  io.logp[0] = W + s.logp_new; io.logp[1] = W + s.logp2;
+  io.rew = bt.rew; io.done = bt.done; io.z3 = nz.z3; io.z4 = nz.z4;
+  for (int p = 0; p < 6; ++p) io.out_q[p] = s.outQ[p] < 0 ? nullptr : W + s.outQ[p];
+  for (int k = 0; k < 2; ++k) {
+    io.d_out_q[k] = s.dOut[k] < 0 ? nullptr : W + s.dOut[k];
+    io.d_out_qa[k] = s.dOut[4 + k] < 0 ? nullptr : W + s.dOut[4 + k];
+    io.d_act[k] = s.dAct[k] < 0 ? nullptr : W + s.dAct[k];   // DSAC_V1 on the MLP engine: no second action-gradient slot
+  }
+  io.d_logits = W + s.dlogits;
+  io.img_act[0] = io.img_act[1] = io.img_q[0] = io.img_q[1] = io.img_qa[0] = io.img_qa[1] = io.img_dlogits = NO_IMG;
+  return io;
+}
+// a launch's blocks: the step's count `natural`, or at most `max_blocks` (> 0, dsact_test_rows / dsact_test_apply) so that
+// few rows take several grid-stride trips
+static int capped(int natural, int max_blocks) { return max_blocks > 0 && natural > max_blocks ? max_blocks : natural; }
+
 // rsample of both policies (utils/act_distribution_cls.py:44-54); also sums the critics' std over the rows (DSAC_V1: of
 // its one critic, and its own logged policy statistics)
-static void enqueue_sample(const dsact_handle* h, int B, const float* eps1, const float* eps2, bool advance_rng,
-                           const ImgOut& img_new_act, const ImgOut& img_act2, Ctx& c) {
-  const StepSlots& s = h->slot;
+static void enqueue_sample(const dsact_handle* h, const RowIo& io, int B, bool advance_rng, Ctx& c, int max_blocks = 0) {
   const StepHyper& p = h->hyper;
-  float* W = h->W();
   SampleArgs a;
-  a.logits[0] = W + s.logitsP; a.logits[1] = W + s.logitsT;
-  a.eps[0] = eps1; a.eps[1] = eps2;
-  a.act[0] = W + s.new_act; a.act[1] = W + s.act2;
-  a.logp[0] = W + s.logp_new; a.logp[1] = W + s.logp2;
+  for (int k = 0; k < 2; ++k) {
+    a.logits[k] = io.logits[k]; a.eps[k] = io.eps[k]; a.act[k] = io.act[k]; a.logp[k] = io.logp[k]; a.img[k] = io.img_act[k];
+  }
   a.hi = h->buf.act_high; a.lo = h->buf.act_low; a.state = h->buf.state;
   a.B = B; a.A = h->act_dim; a.min_log_std = (float)p.min_log_std; a.max_log_std = (float)p.max_log_std; a.gauss = p.act_dist;
-  a.img[0] = img_new_act; a.img[1] = img_act2;
-  a.out_q[0] = W + s.outQ[0]; a.out_q[1] = W + s.outQ[h->v1 ? 0 : 1];
+  a.out_q[0] = io.out_q[0]; a.out_q[1] = io.out_q[h->v1 ? 0 : 1];
   a.advance_rng = advance_rng ? 1 : 0;
   a.v1_stats = h->v1 ? 1 : 0;
   int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-  launch_k(sample_kernel, dim3(blocks, 2), 256, 0, c, a);
+  launch_k(sample_kernel, dim3(capped(blocks, max_blocks), 2), 256, 0, c, a);
   c.done();
 }
 
-// the DSAC-T losses and the gradients of the critics' outputs.  gbias[k]: output-bias gradient of critic k's mean;
-// gbias_raw[k]: of its std output, or null for the element after gbias[k] (one two-output layer)
-static void enqueue_loss(const dsact_handle* h, const dsact_batch& bt, const StepScalars& sc, float* const gbias[2],
-                         float* const gbias_raw[2], const ImgOut img_q[2], const ImgOut img_qa[2], Ctx& c) {
-  const StepSlots& s = h->slot;
-  float* W = h->W();
-  const int B = bt.batch;
+// the DSAC-T losses and the gradients of the critics' outputs
+static void enqueue_loss(const dsact_handle* h, const RowIo& io, int B, const StepScalars& sc, Ctx& c, int max_blocks = 0) {
   LossArgs a;
   a.sc = sc;
-  a.rew = bt.rew; a.done = bt.done; a.z3 = h->pending_z3; a.z4 = h->pending_z4;
-  a.logp2 = W + s.logp2; a.logp_new = W + s.logp_new;
+  a.rew = io.rew; a.done = io.done; a.z3 = io.z3; a.z4 = io.z4;
+  a.logp2 = io.logp[1]; a.logp_new = io.logp[0];
   for (int k = 0; k < 2; ++k) {
-    a.out_q[k] = W + s.outQ[k]; a.out_qt[k] = W + s.outQ[2 + k]; a.out_qa[k] = W + s.outQ[4 + k];
-    a.d_out_q[k] = W + s.dOut[k]; a.d_out_qa[k] = W + s.dOut[4 + k];
-    a.gbias_q[k] = gbias[k]; a.gbias_q_raw[k] = gbias_raw[k];
-    a.img_q[k] = img_q[k]; a.img_qa[k] = img_qa[k];
+    a.out_q[k] = io.out_q[k]; a.out_qt[k] = io.out_q[2 + k]; a.out_qa[k] = io.out_q[4 + k];
+    a.d_out_q[k] = io.d_out_q[k]; a.d_out_qa[k] = io.d_out_qa[k];
+    a.gbias_q[k] = io.gbias_q[k]; a.gbias_q_raw[k] = io.gbias_q_raw[k];
+    a.img_q[k] = io.img_q[k]; a.img_qa[k] = io.img_qa[k];
   }
   a.state = h->buf.state; a.B = B; a.gamma = (float)h->hyper.gamma; a.inv_global_batch = sc.inv_global_batch;
   int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;   // latency bound: spread over the SMs
-  launch_k(loss_kernel, blocks, 64, 0, c, a);
+  launch_k(loss_kernel, capped(blocks, max_blocks), 64, 0, c, a);
   c.done();
 }
 
-// DSAC_V1's losses (one critic, fixed TD bound) and the gradients of the critic's outputs.  gbias: output-bias gradient of
-// the mean; gbias_raw: of the std output, or null for the element after gbias
-static void enqueue_loss_v1(const dsact_handle* h, const dsact_batch& bt, const StepScalars& sc, float* gbias, float* gbias_raw,
-                            const ImgOut& img_q, const ImgOut& img_qa, Ctx& c) {
-  const StepSlots& s = h->slot;
-  float* W = h->W();
-  const int B = bt.batch;
+// DSAC_V1's losses (one critic, fixed TD bound) and the gradients of the critic's outputs (critic 0 of `io`)
+static void enqueue_loss_v1(const dsact_handle* h, const RowIo& io, int B, const StepScalars& sc, Ctx& c, int max_blocks = 0) {
   LossV1Args a;
-  a.rew = bt.rew; a.done = bt.done; a.z = h->pending_z3; a.logp2 = W + s.logp2; a.logp_new = W + s.logp_new;
-  a.out_q = W + s.outQ[0]; a.out_qt = W + s.outQ[2]; a.out_qa = W + s.outQ[4];
-  a.d_out_q = W + s.dOut[0]; a.d_out_qa = W + s.dOut[4];
-  a.gbias_q = gbias; a.gbias_q_raw = gbias_raw;
+  a.rew = io.rew; a.done = io.done; a.z = io.z3; a.logp2 = io.logp[1]; a.logp_new = io.logp[0];
+  a.out_q = io.out_q[0]; a.out_qt = io.out_q[2]; a.out_qa = io.out_q[4];
+  a.d_out_q = io.d_out_q[0]; a.d_out_qa = io.d_out_qa[0];
+  a.gbias_q = io.gbias_q[0]; a.gbias_q_raw = io.gbias_q_raw[0];
   a.state = h->buf.state; a.B = B; a.bound = h->v1_bound; a.gamma = (float)h->hyper.gamma; a.inv_global_batch = sc.inv_global_batch;
   a.td_bound = (float)h->td_bound; a.sc = sc;
-  a.img_q = img_q; a.img_qa = img_qa;
+  a.img_q = io.img_q[0]; a.img_qa = io.img_qa[0];
   int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-  launch_k(loss_v1_kernel, blocks, 64, 0, c, a);
+  launch_k(loss_v1_kernel, capped(blocks, max_blocks), 64, 0, c, a);
   c.done();
 }
 
-// the actor loss's gradient w.r.t. the policy outputs of pi(s).  gbias: output-bias gradient of the mean (the whole
-// (mean | log_std) row when gbias_ls is null); gbias_ls: of a separate log_std head or row
-static void enqueue_policy_grad(const dsact_handle* h, int B, const StepScalars& sc, float* gbias, float* gbias_ls, const ImgOut& img,
-                                Ctx& c) {
-  const StepSlots& s = h->slot;
+// the actor loss's gradient w.r.t. the policy outputs of pi(s)
+static void enqueue_policy_grad(const dsact_handle* h, const RowIo& io, int B, const StepScalars& sc, Ctx& c, int max_blocks = 0) {
   const StepHyper& p = h->hyper;
-  float* W = h->W();
   const int A = h->act_dim;
   PolicyGradArgs a;
-  const bool one_critic = s.dAct[1] < 0;   // DSAC_V1 on the MLP engine: no second action-gradient slot
-  a.logits = W + s.logitsP; a.eps = h->pending_eps1; a.d_act1 = W + s.dAct[0]; a.d_act2 = one_critic ? nullptr : W + s.dAct[1];
+  const bool one_critic = io.d_act[1] == nullptr;
+  a.logits = io.logits[0]; a.eps = io.eps[0]; a.d_act1 = io.d_act[0]; a.d_act2 = io.d_act[1];
   a.hi = h->buf.act_high; a.lo = h->buf.act_low;
-  a.d_logits = W + s.dlogits; a.gbias = gbias; a.gbias_ls = gbias_ls; a.state = h->buf.state;
+  a.d_logits = io.d_logits; a.gbias = io.gbias_pi; a.gbias_ls = io.gbias_ls; a.state = h->buf.state;
   a.B = B; a.A = A; a.min_log_std = (float)p.min_log_std; a.max_log_std = (float)p.max_log_std; a.gauss = p.act_dist;
   a.inv_global_batch = sc.inv_global_batch;
-  a.img = img;
+  a.img = io.img_dlogits;
   a.sc = sc;
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;   // a warp per row
-  launch_k(one_critic ? policy_grad_kernel<1> : policy_grad_kernel<2>, blocks, 256, sizeof(float) * 2 * A, c, a);
+  launch_k(one_critic ? policy_grad_kernel<1> : policy_grad_kernel<2>, capped(blocks, max_blocks), 256, sizeof(float) * 2 * A, c, a);
   c.done();
 }
 
@@ -1124,10 +1146,19 @@ static ApplyArgs apply_args(const dsact_handle* h, int64_t n_q2, int scalars_rea
   a.g_lo = 0; a.g_hi = (a.n_all + 3) / 4; a.finish = 1;
   return a;
 }
-static void launch_apply(const dsact_handle* h, const ApplyArgs& a, Ctx& c) {
+// `part` of the flat buffers: 0 = all of it; 1 = the critics' span only, without closing the step (launched beside the
+// policy backward, see enqueue_phase2); 2 = everything after that span + the end-of-step bookkeeping.  A group straddling
+// the critic / policy boundary goes with part 2.
+static void apply_part(ApplyArgs& a, int part) {
+  const int64_t g_q = a.n_q2 / 4;
+  if (part == 2) a.g_lo = g_q;
+  if (part == 1) { a.g_hi = g_q; a.finish = 0; }
+}
+static void launch_apply(const dsact_handle* h, const ApplyArgs& a, Ctx& c, int max_blocks = 0) {
   int blocks = (int)((a.g_hi - a.g_lo + 255) / 256);   // one 4-element group per thread
   if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
   if (blocks < 1) blocks = 1;
+  blocks = capped(blocks, max_blocks);
   // (its last block also advances the step counters)
   if (a.dp_world > 0) launch_k(apply_kernel<2>, blocks, 256, 0, c, a);
   else if (a.nslabs > 0) launch_k(apply_kernel<1>, blocks, 256, 0, c, a);
@@ -1320,7 +1351,9 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
   const dsact_noise noise = step_noise(h, nz);   // device noise: sample_kernel steps the counter
   const StepPasses sp = step_passes(h, bt);
   enqueue_fwd(h, sp.a, sp.na, B, c);
-  enqueue_sample(h, B, noise.eps1, noise.eps2, !nz, img_out(h, h->ar.i_new_act), img_out(h, h->ar.i_act2), c);
+  RowIo io = step_rows(h, bt, noise);
+  io.img_act[0] = img_out(h, h->ar.i_new_act); io.img_act[1] = img_out(h, h->ar.i_act2);
+  enqueue_sample(h, io, B, !nz, c);
   const bool dp_forked = dp_std_exchange && c.side != nullptr;
   if (dp_forked) fork_branch(c, h->ev_dp_fork, h->ev_dp_join, [&](Ctx& cs) { enqueue_dp_exchange(h, 0, cs); });
   else if (dp_std_exchange) enqueue_dp_exchange(h, 0, c);
@@ -1334,10 +1367,10 @@ static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_nois
 static bool slabs_foldable(const MlpHandle* h) {
   return h->tc() && ((uintptr_t)(h->W() + h->ar.slabs) & 15) == 0 && ((uintptr_t)h->buf.grads & 15) == 0;
 }
-static TailArgs tail_args(const MlpHandle* h, int64_t global_batch, int rows) {
+static TailArgs tail_args(const dsact_handle* h, int64_t global_batch, int rows) {
   TailArgs t;
   t.sc = step_scalars(h, global_batch);
-  t.target_entropy = -(float)h->cfg.act_dim; t.rows = rows; t.enabled = 1;
+  t.target_entropy = -(float)h->act_dim; t.rows = rows; t.enabled = 1;
   return t;
 }
 static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail, bool dp, int part);
@@ -1360,15 +1393,15 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const NetInsts& I = sp.I;
 
   const StepScalars sc = step_scalars(h, global_batch);
-  if (h->v1) {
-    enqueue_loss_v1(h, bt, sc, I.q[0].G + q.b[q.L], nullptr, img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[4]), c);
-  } else {
-    float* const gbias[2] = {I.q[0].G + q.b[q.L], I.q[1].G + q.b[q.L]};
-    float* const gbias_raw[2] = {nullptr, nullptr};   // one two-output layer
-    const ImgOut img_q[2] = {img_out(h, ar.i_dOut[0]), img_out(h, ar.i_dOut[1])};
-    const ImgOut img_qa[2] = {img_out(h, ar.i_dOut[4]), img_out(h, ar.i_dOut[5])};
-    enqueue_loss(h, bt, sc, gbias, gbias_raw, img_q, img_qa, c);
+  RowIo io = step_rows(h, bt, dsact_noise{h->pending_eps1, nullptr, h->pending_z3, h->pending_z4});
+  for (int k = 0; k < h->nq(); ++k) {   // one two-output layer per critic: the std output's bias follows the mean's
+    io.gbias_q[k] = I.q[k].G + q.b[q.L];
+    io.img_q[k] = img_out(h, ar.i_dOut[k]); io.img_qa[k] = img_out(h, ar.i_dOut[4 + k]);
   }
+  io.gbias_pi = I.pi.G + pi.b[pi.L];
+  io.img_dlogits = img_out(h, ar.i_dlogits);
+  if (h->v1) enqueue_loss_v1(h, io, B, sc, c);
+  else enqueue_loss(h, io, B, sc, c);
   // The freeze trick of the reference (dsac_v2.py:166-181) makes the critics' and the policy's backward independent: the
   // critics' dgrad, then, beside a policy backward chain, their weight gradients as a side branch.
   Group gw, ga;   // the critics' weight gradients; the per-layer lowering's dL/da~
@@ -1392,7 +1425,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   launch_group(h, ga, V_DGRAD, c);
   h->join_pending = forked;
 
-  enqueue_policy_grad(h, B, sc, I.pi.G + pi.b[pi.L], nullptr, img_out(h, ar.i_dlogits), c);
+  enqueue_policy_grad(h, io, B, sc, c);
   Group gwp, no_act;   // (the policy pass has no action segment)
   enqueue_dgrad(h, &sp.pi, 1, B, c, no_act);
   add_wgrads(gwp, h, &sp.pi, 1, B);
@@ -1418,21 +1451,23 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   c.check();
 }
 
+// The MLP engine's apply of `part` (see apply_part) with the Adam scalars `scalars_ready` (see ApplyArgs), the step's
+// end-of-backward bookkeeping `tail` (null: none) and the first `nslabs` weight-gradient split slabs folded in
+static ApplyArgs mlp_apply_args(const MlpHandle* h, int scalars_ready, const TailArgs* tail, bool dp, int part, int nslabs) {
+  ApplyArgs a = apply_args(h, h->nq() * h->q.n, scalars_ready, dp);
+  if (tail) a.tail = *tail;
+  if (nslabs > 0) { a.slabs = h->W() + h->ar.slabs; a.nslabs = nslabs; a.slab_stride = h->ar.slab_stride; }
+  apply_part(a, part);
+  a.next_scalars = h->tc() ? 0 : 1;   // the tensor-core modes' prologue (step_prologue_kernel) forms them itself
+  return a;
+}
 // `tail` != null: this apply also does the end-of-backward bookkeeping of the step (see TailArgs) and, single-GPU, folds
 // the weight-gradient split slabs.  `dp`: the gradients are the rank-ordered sum of the exchange blocks.
-// `part`: 0 = the whole flat buffer; 1 = the critics' span only, without closing the step (launched beside the policy
-// backward, see enqueue_phase2); 2 = everything after that span + the end-of-step bookkeeping
 static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
   if (part == 0 && h->apply_early) { part = 2; h->apply_early = false; }   // phase 2 already updated the critics
   // split API: the Adam scalars are formed here; single-call steps: precomputed by the previous apply / prologue if stamped
-  ApplyArgs a = apply_args(h, h->nq() * h->q.n, tail ? 2 : 0, dp);
-  if (tail) a.tail = *tail;
-  if (tail && !dp && slabs_foldable(h)) { a.slabs = h->W() + h->ar.slabs; a.nslabs = h->ar.nslabs; a.slab_stride = h->ar.slab_stride; }
-  const int64_t g_q = a.n_q2 / 4;   // a group straddling the critic / policy boundary goes with part 2
-  if (part == 2) a.g_lo = g_q;
-  if (part == 1) { a.g_hi = g_q; a.finish = 0; }
-  a.next_scalars = h->tc() ? 0 : 1;   // the tensor-core modes' prologue (step_prologue_kernel) forms them itself
-  launch_apply(h, a, c);
+  const int nslabs = tail && !dp && slabs_foldable(h) ? h->ar.nslabs : 0;
+  launch_apply(h, mlp_apply_args(h, tail ? 2 : 0, tail, dp, part, nslabs), c);
 }
 
 // One whole update of the single-call steps: phase 1, phase 2 over `global_batch` rows, then (dp) the logged-sum exchange
@@ -2469,6 +2504,117 @@ int dsact_test_chain(dsact_handle* hh, int32_t dgrad, int32_t L, const int32_t* 
     launch_chain(h, cb, dgrad ? CLS_GEMM_DGRAD : CLS_GEMM_FWD, c);
   }
   return finish_hook(h, c, mem);
+}
+
+static int sync_hook(dsact_handle* h, Ctx& c) {
+  const cudaError_t e = cudaStreamSynchronize(c.s);
+  const cudaError_t err = c.err != cudaSuccess ? c.err : e;
+  if (err != cudaSuccess) return fail(DSACT_ECUDA, "launch failed: %s", cudaGetErrorString(err));
+  h->launches += c.launches;
+  return DSACT_OK;
+}
+
+int dsact_test_rows(dsact_handle* h, const dsact_test_row_io* t, void* stream) {
+  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
+  if (!t) return fail(DSACT_EINVAL, "null rows");
+  if (t->kernel < DSACT_TEST_SAMPLE || t->kernel > DSACT_TEST_STATS) return fail(DSACT_EINVAL, "unknown kernel %d", t->kernel);
+  const int B = t->batch;
+  if (t->kernel != DSACT_TEST_STATS && (B < 1 || B > h->max_batch)) return fail(DSACT_EINVAL, "batch %d outside [1, max_batch]", B);
+  if (t->global_batch < (t->kernel == DSACT_TEST_STATS ? 1 : B)) return fail(DSACT_EINVAL, "global_batch < batch");
+  if (t->max_blocks < 0) return fail(DSACT_EINVAL, "max_blocks < 0");
+  const bool v1 = h->v1, mlp_eng = h->engine == ENGINE_MLP;
+  const bool tc = mlp_eng && mlp(h)->tc();
+  const int A = h->act_dim, nq = v1 ? 1 : 2;
+  const void* imgs[7] = {t->img_act[0], t->img_act[1], t->img_q[0], t->img_q[1], t->img_qa[0], t->img_qa[1], t->img_dlogits};
+  for (const void* p : imgs)
+    if (p && !tc) return fail(DSACT_EINVAL, "images need a tensor-core mode of the MLP engine");
+  auto need = [&](const void* p, const char* what) { return p ? DSACT_OK : fail(DSACT_EINVAL, "%s is null", what); };
+  int rc = DSACT_OK;
+  RowIo io;
+  memset(&io, 0, sizeof(io));
+  auto img = [&](void* p, int width) {
+    if (!p) return NO_IMG;
+    ImgOut o;
+    o.p = static_cast<__nv_bfloat16*>(p); o.pitch = (width + 7) / 8 * 8; o.planes = mlp(h)->passes() == 3 ? 2 : 1;
+    o.plane = (long long)B * o.pitch;
+    return o;
+  };
+  for (int k = 0; k < 2; ++k) {
+    io.logits[k] = t->logits[k]; io.eps[k] = t->eps[k]; io.act[k] = t->act[k]; io.logp[k] = t->logp[k];
+    io.d_out_q[k] = t->d_out_q[k]; io.d_out_qa[k] = t->d_out_qa[k];
+    io.gbias_q[k] = t->gbias_q[k]; io.gbias_q_raw[k] = t->gbias_q_raw[k];
+    io.img_act[k] = img(t->img_act[k], A); io.img_q[k] = img(t->img_q[k], 2); io.img_qa[k] = img(t->img_qa[k], 2);
+  }
+  for (int p = 0; p < 6; ++p) io.out_q[p] = t->out_q[p];
+  io.rew = t->rew; io.done = t->done; io.z3 = t->z3; io.z4 = t->z4;
+  // the step's choice of policy_grad_kernel<1 | 2>: one critic only where the handle has no second action-gradient slot
+  io.d_act[0] = t->d_act[0]; io.d_act[1] = h->slot.dAct[1] < 0 ? nullptr : t->d_act[1];
+  io.d_logits = t->d_logits; io.gbias_pi = t->gbias_pi; io.gbias_ls = t->gbias_ls; io.img_dlogits = img(t->img_dlogits, 2 * A);
+  if (t->kernel == DSACT_TEST_SAMPLE) {
+    for (int k = 0; k < 2 && !rc; ++k)
+      if (!(rc = need(io.logits[k], "logits")) && !(rc = need(io.eps[k], "eps")) && !(rc = need(io.act[k], "act")))
+        rc = need(io.logp[k], "logp");
+    for (int k = 0; k < nq && !rc; ++k) rc = need(io.out_q[k], "out_q");
+  } else if (t->kernel == DSACT_TEST_LOSS) {
+    const void* in[5] = {io.rew, io.done, io.z3, io.logp[0], io.logp[1]};
+    for (const void* p : in) if (!rc) rc = need(p, "a row input");
+    if (!rc && !v1) rc = need(io.z4, "z4");
+    for (int k = 0; k < nq && !rc; ++k)
+      if (!(rc = need(io.out_q[k], "out_q")) && !(rc = need(io.out_q[2 + k], "out_q")) && !(rc = need(io.out_q[4 + k], "out_q")) &&
+          !(rc = need(io.d_out_q[k], "d_out_q")) && !(rc = need(io.d_out_qa[k], "d_out_qa")))
+        rc = need(io.gbias_q[k], "gbias_q");
+  } else if (t->kernel == DSACT_TEST_POLICY_GRAD) {
+    if (!(rc = need(io.logits[0], "logits")) && !(rc = need(io.eps[0], "eps")) && !(rc = need(io.d_act[0], "d_act")) &&
+        !(rc = need(io.d_logits, "d_logits")) && !(rc = need(io.gbias_pi, "gbias_pi")) && h->slot.dAct[1] >= 0)
+      rc = need(io.d_act[1], "d_act[1]");
+  }
+  if (rc) return rc;
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = tc;
+  const StepScalars sc = step_scalars(h, t->global_batch);
+  if (t->kernel == DSACT_TEST_SAMPLE) {
+    enqueue_sample(h, io, B, t->advance_rng != 0, c, t->max_blocks);
+  } else if (t->kernel == DSACT_TEST_LOSS) {
+    if (v1) enqueue_loss_v1(h, io, B, sc, c, t->max_blocks);
+    else enqueue_loss(h, io, B, sc, c, t->max_blocks);
+  } else if (t->kernel == DSACT_TEST_POLICY_GRAD) {
+    enqueue_policy_grad(h, io, B, sc, c, t->max_blocks);
+  } else {
+    float inv_b, inv_pol;
+    stats_scales(h, t->global_batch, &inv_b, &inv_pol);
+    launch_k(finalize_stats_kernel, 1, 32, 0, c, h->buf.state, inv_b, inv_pol, t->stats_out);
+    c.done();
+  }
+  c.check();
+  return sync_hook(h, c);
+}
+
+int dsact_test_apply(dsact_handle* h, int32_t part, int32_t fold_slabs, int32_t scalars_ready, int32_t tail_rows,
+                     int64_t global_batch, int32_t max_blocks, void* stream) {
+  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
+  if (part < 0 || part > 2) return fail(DSACT_EINVAL, "part %d outside 0..2", part);
+  if (scalars_ready < 0 || scalars_ready > 2) return fail(DSACT_EINVAL, "scalars_ready %d outside 0..2", scalars_ready);
+  if (max_blocks < 0 || tail_rows < 0 || (tail_rows > 0 && global_batch < tail_rows)) return fail(DSACT_EINVAL, "bad argument");
+  const bool mlp_eng = h->engine == ENGINE_MLP;
+  const int max_slabs = mlp_eng && slabs_foldable(mlp(h)) ? mlp(h)->ar.nslabs : 0;
+  if (fold_slabs < 0 || fold_slabs > max_slabs)
+    return fail(DSACT_EINVAL, "fold_slabs %d outside [0, %d] (the weight-gradient slabs of this handle)", fold_slabs, max_slabs);
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = mlp_eng && mlp(h)->tc();
+  const TailArgs ta = tail_args(h, tail_rows > 0 ? global_batch : 1, tail_rows);
+  const TailArgs* tail = tail_rows > 0 ? &ta : nullptr;
+  ApplyArgs a;
+  if (mlp_eng) {
+    a = mlp_apply_args(mlp(h), scalars_ready, tail, false, part, fold_slabs);
+  } else {
+    a = apply_args(h, heads(h)->nq() * heads(h)->q.n, scalars_ready, false);
+    if (tail) a.tail = *tail;
+    apply_part(a, part);
+  }
+  launch_apply(h, a, c, max_blocks);
+  return sync_hook(h, c);
 }
 
 }  // extern "C"

@@ -557,3 +557,27 @@ class Engine:
         with torch.cuda.device(self.device):
             check(self.lib.dsact_test_chain(self.h, int(dgrad), len(sizes) - 2, sz, K0, K1, kB1, act, params.data_ptr(), arr,
                                             len(passes), self._stream()))
+
+    def test_rows(self, kernel: str, batch: int, global_batch: Optional[int] = None, max_blocks: int = 0,
+                  advance_rng: bool = False, **arrays):
+        """dsact_test_rows: one step kernel ("sample", "loss", "policy_grad", "stats") on caller tensors.  `arrays` are
+        dsact_test_row_io fields: a tensor, None, or for the array fields a list of them (images [2, batch, pitch] bf16)."""
+        t = _lib.TestRowIo()
+        t.kernel, t.batch = _lib.TEST_KERNELS[kernel], int(batch)
+        t.global_batch = int(batch if global_batch is None else global_batch)
+        t.max_blocks, t.advance_rng = int(max_blocks), int(bool(advance_rng))
+        for k, v in arrays.items():
+            if isinstance(v, (list, tuple)):
+                for i, x in enumerate(v):
+                    getattr(t, k)[i] = _ptr(x)
+            else:
+                setattr(t, k, _ptr(v))
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_test_rows(self.h, C.byref(t), self._stream()))
+
+    def test_apply(self, part: int = 0, fold_slabs: int = 0, scalars_ready: int = 0, tail_rows: int = 0,
+                   global_batch: int = 1, max_blocks: int = 0):
+        """dsact_test_apply: one Adam / Polyak launch on the bound buffers, built as a single-call step builds it."""
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_test_apply(self.h, int(part), int(fold_slabs), int(scalars_ready), int(tail_rows),
+                                            int(global_batch), int(max_blocks), self._stream()))

@@ -368,6 +368,59 @@ typedef struct dsact_test_chain_pass {
 int dsact_test_chain(dsact_handle *h, int32_t dgrad, int32_t L, const int32_t *sizes, int32_t K0, int32_t K1, int32_t kB1,
                      int32_t act, const float *params, const dsact_test_chain_pass *passes, int32_t n_passes, void *stream);
 
+/* Test hooks of the step kernels between the networks, on both engines: the step's own launch code (grid sizing and
+ * argument construction) with the per-row arrays taken from caller buffers instead of the workspace.  Hyperparameters
+ * come from the handle's configuration, the carried state (mean_std, counters, accumulators, iteration) from its bound
+ * `state` and log_alpha from its bound `params`: set them there first.  Both calls synchronise `stream` and return
+ * DSACT_EINVAL with a message, before any launch, for an unknown kernel or part, a batch outside [1, max_batch], a null
+ * pointer the kernel needs, or an image on a handle without tensor-core images.
+ *
+ * dsact_test_rows runs one kernel over `batch` rows (A = act_dim):
+ *  DSACT_TEST_SAMPLE: sample_kernel.  logits[0|1] [batch, 2A] (mean | log_std of pi(s), pi'(s')), eps[0|1] [batch, A] ->
+ *    act[0|1] [batch, A], logp[0|1] [batch]; reads out_q[0] (and out_q[1] on DSAC-T) for the critic-std sums
+ *    (state[DSACT_STATE_STDSUM..+1]) and adds the logged policy sums to the accumulators.  advance_rng: also step the
+ *    generator counter.
+ *  DSACT_TEST_LOSS: loss_kernel (DSAC-T) or loss_v1_kernel (DSAC_V1), chosen by the handle.  rew, done, z3 (DSAC-T: and
+ *    z4), logp[0] (logp_new), logp[1] (logp2) [batch], out_q[p] [batch, 2] (mean, raw std) of Q_k(s,a) (p = k),
+ *    Q'_k(s',a') (p = 2 + k), Q_k(s,a~) (p = 4 + k) -> d_out_q[k], d_out_qa[k] [batch, 2]; gbias_q[k] += the mean's
+ *    bias gradient, gbias_q_raw[k] += the std output's (null: gbias_q[k] + 1).  DSAC_V1 uses k = 0 only.
+ *  DSACT_TEST_POLICY_GRAD: policy_grad_kernel (one critic: DSAC_V1 on the MLP engine, which ignores d_act[1]).
+ *    logits[0], eps[0], d_act[k] [batch, A] -> d_logits [batch, 2A]; gbias_pi += the bias gradient of the mean half
+ *    (of the whole row when gbias_ls is null), gbias_ls += that of the log_std half.
+ *  DSACT_TEST_STATS: finalize_stats_kernel over global_batch rows into stats_out (16 floats; null: the state's slots).
+ * global_batch: the denominator of every batch mean (>= batch).  max_blocks > 0 caps the grid's blocks, so that a small
+ * batch takes several grid-stride trips.  img_* (tensor-core modes of the MLP engine; may be null): bf16 hi / lo images
+ * [2][batch][pitch] of act[k] (width A), d_out_q[k] / d_out_qa[k] (width 2) and d_logits (width 2A), pitch = width
+ * rounded up to 8; the second plane only in bf16x3. */
+enum { DSACT_TEST_SAMPLE = 0, DSACT_TEST_LOSS = 1, DSACT_TEST_POLICY_GRAD = 2, DSACT_TEST_STATS = 3 };
+typedef struct dsact_test_row_io {
+  int32_t kernel, batch;
+  int64_t global_batch;
+  int32_t max_blocks, advance_rng;
+  const float *logits[2], *eps[2];
+  float *act[2], *logp[2];
+  const float *rew, *done, *z3, *z4;
+  const float *out_q[6];
+  float *d_out_q[2], *d_out_qa[2];
+  const float *d_act[2];
+  float *d_logits;
+  float *gbias_q[2], *gbias_q_raw[2], *gbias_pi, *gbias_ls;
+  void *img_act[2], *img_q[2], *img_qa[2], *img_dlogits;
+  float *stats_out;
+} dsact_test_row_io;
+int dsact_test_rows(dsact_handle *h, const dsact_test_row_io *rows, void *stream);
+
+/* dsact_test_apply: one launch of the Adam / Polyak kernel on the handle's bound buffers, built as a single-call step
+ * builds it.  part: 0 the whole flat buffer, 1 the critics' span without closing the step, 2 the rest and the closing
+ * (a 4-element group straddling the boundary goes with part 2).  fold_slabs (tensor-core modes of the MLP engine, 0 to
+ * the number of slabs the workspace holds): fold that many weight-gradient split slabs into `grads` first.
+ * scalars_ready: the Adam step sizes are 0 formed in the kernel, 1 read from state[DSACT_STATE_ADAM..+4], 2 read there
+ * only if stamped with the current counters.  tail_rows > 0: also form the log_alpha gradient over tail_rows rows (of
+ * global_batch) and, when closing, commit the mean_std EMA and stamp the next step's scalars as the step does.
+ * max_blocks > 0 caps the grid's blocks. */
+int dsact_test_apply(dsact_handle *h, int32_t part, int32_t fold_slabs, int32_t scalars_ready, int32_t tail_rows,
+                     int64_t global_batch, int32_t max_blocks, void *stream);
+
 /* Test hook of the head-wise engine's convolution kernels: one layer (NCHW, square k x k window, stride, no padding) on
  * caller buffers, enqueued on `stream` of the current device.
  *  op 0 (forward)        : out[B,cout,hout,wout] = relu(conv(x, w) + b)
