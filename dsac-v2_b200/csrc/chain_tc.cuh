@@ -36,10 +36,6 @@ constexpr int CH_SCRATCH = CH_MMA_THREADS * 16 * 4;       // per-thread 16-float
 // 40 + 232 + 232 = 504.
 constexpr int CH_PRODUCER_REGS = 40;
 constexpr int CH_MMA_REGS = 232;
-// Groups of 16 epilogue values whose global inputs (act' or bias) are loaded ahead of the one being computed; the first
-// CH_PF are loaded before the layer's MMAs retire.  3 of the 4 groups of a 128-column accumulator: with all 4 in flight
-// the bf16x3 kernels spill at 232 registers, with 3 none of the kernels spills.
-constexpr int CH_PF = 3;
 
 struct ChainLayer {
   CUtensorMap mapB;          // weight image; forward: K-major (box = bn rows), dgrad: MN-major (box = 64 x 64)
@@ -93,7 +89,6 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
   E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.N; E.ldz = Lj.N;
   E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
   E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
-  float in[2 * NB][16];   // act'(z) (dgrad) or the bias (forward) of this thread's values
   float acc[128];
 #pragma unroll
   for (int i = 0; i < 32 * NB; ++i) acc[i] = 0.f;
@@ -124,40 +119,51 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
     prev = stage;
     if (++stage == stages) { stage = 0; phase ^= 1; }
   }
-  // The first groups' inputs load under the last k-block's MMAs, so their latency is off the epilogue's path.
-#pragma unroll
-  for (int q = 0; q < CH_PF && q < 2 * NB; ++q) epi_in(in[q], E, m0, n0, q);
+  // The epilogue is a rolled loop over the 16-value groups, each group's global inputs loaded two groups ahead (the first
+  // two under the last k-block's MMAs).  Unrolled, every layer body carried its own copy of the whole epilogue (all
+  // activation variants and stores per group), and each layer ran its epilogue from a cold instruction cache.
+  float nx0[16], nx1[16];
+  epi_in(nx0, E, m0, n0, 0);
+  epi_in(nx1, E, m0, n0, 1);   // 2 NB >= 2 groups
   wg_wait<0>();
   if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
   if (threadIdx.x == 0) TC_STAMP(8 + 3 * j);   // MMAs of layer j retired
-#pragma unroll
+  // The next layer's A operand is written group by group as the epilogue computes it: both warpgroups' MMAs of this
+  // layer must have retired first (each reads all of A).
+  const bool next = j + 1 < P.n_layers;
+  if (next) ch_bar();
+#pragma unroll 1
   for (int q = 0; q < 2 * NB; ++q) {
-    if (q + CH_PF < 2 * NB) epi_in(in[q + CH_PF], E, m0, n0, q + CH_PF);
-    float v[16];
+    float x[16], v[16];
 #pragma unroll
-    for (int t = 0; t < 16; ++t) v[t] = acc[16 * q + t];
-    epi_group<PLANES2>(v, in[q], E, m0, n0, q, row);
+    for (int t = 0; t < 16; ++t) { x[t] = nx0[t]; nx0[t] = nx1[t]; }
+    if (q + 2 < 2 * NB) epi_in(nx1, E, m0, n0, q + 2);
 #pragma unroll
-    for (int t = 0; t < 16; ++t) acc[16 * q + t] = v[t];
-  }
-  if (threadIdx.x == 0) TC_STAMP(9 + 3 * j);
-  if (j + 1 < P.n_layers) {
-    // next layer's A operand: bf16 hi/lo pairs at (row, column) of the swizzled K-major k-block tiles
-    // (16-byte chunk index ^= row & 7).  Both warpgroups' MMAs of this layer have retired before anyone overwrites.
-    ch_bar();
+    for (int c = 0; c < 2 * NB; ++c)   // group q of the accumulator (registers: compile-time indices)
+      if (q == c) {
 #pragma unroll
-    for (int i = 0; i < 8 * NB; ++i) {
-      const int c = n0 + 8 * i + 2 * (lane & 3), cc = c & 63;
+        for (int t = 0; t < 16; ++t) v[t] = acc[16 * c + t];
+      }
+    epi_group<PLANES2>(v, x, E, m0, n0, q, row);
+    if (next) {
+      // bf16 hi/lo pairs at (row, column) of the swizzled K-major k-block tiles (16-byte chunk index ^= row & 7)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = r_lo + 8 * h;
-        uint32_t whi, wlo;
-        split_pack2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], whi, wlo);
-        const uint32_t off = (uint32_t)((c >> 6) * TC_STAGE_A + r * 128 + ((((cc >> 3) ^ (r & 7)) << 4) | ((cc & 7) * 2)));
-        *reinterpret_cast<uint32_t*>(opnd + off) = whi;
-        if (PLANES2) *reinterpret_cast<uint32_t*>(opnd + CH_OPND_PLANE + off) = wlo;
+      for (int ii = 0; ii < 4; ++ii) {
+        const int c = n0 + 8 * (4 * q + ii) + 2 * (lane & 3), cc = c & 63;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r_lo + 8 * h;
+          uint32_t whi, wlo;
+          split_pack2(v[4 * ii + 2 * h], v[4 * ii + 2 * h + 1], whi, wlo);
+          const uint32_t off = (uint32_t)((c >> 6) * TC_STAGE_A + r * 128 + ((((cc >> 3) ^ (r & 7)) << 4) | ((cc & 7) * 2)));
+          *reinterpret_cast<uint32_t*>(opnd + off) = whi;
+          if (PLANES2) *reinterpret_cast<uint32_t*>(opnd + CH_OPND_PLANE + off) = wlo;
+        }
       }
     }
+  }
+  if (threadIdx.x == 0) TC_STAMP(9 + 3 * j);
+  if (next) {
     fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads
     ch_bar();
   }
