@@ -13,13 +13,14 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DSACT_LIB: kernel-development aid (A/B of two builds on one GPU box); the product is libdsact.so beside this file
 LIB_PATH = os.environ.get("DSACT_LIB") or os.path.join(_HERE, "libdsact.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 MAX_HIDDEN = 6
 NUM_STATS = 16
 
 ACTIVATIONS = {"linear": 0, "relu": 1, "gelu": 2, "tanh": 3, "sigmoid": 4, "elu": 5, "selu": 6}
 GEMM_MODES = {"fp32": 0, "bf16x3": 1, "bf16": 2}
 ACT_DISTS = {"TanhGaussDistribution": 0, "GaussDistribution": 1}   # utils/act_distribution_cls.py
+POLICY_STDS = {"mlp_shared": 0, "mlp_separated": 1, "parameter": 2}   # DSACT_STD_*, networks/mlp.py:43-72
 
 # state slots, include/dsact.h
 STATE_STDSUM = 4
@@ -34,7 +35,7 @@ class Config(C.Structure):
         ("hidden_q", C.c_int32 * MAX_HIDDEN), ("hidden_pi", C.c_int32 * MAX_HIDDEN),
         ("act_q", C.c_int32), ("act_pi", C.c_int32), ("max_batch", C.c_int32),
         ("auto_alpha", C.c_int32), ("delay_update", C.c_int32), ("gemm_mode", C.c_int32),
-        ("use_graph", C.c_int32), ("act_dist", C.c_int32),
+        ("use_graph", C.c_int32), ("act_dist", C.c_int32), ("policy_std", C.c_int32),
         ("gamma", C.c_double), ("tau", C.c_double), ("tau_b", C.c_double), ("alpha_fixed", C.c_double),
         ("lr_q", C.c_double), ("lr_pi", C.c_double), ("lr_alpha", C.c_double),
         ("min_log_std", C.c_double), ("max_log_std", C.c_double),
@@ -110,7 +111,7 @@ class TestLayer(C.Structure):
 class TestChainPass(C.Structure):
     """dsact_test_chain_pass: one pass of a dsact_test_chain launch."""
     _fields_ = [("M", C.c_int32), ("x0", _fp), ("x1", _fp), ("Zout", _fp * MAX_HIDDEN), ("Zin", _fp * MAX_HIDDEN),
-                ("img", _fp * MAX_HIDDEN), ("colsum", _fp * MAX_HIDDEN), ("out", _fp)]
+                ("img", _fp * MAX_HIDDEN), ("colsum", _fp * MAX_HIDDEN), ("out", _fp), ("out_ld", C.c_int32)]
 
 
 TEST_KERNELS = {"sample": 0, "loss": 1, "policy_grad": 2, "stats": 3}   # DSACT_TEST_*
@@ -123,7 +124,7 @@ class TestRowIo(C.Structure):
                 ("rew", _fp), ("done", _fp), ("z3", _fp), ("z4", _fp), ("out_q", _fp * 6), ("d_out_q", _fp * 2),
                 ("d_out_qa", _fp * 2), ("d_act", _fp * 2), ("d_logits", _fp), ("gbias_q", _fp * 2), ("gbias_q_raw", _fp * 2),
                 ("gbias_pi", _fp), ("gbias_ls", _fp), ("img_act", _fp * 2), ("img_q", _fp * 2), ("img_qa", _fp * 2),
-                ("img_dlogits", _fp), ("stats_out", _fp)]
+                ("img_dlogits", _fp), ("stats_out", _fp), ("img_dlogits_ls", _fp), ("split_dlogits", C.c_int32)]
 
 
 # every symbol include/dsact.h declares: (restype, argtypes)

@@ -47,9 +47,10 @@ struct ChainLayer {
   float* Zout;               // forward: act'(pre-activation) store, ld = N (null: not needed by a backward pass)
   const float* Zin;          // dgrad: act'(pre-activation) of the layer below, ld = N
   float* colsum;             // dgrad: bias gradient (+=)
-  float* C;                  // fp32 result, ld = N (head layers)
+  float* C;                  // fp32 result, ld = ldc (head layers)
   __nv_bfloat16* img;        // bf16 hi/lo image of the result for the weight-gradient GEMM (null: not needed)
   int img_pitch;
+  int ldc;                   // >= N: a head may write its columns of a wider row (the policy's mean | log_std logits)
   long long img_plane;
 };
 
@@ -86,7 +87,7 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
   const int r_lo = ((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16 + (lane >> 2);   // this thread's rows r_lo, r_lo + 8
   const int nkb = Lj.kblocks[0] + Lj.kblocks[1];
   EpiArgs E;
-  E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.N; E.ldz = Lj.N;
+  E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.ldc; E.ldz = Lj.N;
   E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
   E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
   float acc[128];

@@ -61,6 +61,16 @@ struct Net {
 
 static int64_t round64(int64_t x) { return (x + 63) / 64 * 64; }
 
+// The policy span of the flat layout (DSACT_STD_*): `pi` is the network that produces the mean (mlp_shared: mean | log_std).
+// mean / ls: where that network and the log_std network or row start inside the span (ls -1: none), n: floats in the span.
+struct PiSpan { int64_t mean, ls, n; };
+static PiSpan pi_span(int policy_std, const Net& pi, int A) {
+  if (policy_std == DSACT_STD_SEPARATED) return PiSpan{0, pi.n, 2 * pi.n};
+  if (policy_std == DSACT_STD_PARAMETER) return PiSpan{A, 0, A + pi.n};   // a module's own parameter precedes its children's
+  return PiSpan{0, -1, pi.n};
+}
+static int pi_outputs(const dsact_config& c) { return c.policy_std == DSACT_STD_SHARED ? 2 * c.act_dim : c.act_dim; }
+
 // bf16 image slot inside the arena (TC modes only)
 struct ImgSlot {
   int64_t off = -1;  // floats from the workspace base
@@ -94,12 +104,17 @@ struct Arena : StepSlots {
   int64_t zP[DSACT_MAX_HIDDEN], hP[DSACT_MAX_HIDDEN], hT[DSACT_MAX_HIDDEN];
   int64_t zQ[6][DSACT_MAX_HIDDEN], hQ[6][DSACT_MAX_HIDDEN];
   int64_t dzQ[6][DSACT_MAX_HIDDEN], dzP[DSACT_MAX_HIDDEN];
+  int64_t zL[DSACT_MAX_HIDDEN], hL[DSACT_MAX_HIDDEN], hLT[DSACT_MAX_HIDDEN], dzL[DSACT_MAX_HIDDEN];   // log_std network (mlp_separated)
   // ---- tensor-core modes: bf16 hi/lo images of every GEMM operand + wgrad split slabs
   bool tc;
-  ImgSlot i_obs, i_obs2, i_act, i_new_act, i_act2, i_dlogits;
+  // i_dlogits: dL/d(mean | log_std) [B, 2A] of mlp_shared; with two policy heads, or a log_std row, dL/d(mean) [B, A], and
+  // i_dlogits_ls dL/d(log_std) [B, A] of the log_std network: a TMA operand starts 16-byte aligned, column A of a row does not
+  ImgSlot i_obs, i_obs2, i_act, i_new_act, i_act2, i_dlogits, i_dlogits_ls;
   ImgSlot i_hP[DSACT_MAX_HIDDEN], i_hT[DSACT_MAX_HIDDEN], i_dzP[DSACT_MAX_HIDDEN];
+  ImgSlot i_hL[DSACT_MAX_HIDDEN], i_hLT[DSACT_MAX_HIDDEN], i_dzL[DSACT_MAX_HIDDEN];
   ImgSlot i_hQ[6][DSACT_MAX_HIDDEN], i_dzQ[6][DSACT_MAX_HIDDEN], i_dOut[6];
-  ImgSlot i_wq[4][DSACT_MAX_HIDDEN + 1], i_wpi[2][DSACT_MAX_HIDDEN + 1];  // q1,q2,q1',q2' (DSAC_V1: q, -, q', -) / pi,pi'
+  ImgSlot i_wq[4][DSACT_MAX_HIDDEN + 1], i_wpi[4][DSACT_MAX_HIDDEN + 1];  // q1,q2,q1',q2' (DSAC_V1: q, -, q', -) / pi,pi',
+                                                                          // log_std network of pi, of pi' (mlp_separated)
   int kpad_q0;        // column of the act block inside the Q layer-0 weight image
   int64_t slabs;      // [nslabs][n_params] fp32 wgrad partials, the arena's last region
   int nslabs;
@@ -119,6 +134,8 @@ struct Arena : StepSlots {
     obs = take(B * O); obs2 = take(B * O); act = take(B * A); rew = take(B); done = take(B); logp = take(B); idx = take(2 * B);
     eps1 = take(B * A); eps2 = take(B * A); z3 = take(B); z4 = take(B);
     for (int j = 0; j < pi.L; ++j) { zP[j] = take(B * pi.s[j + 1]); hP[j] = take(B * pi.s[j + 1]); hT[j] = take(B * pi.s[j + 1]); dzP[j] = take(B * pi.s[j + 1]); }
+    const bool two_heads = c.policy_std == DSACT_STD_SEPARATED;
+    for (int j = 0; j < pi.L && two_heads; ++j) { zL[j] = take(B * pi.s[j + 1]); hL[j] = take(B * pi.s[j + 1]); hLT[j] = take(B * pi.s[j + 1]); dzL[j] = take(B * pi.s[j + 1]); }
     logitsP = take(B * 2 * A); logitsT = take(B * 2 * A); dlogits = take(B * 2 * A);
     new_act = take(B * A); act2 = take(B * A); logp_new = take(B); logp2 = take(B);
     for (int p = 0; p < 6; ++p) {
@@ -133,8 +150,10 @@ struct Arena : StepSlots {
     if (tc) {
       const int Bi = (int)B;
       i_obs = img(Bi, (int)O); i_obs2 = img(Bi, (int)O); i_act = img(Bi, (int)A); i_new_act = img(Bi, (int)A); i_act2 = img(Bi, (int)A);
-      i_dlogits = img(Bi, 2 * (int)A);
+      i_dlogits = img(Bi, pi.s[pi.L + 1]);
+      if (two_heads) i_dlogits_ls = img(Bi, (int)A);
       for (int j = 0; j < pi.L; ++j) { i_hP[j] = img(Bi, pi.s[j + 1]); i_hT[j] = img(Bi, pi.s[j + 1]); i_dzP[j] = img(Bi, pi.s[j + 1]); }
+      for (int j = 0; j < pi.L && two_heads; ++j) { i_hL[j] = img(Bi, pi.s[j + 1]); i_hLT[j] = img(Bi, pi.s[j + 1]); i_dzL[j] = img(Bi, pi.s[j + 1]); }
       for (int p = 0; p < 6; ++p) {
         if ((p & 1) >= nq) continue;
         for (int j = 0; j < q.L; ++j) { i_hQ[p][j] = img(Bi, q.s[j + 1]); i_dzQ[p][j] = img(Bi, q.s[j + 1]); }
@@ -142,12 +161,12 @@ struct Arena : StepSlots {
       }
       for (int n = 0; n < 4; ++n)
         for (int j = 0; j <= q.L && (n & 1) < nq; ++j) i_wq[n][j] = img(q.s[j + 1], j == 0 ? kpad_q0 + (int)A : q.s[j]);
-      for (int n = 0; n < 2; ++n)
+      for (int n = 0; n < (two_heads ? 4 : 2); ++n)
         for (int j = 0; j <= pi.L; ++j) i_wpi[n][j] = img(pi.s[j + 1], pi.s[j]);
       // batch split of the weight-gradient GEMMs: at most 4 slabs of >= 256 rows (more slabs mean more partial tiles to
       // write and to fold in apply)
       nslabs = (int)(B / 256); if (nslabs > 4) nslabs = 4; if (nslabs < 1) nslabs = 1;
-      slab_stride = (nq * q.n + pi.n + 1 + 3) / 4 * 4;
+      slab_stride = (nq * q.n + pi_span(c.policy_std, pi, (int)A).n + 1 + 3) / 4 * 4;
       slabs = take((int64_t)nslabs * slab_stride);
     } else {
       slabs = off;   // the (empty) last region
@@ -230,6 +249,7 @@ struct MlpHandle : dsact_handle {
   uint64_t stamp = 0;
   MlpHandle() : dsact_handle(ENGINE_MLP) {}
   int nq() const { return v1 ? 1 : 2; }   // critics: DSAC_V1 has one (flat layout [q | policy | log_alpha])
+  PiSpan span() const { return pi_span(cfg.policy_std, pi, cfg.act_dim); }
   bool tc() const { return cfg.gemm_mode != DSACT_GEMM_FP32; }
   bool fused() const {  // layer-chain kernel: every layer must fit one 256-column wgmma accumulator / A operand
     if (!tc()) return false;
@@ -500,6 +520,7 @@ static GemmProb prob_zero() {
 struct Ten {
   float* f = nullptr;
   Img im;
+  int ld = 0;   // fp32 row pitch when the tensor is a column range of wider rows (0: contiguous)
 };
 struct Wt {       // one layer's weights: fp32 [out, in] + image
   const float* f = nullptr;
@@ -520,7 +541,7 @@ static void add_fwd(Group& G, const Net& net, int j, const Wt& w, const Ten& in0
     x.a[1] = in1.im; x.kB0[1] = kB1;
   }
   x.b = w.im;
-  p.M = B; p.N = net.s[j + 1]; p.C = out.f; p.ldc = net.s[j + 1];
+  p.M = B; p.N = net.s[j + 1]; p.C = out.f; p.ldc = out.ld ? out.ld : net.s[j + 1];
   p.bias = w.bias;
   const bool last = j == net.L;
   p.epi = last ? EPI_STORE : EPI_BIAS_ACT;
@@ -535,7 +556,7 @@ static void add_dgrad(Group& G, const Net& net, int j, const Wt& w, int col0, in
                       const Ten& dX, const float* Zprev, float* gbias_prev, int B, int act) {
   GemmProb p = prob_zero();
   TcExtra x;
-  p.A[0] = dY.f; p.lda[0] = net.s[j + 1]; p.K[0] = net.s[j + 1];
+  p.A[0] = dY.f; p.lda[0] = dY.ld ? dY.ld : net.s[j + 1]; p.K[0] = net.s[j + 1];
   p.B[0] = w.f + col0; p.ldb[0] = net.s[j];
   x.a[0] = dY.im;
   x.b = w.im.cols(img_col0, ncols);
@@ -550,7 +571,7 @@ static void add_dgrad(Group& G, const Net& net, int j, const Wt& w, int col0, in
 static void add_wgrad(Group& G, const Net& net, int j, float* Gw, int col0, int ncols, const Ten& dY, const Ten& X, int B) {
   GemmProb p = prob_zero();
   TcExtra x;
-  p.A[0] = dY.f; p.lda[0] = net.s[j + 1]; p.K[0] = B;
+  p.A[0] = dY.f; p.lda[0] = dY.ld ? dY.ld : net.s[j + 1]; p.K[0] = B;
   p.B[0] = X.f; p.ldb[0] = ncols;
   x.a[0] = dY.im; x.b = X.im;
   p.M = net.s[j + 1]; p.N = ncols; p.C = Gw + col0; p.ldc = net.s[j];
@@ -629,7 +650,7 @@ struct ChainBuild {
   }
   ChainLayer& layer(ChainPass& P, const Img& wimg, bool b_mn, int N, int K0, int K1, int kB1) {
     ChainLayer& L = P.L[P.n_layers++];
-    L.N = N; L.bn = (N + 15) / 16 * 16;
+    L.N = N; L.ldc = N; L.bn = (N + 15) / 16 * 16;
     const int o = b_mn ? 1 : 0;
     if (this->b_mn >= 0 && this->b_mn != o) ok = false;   // the kernel takes one B orientation per launch
     this->b_mn = o;
@@ -645,6 +666,9 @@ struct ChainBuild {
 
 static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
   if (cb.g.n == 0) return;
+  for (int i = 0; i < cb.g.n; ++i)
+    for (int j = 0; j < cb.g.p[i].n_layers; ++j)
+      if (cb.g.p[i].L[j].ldc != cb.g.p[i].L[j].N && cb.g.p[i].L[j].Zout) cb.ok = false;   // Zout rows are N apart
   if (!cb.ok) { c.err = cudaErrorInvalidValue; return; }
   static unsigned long long* dbg = nullptr;
   const bool debug = getenv("DSACT_TC_DEBUG") != nullptr;
@@ -703,7 +727,7 @@ struct ChainIo {
 
 // forward chain of one pass: out = head(act(...act(in W_0^T + b_0)...))
 static ChainPass& chain_fwd_layers(ChainBuild& cb, const Net& net, const float* Wbase, const ChainIo& io, const Img& in0, int k0,
-                                   const Img& in1, int k1, int kB1, int B, int act, float* out) {
+                                   const Img& in1, int k1, int kB1, int B, int act, float* out, int out_ld = 0) {
   ChainPass& P = cb.begin(in0, in1, B);
   for (int j = 0; j <= net.L; ++j) {
     ChainLayer& L = j == 0 ? cb.layer(P, io.w[0], false, net.s[1], k0, k1, kB1) : cb.layer(P, io.w[j], false, net.s[j + 1], net.s[j], 0, 0);
@@ -711,7 +735,8 @@ static ChainPass& chain_fwd_layers(ChainBuild& cb, const Net& net, const float* 
     L.epi = last ? EPI_STORE : EPI_BIAS_ACT;
     L.act = act;
     L.bias = Wbase + net.b[j];
-    if (last) L.C = out;
+    if (last) { L.C = out; if (out_ld) L.ldc = out_ld; }   // only a head layer takes a pitch: the epilogue indexes Zout with
+                                                           // ldc as well, and a head layer has no Zout
     else {
       L.Zout = io.z[j];
       L.img = io.img[j].p; L.img_pitch = io.img[j].pitch; L.img_plane = io.img[j].plane;
@@ -743,7 +768,7 @@ static ChainPass& chain_dgrad_layers(ChainBuild& cb, const Net& net, const Chain
 // A network instance of the step (q_k and q'_k for k < nq, pi, pi'): its fp32 parameters (in params; in targets for q'_k
 // and pi'), gradients (null: a target network), the weight-image slot of every layer and the hidden activation
 struct NetInst { const Net* net; const float* P; float* G; const ImgSlot* wimg; int act; };
-struct NetInsts { NetInst q[2], qt[2], pi, pit; };
+struct NetInsts { NetInst q[2], qt[2], pi, pit, pi_ls, pit_ls; };   // pi_ls / pit_ls: the log_std networks (mlp_separated)
 
 static NetInsts net_insts(const MlpHandle* h) {
   const Net &q = h->q, &pi = h->pi;
@@ -754,8 +779,14 @@ static NetInsts net_insts(const MlpHandle* h) {
     I.q[k] = NetInst{&q, P + k * q.n, G + k * q.n, h->ar.i_wq[k], h->cfg.act_q};
     I.qt[k] = NetInst{&q, T + k * q.n, nullptr, h->ar.i_wq[2 + k], h->cfg.act_q};
   }
-  I.pi = NetInst{&pi, P + nq * q.n, G + nq * q.n, h->ar.i_wpi[0], h->cfg.act_pi};
-  I.pit = NetInst{&pi, T + nq * q.n, nullptr, h->ar.i_wpi[1], h->cfg.act_pi};
+  const PiSpan sp = h->span();
+  const int64_t mean = nq * q.n + sp.mean, ls = nq * q.n + sp.ls;
+  I.pi = NetInst{&pi, P + mean, G + mean, h->ar.i_wpi[0], h->cfg.act_pi};
+  I.pit = NetInst{&pi, T + mean, nullptr, h->ar.i_wpi[1], h->cfg.act_pi};
+  if (h->cfg.policy_std == DSACT_STD_SEPARATED) {
+    I.pi_ls = NetInst{&pi, P + ls, G + ls, h->ar.i_wpi[2], h->cfg.act_pi};
+    I.pit_ls = NetInst{&pi, T + ls, nullptr, h->ar.i_wpi[3], h->cfg.act_pi};
+  }
   return I;
 }
 
@@ -771,6 +802,7 @@ struct FwdPass {
   const ImgSlot* hi;
   bool keep;
   float* out;
+  int out_ld;   // row pitch of `out` when the pass writes its columns of wider rows (0: contiguous)
 };
 
 // The backward of forward pass f: dL/d(output) in slots dout / dout_img, dL/dz_j in slots dz[j] / dz_img[j].  `grads`: it
@@ -779,6 +811,7 @@ struct FwdPass {
 struct BwdPass {
   FwdPass f;
   int64_t dout;
+  int dout_ld;   // row pitch of the fp32 dL/d(output) when it is a column range of wider rows (0: contiguous)
   ImgSlot dout_img;
   const int64_t* dz;
   const ImgSlot* dz_img;
@@ -788,11 +821,13 @@ struct BwdPass {
 
 // The passes of one step in launch order.  Wave A: pi(s), pi'(s'), Q_k(s,a); wave B (it reads a~ ~ pi(s), a' ~ pi'(s')):
 // Q'_k(s',a'), Q_k(s,a~); the critics' backward: Q_k(s,a) with gradients, Q_k(s,a~) with dL/da~; the policy's: pi(s).
+// mlp_separated: pi and pi' are two passes each, the mean network into columns [0, A) of the [B, 2A] logits and the
+// log_std network into [A, 2A), and the policy's backward two.  parameter: the mean network alone, into columns [0, A).
 struct StepPasses {
   NetInsts I;
-  FwdPass a[4], b[4];
-  BwdPass q[4], pi;
-  int na = 0, nb = 0, nqb = 0;
+  FwdPass a[6], b[4];
+  BwdPass q[4], pi[2];
+  int na = 0, nb = 0, nqb = 0, npb = 0;
 };
 
 static Ten ten(const MlpHandle* h, const float* f, const ImgSlot& s, int B) { return Ten{const_cast<float*>(f), h->img(s, B)}; }
@@ -812,15 +847,27 @@ static StepPasses step_passes(const MlpHandle* h, const dsact_batch& bt) {
   const Ten new_act = ten(h, W + ar.new_act, ar.i_new_act, B), act2 = ten(h, W + ar.act2, ar.i_act2, B);
   // the arena holds critic pass Q_k(s,a) at slot k, Q'_k(s',a') at 2 + k and Q_k(s,a~) at 4 + k
   auto critic = [&](const NetInst& n, int p, const Ten& in, const Ten& a, bool store_z, bool keep) {
-    return FwdPass{n, in, a, O, A, ar.kpad_q0, store_z ? ar.zQ[p] : nullptr, ar.hQ[p], ar.i_hQ[p], keep, W + ar.outQ[p]};
+    return FwdPass{n, in, a, O, A, ar.kpad_q0, store_z ? ar.zQ[p] : nullptr, ar.hQ[p], ar.i_hQ[p], keep, W + ar.outQ[p], 0};
   };
   auto critic_bwd = [&](const FwdPass& f, int p, bool grads, float* dact) {
-    return BwdPass{f, ar.dOut[p], ar.i_dOut[p], ar.dzQ[p], ar.i_dzQ[p], grads, dact};
+    return BwdPass{f, ar.dOut[p], 0, ar.i_dOut[p], ar.dzQ[p], ar.i_dzQ[p], grads, dact};
   };
-  const FwdPass pi{s.I.pi, obs, Ten(), O, 0, 0, ar.zP, ar.hP, ar.i_hP, true, W + ar.logitsP};
-  s.a[s.na++] = pi;
-  s.a[s.na++] = FwdPass{s.I.pit, obs2, Ten(), O, 0, 0, nullptr, ar.hT, ar.i_hT, false, W + ar.logitsT};
-  s.pi = BwdPass{pi, ar.dlogits, ar.i_dlogits, ar.dzP, ar.i_dzP, true, nullptr};
+  const int pstd = h->cfg.policy_std;
+  const int ld = pstd == DSACT_STD_SHARED ? 0 : 2 * A;   // an A-wide head writes its columns of the [B, 2A] logits
+  const FwdPass pi{s.I.pi, obs, Ten(), O, 0, 0, ar.zP, ar.hP, ar.i_hP, true, W + ar.logitsP, ld};
+  const FwdPass pit{s.I.pit, obs2, Ten(), O, 0, 0, nullptr, ar.hT, ar.i_hT, false, W + ar.logitsT, ld};
+  s.pi[s.npb++] = BwdPass{pi, ar.dlogits, ld, ar.i_dlogits, ar.dzP, ar.i_dzP, true, nullptr};
+  if (pstd == DSACT_STD_SEPARATED) {
+    const FwdPass pi_ls{s.I.pi_ls, obs, Ten(), O, 0, 0, ar.zL, ar.hL, ar.i_hL, true, W + ar.logitsP + A, ld};
+    s.a[s.na++] = pi;
+    s.a[s.na++] = pi_ls;
+    s.a[s.na++] = pit;
+    s.a[s.na++] = FwdPass{s.I.pit_ls, obs2, Ten(), O, 0, 0, nullptr, ar.hLT, ar.i_hLT, false, W + ar.logitsT + A, ld};
+    s.pi[s.npb++] = BwdPass{pi_ls, ar.dlogits + A, ld, ar.i_dlogits_ls, ar.dzL, ar.i_dzL, true, nullptr};
+  } else {
+    s.a[s.na++] = pi;
+    s.a[s.na++] = pit;
+  }
   const int nq = h->nq();
   for (int k = 0; k < nq; ++k) {
     const FwdPass f = critic(s.I.q[k], k, obs, act, true, true);
@@ -853,14 +900,17 @@ static ChainIo chain_io(const MlpHandle* h, const NetInst& n, int B, const int64
 // one GEMM group per layer depth
 static void enqueue_fwd(MlpHandle* h, const FwdPass* ps, int n, int B, Ctx& c) {
   float* W = h->W();
-  if (h->fused()) {
-    ChainBuild cb(h->passes());
-    for (int i = 0; i < n; ++i) {
-      const FwdPass& p = ps[i];
-      chain_fwd_layers(cb, *p.n.net, p.n.P, chain_io(h, p.n, B, p.z, p.keep ? p.hi : nullptr), p.in0.im, p.k0, p.in1.im, p.k1,
-                       p.kB1, B, p.n.act, p.out);
+  if (h->fused()) {   // a launch carries CH_MAX_PASSES passes: the six of mlp_separated's wave A go out as the four of the
+                      // policies, then the critics'
+    for (int i0 = 0; i0 < n; i0 += CH_MAX_PASSES) {
+      ChainBuild cb(h->passes());
+      for (int i = i0; i < n && i < i0 + CH_MAX_PASSES; ++i) {
+        const FwdPass& p = ps[i];
+        chain_fwd_layers(cb, *p.n.net, p.n.P, chain_io(h, p.n, B, p.z, p.keep ? p.hi : nullptr), p.in0.im, p.k0, p.in1.im, p.k1,
+                         p.kB1, B, p.n.act, p.out, p.out_ld);
+      }
+      launch_chain(h, cb, CLS_GEMM_FWD, c);
     }
-    launch_chain(h, cb, CLS_GEMM_FWD, c);
     return;
   }
   for (int j = 0; j <= DSACT_MAX_HIDDEN; ++j) {
@@ -870,7 +920,7 @@ static void enqueue_fwd(MlpHandle* h, const FwdPass* ps, int n, int B, Ctx& c) {
       const Net& net = *p.n.net;
       if (j > net.L) continue;
       const bool last = j == net.L;
-      const Ten out = last ? Ten{p.out} : ten(h, W + p.hf[j], p.hi[j], B);
+      const Ten out = last ? Ten{p.out, Img(), p.out_ld} : ten(h, W + p.hf[j], p.hi[j], B);
       float* z = last || !p.z ? nullptr : W + p.z[j];
       const Wt w = weight(h, p.n, j);
       if (j == 0) add_fwd(G, net, 0, w, p.in0, p.k0, p.in1, p.k1, p.kB1, out, z, B, p.n.act);
@@ -882,7 +932,10 @@ static void enqueue_fwd(MlpHandle* h, const FwdPass* ps, int n, int B, Ctx& c) {
 
 // dL/d(output of layer j) of a backward pass
 static Ten bwd_dy(const MlpHandle* h, const BwdPass& p, int j, int B) {
-  return j == p.f.n.net->L ? ten(h, h->W() + p.dout, p.dout_img, B) : ten(h, h->W() + p.dz[j], p.dz_img[j], B);
+  if (j < p.f.n.net->L) return ten(h, h->W() + p.dz[j], p.dz_img[j], B);
+  Ten t = ten(h, h->W() + p.dout, p.dout_img, B);
+  t.ld = p.dout_ld;
+  return t;
 }
 
 // The dgrad of a list of backward passes, top layer down: one layer-chain launch (dz stays on chip between layers), or one
@@ -1033,6 +1086,10 @@ struct RowIo {
   // gbias_q[k] (one two-output layer); gbias_pi the policy's mean (the whole (mean | log_std) row when gbias_ls is null)
   float *gbias_q[2], *gbias_q_raw[2], *gbias_pi, *gbias_ls;
   ImgOut img_act[2], img_q[2], img_qa[2], img_dlogits;   // bf16 images (NO_IMG: none)
+  // split_dlogits: img_dlogits is [B, A], the mean half alone, and the log_std half goes to img_dlogits_ls [B, A] (NO_IMG: a
+  // log_std row, which no GEMM reads); otherwise img_dlogits is [B, 2A]
+  bool split_dlogits;
+  ImgOut img_dlogits_ls;
 };
 // the step's row arrays: the arena slots, the minibatch `bt` and the noise `nz`; no bias-gradient targets and no images
 static RowIo step_rows(const dsact_handle* h, const dsact_batch& bt, const dsact_noise& nz) {
@@ -1052,7 +1109,7 @@ static RowIo step_rows(const dsact_handle* h, const dsact_batch& bt, const dsact
     io.d_act[k] = s.dAct[k] < 0 ? nullptr : W + s.dAct[k];   // DSAC_V1 on the MLP engine: no second action-gradient slot
   }
   io.d_logits = W + s.dlogits;
-  io.img_act[0] = io.img_act[1] = io.img_q[0] = io.img_q[1] = io.img_qa[0] = io.img_qa[1] = io.img_dlogits = NO_IMG;
+  io.img_act[0] = io.img_act[1] = io.img_q[0] = io.img_q[1] = io.img_qa[0] = io.img_qa[1] = io.img_dlogits = io.img_dlogits_ls = NO_IMG;
   return io;
 }
 // a launch's blocks: the step's count `natural`, or at most `max_blocks` (> 0, dsact_test_rows / dsact_test_apply) so that
@@ -1122,6 +1179,8 @@ static void enqueue_policy_grad(const dsact_handle* h, const RowIo& io, int B, c
   a.B = B; a.A = A; a.min_log_std = (float)p.min_log_std; a.max_log_std = (float)p.max_log_std; a.gauss = p.act_dist;
   a.inv_global_batch = sc.inv_global_batch;
   a.img = io.img_dlogits;
+  a.img_ls = io.split_dlogits ? io.img_dlogits_ls : io.img_dlogits;
+  a.ls_col = io.split_dlogits ? 0 : A;
   a.sc = sc;
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;   // a warp per row
   launch_k(one_critic ? policy_grad_kernel<1> : policy_grad_kernel<2>, capped(blocks, max_blocks), 256, sizeof(float) * 2 * A, c, a);
@@ -1229,10 +1288,13 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
       }
     };
     for (int k = 0; k < nq; ++k) add_weights(I.q[k]);
+    const bool two_heads = cf.policy_std == DSACT_STD_SEPARATED;
     ib.reserve(h, c, pi.L + 2);
     add_weights(I.pi);
     if (!inputs_imaged) ib.add(bt.obs, O, h->img(ar.i_obs, B), B, O);
+    if (two_heads) add_weights(I.pi_ls);
     for (int k = 0; k < nq; ++k) add_weights(I.qt[k]);
+    if (two_heads) add_weights(I.pit_ls);
     ib.reserve(h, c, pi.L + 3);
     add_weights(I.pit);
     if (!inputs_imaged) {
@@ -1253,6 +1315,13 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
   }
 
   if (want_noise && !tc) enqueue_noise(h, B, c);
+  if (cf.policy_std == DSACT_STD_PARAMETER) {   // the log_std rows of pi and pi' (the head of the policy span) -> their logits
+    const int64_t row = nq * q.n + h->span().ls;
+    int blocks = (B * A + 255) / 256; if (blocks > 2 * h->num_sms) blocks = 2 * h->num_sms;
+    launch_k(log_std_rows_kernel, blocks, 256, 0, c, W + ar.logitsP, W + ar.logitsT, (const float*)(h->buf.params + row),
+             (const float*)(h->buf.targets + row), B, A);
+    c.done();
+  }
   c.check();
 }
 
@@ -1388,7 +1457,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const int B = bt.batch;
   const bool tc = h->tc();
   float* G_ = h->buf.grads;
-  const long long n_flat = h->nq() * q.n + pi.n + 1;
+  const long long n_flat = h->n_params;
   const StepPasses sp = step_passes(h, bt);
   const NetInsts& I = sp.I;
 
@@ -1400,6 +1469,11 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   }
   io.gbias_pi = I.pi.G + pi.b[pi.L];
   io.img_dlogits = img_out(h, ar.i_dlogits);
+  if (cf.policy_std != DSACT_STD_SHARED) {   // the log_std half's gradient: the log_std network's output bias, or the row itself
+    io.gbias_ls = cf.policy_std == DSACT_STD_SEPARATED ? I.pi_ls.G + pi.b[pi.L] : G_ + h->nq() * q.n + h->span().ls;
+    io.split_dlogits = true;
+    io.img_dlogits_ls = cf.policy_std == DSACT_STD_SEPARATED ? img_out(h, ar.i_dlogits_ls) : NO_IMG;
+  }
   if (h->v1) enqueue_loss_v1(h, io, B, sc, c);
   else enqueue_loss(h, io, B, sc, c);
   // The freeze trick of the reference (dsac_v2.py:166-181) makes the critics' and the policy's backward independent: the
@@ -1426,9 +1500,9 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   h->join_pending = forked;
 
   enqueue_policy_grad(h, io, B, sc, c);
-  Group gwp, no_act;   // (the policy pass has no action segment)
-  enqueue_dgrad(h, &sp.pi, 1, B, c, no_act);
-  add_wgrads(gwp, h, &sp.pi, 1, B);
+  Group gwp, no_act;   // (the policy passes have no action segment)
+  enqueue_dgrad(h, sp.pi, sp.npb, B, c, no_act);
+  add_wgrads(gwp, h, sp.pi, sp.npb, B);
   launch_group(h, gwp, V_WGRAD, c);
 
   if (h->join_pending) { cudaStreamWaitEvent(c.s, h->ev_join, 0); h->join_pending = false; }
@@ -1697,6 +1771,16 @@ static int check_noise(const dsact_noise* n) {
 static int check_v2(const dsact_handle* h) {
   return h->v1 ? fail(DSACT_EINVAL, "DSAC_V1 handles have no split or data-parallel update") : DSACT_OK;
 }
+// the peer-memory data-parallel step has not run with two policy heads or a log_std row: refused until it has
+static int check_dp(const dsact_handle* h) {
+  int rc = check_v2(h);
+  if (rc) return rc;
+  if (h->engine == ENGINE_MLP && static_cast<const MlpHandle*>(h)->cfg.policy_std != DSACT_STD_SHARED)
+    return fail(DSACT_EINVAL, "the MLP engine's data-parallel step runs the mlp_shared policy only (policy_std %d): use the split "
+                              "calls (dsact_grad_phase1/2, dsact_apply) with an all-reduce between them",
+                static_cast<const MlpHandle*>(h)->cfg.policy_std);
+  return DSACT_OK;
+}
 // host staging, the replay-fused steps, the profiler and the GEMM test hook exist on the MLP engine only
 static int check_mlp(const dsact_handle* h, const char* fn) {
   return h && h->engine != ENGINE_MLP ? fail(DSACT_EINVAL, "%s: the head-wise engine does not implement this call", fn) : DSACT_OK;
@@ -1754,11 +1838,15 @@ static int validate(const dsact_config* c) {
   if (c->delay_update < 1) return fail(DSACT_EINVAL, "delay_update must be >= 1");
   if (c->gemm_mode < DSACT_GEMM_FP32 || c->gemm_mode > DSACT_GEMM_BF16) return fail(DSACT_EINVAL, "unknown gemm_mode %d", c->gemm_mode);
   if (c->act_dist != 0 && c->act_dist != 1) return fail(DSACT_EINVAL, "act_dist must be 0 (TanhGaussDistribution) or 1 (GaussDistribution)");
+  if (c->policy_std < DSACT_STD_SHARED || c->policy_std > DSACT_STD_PARAMETER)
+    return fail(DSACT_EINVAL, "policy_std must be 0 (mlp_shared), 1 (mlp_separated) or 2 (parameter), got %d", c->policy_std);
   return DSACT_OK;
 }
 
-static int validate_v1(const dsact_v1_options* v) {
+static int validate_v1(const dsact_config* c, const dsact_v1_options* v) {
   if (!v) return fail(DSACT_EINVAL, "null DSAC_V1 options");
+  if (c->policy_std != DSACT_STD_SHARED)
+    return fail(DSACT_EINVAL, "DSAC_V1 on the MLP engine runs the mlp_shared policy only (policy_std %d)", c->policy_std);
   if (v->abi_version != DSACT_ABI_VERSION) return fail(DSACT_EINVAL, "dsact_v1_options.abi_version %d != %d", v->abi_version, DSACT_ABI_VERSION);
   if (v->bound != 0 && v->bound != 1) return fail(DSACT_EINVAL, "DSAC_V1 bound must be 0 (Gaussian NLL) or 1 (bounded loss), got %d", v->bound);
   if (!(v->td_bound > 0.0) || !std::isfinite(v->td_bound)) return fail(DSACT_EINVAL, "DSAC_V1 TD_bound must be finite and > 0, got %g", v->td_bound);
@@ -1770,12 +1858,12 @@ static int mlp_query_layout(const dsact_config* cfg, int nq, dsact_layout* out) 
   if (!out) return fail(DSACT_EINVAL, "null out");
   Net q, pi;
   q.build(cfg->obs_dim + cfg->act_dim, cfg->hidden_q, cfg->n_hidden_q, 2);
-  pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, 2 * cfg->act_dim);
+  pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, pi_outputs(*cfg));
   Arena ar;
   ar.build(*cfg, q, pi, nq);
-  out->n_q = q.n; out->n_pi = pi.n;
-  out->n_params = nq * q.n + pi.n + 1;
-  out->n_targets = nq * q.n + pi.n;
+  out->n_q = q.n; out->n_pi = pi_span(cfg->policy_std, pi, cfg->act_dim).n;
+  out->n_params = nq * q.n + out->n_pi + 1;
+  out->n_targets = nq * q.n + out->n_pi;
   out->workspace_bytes = ar.total * (int64_t)sizeof(float);
   out->state_floats = ST_FLOATS;
   out->max_batch = cfg->max_batch;
@@ -1791,7 +1879,7 @@ int dsact_query_layout(const dsact_config* cfg, dsact_layout* out) {
 
 int dsact_v1_query_layout(const dsact_config* cfg, const dsact_v1_options* v1, dsact_layout* out) {
   int rc = validate(cfg);
-  if (rc || (rc = validate_v1(v1))) return rc;
+  if (rc || (rc = validate_v1(cfg, v1))) return rc;
   return mlp_query_layout(cfg, 1, out);
 }
 
@@ -1808,12 +1896,12 @@ static int mlp_create(const dsact_config* cfg, const dsact_v1_options* v1, int d
   h->num_sms = num_sms;
   if (v1) { h->v1 = true; h->v1_bound = v1->bound; h->td_bound = v1->td_bound; }
   h->q.build(cfg->obs_dim + cfg->act_dim, cfg->hidden_q, cfg->n_hidden_q, 2);
-  h->pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, 2 * cfg->act_dim);
+  h->pi.build(cfg->obs_dim, cfg->hidden_pi, cfg->n_hidden_pi, pi_outputs(*cfg));
   h->ar.build(*cfg, h->q, h->pi, h->nq());
   h->slot = h->ar;
   h->hyper = StepHyper::of(*cfg);
   h->obs_elems = cfg->obs_dim; h->act_dim = cfg->act_dim; h->max_batch = cfg->max_batch;
-  h->n_params = h->nq() * h->q.n + h->pi.n + 1;
+  h->n_params = h->nq() * h->q.n + h->span().n + 1;
   h->arena_imaged = false;
   cudaError_t e = cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking);
@@ -1835,7 +1923,7 @@ int dsact_create(const dsact_config* cfg, int device, dsact_handle** out) {
 
 int dsact_v1_create(const dsact_config* cfg, const dsact_v1_options* v1, int device, dsact_handle** out) {
   int rc = validate(cfg);
-  if (rc || (rc = validate_v1(v1))) return rc;
+  if (rc || (rc = validate_v1(cfg, v1))) return rc;
   return mlp_create(cfg, v1, device, out);
 }
 
@@ -2203,7 +2291,7 @@ int dsact_replay_steps(dsact_handle* hh, int32_t n_steps, int32_t batch, int64_t
 // ---- data parallelism over peer memory (dp_peer.cuh) ------------------------------------------------------------
 int dsact_dp_export(dsact_handle* h, void* handle_out, int64_t* bytes_out) {
   if (!h || !handle_out) return fail(DSACT_EINVAL, "null argument");
-  int rc = check_v2(h);
+  int rc = check_dp(h);
   if (rc) return rc;
   return dp_peer_export(h->dp, h->device, h->n_params, handle_out, bytes_out);
 }
@@ -2211,7 +2299,7 @@ int dsact_dp_export(dsact_handle* h, void* handle_out, int64_t* bytes_out) {
 int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* handles) {
   if (!h || !handles) return fail(DSACT_EINVAL, "null argument");
   if (!h->bound) return fail(DSACT_ESTATE, "dsact_bind has not been called");
-  int rc = check_v2(h);
+  int rc = check_dp(h);
   if (rc) return rc;
   if (!h->dp.buf) return fail(DSACT_ESTATE, "dsact_dp_export has not been called");
   rc = dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
@@ -2224,7 +2312,7 @@ int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* h
 int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t global_batch, int64_t iteration,
                   void* stream) {
   int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise)) || (rc = check_v2(h))) return rc;
+  if (rc || (rc = check_noise(noise)) || (rc = check_dp(h))) return rc;
   if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (global_batch < batch->batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch->batch);
   CUDA_TRY(cudaSetDevice(h->device));
@@ -2254,7 +2342,7 @@ int dsact_dp_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const in
   if (rc) return rc;
   MlpHandle* h = mlp(hh);
   if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if ((rc = check_v2(h))) return rc;
+  if ((rc = check_dp(h))) return rc;
   if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
   if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
   if (global_batch < batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch);
@@ -2456,7 +2544,8 @@ int dsact_test_chain(dsact_handle* hh, int32_t dgrad, int32_t L, const int32_t* 
     return fail(DSACT_EINVAL, "layer-0 segments: K0 + K1 == sizes[0], kB1 >= K0, kB1 %% 8 == 0");
   for (int i = 0; i < n_passes; ++i) {
     const dsact_test_chain_pass& q = passes[i];
-    if (q.M < 1 || !q.x0 || (!dgrad && (!q.out || (K1 > 0 && !q.x1))) || (dgrad && q.out && K1 == 0))
+    if (q.M < 1 || !q.x0 || (!dgrad && (!q.out || (K1 > 0 && !q.x1))) || (dgrad && q.out && K1 == 0) ||
+        (q.out_ld != 0 && (dgrad || q.out_ld < sizes[L + 1])))
       return fail(DSACT_EINVAL, "pass %d: bad argument", i);
     for (int j = 0; j < L && dgrad; ++j)
       if (!q.Zin[j]) return fail(DSACT_EINVAL, "pass %d: Zin[%d] is null", i, j);
@@ -2496,7 +2585,7 @@ int dsact_test_chain(dsact_handle* hh, int32_t dgrad, int32_t L, const int32_t* 
     } else {
       Img in1;
       if (K1 > 0) { in1 = mem.img(q.M, K1); ibt.add(q.x1, K1, in1, q.M, K1); }
-      chain_fwd_layers(cb, net, params, pio, in0, K0, in1, K1, kB1, q.M, act, q.out);
+      chain_fwd_layers(cb, net, params, pio, in0, K0, in1, K1, kB1, q.M, act, q.out, q.out_ld);
     }
   }
   if (mem.err == cudaSuccess) {
@@ -2525,7 +2614,8 @@ int dsact_test_rows(dsact_handle* h, const dsact_test_row_io* t, void* stream) {
   const bool v1 = h->v1, mlp_eng = h->engine == ENGINE_MLP;
   const bool tc = mlp_eng && mlp(h)->tc();
   const int A = h->act_dim, nq = v1 ? 1 : 2;
-  const void* imgs[7] = {t->img_act[0], t->img_act[1], t->img_q[0], t->img_q[1], t->img_qa[0], t->img_qa[1], t->img_dlogits};
+  const void* imgs[8] = {t->img_act[0], t->img_act[1], t->img_q[0], t->img_q[1], t->img_qa[0], t->img_qa[1], t->img_dlogits,
+                         t->img_dlogits_ls};
   for (const void* p : imgs)
     if (p && !tc) return fail(DSACT_EINVAL, "images need a tensor-core mode of the MLP engine");
   auto need = [&](const void* p, const char* what) { return p ? DSACT_OK : fail(DSACT_EINVAL, "%s is null", what); };
@@ -2549,7 +2639,10 @@ int dsact_test_rows(dsact_handle* h, const dsact_test_row_io* t, void* stream) {
   io.rew = t->rew; io.done = t->done; io.z3 = t->z3; io.z4 = t->z4;
   // the step's choice of policy_grad_kernel<1 | 2>: one critic only where the handle has no second action-gradient slot
   io.d_act[0] = t->d_act[0]; io.d_act[1] = h->slot.dAct[1] < 0 ? nullptr : t->d_act[1];
-  io.d_logits = t->d_logits; io.gbias_pi = t->gbias_pi; io.gbias_ls = t->gbias_ls; io.img_dlogits = img(t->img_dlogits, 2 * A);
+  io.d_logits = t->d_logits; io.gbias_pi = t->gbias_pi; io.gbias_ls = t->gbias_ls;
+  io.split_dlogits = t->split_dlogits != 0;
+  io.img_dlogits = img(t->img_dlogits, io.split_dlogits ? A : 2 * A);
+  io.img_dlogits_ls = io.split_dlogits ? img(t->img_dlogits_ls, A) : NO_IMG;
   if (t->kernel == DSACT_TEST_SAMPLE) {
     for (int k = 0; k < 2 && !rc; ++k)
       if (!(rc = need(io.logits[k], "logits")) && !(rc = need(io.eps[k], "eps")) && !(rc = need(io.act[k], "act")))

@@ -562,7 +562,9 @@ struct PolicyGradArgs {
   const float* state;
   int B, A;
   float min_log_std, max_log_std, inv_global_batch;
-  ImgOut img;
+  ImgOut img;        // bf16 image of the mean half (columns [0, A))
+  ImgOut img_ls;     // and of the log_std half, at columns [ls_col, ls_col + A): the same image at column A (one 2A-wide
+  int ls_col;        // head), an image of its own at column 0 (a separate log_std head), or none (a log_std row)
   StepScalars sc;
   int gauss;         // 1: GaussDistribution (a~ = u, log-prob of the Normal only)
 };
@@ -607,7 +609,7 @@ __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
       a.d_logits[(size_t)row * 2 * A + j] = gu;
       a.d_logits[(size_t)row * 2 * A + A + j] = gls;
       img_put(a.img, row, j, gu);
-      img_put(a.img, row, A + j, gls);
+      img_put(a.img_ls, row, a.ls_col + j, gls);
       gb_mean += gu;
       gb_ls += gls;
     }
@@ -619,6 +621,20 @@ __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
     }
   }
   for (int i = threadIdx.x; i < 2 * A; i += blockDim.x) atomicAdd((a.gbias_ls && i >= A) ? a.gbias_ls + (i - A) : a.gbias + i, gb[i]);
+}
+
+// std_type "parameter" (networks/mlp.py:63-64,94-96): log_std is a learnable [1, A] row, the same for every sample.  Writes
+// the rows of pi and pi' into the log_std half of their [B, 2A] logits, where sample_kernel and policy_grad_kernel read
+// any other policy's log_std.
+__global__ void log_std_rows_kernel(float* __restrict__ logitsP, float* __restrict__ logitsT, const float* __restrict__ rowP,
+                                    const float* __restrict__ rowT, int B, int A) {
+  pdl_sync();
+  const int total = B * A;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int r = i / A, j = i - r * A;
+    logitsP[(size_t)r * 2 * A + A + j] = rowP[j];
+    logitsT[(size_t)r * 2 * A + A + j] = rowT[j];
+  }
 }
 
 // __update (dsac_v2.py:320-347): Adam on q1|q2 every step; on policy|log_alpha plus Polyak of all three

@@ -85,8 +85,9 @@ class ApproxContainer(nn.Module):
             self._cfg_args = dict(obs_shape=tuple(q_args["obs_dim"]), act_dim=q_args["act_dim"], kernels=t["kernels"],
                                   channels=t["channels"], strides=t["strides"], hidden=t["heads"],
                                   act_hidden=q_args["hidden_activation"], **common)
-        elif pi_args["std_type"] != "mlp_shared":
-            # separate mean / log_std (reference networks/mlp.py:43-72): the head-wise fp32 engine without an encoder
+        elif pi_args["std_type"] != "mlp_shared" and "dsact_gemm" not in kwargs:
+            # separate mean / log_std (reference networks/mlp.py:43-72): the head-wise fp32 engine without an encoder,
+            # unless the caller names the MLP engine's arithmetic (`dsact_gemm`), as for DSAC_V1
             if q_args["hidden_sizes"] != pi_args["hidden_sizes"] or q_args["hidden_activation"] != pi_args["hidden_activation"]:
                 raise NotImplementedError("policy std_type != 'mlp_shared': critics and policy take one hidden_sizes / activation")
             self._cnn = True     # same engine class and entry points as the CNN approximators
@@ -98,7 +99,8 @@ class ApproxContainer(nn.Module):
                 obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"],
                 hidden_q=q_args["hidden_sizes"], hidden_pi=pi_args["hidden_sizes"],
                 act_q=q_args["hidden_activation"], act_pi=pi_args["hidden_activation"],
-                gemm_mode=kwargs.get("dsact_gemm", "bf16x3"), use_graph=kwargs.get("dsact_graph", True), **common)
+                gemm_mode=kwargs.get("dsact_gemm", "bf16x3"), use_graph=kwargs.get("dsact_graph", True),
+                policy_std=pi_args["std_type"], **common)
         if q_args["output_activation"] != "linear" or pi_args["output_activation"] != "linear":
             raise NotImplementedError("the CUDA engine implements linear output activations")
         self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
@@ -267,6 +269,8 @@ class DSAC_V2:
         # "peer": exchanges inside the step's kernels over NVLink peer memory (falls back to NCCL if the ranks cannot
         # map each other's buffers); "nccl": torch.distributed all-reduces between three graph launches
         self.dp_transport = kwargs.get("dsact_dp_transport", "peer")
+        if not self.networks._cnn and kwargs.get("policy_std_type", "mlp_shared") != "mlp_shared":
+            self.dp_transport = "nccl"   # the MLP engine's peer-memory step serves mlp_shared only (dsact_dp_step refuses)
         self._peer_dp, self._peer_eng = None, None
         self._slots, self._owners, self._cursor = None, [None] * self._RING, 0
 

@@ -35,7 +35,10 @@ STAT_KEYS = [
 def make_config(obs_dim: int, act_dim: int, hidden_q: Sequence[int], hidden_pi: Sequence[int], *, max_batch: int,
                 act_q: str = "gelu", act_pi: str = "gelu", gamma=0.99, tau=0.005, tau_b=None, delay_update=2,
                 auto_alpha=True, alpha=0.2, lr_q=1e-4, lr_pi=1e-4, lr_alpha=3e-4, min_log_std=-20.0,
-                max_log_std=0.5, gemm_mode="fp32", use_graph=True, act_dist="TanhGaussDistribution") -> Config:
+                max_log_std=0.5, gemm_mode="fp32", use_graph=True, act_dist="TanhGaussDistribution",
+                policy_std="mlp_shared") -> Config:
+    """`policy_std`: the policy's std_type (networks/mlp.py:43-72), "mlp_shared", "mlp_separated" or "parameter"; the
+    last two on DSAC-T handles only."""
     if len(hidden_q) > _lib.MAX_HIDDEN or len(hidden_pi) > _lib.MAX_HIDDEN:
         raise ValueError(f"at most {_lib.MAX_HIDDEN} hidden layers")
     for name in (act_q, act_pi):
@@ -54,6 +57,7 @@ def make_config(obs_dim: int, act_dim: int, hidden_q: Sequence[int], hidden_pi: 
     c.auto_alpha, c.delay_update = int(bool(auto_alpha)), int(delay_update)
     c.gemm_mode, c.use_graph = _lib.GEMM_MODES[gemm_mode], int(bool(use_graph))
     c.act_dist = _lib.ACT_DISTS[act_dist]
+    c.policy_std = _lib.POLICY_STDS[policy_std]
     c.gamma, c.tau = float(gamma), float(tau)
     c.tau_b = float(tau if tau_b is None else tau_b)
     c.alpha_fixed = float(alpha)
@@ -475,20 +479,37 @@ class Engine:
     # ---- weights in the reference's state_dict schema -----------------------------------
     def _schema(self):
         """[(key, flat name, offset, shape)] for every tensor of the flat layout (include/dsact.h).  DSAC_V1 handles walk
-        the one critic `q` (dsac_v1.ApproxContainer) instead of `q1`, `q2`."""
+        the one critic `q` (dsac_v1.ApproxContainer) instead of `q1`, `q2`.  The policy span follows `policy_std`
+        (DSACT_STD_*): `policy.policy.*`, or `policy.mean.*` then `policy.log_std.*`, or the row `policy.log_std` then
+        `policy.mean.*`."""
         c = self.cfg
         q_sizes = [c.obs_dim + c.act_dim] + [c.hidden_q[j] for j in range(c.n_hidden_q)] + [2]
-        pi_sizes = [c.obs_dim] + [c.hidden_pi[j] for j in range(c.n_hidden_pi)] + [2 * c.act_dim]
+        pi_in = [c.obs_dim] + [c.hidden_pi[j] for j in range(c.n_hidden_pi)]
         out, off = [], 0
-        critics = ("q",) if getattr(self, "v1", None) is not None else ("q1", "q2")
-        for net, inner, sizes in tuple((n, "q", q_sizes) for n in critics) + (("policy", "policy", pi_sizes),):
+
+        def leaf(net, name, shape):
+            nonlocal off
+            n = 1
+            for d in shape:
+                n *= d
+            out.append((f"{net}.{name}", f"{net}_target.{name}", off, n, shape))
+            off += n
+
+        def mlp(net, inner, sizes):
             for j in range(len(sizes) - 1):
-                for leaf, shape in (("weight", (sizes[j + 1], sizes[j])), ("bias", (sizes[j + 1],))):
-                    n = 1
-                    for d in shape:
-                        n *= d
-                    out.append((f"{net}.{inner}.{2 * j}.{leaf}", f"{net}_target.{inner}.{2 * j}.{leaf}", off, n, shape))
-                    off += n
+                leaf(net, f"{inner}.{2 * j}.weight", (sizes[j + 1], sizes[j]))
+                leaf(net, f"{inner}.{2 * j}.bias", (sizes[j + 1],))
+
+        for net in ("q",) if getattr(self, "v1", None) is not None else ("q1", "q2"):
+            mlp(net, "q", q_sizes)
+        if c.policy_std == _lib.POLICY_STDS["mlp_separated"]:
+            mlp("policy", "mean", pi_in + [c.act_dim])
+            mlp("policy", "log_std", pi_in + [c.act_dim])
+        elif c.policy_std == _lib.POLICY_STDS["parameter"]:
+            leaf("policy", "log_std", (1, c.act_dim))
+            mlp("policy", "mean", pi_in + [c.act_dim])
+        else:
+            mlp("policy", "policy", pi_in + [2 * c.act_dim])
         return out, off
 
     def load_weights(self, weights: dict):
@@ -550,6 +571,7 @@ class Engine:
             t.M = p["M"]
             for k in ("x0", "x1", "out"):
                 setattr(t, k, _ptr(p.get(k)))
+            t.out_ld = int(p.get("out_ld", 0))
             for k in ("Zout", "Zin", "img", "colsum"):
                 for j, v in enumerate(p.get(k) or []):
                     getattr(t, k)[j] = _ptr(v)
@@ -571,7 +593,7 @@ class Engine:
                 for i, x in enumerate(v):
                     getattr(t, k)[i] = _ptr(x)
             else:
-                setattr(t, k, _ptr(v))
+                setattr(t, k, v if isinstance(v, int) else _ptr(v))
         with torch.cuda.device(self.device):
             check(self.lib.dsact_test_rows(self.h, C.byref(t), self._stream()))
 

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define DSACT_ABI_VERSION 3
+#define DSACT_ABI_VERSION 4
 #define DSACT_MAX_HIDDEN 6
 #define DSACT_NUM_STATS 16
 
@@ -57,6 +57,13 @@ enum {
   DSACT_GEMM_BF16 = 2      /* wgmma single-pass bf16, fp32 accumulate (throughput mode) */
 };
 
+/* The policy's std_type (reference networks/mlp.py:43-72) and the flat layout of the policy span it implies:
+ *  DSACT_STD_SHARED    "mlp_shared":    one MLP [O, hidden_pi.., 2A] (mean | log_std);
+ *  DSACT_STD_SEPARATED "mlp_separated": [ mean.* | log_std.* ], two MLPs [O, hidden_pi.., A];
+ *  DSACT_STD_PARAMETER "parameter":     [ log_std row (A floats) | mean.* ], the row a learnable [1, A] parameter.
+ * The last two are the layouts dsact_cnn_query_layout reports for the same networks (n_conv = 0, q_heads = 1). */
+enum { DSACT_STD_SHARED = 0, DSACT_STD_SEPARATED = 1, DSACT_STD_PARAMETER = 2 };
+
 /* What ApproxContainer.__init__ + DSAC_V2.__init__ read from kwargs
  * (reference dsac_v2.py:25-59,79-90; utils/common_utils.py:48-89). */
 typedef struct dsact_config {
@@ -76,6 +83,7 @@ typedef struct dsact_config {
   int32_t use_graph;             /* replay captured CUDA graphs for repeated identical calls */
   int32_t act_dist;              /* policy_act_distribution: 0 TanhGaussDistribution, 1 GaussDistribution
                                     (utils/act_distribution_cls.py:20-79, 82-116) */
+  int32_t policy_std;            /* DSACT_STD_*: the policy's std_type (networks/mlp.py:43-72); DSAC-T handles only */
   /* scalars are doubles because the reference holds them as Python floats and forms
    * 1-beta, lr/(1-beta^t) ... in double before they touch an fp32 tensor */
   double gamma, tau, tau_b;       /* dsac_v2.py:82,83,90 */
@@ -87,7 +95,7 @@ typedef struct dsact_config {
 
 typedef struct dsact_layout {
   int64_t n_q;          /* floats in one Q network */
-  int64_t n_pi;         /* floats in the policy network */
+  int64_t n_pi;         /* floats in the policy span (see DSACT_STD_*) */
   int64_t n_params;     /* 2*n_q + n_pi + 1 (log_alpha last) */
   int64_t n_targets;    /* 2*n_q + n_pi */
   int64_t workspace_bytes; /* activation / scratch arena the caller must provide */
@@ -223,7 +231,9 @@ int dsact_replay_steps(dsact_handle *h, int32_t n_steps, int32_t batch, int64_t 
  * Then dsact_dp_step / dsact_dp_replay_step = dsact_step / dsact_replay_step on this rank's shard, with the critic-std
  * sums, the gradients and the logged sums reduced over all ranks inside the step's own kernels (rank-ordered sums: the
  * replicas stay bit-identical).  `global_batch` = sum of the ranks' batch sizes.  A peer that never arrives makes
- * tb_info slot 14 non-zero (1 + its rank) after DSACT_DP_TIMEOUT_MS (default 10 s) instead of hanging the GPU. */
+ * tb_info slot 14 non-zero (1 + its rank) after DSACT_DP_TIMEOUT_MS (default 10 s) instead of hanging the GPU.
+ * MLP-engine handles with policy_std != DSACT_STD_SHARED return DSACT_EINVAL from all four calls (reduce between the split
+ * calls dsact_grad_phase1/2 and dsact_apply instead). */
 #define DSACT_IPC_HANDLE_BYTES 64
 #define DSACT_DP_MAX_RANKS 8
 int dsact_dp_export(dsact_handle *h, void *handle_out, int64_t *bytes_out);
@@ -235,7 +245,8 @@ int dsact_dp_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int
 
 /* ---- DSAC_V1 on the MLP engine ---------------------------------------------------------------------------------------
  * DSAC_V1 (reference dsac_v1.py:56-273: ONE distributional critic, fixed TD bound) with MLP approximators and the policy's
- * "mlp_shared" std type, on the tensor-core / SIMT engine of dsact_create: the same dsact_config, in which critic and policy
+ * "mlp_shared" std type (policy_std = DSACT_STD_SHARED; any other value is DSACT_EINVAL), on the tensor-core / SIMT engine of
+ * dsact_create: the same dsact_config, in which critic and policy
  * may differ in depth, width and activation, in all three gemm_modes, with use_graph on or off, plus the two settings
  * DSAC-T lacks.
  * Flat layout: params = [ q | policy | log_alpha ], targets = [ q_target | policy_target ] (n_params = n_q + n_pi + 1,
@@ -364,6 +375,7 @@ typedef struct dsact_test_chain_pass {
   void *img[DSACT_MAX_HIDDEN];
   float *colsum[DSACT_MAX_HIDDEN];
   float *out;
+  int32_t out_ld;   /* forward: row pitch of `out` in floats, >= sizes[L+1] (0: contiguous): the head writes its columns of wider rows */
 } dsact_test_chain_pass;
 int dsact_test_chain(dsact_handle *h, int32_t dgrad, int32_t L, const int32_t *sizes, int32_t K0, int32_t K1, int32_t kB1,
                      int32_t act, const float *params, const dsact_test_chain_pass *passes, int32_t n_passes, void *stream);
@@ -407,6 +419,10 @@ typedef struct dsact_test_row_io {
   float *gbias_q[2], *gbias_q_raw[2], *gbias_pi, *gbias_ls;
   void *img_act[2], *img_q[2], *img_qa[2], *img_dlogits;
   float *stats_out;
+  /* DSACT_TEST_POLICY_GRAD with split_dlogits != 0 (two policy heads, or a log_std row): img_dlogits is the image of the
+   * mean half alone (width A) and img_dlogits_ls that of the log_std half (width A; null: not written) */
+  void *img_dlogits_ls;
+  int32_t split_dlogits;
 } dsact_test_row_io;
 int dsact_test_rows(dsact_handle *h, const dsact_test_row_io *rows, void *stream);
 
