@@ -5,8 +5,10 @@
 //   dgrad chain   : dOut -> [dY W_j (.) act'(z_{j-1})] x L (-> dY W_0[:, act columns] for the actor path)
 // Layer 0 takes its A operand from global memory by TMA (the bf16 hi/lo images of obs / act / dOut); every later
 // layer takes A from SHARED MEMORY: the epilogue of layer j writes act(z_j) (or dz_j) as bf16 hi/lo pairs, in the
-// 128-byte-swizzled K-major layout wgmma reads, into the operand buffer, so hidden activations never leave the SM
-// unless the backward pass needs them (act' for the dgrad chain, images for wgrad).
+// 128-byte-swizzled K-major layout wgmma reads, into the operand buffer (stmatrix), so hidden activations never leave the SM
+// unless the backward pass needs them (act' for the dgrad chain, images for wgrad).  The bf16 image a weight gradient
+// needs is that same tile: it leaves as a TMA store of the operand buffer's k-blocks (a layer with an image and no next
+// layer stages it there all the same).
 // The weight tiles of layer j+1 are prefetched by the TMA warp while the epilogue of layer j runs.  The MMAs of a k-block
 // issue back to back and one k-block stays in flight while the next is issued; each warpgroup's share of the layer width
 // (64 or 128 columns) is a compile-time parameter of its layer body, dispatched once per layer.
@@ -39,6 +41,8 @@ constexpr int CH_MMA_REGS = 232;
 
 struct ChainLayer {
   CUtensorMap mapB;          // weight image; forward: K-major (box = bn rows), dgrad: MN-major (box = 64 x 64)
+  CUtensorMap mapImg;        // bf16 hi/lo image of the result for the weight-gradient GEMM, [M, (N + 7) / 8 * 8] (box =
+                             // 64 x 64): stored by TMA from the operand buffer (valid when `img`)
   int kblocks[2];            // k-blocks of 64; layer 0 may have two A segments, later layers use [0] only
   int kB0[2];                // offset of each segment along B's reduction dimension
   int N, bn;                 // outputs; tile width (multiple of 16, <= 256)
@@ -48,10 +52,8 @@ struct ChainLayer {
   const float* Zin;          // dgrad: act'(pre-activation) of the layer below, ld = N
   float* colsum;             // dgrad: bias gradient (+=)
   float* C;                  // fp32 result, ld = ldc (head layers)
-  __nv_bfloat16* img;        // bf16 hi/lo image of the result for the weight-gradient GEMM (null: not needed)
-  int img_pitch;
   int ldc;                   // >= N: a head may write its columns of a wider row (the policy's mean | log_std logits)
-  long long img_plane;
+  int img;                   // nonzero: the image is needed (mapImg)
 };
 
 struct ChainPass {
@@ -65,6 +67,8 @@ struct ChainGroup {
   unsigned long long* dbg;
   ChainPass p[CH_MAX_PASSES];
 };
+// the kernel's parameters (the group, stages, stage_b) within the 32764 bytes a launch may pass (CUDA 12.1+, sm_70+)
+static_assert(sizeof(ChainGroup) + 2 * sizeof(int) <= 32764, "ChainGroup exceeds the kernel-parameter limit");
 
 inline int chain_smem_bytes(int stages, int planes, int stage_b) {
   return stages * planes * stage_b + planes * CH_OPND_PLANE + CH_SCRATCH + 2 * stages * 8 + 1024;
@@ -84,12 +88,11 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
   constexpr int planes = PLANES2 ? 2 : 1;
   const ChainLayer& Lj = P.L[j];
   const int lane = threadIdx.x & 31;
-  const int r_lo = ((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16 + (lane >> 2);   // this thread's rows r_lo, r_lo + 8
   const int nkb = Lj.kblocks[0] + Lj.kblocks[1];
   EpiArgs E;
   E.epi = Lj.epi; E.act = Lj.act; E.M = P.M; E.N = Lj.N; E.ldc = Lj.ldc; E.ldz = Lj.N;
   E.bias = Lj.bias; E.Zout = Lj.Zout; E.Zin = Lj.Zin; E.colsum = Lj.colsum; E.C = Lj.C;
-  E.img = Lj.img; E.img_pitch = Lj.img_pitch; E.img_plane = Lj.img_plane;
+  E.img = nullptr;
   float acc[128];
 #pragma unroll
   for (int i = 0; i < 32 * NB; ++i) acc[i] = 0.f;
@@ -129,10 +132,19 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
   wg_wait<0>();
   if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
   if (threadIdx.x == 0) TC_STAMP(8 + 3 * j);   // MMAs of layer j retired
-  // The next layer's A operand is written group by group as the epilogue computes it: both warpgroups' MMAs of this
-  // layer must have retired first (each reads all of A).
-  const bool next = j + 1 < P.n_layers;
-  if (next) ch_bar();
+  // The result is written group by group into the operand buffer as the epilogue computes it, as the next layer's A
+  // operand and as the source of the image's TMA store: both warpgroups' MMAs of this layer must have retired first
+  // (each reads all of A), and so must the previous layer's image store (thread 0 issued it).
+  const bool opw = j + 1 < P.n_layers || Lj.img;
+  if (opw) {
+    if (threadIdx.x == 0) bulk_wait_read();
+    ch_bar();
+  }
+  // Lane l addresses row l & 7 of 8 x 8 matrix l >> 3 of a stmatrix: matrix m of stmatrix s holds rows 8 (m & 1) .. + 7
+  // of the warp's 16 and the 8 columns ii = 2 s + (m >> 1) of the group (fragment words v[4 ii + 2 h], + 1, h = m & 1).
+  // In the 128-byte-swizzled K-major k-block tiles, the 16-byte chunk of that row and column block is chunk ^ (row & 7).
+  const int m_row = ((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+  const uint32_t s_row = smem_u32(opnd) + (uint32_t)((n0 >> 6) * TC_STAGE_A + m_row * 128);
 #pragma unroll 1
   for (int q = 0; q < 2 * NB; ++q) {
     float x[16], v[16];
@@ -146,27 +158,33 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
         for (int t = 0; t < 16; ++t) v[t] = acc[16 * c + t];
       }
     epi_group<PLANES2>(v, x, E, m0, n0, q, row);
-    if (next) {
-      // bf16 hi/lo pairs at (row, column) of the swizzled K-major k-block tiles (16-byte chunk index ^= row & 7)
+    if (opw) {
+      // bf16 hi/lo pairs, split once: word i = matrix (ii, h) = (i >> 1, i & 1)
+      uint32_t whi[8], wlo[8];
 #pragma unroll
-      for (int ii = 0; ii < 4; ++ii) {
-        const int c = n0 + 8 * (4 * q + ii) + 2 * (lane & 3), cc = c & 63;
+      for (int i = 0; i < 8; ++i) {
+        if (PLANES2) split_pack2(v[2 * i], v[2 * i + 1], whi[i], wlo[i]);
+        else whi[i] = cvt_bf16x2(v[2 * i], v[2 * i + 1]);
+      }
+      const uint32_t s_q = s_row + (uint32_t)((q >> 1) * TC_STAGE_A);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = r_lo + 8 * h;
-          uint32_t whi, wlo;
-          split_pack2(v[4 * ii + 2 * h], v[4 * ii + 2 * h + 1], whi, wlo);
-          const uint32_t off = (uint32_t)((c >> 6) * TC_STAGE_A + r * 128 + ((((cc >> 3) ^ (r & 7)) << 4) | ((cc & 7) * 2)));
-          *reinterpret_cast<uint32_t*>(opnd + off) = whi;
-          if (PLANES2) *reinterpret_cast<uint32_t*>(opnd + CH_OPND_PLANE + off) = wlo;
-        }
+      for (int s = 0; s < 2; ++s) {
+        const uint32_t a = s_q + (uint32_t)((((4 * (q & 1) + 2 * s + (lane >> 4)) ^ (lane & 7))) << 4);
+        stsm_x4(a, whi[4 * s], whi[4 * s + 1], whi[4 * s + 2], whi[4 * s + 3]);
+        if (PLANES2) stsm_x4(a + CH_OPND_PLANE, wlo[4 * s], wlo[4 * s + 1], wlo[4 * s + 2], wlo[4 * s + 3]);
       }
     }
   }
   if (threadIdx.x == 0) TC_STAMP(9 + 3 * j);
-  if (next) {
-    fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads
+  if (opw) {
+    fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads and the TMA store
     ch_bar();
+    // The image: k-block tiles of the layer's columns, clipped by the tensor map to rows < M and columns < (N + 7) / 8 * 8
+    if (Lj.img && threadIdx.x == 0) {
+      for (int kb = 0; kb < (Lj.N + 63) / 64; ++kb)
+        for (int pl = 0; pl < planes; ++pl) tma_store_3d(&Lj.mapImg, opnd + pl * CH_OPND_PLANE + kb * TC_STAGE_A, kb * TC_BK, m0, pl);
+      bulk_commit();
+    }
   }
   if (threadIdx.x == 0) TC_STAMP(10 + 3 * j);
 }
@@ -181,7 +199,7 @@ __device__ __forceinline__ void chain_idle(const ChainPass& P, int j, int stages
     if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[stage]);
     if (++stage == stages) { stage = 0; phase ^= 1; }
   }
-  if (j + 1 < P.n_layers) { ch_bar(); ch_bar(); }
+  if (j + 1 < P.n_layers || P.L[j].img) { ch_bar(); ch_bar(); }
 }
 
 // B_MN: the weight tiles are MN-major (dgrad chains); forward chains read them K-major.
@@ -215,11 +233,12 @@ __global__ void __launch_bounds__(CH_THREADS, 1) tc_chain_kernel(const __grid_co
   }
   if (warp == PRODUCER) {   // descriptor prefetch: every tensor map this CTA will use (kernel parameters: no dependency on the
                      // preceding kernel)
-    for (int i = lane; i < 2 + nl; i += 32) {
+    for (int i = lane; i < 2 + 2 * nl; i += 32) {
       const CUtensorMap* m = nullptr;
       if (i == 0) m = &P.mapA[0];
       else if (i == 1) { if (P.L[0].kblocks[1] > 0) m = &P.mapA[1]; }
-      else m = &P.L[i - 2].mapB;
+      else if (i < 2 + nl) m = &P.L[i - 2].mapB;
+      else if (P.L[i - 2 - nl].img) m = &P.L[i - 2 - nl].mapImg;
       if (m) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
     }
   }
@@ -277,6 +296,7 @@ __global__ void __launch_bounds__(CH_THREADS, 1) tc_chain_kernel(const __grid_co
         default: chain_layer<PLANES2, B_MN, 2>(g, P, j, n0, ringB, opnd, row, stages, stage_b, full, empty, m0, stage, phase); break;
       }
     }
+    if (threadIdx.x == 0) bulk_wait();   // the image stores this thread issued have completed
   }
 
   if (lane == 0 && warp < PRODUCER) { if (g.dbg) atomicMax(&g.dbg[(size_t)blockIdx.x * TC_DBG_SLOTS + 5], gtime()); }

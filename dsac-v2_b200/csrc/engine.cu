@@ -662,6 +662,13 @@ struct ChainBuild {
     flops += 2.0 * P.M * N * ((double)K0 + K1);
     return L;
   }
+  // the bf16 image of layer L's result (p null: none), stored by TMA up to column (N + 7) / 8 * 8 and row im.rows
+  void image(ChainLayer& L, Img im) {
+    if (!im.p) return;
+    im.width = (L.N + 7) / 8 * 8;
+    L.img = 1;
+    ok = ok && make_map(&L.mapImg, im, TC_BM);
+  }
 };
 
 static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
@@ -739,7 +746,7 @@ static ChainPass& chain_fwd_layers(ChainBuild& cb, const Net& net, const float* 
                                                            // ldc as well, and a head layer has no Zout
     else {
       L.Zout = io.z[j];
-      L.img = io.img[j].p; L.img_pitch = io.img[j].pitch; L.img_plane = io.img[j].plane;
+      cb.image(L, io.img[j]);
     }
   }
   return P;
@@ -755,7 +762,7 @@ static ChainPass& chain_dgrad_layers(ChainBuild& cb, const Net& net, const Chain
     L.epi = EPI_DACT; L.act = act;
     L.Zin = io.z[j - 1];
     L.colsum = io.colsum[j - 1];
-    L.img = io.img[j - 1].p; L.img_pitch = io.img[j - 1].pitch; L.img_plane = io.img[j - 1].plane;
+    cb.image(L, io.img[j - 1]);
   }
   if (dact_out) {
     ChainLayer& L = cb.layer(P, io.w[0].cols(act_col_img, act_cols), true, act_cols, net.s[1], 0, 0);

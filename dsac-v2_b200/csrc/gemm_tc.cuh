@@ -116,6 +116,22 @@ template <int N>   // at most N committed wgmma groups of this warp still in fli
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, %0;" ::"n"(TC_MMA_THREADS) : "memory"); }   // the MMA warpgroup only
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// TMA store of one box from shared memory (elements outside the tensor are not written), as part of this thread's next
+// bulk async-group; wait_read: the source of every committed group has been read (shared memory may be rewritten).
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// Four 8 x 8 b16 matrices: lane l passes the shared address of row l & 7 of matrix l >> 3 (16 bytes), and word i of every
+// lane is its fragment of matrix i (row lane >> 2, columns 2 (lane & 3), + 1).
+__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(w0), "r"(w1), "r"(w2), "r"(w3)
+               : "memory");
+}
 
 // Shared-memory matrix descriptor of wgmma, 128-byte swizzle (bits 62-63 = 1).
 //   K-major : rows of 128 B (64 bf16 of K), 8-row groups SBO = 1024 B apart; advance K by 32 B per k16 step.
@@ -350,7 +366,6 @@ template <bool PLANES2>
 __device__ __forceinline__ void epi_group(float (&v)[16], const float (&x)[16], const EpiArgs& E, int m0, int n0, int g,
                                           float* row) {
   EPI_FRAG_COORDS
-  const int img_w = (E.N + 7) / 8 * 8;
   float d[16];
   if (E.epi == EPI_STORE || E.epi == EPI_BIAS_ACT) {
     if (E.bias) {
@@ -371,16 +386,25 @@ __device__ __forceinline__ void epi_group(float (&v)[16], const float (&x)[16], 
 #pragma unroll
     for (int t = 0; t < 16; ++t) v[t] *= x[t];
     if (E.colsum) {  // bias gradient: both rows of the thread, then the eight lanes that share its columns
+      // s[k]: column k = 2 (t >> 2) + (t & 1) of the thread's eight.  A transposing butterfly over lane bits 2, 3, 4: at
+      // each step a lane keeps half of its columns (the upper half if its bit is set), adds the partner's partial sums of
+      // them and sends the other half, so each lane ends with one column's sum over the eight lanes, added in the same
+      // tree (own + partner at every step) as a full xor reduction per column.
+      float s[8];
 #pragma unroll
-      for (int t = 0; t < 16; t += 4)
+      for (int k = 0; k < 8; ++k) s[k] = v[4 * (k >> 1) + (k & 1)] + v[4 * (k >> 1) + 2 + (k & 1)];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float s = v[t + e] + v[t + 2 + e];
-          s += __shfl_xor_sync(0xffffffffu, s, 4);
-          s += __shfl_xor_sync(0xffffffffu, s, 8);
-          s += __shfl_xor_sync(0xffffffffu, s, 16);
-          if (lane < 4 && COL(t + e) < E.N) atomicAdd(E.colsum + COL(t + e), s);
+      for (int h = 4; h >= 1; h >>= 1) {
+        const bool up = lane & (16 / h);
+#pragma unroll
+        for (int i = 0; i < h; ++i) {
+          const float send = up ? s[i] : s[i + h], keep = up ? s[i + h] : s[i];
+          s[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16 / h);
         }
+      }
+      const int k = ((lane >> 2) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 4) & 1);
+      const int c = cq + 32 * g + 8 * (k >> 1) + (k & 1);
+      if (c < E.N) atomicAdd(E.colsum + c, s[0]);
     }
   }
 #pragma unroll
@@ -390,6 +414,14 @@ __device__ __forceinline__ void epi_group(float (&v)[16], const float (&x)[16], 
     for (int t = 0; t < 16; ++t)
       if (ROW_OK(t) && COL(t) < E.N) E.C[(size_t)ROW(t) * E.ldc + COL(t)] = v[t];
   }
+}
+
+// The bf16 hi/lo image of group g's results v (columns >= N are zeros) up to column (N + 7) / 8 * 8.  The layer chain
+// stores its images by TMA from its operand buffer instead.
+template <bool PLANES2>
+__device__ __forceinline__ void epi_img(const float (&v)[16], const EpiArgs& E, int m0, int n0, int g) {
+  EPI_FRAG_COORDS
+  const int img_w = (E.N + 7) / 8 * 8;
   if (E.img) {  // packed bf16 pairs (pitch % 8 == 0, even column): one 4-byte store per plane
 #pragma unroll
     for (int t = 0; t < 16; t += 2) {
@@ -418,6 +450,7 @@ __device__ __forceinline__ void epi_frag(float (&acc)[128], const EpiArgs& E, in
 #pragma unroll
     for (int t = 0; t < 16; ++t) v[t] = acc[16 * g + t];
     epi_group<PLANES2>(v, x, E, m0, n0, g, row);
+    epi_img<PLANES2>(v, E, m0, n0, g);
 #pragma unroll
     for (int t = 0; t < 16; ++t) acc[16 * g + t] = v[t];
   }
