@@ -127,6 +127,15 @@ class TestRowIo(C.Structure):
                 ("img_dlogits", _fp), ("stats_out", _fp), ("img_dlogits_ls", _fp), ("split_dlogits", C.c_int32)]
 
 
+TEST_DP_OPS = {"exchange": 0, "fold": 1, "reduce_scatter": 2, "apply": 3}   # DSACT_TEST_DP_*
+
+
+class TestDpIo(C.Structure):
+    """dsact_test_dp_io: the arguments of one dsact_test_dp operation."""
+    _fields_ = [("kind", C.c_int32), ("ranks", C.POINTER(C.c_void_p)), ("grads", _fp), ("slabs", _fp), ("nslabs", C.c_int32),
+                ("slab_stride", C.c_int64), ("n", C.c_int64), ("tail_rows", C.c_int32), ("global_batch", C.c_int64)]
+
+
 # every symbol include/dsact.h declares: (restype, argtypes)
 IPC_HANDLE_BYTES = 64   # DSACT_IPC_HANDLE_BYTES
 DP_MAX_RANKS = 8        # DSACT_DP_MAX_RANKS
@@ -173,6 +182,9 @@ SYMBOLS = {
                                    C.c_int32, C.c_void_p, C.POINTER(TestChainPass), C.c_int32, C.c_void_p]),
     "dsact_test_rows": (C.c_int, [C.c_void_p, C.POINTER(TestRowIo), C.c_void_p]),
     "dsact_test_apply": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]),
+    "dsact_test_dp_attach": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                       C.POINTER(C.c_int64)]),
+    "dsact_test_dp": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TestDpIo), C.c_void_p]),
 }
 
 _lib = None

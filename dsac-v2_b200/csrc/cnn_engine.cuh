@@ -615,13 +615,9 @@ static void cnn_enqueue_dp_step(HeadsHandle* h, const dsact_batch& bt, const dsa
   enqueue_dp_exchange(h->dp, state, 0, c);
   cnn_enqueue_phase2(h, global_batch, c);
   {   // phase 2 already wrote the log_alpha share: a plain copy of the flat gradients into this rank's block
-    const long long n = h->n_params;
     TailArgs none;
     memset(&none, 0, sizeof(none));
-    int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF, (const float*)h->buf.grads, (const float*)h->buf.grads, n, 0,
-             4LL, (const float*)state, none);
-    c.done();
+    enqueue_dp_fold(h, h->buf.grads, h->buf.grads, 0, 4, h->n_params, none, c);
   }
   enqueue_dp_exchange(h->dp, state, 1, c);
   if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, state, h->num_sms, c);

@@ -78,8 +78,7 @@ __device__ __forceinline__ unsigned long long dp_time_ns() {
 // One block of 32 * world threads.  kind 0: all-reduce state[ST_STDSUM..+1] (SUM) and open epoch e = epoch + 1;
 // kind 1: all-reduce the 16 sums (SUM) and 2 minima (MIN) of state[ST_ACC..] at the epoch kind 0 opened.
 // A peer that does not arrive within `timeout_ns` sets state[ST_DP_ERR] instead of hanging the GPU.
-__global__ void dp_exchange_kernel(const DpComm c, float* __restrict__ state, int kind, unsigned long long timeout_ns) {
-  pdl_sync();
+__device__ __forceinline__ void dp_exchange(const DpComm& c, float* __restrict__ state, int kind, unsigned long long timeout_ns) {
   int* sti = reinterpret_cast<int*>(state);
   const uint32_t e = (uint32_t)sti[ST_DP_EPOCH] + (kind == 0 ? 1u : 0u);
   const int par = (int)(e & 1u);
@@ -115,6 +114,20 @@ __global__ void dp_exchange_kernel(const DpComm c, float* __restrict__ state, in
     src[t] = acc;
   }
   if (kind == 0 && t == 0) sti[ST_DP_EPOCH] = (int)e;
+}
+__global__ void dp_exchange_kernel(const DpComm c, float* __restrict__ state, int kind, unsigned long long timeout_ns) {
+  pdl_sync();
+  dp_exchange(c, state, kind, timeout_ns);
+}
+
+// Test hook only (dsact_test_dp): the exchange of a whole world of ranks on one device in one cooperative launch, block r
+// being rank r.  Cooperative launch keeps the W blocks resident together, so every flag wait can resolve.
+struct DpTestWorld {
+  DpComm comm[DP_MAX_RANKS];
+  float* state[DP_MAX_RANKS];
+};
+__global__ void dp_exchange_world_kernel(const __grid_constant__ DpTestWorld w, int kind, unsigned long long timeout_ns) {
+  dp_exchange(w.comm[blockIdx.x], w.state[blockIdx.x], kind, timeout_ns);
 }
 
 // grads_out[i] = grads[i] + sum of the weight-gradient slabs (the local total, into the exchange buffer)

@@ -1360,6 +1360,16 @@ static void enqueue_dp_exchange(const DpPeer& dp, float* state, int kind, Ctx& c
 }
 static void enqueue_dp_exchange(MlpHandle* h, int kind, Ctx& c) { enqueue_dp_exchange(h->dp, h->buf.state, kind, c); }
 
+// This rank's local gradient total into its exchange block: elements [0, n) of `grads` plus the first `nslabs`
+// weight-gradient slabs (`slab_stride` floats apart); `tail`.enabled: the log_alpha element formed from the logged sum
+static void enqueue_dp_fold(const dsact_handle* h, const float* grads, const float* slabs, int nslabs, long long slab_stride,
+                            long long n, const TailArgs& tail, Ctx& c) {
+  int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
+  launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF, grads, slabs, n, nslabs, slab_stride,
+           (const float*)h->buf.state, tail);
+  c.done();
+}
+
 // ---- exchange-buffer setup (dsact_dp_export / dsact_dp_connect, both engines) ---------------------------------------
 static int dp_peer_export(DpPeer& dp, int device, long long n_params, void* handle_out, int64_t* bytes_out) {
   CUDA_TRY(cudaSetDevice(device));
@@ -1378,7 +1388,8 @@ static int dp_peer_export(DpPeer& dp, int device, long long n_params, void* hand
   return DSACT_OK;
 }
 
-static int dp_peer_connect(DpPeer& dp, int device, float* state, int32_t rank, int32_t world, const void* handles) {
+// the peers' buffers this rank had opened are closed and the map is not ready until dp_peer_start
+static int dp_peer_reset(DpPeer& dp, int device, int32_t rank, int32_t world) {
   if (!dp.buf) return fail(DSACT_ESTATE, "the exchange buffer has not been exported (dp_export)");
   if (world < 2 || world > DP_MAX_RANKS || rank < 0 || rank >= world) return fail(DSACT_EINVAL, "rank %d / world %d outside [2, %d]", rank, world, DP_MAX_RANKS);
   CUDA_TRY(cudaSetDevice(device));
@@ -1386,7 +1397,25 @@ static int dp_peer_connect(DpPeer& dp, int device, float* state, int32_t rank, i
   dp.ready = false;
   for (int r = 0; r < DP_MAX_RANKS; ++r)
     if (dp.opened[r]) { cudaIpcCloseMemHandle(dp.opened[r]); dp.opened[r] = nullptr; }
+  dp.comm = DpComm();
   dp.comm.rank = rank; dp.comm.world = world;
+  return DSACT_OK;
+}
+
+// once every peer's buffer is in dp.comm: every rank starts at epoch 0 with clear flags (the caller synchronises the
+// ranks after this call)
+static int dp_peer_start(DpPeer& dp, float* state) {
+  CUDA_TRY(cudaMemset(dp.buf, 0, sizeof(float) * DP_GRADS_OFF));
+  CUDA_TRY(cudaMemset(state + ST_DP_EPOCH, 0, sizeof(float)));
+  CUDA_TRY(cudaMemset(state + ST_DP_ERR, 0, sizeof(float)));
+  CUDA_TRY(cudaDeviceSynchronize());
+  dp.ready = true;
+  return DSACT_OK;
+}
+
+static int dp_peer_connect(DpPeer& dp, int device, float* state, int32_t rank, int32_t world, const void* handles) {
+  int rc = dp_peer_reset(dp, device, rank, world);
+  if (rc) return rc;
   for (int r = 0; r < world; ++r) {
     if (r == rank) { dp.comm.peer[r] = dp.buf; continue; }
     cudaIpcMemHandle_t ipc;
@@ -1397,13 +1426,7 @@ static int dp_peer_connect(DpPeer& dp, int device, float* state, int32_t rank, i
     dp.opened[r] = p;
     dp.comm.peer[r] = static_cast<float*>(p);
   }
-  // every rank starts at epoch 0 with clear flags (the caller synchronises the ranks after this call)
-  CUDA_TRY(cudaMemset(dp.buf, 0, sizeof(float) * DP_GRADS_OFF));
-  CUDA_TRY(cudaMemset(state + ST_DP_EPOCH, 0, sizeof(float)));
-  CUDA_TRY(cudaMemset(state + ST_DP_ERR, 0, sizeof(float)));
-  CUDA_TRY(cudaDeviceSynchronize());
-  dp.ready = true;
-  return DSACT_OK;
+  return dp_peer_start(dp, state);
 }
 
 static void dp_peer_release(DpPeer& dp) {
@@ -1522,13 +1545,8 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
     launch_k(phase2_tail_kernel, 1, 32, 0, c, G_ + n_flat - 1, h->buf.state, sc, -(float)cf.act_dim, B, adam_hyper(h), 0);
     c.done();
   }
-  if (dp) {  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
-    const long long n = n_flat;
-    int blocks = (int)((n / 4 + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms; if (blocks < 1) blocks = 1;
-    launch_k(dp_grad_fold_kernel, blocks, 256, 0, c, h->dp.buf + DP_GRADS_OFF, (const float*)G_, (const float*)(tc ? W + ar.slabs : G_), n,
-             tc ? ar.nslabs : 0, (long long)(tc ? ar.slab_stride : 4), (const float*)h->buf.state, *tail);
-    c.done();
-  }
+  if (dp)  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
+    enqueue_dp_fold(h, G_, tc ? W + ar.slabs : G_, tc ? ar.nslabs : 0, tc ? ar.slab_stride : 4, n_flat, *tail, c);
   c.check();
 }
 
@@ -2714,6 +2732,90 @@ int dsact_test_apply(dsact_handle* h, int32_t part, int32_t fold_slabs, int32_t 
     apply_part(a, part);
   }
   launch_apply(h, a, c, max_blocks);
+  return sync_hook(h, c);
+}
+
+// ---- test hooks of the peer-memory exchange: every rank of a world on one device -------------------------------------
+static int check_dp_hook(const dsact_handle* h) {
+  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
+  return check_dp(h);
+}
+
+int dsact_test_dp_attach(dsact_handle* h, int32_t rank, int32_t world, dsact_handle* const* peers, void** buffer, int64_t* floats) {
+  if (world < 2 || world > DP_MAX_RANKS || rank < 0 || rank >= world)
+    return fail(DSACT_EINVAL, "rank %d / world %d outside [2, %d]", rank, world, DP_MAX_RANKS);
+  if (!peers) return fail(DSACT_EINVAL, "null peers");
+  int rc = check_dp_hook(h);
+  if (rc) return rc;
+  if (peers[rank] != h) return fail(DSACT_EINVAL, "peers[%d] is not the handle being attached", rank);
+  for (int r = 0; r < world; ++r) {
+    const dsact_handle* p = peers[r];
+    if (!p || !p->dp.buf) return fail(DSACT_ESTATE, "peer %d has not called dsact_dp_export", r);
+    if (p->device != h->device || p->engine != h->engine || p->dp.n_params != h->dp.n_params)
+      return fail(DSACT_EINVAL, "peer %d is on another device or engine, or has another parameter count", r);
+  }
+  if ((rc = dp_peer_reset(h->dp, h->device, rank, world))) return rc;
+  for (int r = 0; r < world; ++r) h->dp.comm.peer[r] = peers[r]->dp.buf;
+  if ((rc = dp_peer_start(h->dp, h->buf.state))) return rc;
+  if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));   // as dsact_dp_connect: captured steps hold the previous peer map
+  if (buffer) *buffer = h->dp.buf;
+  if (floats) *floats = DP_GRADS_OFF + 2 * h->dp.npad();
+  return DSACT_OK;
+}
+
+int dsact_test_dp(dsact_handle* h, int32_t op, const dsact_test_dp_io* io, void* stream) {
+  if (op < DSACT_TEST_DP_EXCHANGE || op > DSACT_TEST_DP_APPLY) return fail(DSACT_EINVAL, "unknown op %d", op);
+  if (!io) return fail(DSACT_EINVAL, "null io");
+  int rc = check_dp_hook(h);
+  if (rc) return rc;
+  if (!h->dp.ready) return fail(DSACT_ESTATE, "not attached (dsact_test_dp_attach)");
+  const DpPeer& dp = h->dp;
+  const int world = dp.comm.world;
+  const bool mlp_eng = h->engine == ENGINE_MLP;
+  DpTestWorld w;
+  memset(&w, 0, sizeof(w));
+  if (op == DSACT_TEST_DP_EXCHANGE) {
+    if (io->kind != 0 && io->kind != 1) return fail(DSACT_EINVAL, "exchange kind %d is not 0 or 1", io->kind);
+    if (!io->ranks) return fail(DSACT_EINVAL, "null ranks");
+    for (int r = 0; r < world; ++r) {
+      const dsact_handle* p = io->ranks[r];
+      if (!p || !p->dp.ready || p->dp.comm.rank != r || p->dp.comm.world != world ||
+          memcmp(p->dp.comm.peer, dp.comm.peer, sizeof(dp.comm.peer)) != 0)
+        return fail(DSACT_EINVAL, "ranks[%d] is not rank %d of this handle's world", r, r);
+      w.comm[r] = p->dp.comm; w.state[r] = p->buf.state;
+    }
+  } else if (op == DSACT_TEST_DP_FOLD) {
+    if (!io->grads || io->n < 1 || io->n > h->n_params || io->nslabs < 0 || io->nslabs > 16 ||
+        (io->nslabs > 0 && (!io->slabs || io->slab_stride < io->n)) || io->tail_rows < 0 ||
+        (io->tail_rows > 0 && io->global_batch < io->tail_rows))
+      return fail(DSACT_EINVAL, "bad fold argument");
+  } else if (op == DSACT_TEST_DP_APPLY && mlp_eng) {
+    if (io->tail_rows < 1 || io->global_batch < io->tail_rows) return fail(DSACT_EINVAL, "tail_rows / global_batch");
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  Ctx c{(cudaStream_t)stream, 0, cudaSuccess};
+  c.pdl = mlp_eng && mlp(h)->tc();
+  if (op == DSACT_TEST_DP_EXCHANGE) {
+    int kind = io->kind;
+    unsigned long long timeout = dp_timeout_ns();
+    void* args[] = {&w, &kind, &timeout};
+    c.err = cudaLaunchCooperativeKernel((const void*)dp_exchange_world_kernel, dim3(world), dim3(32 * world), args, 0, c.s);
+    c.done();
+  } else if (op == DSACT_TEST_DP_FOLD) {
+    TailArgs ta;
+    memset(&ta, 0, sizeof(ta));
+    if (io->tail_rows > 0) ta = tail_args(h, io->global_batch, io->tail_rows);
+    const bool slabs = io->nslabs > 0;   // (none: the steps' arguments, grads and a stride of 4)
+    enqueue_dp_fold(h, io->grads, slabs ? io->slabs : io->grads, io->nslabs, slabs ? io->slab_stride : 4, io->n, ta, c);
+  } else if (op == DSACT_TEST_DP_REDUCE_SCATTER) {
+    enqueue_dp_reduce_scatter(dp, h->buf.state, h->num_sms, c);
+  } else if (mlp_eng) {
+    const TailArgs ta = tail_args(h, io->global_batch, io->tail_rows);
+    enqueue_apply(mlp(h), c, &ta, true);
+  } else {
+    cnn_enqueue_apply(heads(h), c, 1, true);
+  }
+  c.check();
   return sync_hook(h, c);
 }
 

@@ -370,7 +370,10 @@ struct StepScalars {
 __device__ __forceinline__ float step_mean_std(const float* state, const StepScalars& p, int k) {
   const float mean = state[ST_STDSUM + k] * p.inv_global_batch;
   const float old = state[ST_MEAN_STD1 + k];
-  return old < 0.f ? mean : (1.f - p.tau_b) * old + p.tau_b * mean;
+  // each operation rounded, as the reference's float32 arithmetic rounds it.  Left to contraction, nvcc fused a different
+  // product into the add in different kernels, and the split API (phase2_tail_kernel) committed an EMA one ulp away from
+  // the one the single-call and data-parallel steps commit (apply_kernel).
+  return old < 0.f ? mean : __fadd_rn(__fmul_rn(1.f - p.tau_b, old), __fmul_rn(p.tau_b, mean));
 }
 __device__ __forceinline__ float step_alpha(const StepScalars& p) { return p.auto_alpha ? expf(*p.log_alpha) : p.alpha_fixed; }
 

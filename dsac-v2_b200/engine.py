@@ -603,3 +603,36 @@ class Engine:
         with torch.cuda.device(self.device):
             check(self.lib.dsact_test_apply(self.h, int(part), int(fold_slabs), int(scalars_ready), int(tail_rows),
                                             int(global_batch), int(max_blocks), self._stream()))
+
+    def test_dp_attach(self, rank: int, peers: Sequence["Engine"]) -> torch.Tensor:
+        """dsact_test_dp_attach: make this handle rank `rank` of `peers` (engines of this process and device, in rank order,
+        each exported with dp_export).  Returns a float32 view of this rank's whole exchange buffer (header, gradient
+        block, reduced block; csrc/dp_peer.cuh)."""
+        arr = (C.c_void_p * len(peers))(*(p.h.value for p in peers))
+        buf, n = C.c_void_p(), C.c_int64()
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_test_dp_attach(self.h, int(rank), len(peers), arr, C.byref(buf), C.byref(n)))
+        self.dp_world = len(peers)
+        self._dp_peers = list(peers)
+        return _device_view(buf.value, int(n.value), self.device)   # the library owns it: valid while this handle lives
+
+    def test_dp(self, op: str, kind: int = 0, grads: Optional[torch.Tensor] = None, slabs: Optional[torch.Tensor] = None,
+                nslabs: int = 0, slab_stride: int = 0, n: int = 0, tail_rows: int = 0, global_batch: int = 1):
+        """dsact_test_dp: one exchange operation ("exchange", "fold", "reduce_scatter", "apply") on an attached handle.
+        "exchange" runs every rank of the world attached with test_dp_attach."""
+        t = _lib.TestDpIo()
+        t.kind, t.grads, t.slabs, t.nslabs = int(kind), _ptr(grads), _ptr(slabs), int(nslabs)
+        t.slab_stride, t.n, t.tail_rows, t.global_batch = int(slab_stride), int(n), int(tail_rows), int(global_batch)
+        ranks = (C.c_void_p * len(self._dp_peers))(*(p.h.value for p in self._dp_peers))
+        t.ranks = C.cast(ranks, C.POINTER(C.c_void_p))
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_test_dp(self.h, _lib.TEST_DP_OPS[op], C.byref(t), self._stream()))
+
+
+def _device_view(ptr: int, n: int, device: torch.device) -> torch.Tensor:
+    """A float32 tensor over n floats of device memory at `ptr` that torch does not own (through
+    __cuda_array_interface__, no copy)."""
+    class _Mem:
+        __cuda_array_interface__ = {"shape": (n,), "typestr": "<f4", "data": (ptr, False), "version": 3, "strides": None}
+    with torch.cuda.device(device):
+        return torch.as_tensor(_Mem(), device=device)

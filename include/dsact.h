@@ -437,6 +437,42 @@ int dsact_test_rows(dsact_handle *h, const dsact_test_row_io *rows, void *stream
 int dsact_test_apply(dsact_handle *h, int32_t part, int32_t fold_slabs, int32_t scalars_ready, int32_t tail_rows,
                      int64_t global_batch, int32_t max_blocks, void *stream);
 
+/* Test hooks of the peer-memory data-parallel exchange, with every rank of a world on one device.
+ *
+ * dsact_test_dp_attach: make h rank `rank` of the `world` handles peers[0..world-1] (rank order, peers[rank] == h), all
+ * of one process, one device and one engine with the same parameter count, each after dsact_dp_export.  The peers'
+ * exchange buffers are used directly (no CUDA IPC).  Like dsact_dp_connect it resets h's flags, epoch and error slot and
+ * drops the MLP engine's captured graphs.  buffer / floats (may be null): h's exchange buffer and its length in floats
+ * (header, gradient block, reduced block; layout in csrc/dp_peer.cuh).
+ *
+ * dsact_test_dp: one operation on an attached handle, through the data-parallel step's own launch code; synchronises
+ * `stream`.
+ *  DSACT_TEST_DP_EXCHANGE: the exchange of kind io->kind (0 critic-std sums, 1 logged sums) for every rank of the world
+ *    at once: io->ranks holds the world's attached handles in rank order.
+ *  DSACT_TEST_DP_FOLD: io->grads plus io->nslabs slabs at io->slabs (io->slab_stride floats apart) over elements
+ *    [0, io->n) into h's gradient block; io->tail_rows > 0: element n - 1 is the log_alpha gradient of tail_rows rows of
+ *    io->global_batch formed from the logged sum in h's state (the MLP engine's step), 0: a plain sum (the head-wise one).
+ *  DSACT_TEST_DP_REDUCE_SCATTER: h's slice of the two-shot reduction (worlds of 6 and more ranks in the step).
+ *  DSACT_TEST_DP_APPLY: Adam / Polyak on the rank-ordered gradient sum, as the engine's step builds it (one-shot below
+ *    6 ranks, the reduced block from 6 up); the MLP engine's with the end-of-backward bookkeeping over io->tail_rows
+ *    (>= 1) rows of io->global_batch.
+ * Both calls return DSACT_EINVAL or DSACT_ESTATE with a message, before any launch, for an unknown op, a rank or world
+ * outside [2, 8], a handle that is not exported or attached, a DSAC_V1 handle or an MLP handle whose policy_std is not
+ * mlp_shared. */
+int dsact_test_dp_attach(dsact_handle *h, int32_t rank, int32_t world, dsact_handle *const *peers, void **buffer,
+                         int64_t *floats);
+enum { DSACT_TEST_DP_EXCHANGE = 0, DSACT_TEST_DP_FOLD = 1, DSACT_TEST_DP_REDUCE_SCATTER = 2, DSACT_TEST_DP_APPLY = 3 };
+typedef struct dsact_test_dp_io {
+  int32_t kind;
+  dsact_handle *const *ranks;
+  const float *grads, *slabs;
+  int32_t nslabs;
+  int64_t slab_stride, n;
+  int32_t tail_rows;
+  int64_t global_batch;
+} dsact_test_dp_io;
+int dsact_test_dp(dsact_handle *h, int32_t op, const dsact_test_dp_io *io, void *stream);
+
 /* Test hook of the head-wise engine's convolution kernels: one layer (NCHW, square k x k window, stride, no padding) on
  * caller buffers, enqueued on `stream` of the current device.
  *  op 0 (forward)        : out[B,cout,hout,wout] = relu(conv(x, w) + b)

@@ -163,3 +163,18 @@ def test_conv_test_hook_rejects_bad_arguments_before_touching_a_device():
     for op, shape in ((3, (2, 8, 9, 9, 8, 3, 1)), (0, (2, 8, 2, 9, 8, 3, 1)), (1, (0, 8, 9, 9, 8, 3, 1))):
         assert lib.dsact_cnn_test_conv(op, *shape, null, null, null, null, null, null, null, 0, 0, 0, 0, null) == -1
         assert lib.dsact_last_error()
+
+
+def test_dp_test_hooks_reject_bad_arguments_before_touching_a_device():
+    lib = _lib.load()
+    io = _lib.TestDpIo()
+    peers = (C.c_void_p * 2)()
+    for rank, world, want in ((0, 1, b"outside"), (0, 9, b"outside"), (2, 2, b"outside"), (-1, 2, b"outside"),
+                              (0, 2, b"not bound")):
+        assert lib.dsact_test_dp_attach(None, rank, world, peers, None, None) != 0
+        assert want in lib.dsact_last_error(), (rank, world, lib.dsact_last_error())
+    assert lib.dsact_test_dp_attach(None, 0, 2, None, None, None) != 0 and b"null peers" in lib.dsact_last_error()
+    for op, want in ((-1, b"unknown op"), (4, b"unknown op"), (0, b"not bound"), (3, b"not bound")):
+        assert lib.dsact_test_dp(None, op, C.byref(io), None) != 0
+        assert want in lib.dsact_last_error(), (op, lib.dsact_last_error())
+    assert lib.dsact_test_dp(None, 1, None, None) != 0 and b"null io" in lib.dsact_last_error()

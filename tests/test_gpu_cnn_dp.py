@@ -1,4 +1,4 @@
-"""Data-parallel updates of the head-wise engine on 2 / 4 / 8 GPUs (ragged shards) == one GPU on the concatenated
+"""Data-parallel updates of the head-wise engine on 2 to 8 GPUs (ragged shards) == one GPU on the concatenated
 minibatch, for the CNN approximators (config `odd`) and the policy std types "mlp_separated" / "parameter", over both
 transports: "peer" (`dsact_dp_step` on head-wise handles, exchanges inside the step's kernels over NVLink peer memory) and "nccl"
 (`dp.data_parallel_gradients`: torch.distributed all-reduces between the split-API calls).  Each spawn also runs
@@ -93,7 +93,7 @@ def _worker(rank, world, port, out_dir, transport):
     dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("world", [2, 4, 8])
+@pytest.mark.parametrize("world", [2, 3, 4, 5, 6, 7, 8])
 @pytest.mark.parametrize("transport", ["peer", "nccl"])
 def test_data_parallel_equals_single_gpu(tmp_path, transport, world):
     if torch.cuda.device_count() < world:

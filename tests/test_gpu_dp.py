@@ -1,4 +1,4 @@
-"""Data-parallel update on 2 / 4 / 8 GPUs (ragged shards) == single-GPU update on the concatenated minibatch, for both transports:
+"""Data-parallel update on 2 to 8 GPUs (ragged shards) == single-GPU update on the concatenated minibatch, for both transports:
 "peer" (exchanges inside the step's kernels over NVLink peer memory, one graph per rank: dsact_dp_step) and "nccl"
 (torch.distributed all-reduces between the phase launches).  Needs >= 2 CUDA devices; world sizes above the device count are skipped."""
 import os
@@ -57,7 +57,7 @@ def _worker(rank, world, port, out_dir, gemm, transport):
 GLOBAL_ROWS = 250   # not a multiple of 4 or 8: the ranks hold shards of different sizes (dp.shard_rows)
 
 
-@pytest.mark.parametrize("world", [2, 4, 8])
+@pytest.mark.parametrize("world", [2, 3, 4, 5, 6, 7, 8])
 @pytest.mark.parametrize("transport", ["peer", "nccl"])
 @pytest.mark.parametrize("gemm", ["fp32", "bf16x3"])
 def test_data_parallel_equals_single_gpu(tmp_path, gemm, transport, world):
