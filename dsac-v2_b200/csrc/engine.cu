@@ -14,6 +14,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <cmath>
 
 #include <vector>
@@ -23,6 +24,7 @@
 #include "kernels.cuh"
 #include "tc_host.cuh"
 #include "chain_tc.cuh"
+#include "wgrad_tc.cuh"
 #include "dp_peer.cuh"
 
 using namespace dsact;
@@ -243,7 +245,8 @@ struct MlpHandle : dsact_handle {
   int in_set = 0;            // the input set the passes being enqueued read
   cudaStream_t gather_stream = nullptr;   // the next update's gather, forked beside a captured update's backward
   cudaEvent_t ev_gather_fork = nullptr, ev_gather_join = nullptr;
-  bool tc_attr_done = false, chain_attr_done = false;   // cudaFuncSetAttribute is per device: tracked per handle
+  bool tc_attr_done = false, chain_attr_done = false, wgrad_attr_done = false;   // cudaFuncSetAttribute is per device:
+                                                                                 // tracked per handle
   TcGroup tc_scratch;                                   // host-side lowering scratch of launch_tc (~5 KiB)
   std::vector<GraphEntry> graphs;
   uint64_t stamp = 0;
@@ -378,23 +381,76 @@ static void launch_simt(int num_sms, GemmGroup& g, int variant, Ctx& c) {
   else launch_variant<64, 64>(g, variant, grid, c);
 }
 
-// Lower the group onto wgmma: images instead of fp32 operands, TMA tensor maps, 64 x bn tiles.
-// `max_ctas` > 0: issue the group as several launches of at most that many CTAs (one CTA occupies an SM), which leaves
-// the remaining SMs to a concurrent branch of the step graph for the whole duration.
-static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas = 0) {
+// Weight gradients: the persistent two-warpgroup kernel (wgrad_tc.cuh), one launch of at most `max_ctas` CTAs (0: one
+// per SM; a bound leaves the remaining SMs to a concurrent branch of the step graph for the whole duration).  Every
+// problem is split over the batch into the fixed slab count; empty splits store zeros, so the reduction is always valid.
+static void launch_tc_wgrad(MlpHandle* h, Group& G, Ctx& c, int max_ctas) {
   TcGroup& t = h->tc_scratch;
   memset(&t, 0, sizeof(t));
   t.n = G.n;
   t.passes = h->passes();
-  const bool a_mn = variant == V_WGRAD, b_mn = variant != V_FWD;
+  const int nslabs = G.wg_slab ? G.wg_nslabs : h->ar.nslabs;
+  const int budget = max_ctas > 0 && max_ctas < h->num_sms ? max_ctas : h->num_sms;
+  // 128-wide tiles, unless they would leave more than half of the CTAs idle
+  int bn_cap = 128, tiles128 = 0;
+  for (int i = 0; i < G.n; ++i) tiles128 += ((G.prob(i).M + WG_BM - 1) / WG_BM) * ((G.prob(i).N + 127) / 128) * nslabs;
+  if (tiles128 * 2 <= budget) bn_cap = 64;
+  // the list holds the problems by the cost of their tiles (rows x MMA width), largest first: see wgrad_tc.cuh
+  int order[TC_MAXG], cost[TC_MAXG];
+  for (int i = 0; i < G.n; ++i) {
+    const int bn = std::min((G.prob(i).N + 15) / 16 * 16, bn_cap);
+    cost[i] = (G.prob(i).M > TC_BM ? 2 : 1) * ((bn + 63) / 64);
+    order[i] = i;
+  }
+  std::stable_sort(order, order + G.n, [&](int a, int b) { return cost[a] > cost[b]; });
+  int total = 0, bn_max = 16;
+  for (int o = 0; o < G.n; ++o) {
+    const int i = order[o];
+    const GemmProb& s = G.prob(i);
+    const TcExtra& x = G.x[i];
+    TcProb& p = t.p[o];
+    p.M = s.M; p.N = s.N;
+    p.bn = std::min((s.N + 15) / 16 * 16, bn_cap);
+    if (p.bn > bn_max) bn_max = p.bn;
+    p.tiles_m = (s.M + WG_BM - 1) / WG_BM;
+    p.tiles_n = (s.N + p.bn - 1) / p.bn;
+    p.kblocks[0] = (s.K[0] + TC_BK - 1) / TC_BK;
+    p.kB0[0] = x.kB0[0];
+    if (!make_map(&p.mapA[0], x.a[0], 64) || !make_map(&p.mapB, x.b, 64)) { c.err = cudaErrorInvalidValue; return; }
+    p.ksplit = nslabs;
+    p.epi = EPI_PARTIAL;
+    if (G.wg_slab) { p.C = G.wg_slab + G.wg_off[i]; p.split_stride = G.wg_stride; }
+    else { p.C = h->W() + h->ar.slabs + (s.C - h->buf.grads); p.split_stride = h->ar.slab_stride; }
+    p.ldc = s.ldc;
+    p.tile_start = total;
+    total += p.tiles_m * p.tiles_n * p.ksplit;
+  }
+  const int planes = t.passes == 3 ? 2 : 1;
+  const int stage_b = (bn_max + 63) / 64 * 8192;   // bytes of one B plane per stage: 64-column boxes
+  const int stage_bytes = planes * (2 * TC_STAGE_A + stage_b);
+  const int stages = std::min(8, (200 * 1024) / stage_bytes);
+  const int smem = stages * stage_bytes + 2 * stages * 8 + 1024;
+  if (!h->wgrad_attr_done) {
+    cudaFuncSetAttribute(tc_gemm_kernel_wgrad<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc_gemm_kernel_wgrad<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    h->wgrad_attr_done = true;
+  }
+  const int grid = std::min(total, budget);
+  if (planes == 2) launch_k(tc_gemm_kernel_wgrad<true>, grid, WG_THREADS, smem, c, t, total, stages, stage_b);
+  else launch_k(tc_gemm_kernel_wgrad<false>, grid, WG_THREADS, smem, c, t, total, stages, stage_b);
+}
+
+// Lower a forward or dgrad group onto wgmma: images instead of fp32 operands, TMA tensor maps, 64 x bn tiles.
+// `max_ctas` > 0: issue the group as several launches of at most that many CTAs (one CTA occupies an SM).
+static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas = 0) {
+  if (variant == V_WGRAD) { launch_tc_wgrad(h, G, c, max_ctas); return; }
+  TcGroup& t = h->tc_scratch;
+  memset(&t, 0, sizeof(t));
+  t.n = G.n;
+  t.passes = h->passes();
+  const bool b_mn = variant != V_FWD;
   int grid = 0;
   int bn_max = 16;
-  int wg_bn = 128;
-  if (variant == V_WGRAD) {  // a launch that would leave most SMs idle at 128-wide tiles gets 64-wide ones
-    int ctas = 0;
-    for (int i = 0; i < G.n; ++i) ctas += ((G.prob(i).M + TC_BM - 1) / TC_BM) * ((G.prob(i).N + 127) / 128) * (G.wg_slab ? G.wg_nslabs : h->ar.nslabs);
-    if (ctas * 2 <= h->num_sms) wg_bn = 64;
-  }
   for (int i = 0; i < G.n; ++i) {
     const GemmProb& s = G.prob(i);
     const TcExtra& x = G.x[i];
@@ -402,7 +458,6 @@ static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas 
     p.M = s.M; p.N = s.N;
     int bn = (s.N + 15) / 16 * 16;
     if (bn > 256) bn = 256;
-    if (variant == V_WGRAD && bn > wg_bn) bn = wg_bn;  // more tiles for the (few, batch-split) weight-gradient problems
     p.bn = bn;
     if (bn > bn_max) bn_max = bn;
     p.tiles_m = (s.M + TC_BM - 1) / TC_BM;
@@ -410,21 +465,12 @@ static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas 
     for (int sgm = 0; sgm < 2; ++sgm) {
       p.kblocks[sgm] = (s.K[sgm] + TC_BK - 1) / TC_BK;
       p.kB0[sgm] = x.kB0[sgm];
-      if (s.K[sgm] > 0 && !make_map(&p.mapA[sgm], x.a[sgm], a_mn ? 64 : TC_BM)) { c.err = cudaErrorInvalidValue; return; }
+      if (s.K[sgm] > 0 && !make_map(&p.mapA[sgm], x.a[sgm], TC_BM)) { c.err = cudaErrorInvalidValue; return; }
     }
     if (!make_map(&p.mapB, x.b, b_mn ? 64 : bn)) { c.err = cudaErrorInvalidValue; return; }
     p.ksplit = 1;
     p.C = s.C; p.ldc = s.ldc; p.bias = s.bias; p.Zout = s.Zout; p.Zin = s.Zin; p.ldz = s.ldz; p.colsum = s.colsum;
     p.epi = s.epi; p.act = s.act;
-    if (variant == V_WGRAD) {  // fixed slab count: empty splits store zeros so that the reduction is always valid
-      p.epi = EPI_PARTIAL;
-      if (G.wg_slab) { p.ksplit = G.wg_nslabs; p.C = G.wg_slab + G.wg_off[i]; p.split_stride = G.wg_stride; }
-      else {
-        p.ksplit = h->ar.nslabs;
-        p.C = h->W() + h->ar.slabs + (s.C - h->buf.grads);
-        p.split_stride = h->ar.slab_stride;
-      }
-    }
     if (x.out.p) {
       p.img = x.out.p; p.img_pitch = x.out.pitch; p.img_plane = x.out.plane;
       if (p.epi == EPI_BIAS_ACT || p.epi == EPI_DACT) p.C = nullptr;  // the next GEMM reads the image; no fp32 copy
@@ -444,10 +490,8 @@ static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas 
   if (!h->tc_attr_done) {
     cudaFuncSetAttribute(tc_gemm_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(tc_gemm_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(tc_gemm_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(tc_gemm_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(tc_gemm_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(tc_gemm_kernel<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     h->tc_attr_done = true;
   }
   const int total = grid;
@@ -461,12 +505,10 @@ static void launch_tc(MlpHandle* h, Group& G, int variant, Ctx& c, int max_ctas 
     if (t0 > 0) c.launches++;
     if (planes == 2) {
       if (variant == V_FWD) launch_k(tc_gemm_kernel<false, false, true>, n, TC_THREADS, smem, c, t, stages, stage_b);
-      else if (variant == V_DGRAD) launch_k(tc_gemm_kernel<false, true, true>, n, TC_THREADS, smem, c, t, stages, stage_b);
-      else launch_k(tc_gemm_kernel<true, true, true>, n, TC_THREADS, smem, c, t, stages, stage_b);
+      else launch_k(tc_gemm_kernel<false, true, true>, n, TC_THREADS, smem, c, t, stages, stage_b);
     } else {
       if (variant == V_FWD) launch_k(tc_gemm_kernel<false, false, false>, n, TC_THREADS, smem, c, t, stages, stage_b);
-      else if (variant == V_DGRAD) launch_k(tc_gemm_kernel<false, true, false>, n, TC_THREADS, smem, c, t, stages, stage_b);
-      else launch_k(tc_gemm_kernel<true, true, false>, n, TC_THREADS, smem, c, t, stages, stage_b);
+      else launch_k(tc_gemm_kernel<false, true, false>, n, TC_THREADS, smem, c, t, stages, stage_b);
     }
   }
   grid = total;
@@ -2538,6 +2580,8 @@ int dsact_test_gemm(dsact_handle* hh, int32_t variant, const dsact_test_layer* p
     if (variant == V_WGRAD) {
       G.wg_slab = static_cast<float*>(mem.get(sizeof(float) * (size_t)nslabs * slab_floats));
       G.wg_stride = slab_floats; G.wg_nslabs = nslabs;
+      // NaN: a slab element the kernel leaves unwritten reaches C
+      if (G.wg_slab) c.err = cudaMemsetAsync(G.wg_slab, 0xff, sizeof(float) * (size_t)nslabs * slab_floats, c.s);
     }
   }
   if (mem.err == cudaSuccess) launch_group(h, G, variant, c, max_ctas);

@@ -13,7 +13,9 @@
 //   forward  y  = x W^T   : A K-major (x image),   B K-major  (W image)
 //   dgrad    dx = dy W    : A K-major (dy image),  B MN-major (W image)
 //   wgrad    dW = dy^T x  : A MN-major (dy image), B MN-major (x image); split over the batch, each split
-//                           stores its partial tile to a workspace slab (no atomics), reduced later.
+//                           stores its partial tile to a workspace slab (no atomics), reduced later.  The step's
+//                           weight gradients run on the persistent 128-row kernel of wgrad_tc.cuh, which reads the
+//                           same images with the same tensor maps.
 #pragma once
 #include <stdio.h>
 #include <cuda.h>
