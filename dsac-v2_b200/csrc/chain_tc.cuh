@@ -98,6 +98,15 @@ __device__ __forceinline__ void chain_layer(const ChainGroup& g, const ChainPass
   for (int i = 0; i < 32 * NB; ++i) acc[i] = 0.f;
   int prev = -1;
   for (int kb = 0; kb < nkb; ++kb) {
+    // When k-block kb has not landed yet, the MMAs of kb - 1 retire before it does: drain them and release kb - 1's slot
+    // now, so that the producer loads kb + 1 while kb is still in flight.  With two stages, releasing only after kb is
+    // issued leaves one load in flight, and the layer's MMA phase is set by the load latency.  The four-stage ring of
+    // one plane already has three loads in flight; draining there only loses the MMA overlap.
+    if (stages == 2 && prev >= 0 && !__all_sync(0xffffffffu, mbar_test(&full[stage], phase))) {
+      wg_wait<0>();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      prev = -1;
+    }
     mbar_wait(&full[stage], phase);
     if (j == 0 && kb == 0 && threadIdx.x == 0) TC_STAMP(2);
     // this warpgroup's columns of the stage: K-major rows of 128 B, MN-major 64-column boxes of 8 KiB (1024-byte aligned)
