@@ -180,6 +180,9 @@ SYMBOLS = {
     "dsact_test_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TestLayer), C.c_int32, C.c_int32, C.c_void_p]),
     "dsact_test_chain": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_void_p, C.POINTER(TestChainPass), C.c_int32, C.c_void_p]),
+    "dsact_test_chain_tiling": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_int32,
+                                          C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(TestChainPass), C.c_int32,
+                                          C.c_void_p]),
     "dsact_test_rows": (C.c_int, [C.c_void_p, C.POINTER(TestRowIo), C.c_void_p]),
     "dsact_test_apply": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]),
     "dsact_test_dp_attach": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),

@@ -23,7 +23,7 @@
 #include "gemm_simt.cuh"
 #include "kernels.cuh"
 #include "tc_host.cuh"
-#include "chain_tc.cuh"
+#include "chain_pp.cuh"
 #include "wgrad_tc.cuh"
 #include "dp_peer.cuh"
 
@@ -679,6 +679,7 @@ struct ChainBuild {
   ChainGroup g;
   int grid = 0, stage_b = 16 * 128;
   int b_mn = -1;   // B orientation, one per launch: forward chains K-major, dgrad chains MN-major
+  Img w[CH_MAX_PASSES][CH_MAX_LAYERS];   // each layer's weight image (the ping-pong kernel's K-major maps differ)
   double flops = 0.0;
   bool ok = true;
   explicit ChainBuild(int passes) { memset(&g, 0, sizeof(g)); g.passes = passes; }
@@ -699,6 +700,7 @@ struct ChainBuild {
     L.kblocks[0] = (K0 + TC_BK - 1) / TC_BK; L.kblocks[1] = (K1 + TC_BK - 1) / TC_BK;
     L.kB0[0] = 0; L.kB0[1] = kB1;
     ok = ok && make_map(&L.mapB, wimg, b_mn ? 64 : L.bn);
+    w[&P - g.p][P.n_layers - 1] = wimg;
     const int sb = (L.bn + 63) / 64 * 8192;   // the wgmma N (64 multiple) reads that many rows of a K-major tile
     if (sb > stage_b) stage_b = sb;
     flops += 2.0 * P.M * N * ((double)K0 + K1);
@@ -713,7 +715,12 @@ struct ChainBuild {
   }
 };
 
-static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
+// The layer-chain kernel of a launch: the column split (tc_chain_kernel, one 64-row tile per CTA) when its grid fits one
+// wave, the ping-pong kernel (tc_pingpong_kernel, two tiles per CTA) when it needs more.  `tiling` (tests): 0 / 1 forces
+// the column split / the ping-pong kernel, -1 selects by shape.
+enum { CHAIN_BY_SHAPE = -1, CHAIN_COLUMN_SPLIT = 0, CHAIN_PINGPONG = 1 };
+
+static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c, int tiling = CHAIN_BY_SHAPE) {
   if (cb.g.n == 0) return;
   for (int i = 0; i < cb.g.n; ++i)
     for (int j = 0; j < cb.g.p[i].n_layers; ++j)
@@ -726,14 +733,39 @@ static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
   const int planes = cb.g.passes == 3 ? 2 : 1;
   const int stages = planes == 2 ? 2 : 4;   // layer 0's A ring lives in the 4-k-block operand buffer
   const int smem = chain_smem_bytes(stages, planes, cb.stage_b);
+  const int pp_smem = pp_smem_bytes(stages, planes);
   if (!h->chain_attr_done) {
     cudaFuncSetAttribute(tc_chain_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(tc_chain_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(tc_chain_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(tc_chain_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaFuncSetAttribute(tc_pingpong_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    cudaFuncSetAttribute(tc_pingpong_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    cudaFuncSetAttribute(tc_pingpong_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    cudaFuncSetAttribute(tc_pingpong_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
     h->chain_attr_done = true;
   }
-  if (planes == 2) {
+  if (tiling == CHAIN_BY_SHAPE) {   // the column split's resident CTAs on the device
+    int per_sm = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc_chain_kernel<true, false>, CH_THREADS, smem);
+    if (e != cudaSuccess) { c.err = e; return; }
+    tiling = cb.grid > std::max(per_sm, 1) * h->num_sms ? CHAIN_PINGPONG : CHAIN_COLUMN_SPLIT;
+  }
+  if (tiling == CHAIN_PINGPONG) {
+    // K-major weight maps load one column half (min(bn, 128) weight rows) per ring stage
+    for (int i = 0; i < cb.g.n && !cb.b_mn; ++i)
+      for (int j = 0; j < cb.g.p[i].n_layers; ++j)
+        if (cb.g.p[i].L[j].bn > PP_HALF && !make_map(&cb.g.p[i].L[j].mapB, cb.w[i][j], PP_HALF)) { c.err = cudaErrorInvalidValue; return; }
+    int ctas = 0;
+    for (int i = 0; i < cb.g.n; ++i) ctas += (cb.g.p[i].M + 2 * TC_BM - 1) / (2 * TC_BM);
+    if (planes == 2) {
+      if (cb.b_mn) launch_k(tc_pingpong_kernel<true, true>, ctas, PP_THREADS, pp_smem, c, cb.g, stages);
+      else launch_k(tc_pingpong_kernel<true, false>, ctas, PP_THREADS, pp_smem, c, cb.g, stages);
+    } else {
+      if (cb.b_mn) launch_k(tc_pingpong_kernel<false, true>, ctas, PP_THREADS, pp_smem, c, cb.g, stages);
+      else launch_k(tc_pingpong_kernel<false, false>, ctas, PP_THREADS, pp_smem, c, cb.g, stages);
+    }
+  } else if (planes == 2) {
     if (cb.b_mn) launch_k(tc_chain_kernel<true, true>, cb.grid, CH_THREADS, smem, c, cb.g, stages, cb.stage_b);
     else launch_k(tc_chain_kernel<true, false>, cb.grid, CH_THREADS, smem, c, cb.g, stages, cb.stage_b);
   } else {
@@ -752,14 +784,21 @@ static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c) {
       if (d[0] < tmin) tmin = d[0];
       if (d[6] > tmax) tmax = d[6];
     }
-    fprintf(stderr, "[chain_debug] class %d passes %d grid %d span %.1f us\n", cls, cb.g.n, cb.grid, (tmax - tmin) / 1000.0);
-    for (int pi = 0; pi < cb.g.n; ++pi) {  // first CTA of every pass: per-layer timeline relative to its start (us)
-      const unsigned long long* d = &hbuf[TC_DBG_SLOTS * (size_t)cb.g.p[pi].tile_start];
-      fprintf(stderr, "  pass %d: setup %.1f first-load %.1f |", pi, (d[1] - d[0]) / 1e3, (d[2] - d[0]) / 1e3);
-      for (int j = 0; j < cb.g.p[pi].n_layers; ++j)
-        fprintf(stderr, " L%d mma-done %.1f epilogue %.1f operand %.1f |", j, (d[8 + 3 * j] - d[0]) / 1e3, (d[9 + 3 * j] - d[0]) / 1e3,
-                (d[10 + 3 * j] - d[0]) / 1e3);
-      fprintf(stderr, " end %.1f\n", (d[6] - d[0]) / 1e3);
+    fprintf(stderr, "[chain_debug] class %d passes %d grid %d span %.1f us %s\n", cls, cb.g.n, cb.grid, (tmax - tmin) / 1000.0,
+            tiling == CHAIN_PINGPONG ? "ping-pong" : "column split");
+    // first CTA of every pass (ping-pong: both of its tiles, one per warpgroup): per-layer timeline relative to the CTA's
+    // start (us)
+    for (int pi = 0; pi < cb.g.n; ++pi) {
+      const int t0 = cb.g.p[pi].tile_start, tend = pi + 1 < cb.g.n ? cb.g.p[pi + 1].tile_start : cb.grid;
+      const unsigned long long* d0 = &hbuf[TC_DBG_SLOTS * (size_t)t0];
+      for (int t = t0; t < (tiling == CHAIN_PINGPONG ? std::min(t0 + 2, tend) : t0 + 1); ++t) {
+        const unsigned long long* d = &hbuf[TC_DBG_SLOTS * (size_t)t];
+        fprintf(stderr, "  pass %d tile %d: setup %.1f first-load %.1f |", pi, t - t0, (d[1] - d0[0]) / 1e3, (d[2] - d0[0]) / 1e3);
+        for (int j = 0; j < cb.g.p[pi].n_layers; ++j)
+          fprintf(stderr, " L%d mma-done %.1f epilogue %.1f operand %.1f |", j, (d[8 + 3 * j] - d0[0]) / 1e3,
+                  (d[9 + 3 * j] - d0[0]) / 1e3, (d[10 + 3 * j] - d0[0]) / 1e3);
+        fprintf(stderr, " end %.1f\n", (d[6] - d0[0]) / 1e3);
+      }
     }
   }
 }
@@ -2596,8 +2635,9 @@ int dsact_test_gemm(dsact_handle* hh, int32_t variant, const dsact_test_layer* p
   return finish_hook(h, c, mem);
 }
 
-int dsact_test_chain(dsact_handle* hh, int32_t dgrad, int32_t L, const int32_t* sizes, int32_t K0, int32_t K1, int32_t kB1,
-                     int32_t act, const float* params, const dsact_test_chain_pass* passes, int32_t n_passes, void* stream) {
+static int test_chain(dsact_handle* hh, int tiling, int32_t dgrad, int32_t L, const int32_t* sizes, int32_t K0, int32_t K1,
+                      int32_t kB1, int32_t act, const float* params, const dsact_test_chain_pass* passes, int32_t n_passes,
+                      void* stream) {
   if (!hh) return fail(DSACT_EINVAL, "null handle");
   int rc = check_mlp(hh, "dsact_test_chain");
   if (rc) return rc;
@@ -2659,9 +2699,22 @@ int dsact_test_chain(dsact_handle* hh, int32_t dgrad, int32_t L, const int32_t* 
   }
   if (mem.err == cudaSuccess) {
     ibt.launch(h, c);
-    launch_chain(h, cb, dgrad ? CLS_GEMM_DGRAD : CLS_GEMM_FWD, c);
+    launch_chain(h, cb, dgrad ? CLS_GEMM_DGRAD : CLS_GEMM_FWD, c, tiling);
   }
   return finish_hook(h, c, mem);
+}
+
+int dsact_test_chain(dsact_handle* h, int32_t dgrad, int32_t L, const int32_t* sizes, int32_t K0, int32_t K1, int32_t kB1,
+                     int32_t act, const float* params, const dsact_test_chain_pass* passes, int32_t n_passes, void* stream) {
+  return test_chain(h, CHAIN_BY_SHAPE, dgrad, L, sizes, K0, K1, kB1, act, params, passes, n_passes, stream);
+}
+
+int dsact_test_chain_tiling(dsact_handle* h, int32_t tiling, int32_t dgrad, int32_t L, const int32_t* sizes, int32_t K0,
+                            int32_t K1, int32_t kB1, int32_t act, const float* params, const dsact_test_chain_pass* passes,
+                            int32_t n_passes, void* stream) {
+  if (tiling != CHAIN_COLUMN_SPLIT && tiling != CHAIN_PINGPONG)
+    return fail(DSACT_EINVAL, "dsact_test_chain_tiling: tiling %d is neither 0 (column split) nor 1 (ping-pong)", tiling);
+  return test_chain(h, tiling, dgrad, L, sizes, K0, K1, kB1, act, params, passes, n_passes, stream);
 }
 
 static int sync_hook(dsact_handle* h, Ctx& c) {

@@ -563,9 +563,11 @@ class Engine:
         with torch.cuda.device(self.device):
             check(self.lib.dsact_test_gemm(self.h, variant, arr, len(probs), max_ctas, self._stream()))
 
-    def test_chain(self, dgrad: bool, sizes, K0: int, K1: int, kB1: int, act: int, params: torch.Tensor, passes):
+    def test_chain(self, dgrad: bool, sizes, K0: int, K1: int, kB1: int, act: int, params: torch.Tensor, passes,
+                   tiling: Optional[int] = None):
         """dsact_test_chain: one launch of the layer-chain kernel; `passes` are dicts of dsact_test_chain_pass fields
-        (Zout / Zin / img / colsum: lists per hidden layer, entries may be None; `img` entries [2, M, pitch] bf16)."""
+        (Zout / Zin / img / colsum: lists per hidden layer, entries may be None; `img` entries [2, M, pitch] bf16).
+        `tiling` (dsact_test_chain_tiling): 0 = the column-split kernel, 1 = the ping-pong kernel, None = by shape."""
         arr = (_lib.TestChainPass * len(passes))()
         for t, p in zip(arr, passes):
             t.M = p["M"]
@@ -577,8 +579,12 @@ class Engine:
                     getattr(t, k)[j] = _ptr(v)
         sz = (C.c_int32 * len(sizes))(*sizes)
         with torch.cuda.device(self.device):
-            check(self.lib.dsact_test_chain(self.h, int(dgrad), len(sizes) - 2, sz, K0, K1, kB1, act, params.data_ptr(), arr,
-                                            len(passes), self._stream()))
+            if tiling is None:
+                check(self.lib.dsact_test_chain(self.h, int(dgrad), len(sizes) - 2, sz, K0, K1, kB1, act, params.data_ptr(),
+                                                arr, len(passes), self._stream()))
+            else:
+                check(self.lib.dsact_test_chain_tiling(self.h, int(tiling), int(dgrad), len(sizes) - 2, sz, K0, K1, kB1, act,
+                                                       params.data_ptr(), arr, len(passes), self._stream()))
 
     def test_rows(self, kernel: str, batch: int, global_batch: Optional[int] = None, max_blocks: int = 0,
                   advance_rng: bool = False, **arrays):

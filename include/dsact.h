@@ -379,6 +379,11 @@ typedef struct dsact_test_chain_pass {
 } dsact_test_chain_pass;
 int dsact_test_chain(dsact_handle *h, int32_t dgrad, int32_t L, const int32_t *sizes, int32_t K0, int32_t K1, int32_t kB1,
                      int32_t act, const float *params, const dsact_test_chain_pass *passes, int32_t n_passes, void *stream);
+/* dsact_test_chain_tiling: the same launch on a chosen layer-chain kernel instead of the one the launch shape selects:
+ * tiling 0 = the column split (one 64-row tile per CTA), 1 = the ping-pong kernel (two 64-row tiles per CTA). */
+int dsact_test_chain_tiling(dsact_handle *h, int32_t tiling, int32_t dgrad, int32_t L, const int32_t *sizes, int32_t K0,
+                            int32_t K1, int32_t kB1, int32_t act, const float *params, const dsact_test_chain_pass *passes,
+                            int32_t n_passes, void *stream);
 
 /* Test hooks of the step kernels between the networks, on both engines: the step's own launch code (grid sizing and
  * argument construction) with the per-row arrays taken from caller buffers instead of the workspace.  Hyperparameters
