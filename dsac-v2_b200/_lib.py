@@ -99,6 +99,12 @@ class Replay(C.Structure):
                 ("capacity", C.c_int64)]
 
 
+class FrameReplay(C.Structure):
+    """dsact_frame_replay: the frame ring (include/dsact.h)."""
+    _fields_ = [("frames", _fp), ("obs_frames", _fp), ("obs2_frames", _fp), ("act", _fp), ("rew", _fp), ("done", _fp),
+                ("logp", _fp), ("capacity", C.c_int64), ("frame_capacity", C.c_int64), ("frames_per_obs", C.c_int32)]
+
+
 class TestLayer(C.Structure):
     """dsact_test_layer: one problem of a dsact_test_gemm group."""
     _fields_ = [("M", C.c_int32), ("N", C.c_int32), ("K0", C.c_int32), ("K1", C.c_int32), ("kB1", C.c_int32),
@@ -160,6 +166,9 @@ SYMBOLS = {
     "dsact_read_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "dsact_replay_bind": (C.c_int, [C.c_void_p, C.POINTER(Replay)]),
     "dsact_replay_add": (C.c_int, [C.c_void_p] + [C.c_void_p] * 6 + [C.c_int64, C.c_int64, C.c_void_p]),
+    "dsact_replay_bind_frames": (C.c_int, [C.c_void_p, C.POINTER(FrameReplay)]),
+    "dsact_replay_add_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 6
+                                + [C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_replay_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Batch), C.c_void_p]),
     "dsact_replay_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_int64, C.c_void_p]),
     "dsact_replay_steps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_void_p,

@@ -206,6 +206,8 @@ struct dsact_handle {
   int64_t dev_iter = -1;     // what state[ST_ITER] will hold when the next enqueued work runs (-1 unknown)
   int64_t dev_rb_size = -1;  // what state[ST_RB_SIZE] holds
   dsact_replay rb = {};
+  dsact_frame_replay fr = {};   // the frame ring, when rb_frames (binding either ring kind replaces the other)
+  bool rb_frames = false;
   DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   int32_t pending_batch = 0; // rows of the shard phase1 processed (phase2 must match)
   dsact_batch pending = {};  // batch pointers of phase1
@@ -214,6 +216,7 @@ struct dsact_handle {
   int32_t last_launches = 0;
   explicit dsact_handle(int e) : engine(e) {}
   float* W() const { return reinterpret_cast<float*>(buf.workspace); }
+  int64_t rb_rows() const { return rb_frames ? fr.capacity : rb.capacity; }
 };
 
 struct MlpHandle : dsact_handle {
@@ -1329,9 +1332,18 @@ static void enqueue_gather(const dsact_handle* h, int B, const int64_t* idx, con
     for (int i = 0; i < 6; ++i) d[i] = const_cast<float*>(o[i]);
   }
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
-  launch_k(gather_kernel, blocks, 256, 0, c, h->rb.obs, h->rb.obs2, h->rb.act, h->rb.rew, h->rb.done, h->rb.logp, idx,
-           d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
-           img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0);
+  if (h->rb_frames) {
+    const dsact_frame_replay& r = h->fr;
+    launch_k(gather_kernel<true>, blocks, 256, 0, c, (const float*)r.frames, (const float*)r.frames, r.act, r.rew, r.done,
+             r.logp, idx, d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
+             img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0,
+             (const int32_t*)r.obs_frames, (const int32_t*)r.obs2_frames, (int)r.frames_per_obs);
+  } else {
+    launch_k(gather_kernel<false>, blocks, 256, 0, c, h->rb.obs, h->rb.obs2, h->rb.act, h->rb.rew, h->rb.done, h->rb.logp, idx,
+             d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
+             img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0,
+             (const int32_t*)nullptr, (const int32_t*)nullptr, 1);
+  }
   c.done();
   c.check();
 }
@@ -1903,7 +1915,7 @@ static int sync_iteration(dsact_handle* h, int64_t iteration, cudaStream_t s) {
 }
 
 static int sync_rb_size(dsact_handle* h, int64_t size, cudaStream_t s) {
-  if (size < 1 || size > h->rb.capacity) return fail(DSACT_EINVAL, "size %lld outside [1, capacity]", (long long)size);
+  if (size < 1 || size > h->rb_rows()) return fail(DSACT_EINVAL, "size %lld outside [1, capacity]", (long long)size);
   if (h->dev_rb_size != size) {
     set_rb_size_kernel<<<1, 32, 0, s>>>(h->buf.state, size);
     CUDA_TRY(cudaGetLastError());
@@ -2286,13 +2298,81 @@ int dsact_replay_bind(dsact_handle* h, const dsact_replay* rb) {
     return fail(DSACT_EINVAL, "bad replay buffers");
   h->rb = *rb;
   h->rb_bound = true;
+  h->rb_frames = false;
   if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
+  return DSACT_OK;
+}
+
+int dsact_replay_bind_frames(dsact_handle* h, const dsact_frame_replay* rb) {
+  if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
+  const int64_t K = rb->frames_per_obs;
+  if (K < 1 || K > 64 || h->obs_elems % K != 0)
+    return fail(DSACT_EINVAL, "frames_per_obs %lld must be in [1, 64] and divide obs_elems %lld", (long long)K,
+                (long long)h->obs_elems);
+  if (rb->frame_capacity < K || rb->frame_capacity > 0x7fffffff)
+    return fail(DSACT_EINVAL, "frame_capacity %lld outside [frames_per_obs, 2^31 - 1]", (long long)rb->frame_capacity);
+  if (rb->capacity < 1) return fail(DSACT_EINVAL, "capacity %lld < 1", (long long)rb->capacity);
+  if (!rb->frames || !rb->obs_frames || !rb->obs2_frames || !rb->act || !rb->rew || !rb->done || !rb->logp)
+    return fail(DSACT_EINVAL, "null frame-ring pointer");
+  h->fr = *rb;
+  h->rb_bound = true;
+  h->rb_frames = true;
+  if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
+  return DSACT_OK;
+}
+
+// the first n entries of a HOST frame-id table (nullptr: not host memory, or an id outside [0, frame_capacity))
+static const char* check_frame_ids(const int32_t* ids, int64_t n, int64_t frame_capacity) {
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, ids) != cudaSuccess) { cudaGetLastError(); return "not a valid pointer"; }
+  if (at.type == cudaMemoryTypeDevice) return "device memory (frame-id tables must be host memory)";
+  for (int64_t i = 0; i < n; ++i)
+    if (ids[i] < 0 || ids[i] >= frame_capacity) return "an id outside [0, frame_capacity)";
+  return nullptr;
+}
+
+int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_frames, int64_t frame_ptr,
+                            const int32_t* obs_frames, const int32_t* obs2_frames, const float* act, const float* rew,
+                            const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
+  if (!h || !h->rb_bound || !h->rb_frames) return fail(DSACT_ESTATE, "frame replay ring not bound");
+  const dsact_frame_replay& r = h->fr;
+  if (n < 0 || n > r.capacity || ptr < 0 || ptr >= r.capacity) return fail(DSACT_EINVAL, "bad n/ptr");
+  if (n_frames < 0 || n_frames > r.frame_capacity || frame_ptr < 0 || frame_ptr >= r.frame_capacity)
+    return fail(DSACT_EINVAL, "bad n_frames/frame_ptr");
+  if (n_frames > 0 && !frames) return fail(DSACT_EINVAL, "null frame staging pointer");
+  if (n > 0 && (!obs_frames || !obs2_frames || !act || !rew || !done || !logp)) return fail(DSACT_EINVAL, "null staging pointer");
+  const int64_t K = r.frames_per_obs;
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (n > 0) {   // the gather follows these ids: every one is checked before anything is copied
+    const char* bad = check_frame_ids(obs_frames, n * K, r.frame_capacity);
+    if (!bad) bad = check_frame_ids(obs2_frames, n * K, r.frame_capacity);
+    if (bad) return fail(DSACT_EINVAL, "frame-id table: %s", bad);
+  }
+  const cudaStream_t s = (cudaStream_t)stream;
+  // n items of w elements of `bytes` each from src into ring dst of `cap` items, starting at item p
+  auto put = [&](void* dst, const void* src, int64_t cnt, int64_t p, int64_t cap, int64_t w, size_t bytes) -> cudaError_t {
+    const int64_t first = (p + cnt <= cap) ? cnt : cap - p;
+    cudaError_t e = cudaMemcpyAsync((char*)dst + p * w * bytes, src, first * w * bytes, cudaMemcpyDefault, s);
+    if (e == cudaSuccess && first < cnt)
+      e = cudaMemcpyAsync(dst, (const char*)src + first * w * bytes, (cnt - first) * w * bytes, cudaMemcpyDefault, s);
+    return e;
+  };
+  if (n_frames > 0) CUDA_TRY(put(r.frames, frames, n_frames, frame_ptr, r.frame_capacity, h->obs_elems / K, sizeof(float)));
+  if (n > 0) {
+    CUDA_TRY(put(r.obs_frames, obs_frames, n, ptr, r.capacity, K, sizeof(int32_t)));
+    CUDA_TRY(put(r.obs2_frames, obs2_frames, n, ptr, r.capacity, K, sizeof(int32_t)));
+    CUDA_TRY(put(r.act, act, n, ptr, r.capacity, h->act_dim, sizeof(float)));
+    CUDA_TRY(put(r.rew, rew, n, ptr, r.capacity, 1, sizeof(float)));
+    CUDA_TRY(put(r.done, done, n, ptr, r.capacity, 1, sizeof(float)));
+    CUDA_TRY(put(r.logp, logp, n, ptr, r.capacity, 1, sizeof(float)));
+  }
   return DSACT_OK;
 }
 
 int dsact_replay_add(dsact_handle* h, const float* obs, const float* obs2, const float* act, const float* rew,
                      const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
   if (!h || !h->rb_bound) return fail(DSACT_ESTATE, "replay buffer not bound");
+  if (h->rb_frames) return fail(DSACT_ESTATE, "a frame replay ring is bound: rows go in through dsact_replay_add_frames");
   if (n < 0 || n > h->rb.capacity || ptr < 0 || ptr >= h->rb.capacity) return fail(DSACT_EINVAL, "bad n/ptr");
   if (n == 0) return DSACT_OK;
   if (!obs || !obs2 || !act || !rew || !done || !logp) return fail(DSACT_EINVAL, "null staging pointer");

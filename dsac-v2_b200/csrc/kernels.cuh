@@ -198,17 +198,28 @@ __device__ __forceinline__ int64_t replay_index(int row, uint32_t step, int64_t 
   return (int64_t)__umul64hi(a, (uint64_t)size);
 }
 // Replay gather (training/replay_buffer.py:87-90): one warp per sampled row, vectorised over obs columns.
+// FRAMES = false: the flat ring (dsact_replay), rows r_obs / r_obs2 [capacity, O].
+// FRAMES = true: the frame ring (dsact_frame_replay): r_obs = r_obs2 = the frame store [frame_capacity, F = O / K]; frame
+// k of row src's obs is frame f_obs[src * K + k] (obs2: f_obs2), i.e. floats [k * F, (k + 1) * F) of the observation.
+template <bool FRAMES>
 __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __restrict__ r_obs2,
                               const float* __restrict__ r_act, const float* __restrict__ r_rew,
                               const float* __restrict__ r_done, const float* __restrict__ r_logp,
                               const int64_t* __restrict__ idx, float* __restrict__ obs, float* __restrict__ obs2,
                               float* __restrict__ act, float* __restrict__ rew, float* __restrict__ done,
                               float* __restrict__ logp, int B, int O, int A, ImgOut i_obs, ImgOut i_obs2, ImgOut i_act,
-                              int64_t* __restrict__ draw_idx, uint64_t seed, const float* __restrict__ state, int write_f32) {
+                              int64_t* __restrict__ draw_idx, uint64_t seed, const float* __restrict__ state, int write_f32,
+                              const int32_t* __restrict__ f_obs, const int32_t* __restrict__ f_obs2, int K) {
   pdl_sync();
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
-  const bool v4 = (O & 3) == 0;
+  const int F = FRAMES ? O / K : O;   // floats of one frame (a float4 never straddles two frames when F % 4 == 0)
+  const bool v4 = (F & 3) == 0;
+  // address of float e of row src's observation in the frame store (row slots `fs`)
+  auto frame_at = [&](const int32_t* fs, int e) {
+    const int k = e / F;
+    return r_obs + (int64_t)__ldg(fs + k) * F + (e - k * F);
+  };
   // draw_idx != null: no index list was given; every warp draws its row's index itself  and records it in draw_idx
   uint32_t step = 0;
   int64_t size = 1;
@@ -227,6 +238,8 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
     }
     const float* so = r_obs + src * O;
     const float* so2 = r_obs2 + src * O;
+    const int32_t* fo = FRAMES ? f_obs + src * K : nullptr;
+    const int32_t* fo2 = FRAMES ? f_obs2 + src * K : nullptr;
     float* dobs = obs + (size_t)row * O;
     float* dobs2 = obs2 + (size_t)row * O;
     if (v4) {
@@ -237,7 +250,14 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
 #pragma unroll
         for (int u = 0; u < 3; ++u) {
           const int c = c0 + 32 * u;
-          if (c < O / 4) { a[u] = __ldg(reinterpret_cast<const float4*>(so) + c); b[u] = __ldg(reinterpret_cast<const float4*>(so2) + c); }
+          if (c < O / 4) {
+            if constexpr (FRAMES) {
+              a[u] = __ldg(reinterpret_cast<const float4*>(frame_at(fo, 4 * c)));
+              b[u] = __ldg(reinterpret_cast<const float4*>(frame_at(fo2, 4 * c)));
+            } else {
+              a[u] = __ldg(reinterpret_cast<const float4*>(so) + c); b[u] = __ldg(reinterpret_cast<const float4*>(so2) + c);
+            }
+          }
         }
 #pragma unroll
         for (int u = 0; u < 3; ++u) {
@@ -254,7 +274,9 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
       }
     } else {
       for (int c = lane; c < O; c += 32) {
-        const float a = __ldg(so + c), b = __ldg(so2 + c);
+        float a, b;
+        if constexpr (FRAMES) { a = __ldg(frame_at(fo, c)); b = __ldg(frame_at(fo2, c)); }
+        else { a = __ldg(so + c); b = __ldg(so2 + c); }
         if (write_f32) { dobs[c] = a; dobs2[c] = b; }
         img_put(i_obs, row, c, a); img_put(i_obs2, row, c, b);
       }

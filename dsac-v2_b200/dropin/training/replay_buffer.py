@@ -8,11 +8,19 @@ Uniform sampling with replacement, like `np.random.randint` (reference :86).
 `index_source="numpy"` draws the indices from numpy's global generator exactly as
 the reference does (same seed -> same minibatch rows); the default "device" draws
 them with Philox on the GPU.
+
+`dsact_replay_frames=K` stores each observation frame once instead (the frame ring, include/dsact.h): an observation
+is K frames of obs_elems / K floats (an NCHW image with K = C: one channel each; K = 1: the whole observation), and a
+row refers to the frames of the previous row's obs2 or of its own obs that it repeats (dsac_v2_b200/frame_plan.py).
+The minibatches are bit for bit those of the flat ring; the device memory is about half of it (K = 1, obs2_t = obs_{t+1})
+or less (stacked frames: one new frame per row).
 """
 __all__ = ["ReplayBuffer"]
 
 import numpy as np
 import torch
+
+from dsac_v2_b200.frame_plan import FramePlanner
 
 
 class ReplayBuffer:
@@ -32,6 +40,10 @@ class ReplayBuffer:
             raise NotImplementedError("additional_info fields are not supported by the device ring buffer")
         self.index_source = kwargs.get("dsact_index_source",
                                        "numpy" if kwargs.get("dsact_noise") == "reference" else "device")
+        self.frames_per_obs = kwargs.get("dsact_replay_frames")
+        self.planner = None
+        if self.frames_per_obs is not None:
+            self.planner = FramePlanner(self.max_size, int(self.frames_per_obs), self.obs_elems)
         self.ptr, self.size = 0, 0
         self.engine = None
         self._stage = None      # pinned staging buffers
@@ -46,13 +58,22 @@ class ReplayBuffer:
         if eng_obs != self.obs_elems or engine.cfg.act_dim != self.act_dim:
             raise ValueError("replay buffer and engine disagree on obs/act dimensions")
         self.engine = engine
-        engine.bind_replay(self.max_size)
         O, A = self.obs_elems, self.act_dim
         R = min(self._STAGE_ROWS if self.obs_shape is None else max(8, self._STAGE_ROWS * 400 // O), self.max_size)   # ~6 MB per staging set
         self._rows = R
         pin = lambda *s: torch.zeros(*s, dtype=torch.float32).pin_memory()
-        self._stage = [dict(obs=pin(R, O), obs2=pin(R, O), act=pin(R, A), rew=pin(R), done=pin(R), logp=pin(R))
-                       for _ in range(self._STAGES)]
+        if self.planner is None:
+            engine.bind_replay(self.max_size)
+            self._stage = [dict(obs=pin(R, O), obs2=pin(R, O), act=pin(R, A), rew=pin(R), done=pin(R), logp=pin(R))
+                           for _ in range(self._STAGES)]
+        else:
+            pl = self.planner
+            engine.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K)
+            ids = lambda: torch.zeros(R, pl.K, dtype=torch.int32).pin_memory()
+            # up to 2K new frames per row: the same bytes as the flat ring's obs + obs2 staging
+            self._stage = [dict(frames=pin(2 * R * pl.K, pl.F), obs_frames=ids(), obs2_frames=ids(), act=pin(R, A),
+                                rew=pin(R), done=pin(R), logp=pin(R)) for _ in range(self._STAGES)]
+            self._nframes, self._frame_ptr = 0, 0
         self._np = [{k: v.numpy() for k, v in s.items()} for s in self._stage]
         self._events = [None] * self._STAGES
         pending, self._pending = self._pending, []
@@ -65,7 +86,10 @@ class ReplayBuffer:
             return
         self.flush()
         torch.cuda.current_stream(old.device).synchronize()
-        new.bind_replay(self.max_size)
+        if self.planner is None:
+            new.bind_replay(self.max_size)
+        else:
+            new.bind_replay_frames(self.max_size, self.planner.frame_capacity, self.planner.K)
         for k, v in old.replay.items():
             new.replay[k].copy_(v)
         self.engine = new
@@ -79,19 +103,38 @@ class ReplayBuffer:
         return self.size
 
     def __get_RAM__(self):
-        """MB of device memory holding valid transitions."""
+        """MB of device memory holding valid transitions (frame ring: the frames they refer to, and their frame ids)."""
+        if self.planner is not None:
+            pl = self.planner
+            return (4 * pl.F * pl.held() + 4 * (2 * pl.K + self.act_dim + 3) * self.size) / 1e6
         row_bytes = 4 * (2 * self.obs_elems + self.act_dim + 3)
         return row_bytes * self.size / 1e6
 
     # ---- store ----------------------------------------------------------------------
     def _store_row(self, obs, act, rew, next_obs, done, logp):
+        if self.planner is not None:
+            plan = self.planner.plan(obs, next_obs)
+            if plan.need > self.planner.frame_capacity:
+                self._grow(self.planner.grown_capacity(plan.need))
+            # a flush copies at most frame_capacity frames: no two of its frames share a slot
+            if self._fill and self._nframes + len(plan.new) > self.planner.frame_capacity:
+                self.flush()
         if self._fill == self._rows:
             self.flush()
         if self._fill == 0 and self._events[self._cur] is not None:
             self._events[self._cur].synchronize()  # the async copy out of this staging buffer has finished
         s, i = self._np[self._cur], self._fill
-        s["obs"][i] = obs.reshape(-1)
-        s["obs2"][i] = next_obs.reshape(-1)
+        if self.planner is None:
+            s["obs"][i] = obs.reshape(-1)
+            s["obs2"][i] = next_obs.reshape(-1)
+        else:
+            _, slots, new, frame_ptr = self.planner.commit(plan)
+            K, m = self.planner.K, len(new)
+            if self._fill == 0:
+                self._frame_ptr = frame_ptr
+            s["frames"][self._nframes:self._nframes + m] = new
+            self._nframes += m
+            s["obs_frames"][i], s["obs2_frames"][i] = slots[:K], slots[K:]
         s["act"][i] = act
         s["rew"][i] = rew
         s["done"][i] = done
@@ -116,7 +159,12 @@ class ReplayBuffer:
         if self.engine is None or self._fill == 0:
             return
         n = self._fill
-        self.engine.replay_add(self._stage[self._cur], n, self.ptr)
+        if self.planner is None:
+            self.engine.replay_add(self._stage[self._cur], n, self.ptr)
+        else:
+            st = self._stage[self._cur]
+            self.engine.replay_add_frames(st["frames"], self._nframes, self._frame_ptr, st, n, self.ptr)
+            self._nframes = 0
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.engine.device))
         self._events[self._cur] = ev
@@ -124,21 +172,67 @@ class ReplayBuffer:
         self._cur = (self._cur + 1) % self._STAGES
         self._fill = 0
 
+    def _grow(self, frame_capacity: int):
+        """Move the frame store to `frame_capacity` slots: every live frame to its new slot, every row's ids rewritten."""
+        self.flush()
+        eng, pl = self.engine, self.planner
+        with torch.cuda.device(eng.device):
+            old = eng.replay
+            src, dst = (torch.from_numpy(x).to(eng.device) for x in pl.moves(frame_capacity))
+            eng.bind_replay_frames(self.max_size, frame_capacity, pl.K)
+            eng.replay["frames"][dst] = old["frames"][src]
+            for k in ("act", "rew", "done", "logp"):
+                eng.replay[k].copy_(old[k])
+            pl.frame_capacity = frame_capacity
+            self._put_ids()
+            torch.cuda.current_stream(eng.device).synchronize()   # `old` may go
+
+    def _put_ids(self):
+        slots = torch.from_numpy(self.planner.slots())
+        K = self.planner.K
+        self.engine.replay["obs_frames"].copy_(slots[:, :K])
+        self.engine.replay["obs2_frames"].copy_(slots[:, K:])
+
     # ---- full-state checkpoint (SURVEY §8f rank 3) ---------------------------------------
     def state_dict(self, with_data: bool = True) -> dict:
-        """ptr/size (+ the valid transitions, fetched from the device ring) for an exact resume."""
+        """ptr/size (+ the valid transitions, fetched from the device ring) for an exact resume.  Frame ring: the planner's
+        state and the frames its rows refer to, in serial order, instead of obs / obs2 rows."""
         self.flush()
         out = {"ptr": self.ptr, "size": self.size, "max_size": self.max_size}
+        if self.planner is not None:
+            out["frame_planner"] = self.planner.state_dict()
         if with_data and self.engine is not None:
             torch.cuda.current_stream(self.engine.device).synchronize()
-            out["data"] = {k: v[:self.size].cpu().clone() for k, v in self.engine.replay.items()}
+            if self.planner is None:
+                out["data"] = {k: v[:self.size].cpu().clone() for k, v in self.engine.replay.items()}
+            else:
+                r = self.engine.replay
+                src, _ = self.planner.moves(self.planner.frame_capacity)
+                out["data"] = {k: r[k][:self.size].cpu().clone() for k in ("act", "rew", "done", "logp")}
+                out["data"]["frames"] = r["frames"][torch.from_numpy(src).to(r["frames"].device)].cpu()
         return out
 
     def load_state_dict(self, state: dict) -> None:
         self._require_engine()
         if state["max_size"] != self.max_size:
             raise ValueError("replay capacity differs from the checkpoint")
+        if ("frame_planner" in state) != (self.planner is not None):
+            raise ValueError("the checkpoint's replay ring kind (flat / frame ring) differs from this buffer's")
         self.ptr, self.size, self._fill = int(state["ptr"]), int(state["size"]), 0
+        if self.planner is not None:
+            pl = self.planner
+            pl.load_state_dict(state["frame_planner"])
+            eng = self.engine
+            if eng.replay["frames"].shape[0] != pl.frame_capacity:
+                eng.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K)
+            self._nframes = 0
+            self._put_ids()
+            if "data" in state:
+                _, dst = pl.moves(pl.frame_capacity)
+                eng.replay["frames"][torch.from_numpy(dst).to(eng.device)] = state["data"]["frames"].to(eng.device)
+                for k in ("act", "rew", "done", "logp"):
+                    eng.replay[k][:self.size].copy_(state["data"][k])
+            return
         if "data" in state:
             for k, v in state["data"].items():
                 self.engine.replay[k][:self.size].copy_(v)

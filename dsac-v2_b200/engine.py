@@ -351,6 +351,42 @@ class Engine:
             check(self.lib.dsact_replay_bind(self.h, C.byref(rb)))
         self.capacity = int(capacity)
 
+    def bind_replay_frames(self, capacity: int, frame_capacity: int, frames_per_obs: int):
+        """Bind a frame ring (dsact_replay_bind_frames): `capacity` rows whose obs / obs2 are `frames_per_obs` (K) frame
+        ids each into a store of `frame_capacity` frames of obs_elems / K floats.  `replay` then holds `frames`,
+        `obs_frames`, `obs2_frames` (int32 [capacity, K]), `act`, `rew`, `done`, `logp`."""
+        O, A, K = self.obs_elems, self.cfg.act_dim, int(frames_per_obs)
+        capacity, frame_capacity = int(capacity), int(frame_capacity)
+        if not 1 <= K <= 64 or O % K:
+            raise ValueError(f"frames_per_obs {K} must be in [1, 64] and divide the observation's {O} floats")
+        if not K <= frame_capacity <= 2 ** 31 - 1 or capacity < 1:
+            raise ValueError(f"frame_capacity {frame_capacity} outside [{K}, 2^31 - 1] or capacity {capacity} < 1")
+        with torch.cuda.device(self.device):
+            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)
+            ids = lambda: torch.zeros(capacity, K, dtype=torch.int32, device=self.device)
+            self.replay = dict(frames=z(frame_capacity, O // K), obs_frames=ids(), obs2_frames=ids(), act=z(capacity, A),
+                               rew=z(capacity), done=z(capacity), logp=z(capacity))
+            r = self.replay
+            rb = _lib.FrameReplay(*(r[k].data_ptr() for k in ("frames", "obs_frames", "obs2_frames", "act", "rew", "done",
+                                                              "logp")), capacity, frame_capacity, K)
+            check(self.lib.dsact_replay_bind_frames(self.h, C.byref(rb)))
+        self.capacity = capacity
+
+    def replay_add_frames(self, frames: Optional[torch.Tensor], n_frames: int, frame_ptr: int, rows: Dict[str, torch.Tensor],
+                          n: int, ptr: int):
+        """dsact_replay_add_frames: `n_frames` frames (contiguous fp32, host or device) -> frame slots
+        (frame_ptr + i) % frame_capacity; rows' `obs_frames` / `obs2_frames` (contiguous int32 HOST tensors [n, K]) and
+        `act`, `rew`, `done`, `logp` (host or device) -> rows (ptr + i) % capacity."""
+        r = rows
+        for k in ("obs_frames", "obs2_frames"):
+            if r[k].device.type != "cpu" or r[k].dtype != torch.int32 or not r[k].is_contiguous():
+                raise ValueError(f"{k} must be a contiguous int32 host tensor")
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_replay_add_frames(self.h, _ptr(frames), int(n_frames), int(frame_ptr),
+                                                   r["obs_frames"].data_ptr(), r["obs2_frames"].data_ptr(),
+                                                   r["act"].data_ptr(), r["rew"].data_ptr(), r["done"].data_ptr(),
+                                                   r["logp"].data_ptr(), int(n), int(ptr), self._stream()))
+
     def replay_add(self, staging: Dict[str, torch.Tensor], n: int, ptr: int):
         """Rows of contiguous fp32 staging tensors (pinned host or device) -> ring rows (ptr+i) % capacity."""
         s = staging

@@ -198,6 +198,31 @@ int dsact_replay_bind(dsact_handle *h, const dsact_replay *rb);
 int dsact_replay_add(dsact_handle *h, const float *obs, const float *obs2, const float *act,
                      const float *rew, const float *done, const float *logp,
                      int64_t n, int64_t ptr, void *stream);
+/* ---- frame replay ring: each observation frame stored once ----
+ * The flat ring above stores obs and obs2 of every row as separate copies, although obs2 of row t is usually obs of row
+ * t + 1 (and, with stacked frames, obs2 is obs shifted by one frame).  This ring stores frames instead: an observation
+ * of O = obs_elems floats is K = frames_per_obs frames of F = O / K floats, frame k being floats [k*F, (k+1)*F) (for an
+ * NCHW image and K = C, one channel).  Row r's obs is frames[obs_frames[r*K + k]], k = 0..K-1; obs2 likewise through
+ * obs2_frames.  Which frames rows share is the caller's decision; every gather reads the ring that is bound, and yields
+ * bit for bit the rows a flat ring holding the same observations would.
+ * dsact_replay_bind_frames: DSACT_EINVAL unless frames_per_obs is in [1, 64] and divides obs_elems, frame_capacity is in
+ * [frames_per_obs, 2^31 - 1], capacity >= 1 and no pointer is null.  Binding either ring kind replaces the other. */
+typedef struct dsact_frame_replay {
+  float *frames;                      /* [frame_capacity, obs_elems / frames_per_obs] */
+  int32_t *obs_frames, *obs2_frames;  /* [capacity, frames_per_obs]: frame slots of each row */
+  float *act, *rew, *done, *logp;     /* as in dsact_replay */
+  int64_t capacity, frame_capacity;
+  int32_t frames_per_obs;             /* K: 1 = the whole observation is one frame */
+} dsact_frame_replay;
+
+int dsact_replay_bind_frames(dsact_handle *h, const dsact_frame_replay *rb);
+/* copy n_frames frames (host or device) into frame slots (frame_ptr + i) % frame_capacity, and n rows into rows
+ * (ptr + i) % capacity: their frame ids (HOST int32 [n, frames_per_obs] each), act, rew, done, logp (host or device).
+ * Every id is checked against [0, frame_capacity) before anything is copied (DSACT_EINVAL otherwise).  A handle with a
+ * frame ring bound refuses dsact_replay_add (DSACT_ESTATE), and one with a flat ring refuses this call. */
+int dsact_replay_add_frames(dsact_handle *h, const float *frames, int64_t n_frames, int64_t frame_ptr,
+                            const int32_t *obs_frames, const int32_t *obs2_frames, const float *act, const float *rew,
+                            const float *done, const float *logp, int64_t n, int64_t ptr, void *stream);
 /* sample_batch(): gather rows idx[i] (device int64, or NULL = draw uniformly in [0,size) on
  * the device) into the engine's batch arena; `out` receives the arena's device pointers */
 int dsact_replay_sample(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx,
