@@ -16,6 +16,11 @@
 //
 // Every output element accumulates over the same k16 steps, in the same order and with the same planes, as in the column
 // split, so the outputs, act', images and column sums are the same bits (the column sums' float atomics aside).
+//
+// Epilogue bodies: a full tile (64 rows < M) of a layer whose kind the host set (ChainLayer::kind: forward hidden GELU /
+// ReLU with or without act', dgrad hidden with or without column sums) runs a straight-line body templated on (NB, kind):
+// one activation, no row or column checks, unconditional 8-byte loads and stores.  Every other tile and layer runs the
+// runtime body.  The per-value arithmetic is the same in both.
 #pragma once
 #include "chain_tc.cuh"
 
@@ -87,6 +92,71 @@ __device__ __forceinline__ void pp_step_hi(float (&d)[128], uint64_t a_hi, uint6
 __shared__ int pp_dbg_tile[2];
 #define PP_STAMP(slot) do { if (g.dbg) g.dbg[(size_t)pp_dbg_tile[pp_wg()] * TC_DBG_SLOTS + (slot)] = gtime(); } while (0)
 
+// The epilogue of one layer of one tile: the rolled loop of the column split over all 2 NB groups, each group's global
+// inputs loaded one group ahead (the first under the last item's MMAs).  A group's inputs (bias or act') are applied
+// (epi_apply) before the next group's loads go into the same registers: a 256-column accumulator leaves no room for a
+// second 16-value input buffer.  `prev`: the ring slot of the layer's last item, released once its MMAs retire.
+template <bool PLANES2, int NB, int KIND>
+__device__ __forceinline__ void pp_epilogue(const ChainGroup& g, const ChainPass& P, int j, const EpiArgs& E,
+                                            float (&acc)[128], uint8_t* opnd, float* row, uint64_t* empty, int prev, int m0) {
+  constexpr int planes = PLANES2 ? 2 : 1;
+  const ChainLayer& Lj = P.L[j];
+  const int lane = threadIdx.x & 31;
+  float nx[16];
+  epi_in<KIND>(nx, E, m0, 0, 0);
+  wg_wait<0>();
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+  if (pp_lead()) PP_STAMP(8 + 3 * j);   // MMAs of layer j retired
+  // The operand buffer is this tile's alone: its warpgroup's MMAs of this layer must have retired (each warp reads all of
+  // A), and so must the previous layer's image store (the lead thread issued it).
+  const bool opw = j + 1 < P.n_layers || Lj.img;
+  if (opw) {
+    if (pp_lead()) bulk_wait_read();
+    pp_bar();
+  }
+  const int m_row = ((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+  const uint32_t s_row = smem_u32(opnd) + (uint32_t)(m_row * 128);
+#pragma unroll 1
+  for (int q = 0; q < 2 * NB; ++q) {
+    float v[16];
+#pragma unroll
+    for (int c = 0; c < 2 * NB; ++c)
+      if (q == c) {
+#pragma unroll
+        for (int t = 0; t < 16; ++t) v[t] = acc[16 * c + t];
+      }
+    epi_apply<KIND>(v, nx, E);
+    if (q + 1 < 2 * NB) epi_in<KIND>(nx, E, m0, 0, q + 1);
+    epi_group<PLANES2, KIND, true>(v, nx, E, m0, 0, q, row);
+    if (opw) {   // as chain_layer: bf16 hi/lo pairs split once, two stmatrix per plane
+      uint32_t whi[8], wlo[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        if (PLANES2) split_pack2(v[2 * i], v[2 * i + 1], whi[i], wlo[i]);
+        else whi[i] = cvt_bf16x2(v[2 * i], v[2 * i + 1]);
+      }
+      const uint32_t s_q = s_row + (uint32_t)((q >> 1) * TC_STAGE_A);
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const uint32_t a = s_q + (uint32_t)((((4 * (q & 1) + 2 * s + (lane >> 4)) ^ (lane & 7))) << 4);
+        stsm_x4(a, whi[4 * s], whi[4 * s + 1], whi[4 * s + 2], whi[4 * s + 3]);
+        if (PLANES2) stsm_x4(a + CH_OPND_PLANE, wlo[4 * s], wlo[4 * s + 1], wlo[4 * s + 2], wlo[4 * s + 3]);
+      }
+    }
+  }
+  if (pp_lead()) PP_STAMP(9 + 3 * j);
+  if (opw) {
+    fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads and the TMA store
+    pp_bar();
+    if (Lj.img && pp_lead()) {
+      for (int kb = 0; kb < (Lj.N + 63) / 64; ++kb)
+        for (int pl = 0; pl < planes; ++pl) tma_store_3d(&Lj.mapImg, opnd + pl * CH_OPND_PLANE + kb * TC_STAGE_A, kb * TC_BK, m0, pl);
+      bulk_commit();
+    }
+  }
+  if (pp_lead()) PP_STAMP(10 + 3 * j);
+}
+
 // One layer of one tile on its warpgroup: 64 x (64 NB) outputs.  The MMAs of each ring item (one k-block of one column
 // half) issue back to back and one item stays in flight while the next is issued; then the epilogue on the accumulator,
 // which writes the next layer's A operand into this tile's operand buffer.  `pos`: the ring position of the warpgroup's
@@ -147,75 +217,27 @@ __device__ __forceinline__ void pp_layer(const ChainGroup& g, const ChainPass& P
     }
   }
   if (give_turn) pp_give_turn();
-  // The rolled epilogue of the column split over all 2 NB groups of the tile, each group's global inputs loaded one group
-  // ahead (the first under the last item's MMAs).  A group's inputs (bias or act') are applied here, exactly as epi_group
-  // applies them, so that the next group's loads go into the same registers: a 256-column accumulator leaves no room for
-  // a second 16-value input buffer.  epi_group then sees no bias (Eg) and act' = 1.
-  const bool add_bias = (E.epi == EPI_STORE || E.epi == EPI_BIAS_ACT) && E.bias;
-  EpiArgs Eg = E;
-  Eg.bias = nullptr;
-  float one[16];
-#pragma unroll
-  for (int t = 0; t < 16; ++t) one[t] = 1.f;
-  float nx[16];
-  epi_in(nx, E, m0, 0, 0);
-  wg_wait<0>();
-  if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-  if (pp_lead()) PP_STAMP(8 + 3 * j);   // MMAs of layer j retired
-  // The operand buffer is this tile's alone: its warpgroup's MMAs of this layer must have retired (each warp reads all of
-  // A), and so must the previous layer's image store (the lead thread issued it).
-  const bool opw = j + 1 < P.n_layers || Lj.img;
-  if (opw) {
-    if (pp_lead()) bulk_wait_read();
-    pp_bar();
-  }
-  const int m_row = ((threadIdx.x & (TC_MMA_THREADS - 1)) >> 5) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
-  const uint32_t s_row = smem_u32(opnd) + (uint32_t)(m_row * 128);
-#pragma unroll 1
-  for (int q = 0; q < 2 * NB; ++q) {
-    float v[16];
-#pragma unroll
-    for (int c = 0; c < 2 * NB; ++c)
-      if (q == c) {
-#pragma unroll
-        for (int t = 0; t < 16; ++t) v[t] = acc[16 * c + t];
-      }
-    if (add_bias) {
-#pragma unroll
-      for (int t = 0; t < 16; ++t) v[t] += nx[2 * (t >> 2) + (t & 1)];
-    } else if (E.epi == EPI_DACT) {
-#pragma unroll
-      for (int t = 0; t < 16; ++t) v[t] *= nx[t];
+  // The epilogue body, chosen once per layer: a full tile of a layer with an epilogue kind (ChainLayer::kind) runs that
+  // kind's straight-line body, anything else the runtime body with its row and column checks.  Each kernel holds only the
+  // kinds of its direction.
+  const int kind = m0 + TC_BM <= P.M ? Lj.kind : EK_RUNTIME;
+#define PP_EPI(K) pp_epilogue<PLANES2, NB, K>(g, P, j, E, acc, opnd, row, empty, prev, m0)
+  if constexpr (B_MN) {
+    switch (kind) {
+      case EK_DACT: PP_EPI(EK_DACT); break;
+      case EK_DACT_SUM: PP_EPI(EK_DACT_SUM); break;
+      default: PP_EPI(EK_RUNTIME); break;
     }
-    if (q + 1 < 2 * NB) epi_in(nx, E, m0, 0, q + 1);
-    epi_group<PLANES2>(v, one, Eg, m0, 0, q, row);
-    if (opw) {   // as chain_layer: bf16 hi/lo pairs split once, two stmatrix per plane
-      uint32_t whi[8], wlo[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        if (PLANES2) split_pack2(v[2 * i], v[2 * i + 1], whi[i], wlo[i]);
-        else whi[i] = cvt_bf16x2(v[2 * i], v[2 * i + 1]);
-      }
-      const uint32_t s_q = s_row + (uint32_t)((q >> 1) * TC_STAGE_A);
-#pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        const uint32_t a = s_q + (uint32_t)((((4 * (q & 1) + 2 * s + (lane >> 4)) ^ (lane & 7))) << 4);
-        stsm_x4(a, whi[4 * s], whi[4 * s + 1], whi[4 * s + 2], whi[4 * s + 3]);
-        if (PLANES2) stsm_x4(a + CH_OPND_PLANE, wlo[4 * s], wlo[4 * s + 1], wlo[4 * s + 2], wlo[4 * s + 3]);
-      }
+  } else {
+    switch (kind) {
+      case EK_GELU: PP_EPI(EK_GELU); break;
+      case EK_GELU_Z: PP_EPI(EK_GELU_Z); break;
+      case EK_RELU: PP_EPI(EK_RELU); break;
+      case EK_RELU_Z: PP_EPI(EK_RELU_Z); break;
+      default: PP_EPI(EK_RUNTIME); break;
     }
   }
-  if (pp_lead()) PP_STAMP(9 + 3 * j);
-  if (opw) {
-    fence_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads and the TMA store
-    pp_bar();
-    if (Lj.img && pp_lead()) {
-      for (int kb = 0; kb < (Lj.N + 63) / 64; ++kb)
-        for (int pl = 0; pl < planes; ++pl) tma_store_3d(&Lj.mapImg, opnd + pl * CH_OPND_PLANE + kb * TC_STAGE_A, kb * TC_BK, m0, pl);
-      bulk_commit();
-    }
-  }
-  if (pp_lead()) PP_STAMP(10 + 3 * j);
+#undef PP_EPI
 }
 
 // Ring items of layer j for one tile: k-blocks x column halves.
@@ -323,9 +345,10 @@ __global__ void __launch_bounds__(PP_THREADS, 1) tc_pingpong_kernel(const __grid
       int pos = 0;   // ring position of tile 0's first item of layer j
       for (int j = 0; j < nl; ++j) {
         const int items = pp_items(P.L[j]);
-        const int mine = pos + w * items;
+        const int wg = pp_wg();   // read afresh: not kept in a register through the layer bodies
+        const int mine = pos + wg * items;
         // turns: warpgroup 0's layer j, warpgroup 1's layer j, warpgroup 0's layer j + 1, ...
-        const bool wait = ntiles == 2 && (w == 1 || j > 0), give = ntiles == 2 && (w == 0 || j + 1 < nl);
+        const bool wait = ntiles == 2 && (wg == 1 || j > 0), give = ntiles == 2 && (wg == 0 || j + 1 < nl);
         switch ((P.L[j].bn + 63) / 64) {
           case 1: pp_layer<PLANES2, B_MN, 1>(g, P, j, ringB, opnd, row, stages, full, empty, m0, mine, wait, give); break;
           case 2: pp_layer<PLANES2, B_MN, 2>(g, P, j, ringB, opnd, row, stages, full, empty, m0, mine, wait, give); break;
@@ -338,9 +361,9 @@ __global__ void __launch_bounds__(PP_THREADS, 1) tc_pingpong_kernel(const __grid
     }
   }
 
-  if (lane == 0 && w < ntiles) { if (g.dbg) atomicMax(&g.dbg[(size_t)pp_dbg_tile[w] * TC_DBG_SLOTS + 5], gtime()); }
+  if ((pp_tid() & 31) == 0 && pp_wg() < ntiles) { if (g.dbg) atomicMax(&g.dbg[(size_t)pp_dbg_tile[pp_wg()] * TC_DBG_SLOTS + 5], gtime()); }
   __syncthreads();
-  if (w < ntiles && (threadIdx.x & (TC_MMA_THREADS - 1)) == 0) PP_STAMP(6);
+  if (pp_wg() < ntiles && pp_lead()) PP_STAMP(6);
 }
 
 #undef PP_STAMP

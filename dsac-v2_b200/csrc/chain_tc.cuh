@@ -54,6 +54,7 @@ struct ChainLayer {
   float* C;                  // fp32 result, ld = ldc (head layers)
   int ldc;                   // >= N: a head may write its columns of a wider row (the policy's mean | log_std logits)
   int img;                   // nonzero: the image is needed (mapImg)
+  int kind;                  // epilogue kind of the ping-pong kernel's full tiles (EK_*, gemm_tc.cuh), set by the host
 };
 
 struct ChainPass {

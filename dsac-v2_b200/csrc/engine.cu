@@ -723,11 +723,30 @@ struct ChainBuild {
 // the column split / the ping-pong kernel, -1 selects by shape.
 enum { CHAIN_BY_SHAPE = -1, CHAIN_COLUMN_SPLIT = 0, CHAIN_PINGPONG = 1 };
 
+// The epilogue kind of a layer's full tiles in the ping-pong kernel (gemm_tc.cuh): a forward hidden layer (bias, GELU or
+// ReLU, with or without Zout) or a dgrad hidden layer (with or without column sums), N a multiple of 64 (every column
+// of the accumulator is an output) and 8-byte aligned inputs and act' stores.  Anything else (heads, C stores, the other
+// activations) keeps the runtime body.
+static int chain_epi_kind(const ChainLayer& L) {
+  const auto al8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };
+  if (L.N % 64 != 0 || L.C) return EK_RUNTIME;
+  if (L.epi == EPI_BIAS_ACT && L.bias && al8(L.bias) && (L.act == ACT_GELU || L.act == ACT_RELU) &&
+      (!L.Zout || (al8(L.Zout) && L.ldc == L.N))) {
+    if (L.act == ACT_GELU) return L.Zout ? EK_GELU_Z : EK_GELU;
+    return L.Zout ? EK_RELU_Z : EK_RELU;
+  }
+  if (L.epi == EPI_DACT && L.Zin && al8(L.Zin)) return L.colsum ? EK_DACT_SUM : EK_DACT;
+  return EK_RUNTIME;
+}
+
 static void launch_chain(MlpHandle* h, ChainBuild& cb, int cls, Ctx& c, int tiling = CHAIN_BY_SHAPE) {
   if (cb.g.n == 0) return;
   for (int i = 0; i < cb.g.n; ++i)
-    for (int j = 0; j < cb.g.p[i].n_layers; ++j)
-      if (cb.g.p[i].L[j].ldc != cb.g.p[i].L[j].N && cb.g.p[i].L[j].Zout) cb.ok = false;   // Zout rows are N apart
+    for (int j = 0; j < cb.g.p[i].n_layers; ++j) {
+      ChainLayer& L = cb.g.p[i].L[j];
+      if (L.ldc != L.N && L.Zout) cb.ok = false;   // Zout rows are N apart
+      L.kind = chain_epi_kind(L);
+    }
   if (!cb.ok) { c.err = cudaErrorInvalidValue; return; }
   static unsigned long long* dbg = nullptr;
   const bool debug = getenv("DSACT_TC_DEBUG") != nullptr;

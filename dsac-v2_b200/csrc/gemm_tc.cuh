@@ -336,6 +336,23 @@ __device__ __forceinline__ void st_pair(float* p, int c, int n, bool pair, float
   }
 }
 __device__ __forceinline__ bool pairs_ok(const float* p, int ld) { return ((ld | (int)(reinterpret_cast<uintptr_t>(p) >> 2)) & 1) == 0; }
+// An unconditional 8-byte read-only load, kept where it is written as ldg2_if is.
+__device__ __forceinline__ void ldg2(const float* p, float& a, float& b) {
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(a), "=f"(b) : "l"(p));
+}
+
+// Epilogue kinds.  EK_RUNTIME reads the variant (epi, act, which optional pointers are set) from EpiArgs and checks every
+// value's row against M and column against N.  The others fix the variant at compile time for a FULL tile: all rows of the
+// 64-row tile are < M, every column of the accumulator is < N, the bias / act' / Zout pointers are 8-byte aligned with
+// rows N floats apart, and there is no fp32 C store.  Each kind body then holds one activation and no masking.  The layer
+// chain decides a layer's kind on the host (ChainLayer::kind) and checks the rows per tile.
+//   EK_GELU / EK_RELU     : EPI_BIAS_ACT with a bias, without Zout;  EK_GELU_Z / EK_RELU_Z: with Zout
+//   EK_DACT / EK_DACT_SUM : EPI_DACT without / with colsum
+enum { EK_RUNTIME = 0, EK_GELU, EK_GELU_Z, EK_RELU, EK_RELU_Z, EK_DACT, EK_DACT_SUM };
+__host__ __device__ constexpr bool ek_fwd(int k) { return k >= EK_GELU && k <= EK_RELU_Z; }
+__host__ __device__ constexpr int ek_epi(int k) { return ek_fwd(k) ? EPI_BIAS_ACT : EPI_DACT; }
+__host__ __device__ constexpr int ek_act(int k) { return k == EK_GELU || k == EK_GELU_Z ? ACT_GELU : ACT_RELU; }
+__host__ __device__ constexpr bool ek_zout(int k) { return k == EK_GELU_Z || k == EK_RELU_Z; }
 
 // Epilogue of the warpgroup's 64 x (64 NB) accumulator, element (0, 0) = output (m0, n0), straight from the wgmma
 // fragment: acc[16 g + t] sits in row ra (t & 2 == 0) or ra + 8, column n0 + 32 g + 8 (t >> 2) + 2 (lane & 3) + (t & 1).
@@ -352,8 +369,19 @@ __device__ __forceinline__ bool pairs_ok(const float* p, int ld) { return ((ld |
 
 // The global inputs of group g: x[t] = act'(z) of value t (EPI_DACT), or x[2 (t >> 2) + (t & 1)] = the bias of value t's
 // column (EPI_STORE / EPI_BIAS_ACT with a bias).
+template <int KIND = EK_RUNTIME>
 __device__ __forceinline__ void epi_in(float (&x)[16], const EpiArgs& E, int m0, int n0, int g) {
   EPI_FRAG_COORDS
+  if constexpr (KIND != EK_RUNTIME) {   // full tile: unconditional 8-byte loads
+    if constexpr (ek_epi(KIND) == EPI_DACT) {
+#pragma unroll
+      for (int t = 0; t < 16; t += 2) ldg2(E.Zin + (size_t)ROW(t) * E.ldz + COL(t), x[t], x[t + 1]);
+    } else {
+#pragma unroll
+      for (int t = 0; t < 16; t += 4) ldg2(E.bias + COL(t), x[t / 2], x[t / 2 + 1]);
+    }
+    return;
+  }
   // one loop body per access width, so that `pair` is a constant inside it
 #define EPI_IN_ZIN(pair) \
   _Pragma("unroll") for (int t = 0; t < 16; t += 2) ld_pair(E.Zin + (size_t)ROW(t) * E.ldz, COL(t), ROW_OK(t) ? E.N : 0, pair, x[t], x[t + 1]);
@@ -368,33 +396,57 @@ __device__ __forceinline__ void epi_in(float (&x)[16], const EpiArgs& E, int m0,
 #undef EPI_IN_BIAS
 }
 
-// Arithmetic and stores of group g: v = the accumulator values on entry, the result on return.  Columns >= N leave as
-// zeros (they are the next layer's K padding and the image padding).  `row`: this thread's 16-float shared-memory row
-// (generic activations).
-template <bool PLANES2>
+// Group g's global inputs x (epi_in) applied to its values v as epi_group applies them: the bias added or act'
+// multiplied.  A caller that loads the next group's inputs into the same registers applies them first (APPLIED).
+template <int KIND = EK_RUNTIME>
+__device__ __forceinline__ void epi_apply(float (&v)[16], const float (&x)[16], const EpiArgs& E) {
+  const int epi = KIND == EK_RUNTIME ? E.epi : ek_epi(KIND);
+  if ((epi == EPI_STORE || epi == EPI_BIAS_ACT) && (KIND != EK_RUNTIME || E.bias)) {
+#pragma unroll
+    for (int t = 0; t < 16; ++t) v[t] += x[2 * (t >> 2) + (t & 1)];
+  } else if (epi == EPI_DACT) {
+#pragma unroll
+    for (int t = 0; t < 16; ++t) v[t] *= x[t];
+  }
+}
+
+// Arithmetic and stores of group g: v = the accumulator values on entry, the result on return; x = its inputs (epi_in),
+// unused when the caller has APPLIED them.  Columns >= N leave as zeros (they are the next layer's K padding and the image
+// padding).  `row`: this thread's 16-float shared-memory row (generic activations).
+template <bool PLANES2, int KIND = EK_RUNTIME, bool APPLIED = false>
 __device__ __forceinline__ void epi_group(float (&v)[16], const float (&x)[16], const EpiArgs& E, int m0, int n0, int g,
                                           float* row) {
   EPI_FRAG_COORDS
+  constexpr bool RT = KIND == EK_RUNTIME;
+  const int epi = RT ? E.epi : ek_epi(KIND);
+  const int act = RT ? E.act : ek_act(KIND);
   float d[16];
-  if (E.epi == EPI_STORE || E.epi == EPI_BIAS_ACT) {
-    if (E.bias) {
+  if (epi == EPI_STORE || epi == EPI_BIAS_ACT) {
+    if (!APPLIED && (!RT || E.bias)) {
 #pragma unroll
       for (int t = 0; t < 16; ++t) v[t] += x[2 * (t >> 2) + (t & 1)];
     }
-    if (E.epi == EPI_BIAS_ACT) {
-      if (E.Zout) {
-        act_fwdN<true, 16>(v, d, E.act, row);
-        const bool pair = pairs_ok(E.Zout, E.ldc);
+    if (epi == EPI_BIAS_ACT) {
+      if (RT ? E.Zout != nullptr : ek_zout(KIND)) {
+        act_fwdN<true, 16>(v, d, act, row);
+        if constexpr (RT) {
+          const bool pair = pairs_ok(E.Zout, E.ldc);
 #pragma unroll
-        for (int t = 0; t < 16; t += 2) st_pair(E.Zout + (size_t)ROW(t) * E.ldc, COL(t), ROW_OK(t) ? E.N : 0, pair, d[t], d[t + 1]);
+          for (int t = 0; t < 16; t += 2) st_pair(E.Zout + (size_t)ROW(t) * E.ldc, COL(t), ROW_OK(t) ? E.N : 0, pair, d[t], d[t + 1]);
+        } else {   // full tile: unconditional 8-byte stores
+#pragma unroll
+          for (int t = 0; t < 16; t += 2) *reinterpret_cast<float2*>(E.Zout + (size_t)ROW(t) * E.ldc + COL(t)) = make_float2(d[t], d[t + 1]);
+        }
       } else {
-        act_fwdN<false, 16>(v, d, E.act, row);
+        act_fwdN<false, 16>(v, d, act, row);
       }
     }
-  } else if (E.epi == EPI_DACT) {
+  } else if (epi == EPI_DACT) {
+    if (!APPLIED) {
 #pragma unroll
-    for (int t = 0; t < 16; ++t) v[t] *= x[t];
-    if (E.colsum) {  // bias gradient: both rows of the thread, then the eight lanes that share its columns
+      for (int t = 0; t < 16; ++t) v[t] *= x[t];
+    }
+    if (RT ? E.colsum != nullptr : KIND == EK_DACT_SUM) {  // bias gradient: both rows of the thread, then the eight lanes that share its columns
       // s[k]: column k = 2 (t >> 2) + (t & 1) of the thread's eight.  A transposing butterfly over lane bits 2, 3, 4: at
       // each step a lane keeps half of its columns (the upper half if its bit is set), adds the partner's partial sums of
       // them and sends the other half, so each lane ends with one column's sum over the eight lanes, added in the same
@@ -413,15 +465,17 @@ __device__ __forceinline__ void epi_group(float (&v)[16], const float (&x)[16], 
       }
       const int k = ((lane >> 2) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 4) & 1);
       const int c = cq + 32 * g + 8 * (k >> 1) + (k & 1);
-      if (c < E.N) atomicAdd(E.colsum + c, s[0]);
+      if (!RT || c < E.N) atomicAdd(E.colsum + c, s[0]);
     }
   }
+  if constexpr (RT) {
 #pragma unroll
-  for (int t = 0; t < 16; ++t) v[t] = COL(t) < E.N ? v[t] : 0.f;
-  if (E.C) {   // scalar: head outputs have odd widths (e.g. the action columns)
+    for (int t = 0; t < 16; ++t) v[t] = COL(t) < E.N ? v[t] : 0.f;
+    if (E.C) {   // scalar: head outputs have odd widths (e.g. the action columns)
 #pragma unroll
-    for (int t = 0; t < 16; ++t)
-      if (ROW_OK(t) && COL(t) < E.N) E.C[(size_t)ROW(t) * E.ldc + COL(t)] = v[t];
+      for (int t = 0; t < 16; ++t)
+        if (ROW_OK(t) && COL(t) < E.N) E.C[(size_t)ROW(t) * E.ldc + COL(t)] = v[t];
+    }
   }
 }
 
