@@ -32,7 +32,11 @@ POWER = 5.0        # every gate must sit at least this factor below the signal o
 # 0.91, smallest signal_k / gate_k 5.7 (the log_alpha gradient at halfcheetah B=8192).  layered_q's six tanh critic
 # layers carry the split-bf16 rounding through six dgrad GEMMs into the first layer's weight gradient: there err_k reaches
 # 1.15 x the floor on an H100, and the float64 oracle with its GEMMs restated as hi*hi + hi*lo + lo*hi of bf16 splits
-# reaches 1.19 x.  That case's bf16x3 gates are doubled; its smallest signal_k / gate_k stays above 80.
+# reaches 1.19 x.  That case's bf16x3 gates are doubled; its smallest signal_k / gate_k stays above 80.  deep_pi at
+# B = 2200 in bf16x3: q1.q.0.weight, the gradient of the first critic layer (109 inputs: 13 observation and 96 action
+# columns), comes out at 9.59 x the floor on an H100, and the float64 oracle with every GEMM restated as split-bf16
+# products reaches 9.59 x as well (the other tensors stay below 0.52 x).  Only that tensor's gate is widened, 12 x: its
+# signal_k / gate_k is 467, while a case-wide factor would leave log_alpha's lost-tile signal (5.4 x its gate) unseen.
 GATES = {"fp32": (4.0, 2e-6), "heads": (4.0, 2e-6), "bf16x3": (8.0, 1e-5)}
 BF16_LIMIT = 5e-2  # the single-pass bf16 mode is not a parity mode: finite gradients within this relative error
 TB_RTOL = 1e-4
@@ -56,6 +60,7 @@ class Case:
     hyper: Tuple[Tuple[str, float], ...] = ()   # overrides of synth.HYPER
     fp32_only: bool = False        # MLP engine: skip the bf16x3 mode (see REGIME_CASES)
     bf16x3_scale: float = 1.0      # widens this case's bf16x3 gates (see SHAPE_CASES)
+    bf16x3_keys: Tuple[Tuple[str, float], ...] = ()   # widens the bf16x3 gates of single tensors instead (see SHAPE_CASES)
 
     @property
     def cnn(self) -> bool:
@@ -85,6 +90,11 @@ SHAPE_CASES = [Case(f"ragged_b{b}", "mlp", "ragged", b) for b in (63, 64, 65, 12
     Case("wide_b200", "mlp", "wide", 200),
 ] + [Case(f"{name}_b200", "mlp", name, 200, bf16x3_scale=2.0 if name == "layered_q" else 1.0)
       for name in synth.ASYM_CONFIGS] + [   # critics and policy of different shapes
+    # B = 2200: a four-pass chain launch has 4 x 35 row tiles, more than one wave of 132 CTAs, so both forward chains and
+    # the critic dgrad chain run on the ping-pong kernel, with ELU, SELU and tanh, six-layer critics and policies, the
+    # narrow ragged widths, and a last CTA holding one ragged 24-row tile
+    Case(f"{name}_b2200", "mlp", name, 2200, bf16x3_keys=(("q1.q.0.weight", 12.0),) if name == "deep_pi" else ())
+    for name in ("asym", "deep_pi", "ragged")] + [
     Case("separated_ragged_b1000", "heads", "ragged", 1000, std_type="mlp_separated"),
     Case("parameter_ragged_b1000", "heads", "ragged", 1000, std_type="parameter"),
     Case("gauss_tiny_b1000", "heads", "tiny", 1000, act_dist="GaussDistribution"),
@@ -264,8 +274,10 @@ def reference(name: str) -> Reference:
 
 def gates(name: str, mode: str) -> Dict[str, float]:
     c, floor = GATES[mode]
-    scale = CASES[name].bf16x3_scale if mode == "bf16x3" else 1.0
-    return {k: scale * max(c * r, floor) for k, r in reference(name).ref.items()}
+    case = CASES[name]
+    keys = dict(case.bf16x3_keys)
+    scale = lambda k: keys.get(k, case.bf16x3_scale) if mode == "bf16x3" else 1.0
+    return {k: scale(k) * max(c * r, floor) for k, r in reference(name).ref.items()}
 
 
 def power_violations(name: str, mode: str) -> Dict[str, Tuple[float, float]]:

@@ -30,6 +30,12 @@ CASES = {
     "dgrad_wide": (True, [256, 256, 256], 376, 17, 384, 2),
     "dgrad_mixed": (True, [64, 136, 200, 128], 14, 0, 0, 2),
     "dgrad_narrow": (True, [8, 72, 256, 248], 5, 0, 0, 34),
+    # five and six hidden layers; the six-layer chain's ring items per tile mix odd and even counts (forward: 1, 2, 3, 2,
+    # 4, 4, then 3 for the head), so the warpgroups' turns and the ring's parity waits go through many phases
+    "fwd_deep5": (False, [256, 64, 128, 200, 136], 14, 3, 16, 2),
+    "fwd_parity6": (False, [64, 192, 8, 256, 72, 136], 5, 0, 0, 2),
+    "dgrad_deep5": (True, [256, 64, 128, 200, 136], 14, 3, 16, 2),
+    "dgrad_parity6": (True, [64, 192, 8, 256, 72, 136], 5, 0, 0, 2),
 }
 # the rows of each pass of one launch: one tile, a full and a partial CTA, a CTA whose second tile is missing (129, 8449)
 PASS_SETS = {
@@ -92,16 +98,17 @@ def _build(case, Ms, seed):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("act", list(ACT))
 @pytest.mark.parametrize("pset", list(PASS_SETS))
 @pytest.mark.parametrize("name", list(CASES))
-def test_pingpong_gives_the_column_split_bits(tc_eng, name, pset):
+def test_pingpong_gives_the_column_split_bits(tc_eng, name, pset, act):
     case = CASES[name]
     dgrad, hidden, K0, K1, kB1 = case[:5]
     Ms = PASS_SETS[pset]
     res = []
     for tiling in (0, 1):
         sizes, params, passes, bufs = _build(case, Ms, 23)
-        tc_eng.test_chain(dgrad, sizes, K0, K1, kB1, ACT["gelu"], params, passes, tiling=tiling)
+        tc_eng.test_chain(dgrad, sizes, K0, K1, kB1, ACT[act], params, passes, tiling=tiling)
         torch.cuda.synchronize()
         res.append(bufs)
     for i, ((exact0, sums0), (exact1, sums1)) in enumerate(zip(*res)):

@@ -202,7 +202,35 @@ CHAIN_CASES = {c["name"]: c for c in [
     chain_case("w136_8", [136, 8], 376, 2, 64, "selu", K1=17, kB1=384),
     chain_case("w64x5", [64] * 5, 5, 2, 65, "sigmoid"),
     chain_case("w256_4pass_m8192", [256, 256], 376, 2, 8192, "gelu", K1=17, kB1=384, passes=4),
+    chain_case("w248_40_linear", [248, 40], 120, 2, 97, "linear"),
+    # six hidden layers whose ring items per tile (k-blocks x column halves) mix odd and even: 1, 2, 3, 2, 4, 4, then 3 for
+    # the head; the ping-pong kernel's turns and parity waits go through many ring phases
+    chain_case("ring_parity6", [64, 192, 8, 256, 72, 136], 5, 2, 1000, "elu"),
 ]}
+# tiling: None selects the kernel by launch shape, 0 forces the column split, 1 the ping-pong kernel
+TILINGS = {"by_shape": None, "column_split": 0, "pingpong": 1}
+# the passes the ping-pong runs add: 161 rows (two full tiles, the kind bodies; then a CTA whose only tile is ragged) and
+# 97 rows (a CTA whose second tile is ragged)
+PP_EXTRA_ROWS = [161, 97]
+MAX_PASSES = 4
+
+
+def chain_rows(case, tiling):
+    """The rows of each pass of one launch of the case: its own passes, and under the ping-pong kernel PP_EXTRA_ROWS from
+    the second pass on (at most MAX_PASSES passes)."""
+    rows = [case["M"]] * case["passes"]
+    if tiling == 1:
+        rows = (rows[:1] + PP_EXTRA_ROWS + rows[1:])[:MAX_PASSES]
+    return rows
+
+
+def pp_ctas(M):
+    """The kinds of ping-pong CTA a pass of M rows has: "full" (a tile of 64 rows), "ragged2" (a second tile below 64
+    rows), "missing2" (no second tile)."""
+    tiles = (M + 63) // 64
+    kinds = {"full"} if M >= 64 else set()
+    kinds.add("missing2" if tiles % 2 else ("ragged2" if M % 64 else "full"))
+    return kinds
 
 
 def _chain_params(sizes, g):
@@ -265,12 +293,14 @@ def _check_fwd_chain(mode, case, sizes, parts, x, p):
     return ratios
 
 
+@pytest.mark.parametrize("tiling", list(TILINGS.values()), ids=list(TILINGS))
 @pytest.mark.parametrize("name", list(CHAIN_CASES))
-def test_forward_chain_against_float64(tc_eng, name):
+def test_forward_chain_against_float64(tc_eng, name, tiling):
     case = CHAIN_CASES[name]
     sizes, parts, params, g = _chain_setup(case, 7)
-    runs = [_fwd_pass(case, sizes, g, case["M"]) for _ in range(case["passes"])]
-    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], ACT[case["act"]], params, [p for _, p in runs])
+    runs = [_fwd_pass(case, sizes, g, M) for M in chain_rows(case, tiling)]
+    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], ACT[case["act"]], params, [p for _, p in runs],
+                      tiling=tiling)
     torch.cuda.synchronize()
     ratios = {}
     for i, (x, p) in enumerate(runs):
@@ -279,20 +309,21 @@ def test_forward_chain_against_float64(tc_eng, name):
     _report(tc_eng.mode, f"chain_fwd.{name}", ratios)
 
 
-def test_forward_pass_is_the_same_alone_in_a_group_and_without_stores(tc_eng):
+@pytest.mark.parametrize("tiling", list(TILINGS.values()), ids=list(TILINGS))
+def test_forward_pass_is_the_same_alone_in_a_group_and_without_stores(tc_eng, tiling):
     """One pass gives the same bits run alone, as the second of 4 passes of different lengths, and without its act' and
     image stores."""
     case = dict(CHAIN_CASES["w128_192_200_248"], K1=17, kB1=384, K0=64)
     sizes, parts, params, g = _chain_setup(case, 11)
     runs = [_fwd_pass(case, sizes, g, m) for m in (65, 200, 1, 130)]
     act = ACT[case["act"]]
-    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], act, params, [p for _, p in runs])
+    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], act, params, [p for _, p in runs], tiling=tiling)
     x, p = runs[1]
     alone = dict(p, out=torch.full_like(p["out"], NAN), Zout=[torch.full_like(z, NAN) for z in p["Zout"]],
                  img=[torch.full_like(i, NAN) for i in p["img"]])
     bare = dict(p, out=torch.full_like(p["out"], NAN), Zout=None, img=None)
-    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], act, params, [alone])
-    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], act, params, [bare])
+    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], act, params, [alone], tiling=tiling)
+    tc_eng.test_chain(False, sizes, case["K0"], case["K1"], case["kB1"], act, params, [bare], tiling=tiling)
     torch.cuda.synchronize()
     assert torch.equal(p["out"], alone["out"]) and torch.equal(p["out"], bare["out"])
     for a, b in zip(p["Zout"], alone["Zout"]):
@@ -302,8 +333,9 @@ def test_forward_pass_is_the_same_alone_in_a_group_and_without_stores(tc_eng):
     _report(tc_eng.mode, "chain_fwd.group_of_4", _check_fwd_chain(tc_eng.mode, case, sizes, parts, x, p))
 
 
+@pytest.mark.parametrize("tiling", list(TILINGS.values()), ids=list(TILINGS))
 @pytest.mark.parametrize("name", list(CHAIN_CASES))
-def test_dgrad_chain_against_float64(tc_eng, name):
+def test_dgrad_chain_against_float64(tc_eng, name, tiling):
     """dz_{j-1} = (dz_j W_j) * act'(z_{j-1}) down the hidden layers, the bias gradients (accumulated onto non-zero
     values) and the action columns' gradient read through the dact window at the step's column kB1 of W_0's image."""
     case = CHAIN_CASES[name]
@@ -311,8 +343,7 @@ def test_dgrad_chain_against_float64(tc_eng, name):
     sizes, parts, params, g = _chain_setup(case, 13)
     L = len(sizes) - 2
     runs = []
-    for _ in range(case["passes"]):
-        M = case["M"]
+    for M in chain_rows(case, tiling):
         dout = torch.randn(M, sizes[-1], generator=g)
         dout[3::7] = 0.0
         D = [torch.rand(M, sizes[j + 1], generator=g) * 2.0 - 0.25 for j in range(L)]
@@ -322,7 +353,8 @@ def test_dgrad_chain_against_float64(tc_eng, name):
         if case["K1"]:
             p["out"] = torch.full((M, case["K1"]), NAN, device="cuda")
         runs.append((dout, D, cs0, p))
-    tc_eng.test_chain(True, sizes, case["K0"], case["K1"], case["kB1"], ACT[case["act"]], params, [r[3] for r in runs])
+    tc_eng.test_chain(True, sizes, case["K0"], case["K1"], case["kB1"], ACT[case["act"]], params, [r[3] for r in runs],
+                      tiling=tiling)
     torch.cuda.synchronize()
     ratios = {}
     for i, (dout, D, cs0, p) in enumerate(runs):
@@ -355,3 +387,10 @@ def test_chain_case_table_covers_the_layer_bodies():
     assert {1, 2, 34, 192} <= {c["head"] for c in CHAIN_CASES.values()}
     assert {(5, 0), (64, 0), (376, 0), (11, 3), (64, 5), (376, 17)} <= {(c["K0"], c["K1"]) for c in CHAIN_CASES.values()}
     assert {1, 63, 64, 65, 200, 4096, 8192} <= {c["M"] for c in CHAIN_CASES.values()}
+    assert set(ACT) == {c["act"] for c in CHAIN_CASES.values()}
+    # under the ping-pong kernel every activation meets a full tile, a CTA whose second tile is ragged and one whose
+    # second tile is missing
+    for act in ACT:
+        kinds = {k for c in CHAIN_CASES.values() if c["act"] == act for M in chain_rows(c, 1) for k in pp_ctas(M)}
+        assert kinds == {"full", "ragged2", "missing2"}, (act, kinds)
+    assert all(len(chain_rows(c, t)) <= MAX_PASSES for c in CHAIN_CASES.values() for t in TILINGS.values())

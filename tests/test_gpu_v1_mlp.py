@@ -70,11 +70,14 @@ def _v1_case(name, cfg_name, batch, hyper=(), bf16x3_scale=1.0):
 
 HOPPER_HYPER = (("TD_bound", 10.0), ("gamma", 0.999))
 # ragged at the tile edges and multi-tile, the reference example's shape, critics and policy of different shapes, and a
-# TD bound that clips (v1_ragged_tight's).  layered_q's six tanh critic layers: bf16x3 gates doubled, as in gradcheck64.
+# TD bound that clips (v1_ragged_tight's), and asym at a batch whose chain launches all run on the ping-pong kernel.
+# layered_q's six tanh critic layers: bf16x3 gates doubled, as in gradcheck64.
 F64_CASES = {c.name: c for c in [_v1_case(f"v1mlp_ragged_b{b}", "ragged", b) for b in (63, 65, 129, 1000)] + [
     _v1_case("v1mlp_hopper_b256", "hopper", 256, HOPPER_HYPER)] + [
     _v1_case(f"v1mlp_{n}_b200", n, 200, bf16x3_scale=2.0 if n == "layered_q" else 1.0) for n in synth.ASYM_CONFIGS] + [
-    _v1_case("v1mlp_tight_ragged_b129", "ragged", 129, (("TD_bound", 0.5), ("delay_update", 3)))]}
+    _v1_case("v1mlp_tight_ragged_b129", "ragged", 129, (("TD_bound", 0.5), ("delay_update", 3))),
+    # one critic: launches of 3, 2 and 2 passes, each more than one wave of row tiles at B = 4300 (the ping-pong kernel)
+    _v1_case("v1mlp_asym_b4300", "asym", 4300)]}
 
 
 def _oracle_grads(case, dtype, rows=None):
