@@ -64,11 +64,12 @@ _ACT = {
 }
 
 
-def mlp_forward(layers: Sequence[torch.Tensor], x: torch.Tensor, act: str) -> torch.Tensor:
-    """networks/mlp.py:15-20 — Linear+act per hidden layer, Identity on the last."""
+def mlp_forward(layers: Sequence[torch.Tensor], x: torch.Tensor, act: str, linear=F.linear) -> torch.Tensor:
+    """networks/mlp.py:15-20 — Linear+act per hidden layer, Identity on the last.  `linear(x, W, b)`: the dense layer
+    (tests/gradcheck_rounded.py restates it with the tensor-core kernels' bf16 operands)."""
     n = len(layers) // 2
     for j in range(n):
-        x = F.linear(x, layers[2 * j], layers[2 * j + 1])
+        x = linear(x, layers[2 * j], layers[2 * j + 1])
         if j < n - 1:
             x = _ACT[act](x)
     return x
@@ -92,9 +93,10 @@ class OracleDSACT:
                  policy_learning_rate=1e-4, alpha_learning_rate=3e-4,
                  policy_min_log_std=-20.0, policy_max_log_std=0.5, hidden_activation="gelu",
                  value_hidden_activation=None, policy_hidden_activation=None,
-                 policy_act_distribution="TanhGaussDistribution", dtype=torch.float32, **_ignored):
+                 policy_act_distribution="TanhGaussDistribution", dtype=torch.float32, linear=F.linear, **_ignored):
         self.O, self.A = int(obs_dim), int(act_dim)
         self.dtype = dtype
+        self.linear = linear   # every dense layer of every network (mlp_forward); F.linear is the reference's nn.Linear
         # critics / policy: the reference's value_* / policy_* kwargs, else `hidden_activation` for both networks
         self.act_q = value_hidden_activation or hidden_activation
         self.act_pi = policy_hidden_activation or hidden_activation
@@ -158,13 +160,13 @@ class OracleDSACT:
     # ---- network pieces -------------------------------------------------
     def policy_logits(self, layers, obs):
         """StochaPolicy.forward, std_type='mlp_shared' (networks/mlp.py:85-100)."""
-        out = mlp_forward(layers, obs, self.act_pi)
+        out = mlp_forward(layers, obs, self.act_pi, self.linear)
         mean, log_std = torch.chunk(out, 2, dim=-1)
         return mean, torch.clamp(log_std, self.min_log_std, self.max_log_std).exp()
 
     def q_dist(self, layers, obs, act):
         """ActionValueDistri.forward (networks/mlp.py:122-127): mean, softplus(std)."""
-        out = mlp_forward(layers, torch.cat([obs, act], dim=-1), self.act_q)
+        out = mlp_forward(layers, torch.cat([obs, act], dim=-1), self.act_q, self.linear)
         return out[..., 0], F.softplus(out[..., 1])
 
     def tanh_gauss_rsample(self, mean, std, eps):
@@ -358,7 +360,7 @@ class OracleDSACTStd(OracleDSACT):
             while f"{name}.{2 * j}.weight" in w:
                 ls += [w[f"{name}.{2 * j}.weight"], w[f"{name}.{2 * j}.bias"]]
                 j += 1
-            return mlp_forward(ls, obs, self.act_pi)
+            return mlp_forward(ls, obs, self.act_pi, self.linear)
 
         mean = head("mean")
         log_std = head("log_std") if self.std_type == "mlp_separated" else w["log_std"] + torch.zeros_like(mean)
@@ -425,7 +427,7 @@ class OracleDSACTCNN(OracleDSACT):
         while f"{head}.{2 * j}.weight" in w:
             layers += [w[f"{head}.{2 * j}.weight"], w[f"{head}.{2 * j}.bias"]]
             j += 1
-        return mlp_forward(layers, x, act)
+        return mlp_forward(layers, x, act, self.linear)
 
     def policy_logits(self, layers, obs):
         """StochaPolicy.forward (networks/cnn.py:233-240): mean head, exp(clamp(log_std head))."""

@@ -37,6 +37,7 @@ POWER = 5.0        # every gate must sit at least this factor below the signal o
 # columns), comes out at 9.59 x the floor on an H100, and the float64 oracle with every GEMM restated as split-bf16
 # products reaches 9.59 x as well (the other tensors stay below 0.52 x).  Only that tensor's gate is widened, 12 x: its
 # signal_k / gate_k is 467, while a case-wide factor would leave log_alpha's lost-tile signal (5.4 x its gate) unseen.
+# The restated oracle is tests/gradcheck_rounded.py; tests/test_grad_rounded.py recomputes both widenings' numbers.
 GATES = {"fp32": (4.0, 2e-6), "heads": (4.0, 2e-6), "bf16x3": (8.0, 1e-5)}
 BF16_LIMIT = 5e-2  # the single-pass bf16 mode is not a parity mode: finite gradients within this relative error
 TB_RTOL = 1e-4
@@ -346,12 +347,13 @@ def make_engine(case: Case, mode: str):
     return CnnEngine(c, torch.device("cuda", 0), lim, -lim)
 
 
-def engine_grads(name: str, mode: str):
-    """(gradients in the schema of the oracle's grad_dict, tb_info) of one step-0 gradient computation on cuda:0.
-    DSAC-T runs the gradient-message seam (`compute_grads`); DSAC_V1 has none, so it runs one whole step, which leaves the
-    step's gradients in the gradient buffer and the statistics of its forward pass."""
+def engine_grads(name, mode: str):
+    """(gradients in the schema of the oracle's grad_dict, tb_info) of one step-0 gradient computation on cuda:0 for the
+    case named `name` (or the Case itself).  DSAC-T runs the gradient-message seam (`compute_grads`); DSAC_V1 has none, so
+    it runs one whole step, which leaves the step's gradients in the gradient buffer and the statistics of its forward
+    pass."""
     from dsac_v2_b200.engine import STAT_KEYS
-    case = CASES[name]
+    case = name if isinstance(name, Case) else CASES[name]
     w, b, n = inputs(case)
     eng = make_engine(case, "fp32" if mode == "heads" else mode)
     try:

@@ -399,7 +399,8 @@ F64_CASES = [(s, b, False) for s in STD_TYPES for b in (200, 1000, 2200)] + [(s,
 # operand rounding carried through the three dgrad GEMMs above that layer, as for gradcheck64's layered_q; that case's
 # bf16x3 gates are doubled like layered_q's, and the power rule still has to hold for the doubled gate.  At B = 2200 the
 # same tensor comes out at 1.03 x the floor, and the float64 oracle with every GEMM restated as split-bf16 products at
-# 0.93 x (at B = 200: 1.08 x against the engine's 1.09 x); its gates are doubled too.
+# 0.94 x (at B = 200: 1.07 x against the engine's 1.09 x; tests/test_grad_rounded.py recomputes both); its gates are
+# doubled too.
 F64_BF16X3_SCALE = {("parameter", 200, False): 2.0, ("parameter", 2200, False): 2.0}
 
 
