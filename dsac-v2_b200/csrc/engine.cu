@@ -208,6 +208,8 @@ struct dsact_handle {
   dsact_replay rb = {};
   dsact_frame_replay fr = {};   // the frame ring, when rb_frames (binding either ring kind replaces the other)
   bool rb_frames = false;
+  bool rb_codes = false;        // rb_frames and fr.frames holds uint8 codes, decoded through fr_table
+  float* fr_table = nullptr;    // the coded ring's device table [256]
   DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   int32_t pending_batch = 0; // rows of the shard phase1 processed (phase2 must match)
   dsact_batch pending = {};  // batch pointers of phase1
@@ -1353,15 +1355,16 @@ static void enqueue_gather(const dsact_handle* h, int B, const int64_t* idx, con
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
   if (h->rb_frames) {
     const dsact_frame_replay& r = h->fr;
-    launch_k(gather_kernel<true>, blocks, 256, 0, c, (const float*)r.frames, (const float*)r.frames, r.act, r.rew, r.done,
+    launch_k(h->rb_codes ? gather_kernel<true, true> : gather_kernel<true>, blocks, 256, 0, c, (const float*)r.frames,
+             (const float*)r.frames, r.act, r.rew, r.done,
              r.logp, idx, d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
              img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0,
-             (const int32_t*)r.obs_frames, (const int32_t*)r.obs2_frames, (int)r.frames_per_obs);
+             (const int32_t*)r.obs_frames, (const int32_t*)r.obs2_frames, (int)r.frames_per_obs, (const float*)h->fr_table);
   } else {
     launch_k(gather_kernel<false>, blocks, 256, 0, c, h->rb.obs, h->rb.obs2, h->rb.act, h->rb.rew, h->rb.done, h->rb.logp, idx,
              d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
              img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0,
-             (const int32_t*)nullptr, (const int32_t*)nullptr, 1);
+             (const int32_t*)nullptr, (const int32_t*)nullptr, 1, (const float*)nullptr);
   }
   c.done();
   c.check();
@@ -2318,12 +2321,13 @@ int dsact_replay_bind(dsact_handle* h, const dsact_replay* rb) {
   h->rb = *rb;
   h->rb_bound = true;
   h->rb_frames = false;
+  h->rb_codes = false;
   if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
   return DSACT_OK;
 }
 
-int dsact_replay_bind_frames(dsact_handle* h, const dsact_frame_replay* rb) {
-  if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
+// the shape and pointers of a frame ring of either kind (DSACT_OK, or DSACT_EINVAL with the reason)
+static int check_frame_ring(const dsact_handle* h, const dsact_frame_replay* rb) {
   const int64_t K = rb->frames_per_obs;
   if (K < 1 || K > 64 || h->obs_elems % K != 0)
     return fail(DSACT_EINVAL, "frames_per_obs %lld must be in [1, 64] and divide obs_elems %lld", (long long)K,
@@ -2333,11 +2337,30 @@ int dsact_replay_bind_frames(dsact_handle* h, const dsact_frame_replay* rb) {
   if (rb->capacity < 1) return fail(DSACT_EINVAL, "capacity %lld < 1", (long long)rb->capacity);
   if (!rb->frames || !rb->obs_frames || !rb->obs2_frames || !rb->act || !rb->rew || !rb->done || !rb->logp)
     return fail(DSACT_EINVAL, "null frame-ring pointer");
+  return DSACT_OK;
+}
+
+static int bind_frame_ring(dsact_handle* h, const dsact_frame_replay* rb, const float* table) {
   h->fr = *rb;
+  h->fr_table = const_cast<float*>(table);
   h->rb_bound = true;
   h->rb_frames = true;
+  h->rb_codes = table != nullptr;
   if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
   return DSACT_OK;
+}
+
+int dsact_replay_bind_frames(dsact_handle* h, const dsact_frame_replay* rb) {
+  if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
+  if (int rc = check_frame_ring(h, rb)) return rc;
+  return bind_frame_ring(h, rb, nullptr);
+}
+
+int dsact_replay_bind_coded_frames(dsact_handle* h, const dsact_frame_replay* rb, const float* table) {
+  if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
+  if (int rc = check_frame_ring(h, rb)) return rc;
+  if (!table) return fail(DSACT_EINVAL, "null table");
+  return bind_frame_ring(h, rb, table);
 }
 
 // the first n entries of a HOST frame-id table (nullptr: not host memory, or an id outside [0, frame_capacity))
@@ -2350,10 +2373,10 @@ static const char* check_frame_ids(const int32_t* ids, int64_t n, int64_t frame_
   return nullptr;
 }
 
-int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_frames, int64_t frame_ptr,
+// the arguments of an add to a frame ring of either kind, every frame id included (DSACT_OK: nothing has been copied yet)
+static int check_frame_rows(dsact_handle* h, const void* frames, int64_t n_frames, int64_t frame_ptr,
                             const int32_t* obs_frames, const int32_t* obs2_frames, const float* act, const float* rew,
-                            const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
-  if (!h || !h->rb_bound || !h->rb_frames) return fail(DSACT_ESTATE, "frame replay ring not bound");
+                            const float* done, const float* logp, int64_t n, int64_t ptr) {
   const dsact_frame_replay& r = h->fr;
   if (n < 0 || n > r.capacity || ptr < 0 || ptr >= r.capacity) return fail(DSACT_EINVAL, "bad n/ptr");
   if (n_frames < 0 || n_frames > r.frame_capacity || frame_ptr < 0 || frame_ptr >= r.frame_capacity)
@@ -2367,7 +2390,15 @@ int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_fram
     if (!bad) bad = check_frame_ids(obs2_frames, n * K, r.frame_capacity);
     if (bad) return fail(DSACT_EINVAL, "frame-id table: %s", bad);
   }
-  const cudaStream_t s = (cudaStream_t)stream;
+  return DSACT_OK;
+}
+
+// the copies of a checked add: frames of F elements of `elem_bytes` each, and the rows
+static int put_frame_rows(dsact_handle* h, const void* frames, size_t elem_bytes, int64_t n_frames, int64_t frame_ptr,
+                          const int32_t* obs_frames, const int32_t* obs2_frames, const float* act, const float* rew,
+                          const float* done, const float* logp, int64_t n, int64_t ptr, cudaStream_t s) {
+  const dsact_frame_replay& r = h->fr;
+  const int64_t K = r.frames_per_obs;
   // n items of w elements of `bytes` each from src into ring dst of `cap` items, starting at item p
   auto put = [&](void* dst, const void* src, int64_t cnt, int64_t p, int64_t cap, int64_t w, size_t bytes) -> cudaError_t {
     const int64_t first = (p + cnt <= cap) ? cnt : cap - p;
@@ -2376,7 +2407,7 @@ int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_fram
       e = cudaMemcpyAsync(dst, (const char*)src + first * w * bytes, (cnt - first) * w * bytes, cudaMemcpyDefault, s);
     return e;
   };
-  if (n_frames > 0) CUDA_TRY(put(r.frames, frames, n_frames, frame_ptr, r.frame_capacity, h->obs_elems / K, sizeof(float)));
+  if (n_frames > 0) CUDA_TRY(put(r.frames, frames, n_frames, frame_ptr, r.frame_capacity, h->obs_elems / K, elem_bytes));
   if (n > 0) {
     CUDA_TRY(put(r.obs_frames, obs_frames, n, ptr, r.capacity, K, sizeof(int32_t)));
     CUDA_TRY(put(r.obs2_frames, obs2_frames, n, ptr, r.capacity, K, sizeof(int32_t)));
@@ -2386,6 +2417,37 @@ int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_fram
     CUDA_TRY(put(r.logp, logp, n, ptr, r.capacity, 1, sizeof(float)));
   }
   return DSACT_OK;
+}
+
+int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_frames, int64_t frame_ptr,
+                            const int32_t* obs_frames, const int32_t* obs2_frames, const float* act, const float* rew,
+                            const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
+  if (!h || !h->rb_bound || !h->rb_frames) return fail(DSACT_ESTATE, "frame replay ring not bound");
+  if (h->rb_codes) return fail(DSACT_ESTATE, "a coded frame ring is bound: frames go in through dsact_replay_add_coded_frames");
+  if (int rc = check_frame_rows(h, frames, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr)) return rc;
+  return put_frame_rows(h, frames, sizeof(float), n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr,
+                        (cudaStream_t)stream);
+}
+
+int dsact_replay_add_coded_frames(dsact_handle* h, const uint8_t* codes, int64_t n_frames, int64_t frame_ptr,
+                                  const float* table, int32_t n_codes, const int32_t* obs_frames, const int32_t* obs2_frames,
+                                  const float* act, const float* rew, const float* done, const float* logp, int64_t n,
+                                  int64_t ptr, void* stream) {
+  if (!h || !h->rb_bound || !h->rb_codes) return fail(DSACT_ESTATE, "coded frame replay ring not bound");
+  if (n_codes < 0 || n_codes > 256) return fail(DSACT_EINVAL, "n_codes %d outside [0, 256]", (int)n_codes);
+  if (n_codes > 0 && !table) return fail(DSACT_EINVAL, "null table");
+  if (int rc = check_frame_rows(h, codes, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr)) return rc;
+  if (n_frames > 0) {   // the gather decodes through these codes: every one is checked before anything is copied
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, codes) != cudaSuccess) { cudaGetLastError(); return fail(DSACT_EINVAL, "codes: not a valid pointer"); }
+    if (at.type == cudaMemoryTypeDevice) return fail(DSACT_EINVAL, "codes: device memory (staged codes must be host memory)");
+    const int64_t m = n_frames * (h->obs_elems / h->fr.frames_per_obs);
+    for (int64_t i = 0; i < m; ++i)
+      if (codes[i] >= n_codes) return fail(DSACT_EINVAL, "codes: code %d at %lld is not below n_codes %d", (int)codes[i], (long long)i, (int)n_codes);
+  }
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (n_codes > 0) CUDA_TRY(cudaMemcpyAsync(h->fr_table, table, n_codes * sizeof(float), cudaMemcpyDefault, s));
+  return put_frame_rows(h, codes, 1, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr, s);
 }
 
 int dsact_replay_add(dsact_handle* h, const float* obs, const float* obs2, const float* act, const float* rew,

@@ -14,13 +14,19 @@ is K frames of obs_elems / K floats (an NCHW image with K = C: one channel each;
 row refers to the frames of the previous row's obs2 or of its own obs that it repeats (dsac_v2_b200/frame_plan.py).
 The minibatches are bit for bit those of the flat ring; the device memory is about half of it (K = 1, obs2_t = obs_{t+1})
 or less (stacked frames: one new frame per row).
+
+`dsact_replay_codes=True` (with `dsact_replay_frames`) stores the frames as 8-bit codes into a table of at most 256
+float32 values (the coded frame ring): a quarter of the frame bytes, for observations with at most 256 distinct values
+(8-bit images scaled to floats, such as `gym_carracingraw`'s rgb / 255).  Values are matched bit for bit; a store that
+brings a 257th distinct value raises ValueError and leaves the buffer as it was.  The minibatches are still bit for bit
+those of the flat ring.
 """
 __all__ = ["ReplayBuffer"]
 
 import numpy as np
 import torch
 
-from dsac_v2_b200.frame_plan import FramePlanner
+from dsac_v2_b200.frame_plan import FrameCoder, FramePlanner
 
 
 class ReplayBuffer:
@@ -44,6 +50,11 @@ class ReplayBuffer:
         self.planner = None
         if self.frames_per_obs is not None:
             self.planner = FramePlanner(self.max_size, int(self.frames_per_obs), self.obs_elems)
+        self.coder = None
+        if kwargs.get("dsact_replay_codes"):
+            if self.planner is None:
+                raise ValueError("dsact_replay_codes codes the frames of the frame ring: it needs dsact_replay_frames")
+            self.coder = FrameCoder()
         self.ptr, self.size = 0, 0
         self.engine = None
         self._stage = None      # pinned staging buffers
@@ -68,11 +79,13 @@ class ReplayBuffer:
                            for _ in range(self._STAGES)]
         else:
             pl = self.planner
-            engine.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K)
+            engine.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K, coded=self.coder is not None)
             ids = lambda: torch.zeros(R, pl.K, dtype=torch.int32).pin_memory()
-            # up to 2K new frames per row: the same bytes as the flat ring's obs + obs2 staging
-            self._stage = [dict(frames=pin(2 * R * pl.K, pl.F), obs_frames=ids(), obs2_frames=ids(), act=pin(R, A),
-                                rew=pin(R), done=pin(R), logp=pin(R)) for _ in range(self._STAGES)]
+            # up to 2K new frames per row: the same bytes as the flat ring's obs + obs2 staging (a quarter when coded)
+            fdt = torch.float32 if self.coder is None else torch.uint8
+            self._stage = [dict(frames=torch.zeros(2 * R * pl.K, pl.F, dtype=fdt).pin_memory(), obs_frames=ids(),
+                                obs2_frames=ids(), act=pin(R, A), rew=pin(R), done=pin(R), logp=pin(R))
+                           for _ in range(self._STAGES)]
             self._nframes, self._frame_ptr = 0, 0
         self._np = [{k: v.numpy() for k, v in s.items()} for s in self._stage]
         self._events = [None] * self._STAGES
@@ -89,7 +102,7 @@ class ReplayBuffer:
         if self.planner is None:
             new.bind_replay(self.max_size)
         else:
-            new.bind_replay_frames(self.max_size, self.planner.frame_capacity, self.planner.K)
+            new.bind_replay_frames(self.max_size, self.planner.frame_capacity, self.planner.K, coded=self.coder is not None)
         for k, v in old.replay.items():
             new.replay[k].copy_(v)
         self.engine = new
@@ -103,10 +116,12 @@ class ReplayBuffer:
         return self.size
 
     def __get_RAM__(self):
-        """MB of device memory holding valid transitions (frame ring: the frames they refer to, and their frame ids)."""
+        """MB of device memory holding valid transitions (frame ring: the frames they refer to, and their frame ids; coded
+        frame ring: one byte per frame value, and the table)."""
         if self.planner is not None:
             pl = self.planner
-            return (4 * pl.F * pl.held() + 4 * (2 * pl.K + self.act_dim + 3) * self.size) / 1e6
+            frames = 4 * pl.F * pl.held() if self.coder is None else pl.F * pl.held() + 4 * FrameCoder.N
+            return (frames + 4 * (2 * pl.K + self.act_dim + 3) * self.size) / 1e6
         row_bytes = 4 * (2 * self.obs_elems + self.act_dim + 3)
         return row_bytes * self.size / 1e6
 
@@ -114,6 +129,8 @@ class ReplayBuffer:
     def _store_row(self, obs, act, rew, next_obs, done, logp):
         if self.planner is not None:
             plan = self.planner.plan(obs, next_obs)
+            if self.coder is not None:   # (raises before anything changes)
+                codes, new_values = self.coder.encode(plan.bits[plan.new].view(np.float32))
             if plan.need > self.planner.frame_capacity:
                 self._grow(self.planner.grown_capacity(plan.need))
             # a flush copies at most frame_capacity frames: no two of its frames share a slot
@@ -132,6 +149,9 @@ class ReplayBuffer:
             K, m = self.planner.K, len(new)
             if self._fill == 0:
                 self._frame_ptr = frame_ptr
+            if self.coder is not None:
+                self.coder.commit(new_values)
+                new = codes
             s["frames"][self._nframes:self._nframes + m] = new
             self._nframes += m
             s["obs_frames"][i], s["obs2_frames"][i] = slots[:K], slots[K:]
@@ -145,6 +165,9 @@ class ReplayBuffer:
         row = (np.asarray(obs, dtype=np.float32), np.asarray(act, dtype=np.float32), float(rew),
                np.asarray(next_obs, dtype=np.float32), float(done), float(np.asarray(logp)))
         if self.engine is None:
+            if self.coder is not None:   # refuse an uncodable row now, not when the buffer is attached
+                _, new_values = self.coder.encode(np.concatenate([row[0].reshape(-1), row[3].reshape(-1)]))
+                self.coder.commit(new_values)
             self._pending.append(row)
         else:
             self._store_row(*row)
@@ -163,7 +186,11 @@ class ReplayBuffer:
             self.engine.replay_add(self._stage[self._cur], n, self.ptr)
         else:
             st = self._stage[self._cur]
-            self.engine.replay_add_frames(st["frames"], self._nframes, self._frame_ptr, st, n, self.ptr)
+            if self.coder is None:
+                self.engine.replay_add_frames(st["frames"], self._nframes, self._frame_ptr, st, n, self.ptr)
+            else:
+                self.engine.replay_add_coded_frames(st["frames"], self._nframes, self._frame_ptr, self.coder.table,
+                                                    self.coder.n, st, n, self.ptr)
             self._nframes = 0
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.engine.device))
@@ -179,9 +206,9 @@ class ReplayBuffer:
         with torch.cuda.device(eng.device):
             old = eng.replay
             src, dst = (torch.from_numpy(x).to(eng.device) for x in pl.moves(frame_capacity))
-            eng.bind_replay_frames(self.max_size, frame_capacity, pl.K)
+            eng.bind_replay_frames(self.max_size, frame_capacity, pl.K, coded=self.coder is not None)
             eng.replay["frames"][dst] = old["frames"][src]
-            for k in ("act", "rew", "done", "logp"):
+            for k in ("act", "rew", "done", "logp") + (("table",) if self.coder is not None else ()):
                 eng.replay[k].copy_(old[k])
             pl.frame_capacity = frame_capacity
             self._put_ids()
@@ -196,11 +223,14 @@ class ReplayBuffer:
     # ---- full-state checkpoint (SURVEY §8f rank 3) ---------------------------------------
     def state_dict(self, with_data: bool = True) -> dict:
         """ptr/size (+ the valid transitions, fetched from the device ring) for an exact resume.  Frame ring: the planner's
-        state and the frames its rows refer to, in serial order, instead of obs / obs2 rows."""
+        state and the frames its rows refer to, in serial order, instead of obs / obs2 rows.  Coded frame ring: those
+        frames' codes, and the coder's table."""
         self.flush()
         out = {"ptr": self.ptr, "size": self.size, "max_size": self.max_size}
         if self.planner is not None:
             out["frame_planner"] = self.planner.state_dict()
+        if self.coder is not None:
+            out["frame_coder"] = self.coder.state_dict()
         if with_data and self.engine is not None:
             torch.cuda.current_stream(self.engine.device).synchronize()
             if self.planner is None:
@@ -216,17 +246,20 @@ class ReplayBuffer:
         self._require_engine()
         if state["max_size"] != self.max_size:
             raise ValueError("replay capacity differs from the checkpoint")
-        if ("frame_planner" in state) != (self.planner is not None):
-            raise ValueError("the checkpoint's replay ring kind (flat / frame ring) differs from this buffer's")
+        if ("frame_planner" in state) != (self.planner is not None) or ("frame_coder" in state) != (self.coder is not None):
+            raise ValueError("the checkpoint's replay ring kind (flat / frame / coded frame ring) differs from this buffer's")
         self.ptr, self.size, self._fill = int(state["ptr"]), int(state["size"]), 0
         if self.planner is not None:
             pl = self.planner
             pl.load_state_dict(state["frame_planner"])
             eng = self.engine
             if eng.replay["frames"].shape[0] != pl.frame_capacity:
-                eng.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K)
+                eng.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K, coded=self.coder is not None)
             self._nframes = 0
             self._put_ids()
+            if self.coder is not None:
+                self.coder.load_state_dict(state["frame_coder"])
+                eng.replay["table"].copy_(torch.from_numpy(self.coder.table.copy()))
             if "data" in state:
                 _, dst = pl.moves(pl.frame_capacity)
                 eng.replay["frames"][torch.from_numpy(dst).to(eng.device)] = state["data"]["frames"].to(eng.device)

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -351,10 +352,12 @@ class Engine:
             check(self.lib.dsact_replay_bind(self.h, C.byref(rb)))
         self.capacity = int(capacity)
 
-    def bind_replay_frames(self, capacity: int, frame_capacity: int, frames_per_obs: int):
+    def bind_replay_frames(self, capacity: int, frame_capacity: int, frames_per_obs: int, coded: bool = False):
         """Bind a frame ring (dsact_replay_bind_frames): `capacity` rows whose obs / obs2 are `frames_per_obs` (K) frame
         ids each into a store of `frame_capacity` frames of obs_elems / K floats.  `replay` then holds `frames`,
-        `obs_frames`, `obs2_frames` (int32 [capacity, K]), `act`, `rew`, `done`, `logp`."""
+        `obs_frames`, `obs2_frames` (int32 [capacity, K]), `act`, `rew`, `done`, `logp`.
+        coded: the coded frame ring (dsact_replay_bind_coded_frames): `frames` holds uint8 codes, and `table` (256
+        floats, zeros until replay_add_coded_frames fills them) their values."""
         O, A, K = self.obs_elems, self.cfg.act_dim, int(frames_per_obs)
         capacity, frame_capacity = int(capacity), int(frame_capacity)
         if not 1 <= K <= 64 or O % K:
@@ -364,13 +367,42 @@ class Engine:
         with torch.cuda.device(self.device):
             z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)
             ids = lambda: torch.zeros(capacity, K, dtype=torch.int32, device=self.device)
-            self.replay = dict(frames=z(frame_capacity, O // K), obs_frames=ids(), obs2_frames=ids(), act=z(capacity, A),
+            frames = (torch.zeros(frame_capacity, O // K, dtype=torch.uint8, device=self.device) if coded
+                      else z(frame_capacity, O // K))
+            self.replay = dict(frames=frames, obs_frames=ids(), obs2_frames=ids(), act=z(capacity, A),
                                rew=z(capacity), done=z(capacity), logp=z(capacity))
+            if coded:
+                self.replay["table"] = z(256)
             r = self.replay
             rb = _lib.FrameReplay(*(r[k].data_ptr() for k in ("frames", "obs_frames", "obs2_frames", "act", "rew", "done",
                                                               "logp")), capacity, frame_capacity, K)
-            check(self.lib.dsact_replay_bind_frames(self.h, C.byref(rb)))
+            if coded:
+                check(self.lib.dsact_replay_bind_coded_frames(self.h, C.byref(rb), r["table"].data_ptr()))
+            else:
+                check(self.lib.dsact_replay_bind_frames(self.h, C.byref(rb)))
         self.capacity = capacity
+
+    def bind_replay_coded_frames(self, capacity: int, frame_capacity: int, frames_per_obs: int):
+        """Bind a coded frame ring (dsact_replay_bind_coded_frames): bind_replay_frames with uint8 codes for frames."""
+        self.bind_replay_frames(capacity, frame_capacity, frames_per_obs, coded=True)
+
+    def replay_add_coded_frames(self, codes: Optional[torch.Tensor], n_frames: int, frame_ptr: int, table: np.ndarray,
+                                n_codes: int, rows: Dict[str, torch.Tensor], n: int, ptr: int):
+        """dsact_replay_add_coded_frames: `n_frames` frames of codes (contiguous uint8 HOST tensor) -> frame slots
+        (frame_ptr + i) % frame_capacity, table[:n_codes] (float32, host) -> the device table; the rows as in
+        replay_add_frames."""
+        r = rows
+        for k, dt, t in (("codes", torch.uint8, codes), ("obs_frames", torch.int32, r["obs_frames"]),
+                         ("obs2_frames", torch.int32, r["obs2_frames"])):
+            if t is not None and (t.device.type != "cpu" or t.dtype != dt or not t.is_contiguous()):
+                raise ValueError(f"{k} must be a contiguous {dt} host tensor")
+        table = np.ascontiguousarray(table, np.float32)
+        with torch.cuda.device(self.device):
+            check(self.lib.dsact_replay_add_coded_frames(self.h, _ptr(codes), int(n_frames), int(frame_ptr),
+                                                         table.ctypes.data, int(n_codes), r["obs_frames"].data_ptr(),
+                                                         r["obs2_frames"].data_ptr(), r["act"].data_ptr(),
+                                                         r["rew"].data_ptr(), r["done"].data_ptr(), r["logp"].data_ptr(),
+                                                         int(n), int(ptr), self._stream()))
 
     def replay_add_frames(self, frames: Optional[torch.Tensor], n_frames: int, frame_ptr: int, rows: Dict[str, torch.Tensor],
                           n: int, ptr: int):

@@ -134,3 +134,84 @@ class FramePlanner:
         self.serials, self.first = np.array(st["serials"], np.int64), np.array(st["first"], np.int64)
         self.prev_bits = None if st["prev_bits"] is None else np.array(st["prev_bits"], np.uint32)
         self.prev_serials = None if st["prev_serials"] is None else np.array(st["prev_serials"], np.int64)
+
+
+class FrameCoder:
+    """Host coder of the coded frame ring (dsact_replay_bind_coded_frames): float32 values -> uint8 codes through a table
+    of up to 256 values.  Values are matched on their bit patterns (so -0.0 and 0.0, and NaNs of different payloads, are
+    different values) and take codes in order of first appearance.  The table is a bijection between codes and the bit
+    patterns seen, so comparing codes is comparing values.
+
+    Lookup: a multiplicative hash (bits * mul mod 2^32) >> 16 into 65536 slots, with `mul` chosen so that no two table
+    entries share a slot; a value is known when its slot holds its own bit pattern.  A few vector operations per value,
+    and no Python loop over values."""
+    N = 256
+    _SHIFT = 16
+
+    def __init__(self):
+        self.bits = np.zeros(self.N, np.uint32)   # table: code -> bit pattern
+        self.n = 0
+        self._mul = np.uint32(0x9E3779B1)
+        self._used = np.zeros(1 << (32 - self._SHIFT), bool)    # slot -> (holds an entry, its pattern, its code)
+        self._slot_bits = np.zeros(1 << (32 - self._SHIFT), np.uint32)
+        self._slot_code = np.zeros(1 << (32 - self._SHIFT), np.uint8)
+
+    @property
+    def table(self) -> np.ndarray:
+        """float32 [256]: code -> value (entries from n on are unused)."""
+        return self.bits.view(np.float32)
+
+    def _slots(self, flat: np.ndarray, mul) -> np.ndarray:
+        return (flat * mul) >> np.uint32(self._SHIFT)
+
+    def encode(self, values: np.ndarray):
+        """(uint8 codes of `values`' shape, bit patterns the table does not hold yet, in order of first appearance).
+        Changes nothing; ValueError when the table would need more than 256 entries."""
+        b = np.ascontiguousarray(values, np.float32).view(np.uint32)
+        flat = b.reshape(-1)
+        s = self._slots(flat, self._mul)
+        known = self._used[s] & (self._slot_bits[s] == flat)
+        codes = self._slot_code[s]
+        if known.all():
+            return codes.reshape(b.shape), flat[:0]
+        miss = ~known
+        uniq, first, inv = np.unique(flat[miss], return_index=True, return_inverse=True)
+        order = np.argsort(first)
+        new = uniq[order]
+        if self.n + len(new) > self.N:
+            v = new[self.N - self.n]
+            raise ValueError(f"the coded replay ring holds at most {self.N} distinct observation values; "
+                             f"{np.array(v, np.uint32).view(np.float32).item()!r} (bits 0x{int(v):08x}) would be value "
+                             f"{self.N + 1}: the observations are not 8-bit quantised")
+        rank = np.empty(len(uniq), np.int64)
+        rank[order] = np.arange(len(uniq))
+        codes[miss] = (self.n + rank[inv.reshape(-1)]).astype(np.uint8)
+        return codes.reshape(b.shape), new
+
+    def commit(self, new: np.ndarray) -> None:
+        """Append the patterns `encode` returned to the table."""
+        if len(new) == 0:
+            return
+        self.bits[self.n:self.n + len(new)] = new
+        self.n += len(new)
+        bits = self.bits[:self.n]
+        mul, g = self._mul, np.random.default_rng(self.n)
+        while len(np.unique(self._slots(bits, mul))) != self.n:   # a collision: another odd multiplier
+            mul = np.uint32(int(g.integers(0, 2 ** 31)) * 2 + 1)
+        self._mul = mul
+        s = self._slots(bits, mul)
+        self._used[:] = False
+        self._used[s] = True
+        self._slot_bits[s] = bits
+        self._slot_code[s] = np.arange(self.n).astype(np.uint8)
+
+    def state_dict(self) -> dict:
+        return {"bits": self.bits[:self.n].copy()}
+
+    def load_state_dict(self, st: dict) -> None:
+        bits = np.asarray(st["bits"], np.uint32)
+        if len(bits) > self.N or len(np.unique(bits)) != len(bits):
+            raise ValueError("frame coder state: not a table of at most 256 distinct values")
+        self.bits[:] = 0
+        self.n = 0
+        self.commit(bits)

@@ -223,6 +223,22 @@ int dsact_replay_bind_frames(dsact_handle *h, const dsact_frame_replay *rb);
 int dsact_replay_add_frames(dsact_handle *h, const float *frames, int64_t n_frames, int64_t frame_ptr,
                             const int32_t *obs_frames, const int32_t *obs2_frames, const float *act, const float *rew,
                             const float *done, const float *logp, int64_t n, int64_t ptr, void *stream);
+/* ---- coded frame replay ring: frames of 8-bit codes ----
+ * A frame ring whose frame store holds one uint8 code per value (rb->frames points to uint8 [frame_capacity,
+ * obs_elems / frames_per_obs]) and a device table of 256 floats: code c stands for table[c], bit for bit.  For sources
+ * with at most 256 distinct values (8-bit images scaled to floats) it stores a quarter of the fp32 frame ring's bytes,
+ * and every gather yields bit for bit what the fp32 frame ring holding the decoded frames would.
+ * dsact_replay_bind_coded_frames: the checks of dsact_replay_bind_frames, and DSACT_EINVAL for a null table.  Binding
+ * any ring kind replaces the others. */
+int dsact_replay_bind_coded_frames(dsact_handle *h, const dsact_frame_replay *rb, const float *table);
+/* dsact_replay_add_frames for a coded ring: n_frames frames of codes (HOST uint8) and table[0, n_codes) (host or device)
+ * copied into the device table's first n_codes entries.  Every code is checked against n_codes, and n_codes against
+ * [0, 256], before anything is copied (DSACT_EINVAL otherwise).  A coded ring refuses dsact_replay_add_frames
+ * (DSACT_ESTATE), and every other ring kind refuses this call. */
+int dsact_replay_add_coded_frames(dsact_handle *h, const uint8_t *codes, int64_t n_frames, int64_t frame_ptr,
+                                  const float *table, int32_t n_codes, const int32_t *obs_frames,
+                                  const int32_t *obs2_frames, const float *act, const float *rew, const float *done,
+                                  const float *logp, int64_t n, int64_t ptr, void *stream);
 /* sample_batch(): gather rows idx[i] (device int64, or NULL = draw uniformly in [0,size) on
  * the device) into the engine's batch arena; `out` receives the arena's device pointers */
 int dsact_replay_sample(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx,
