@@ -153,6 +153,7 @@ SYMBOLS = {
     "dsact_create": (C.c_int, [C.POINTER(Config), C.c_int, C.POINTER(C.c_void_p)]),
     "dsact_destroy": (None, [C.c_void_p]),
     "dsact_bind": (C.c_int, [C.c_void_p, C.POINTER(Buffers)]),
+    "dsact_set_output_activations": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "dsact_seed": (C.c_int, [C.c_void_p, C.c_uint64]),
     "dsact_set_carry": (C.c_int, [C.c_void_p, C.c_float, C.c_float, C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_void_p]),

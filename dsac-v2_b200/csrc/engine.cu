@@ -200,6 +200,10 @@ struct dsact_handle {
   double td_bound = 20.0;    // DSAC_V1's TD bound (dsac_v1.py:79)
   StepSlots slot = {};
   StepHyper hyper = {};
+  // output activations (dsact_set_output_activations; fixed at bind): ACT_* codes of the critics' outputs and of the
+  // policy's mean / log_std halves
+  OutActs oa = {ACT_LINEAR, ACT_LINEAR, ACT_LINEAR};
+  bool outact() const { return oa.q != ACT_LINEAR || oa.mean != ACT_LINEAR || oa.ls != ACT_LINEAR; }
   dsact_buffers buf = {};
   bool bound = false, rb_bound = false;
   uint64_t seed = 0x5DEECE66Dull;
@@ -1241,8 +1245,9 @@ static void enqueue_sample(const dsact_handle* h, const RowIo& io, int B, bool a
   a.out_q[0] = io.out_q[0]; a.out_q[1] = io.out_q[h->v1 ? 0 : 1];
   a.advance_rng = advance_rng ? 1 : 0;
   a.v1_stats = h->v1 ? 1 : 0;
+  a.oa = h->oa;
   int blocks = (B + 7) / 8; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-  launch_k(sample_kernel, dim3(capped(blocks, max_blocks), 2), 256, 0, c, a);
+  launch_k(h->outact() ? sample_kernel<true> : sample_kernel<false>, dim3(capped(blocks, max_blocks), 2), 256, 0, c, a);
   c.done();
 }
 
@@ -1259,8 +1264,9 @@ static void enqueue_loss(const dsact_handle* h, const RowIo& io, int B, const St
     a.img_q[k] = io.img_q[k]; a.img_qa[k] = io.img_qa[k];
   }
   a.state = h->buf.state; a.B = B; a.gamma = (float)h->hyper.gamma; a.inv_global_batch = sc.inv_global_batch;
+  a.act_q = h->oa.q;
   int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;   // latency bound: spread over the SMs
-  launch_k(loss_kernel, capped(blocks, max_blocks), 64, 0, c, a);
+  launch_k(h->outact() ? loss_kernel<true> : loss_kernel<false>, capped(blocks, max_blocks), 64, 0, c, a);
   c.done();
 }
 
@@ -1274,8 +1280,9 @@ static void enqueue_loss_v1(const dsact_handle* h, const RowIo& io, int B, const
   a.state = h->buf.state; a.B = B; a.bound = h->v1_bound; a.gamma = (float)h->hyper.gamma; a.inv_global_batch = sc.inv_global_batch;
   a.td_bound = (float)h->td_bound; a.sc = sc;
   a.img_q = io.img_q[0]; a.img_qa = io.img_qa[0];
+  a.act_q = h->oa.q;
   int blocks = (B + 63) / 64; if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
-  launch_k(loss_v1_kernel, capped(blocks, max_blocks), 64, 0, c, a);
+  launch_k(h->outact() ? loss_v1_kernel<true> : loss_v1_kernel<false>, capped(blocks, max_blocks), 64, 0, c, a);
   c.done();
 }
 
@@ -1294,8 +1301,11 @@ static void enqueue_policy_grad(const dsact_handle* h, const RowIo& io, int B, c
   a.img_ls = io.split_dlogits ? io.img_dlogits_ls : io.img_dlogits;
   a.ls_col = io.split_dlogits ? 0 : A;
   a.sc = sc;
+  a.oa = h->oa;
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms; if (blocks < 1) blocks = 1;   // a warp per row
-  launch_k(one_critic ? policy_grad_kernel<1> : policy_grad_kernel<2>, capped(blocks, max_blocks), 256, sizeof(float) * 2 * A, c, a);
+  auto* k = h->outact() ? (one_critic ? policy_grad_kernel<1, true> : policy_grad_kernel<2, true>)
+                        : (one_critic ? policy_grad_kernel<1, false> : policy_grad_kernel<2, false>);
+  launch_k(k, capped(blocks, max_blocks), 256, sizeof(float) * 2 * A, c, a);
   c.done();
 }
 
@@ -2112,6 +2122,18 @@ int dsact_bind(dsact_handle* h, const dsact_buffers* b) {
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMemset(m->W() + m->ar.slabs, 0, sizeof(float) * (size_t)m->ar.nslabs * m->ar.slab_stride));
   }
+  return DSACT_OK;
+}
+
+int dsact_set_output_activations(dsact_handle* h, int32_t value_act, int32_t policy_act) {
+  if (!h) return fail(DSACT_EINVAL, "null handle");
+  if (h->bound) return fail(DSACT_ESTATE, "dsact_set_output_activations: call it before dsact_bind");
+  for (int32_t a : {value_act, policy_act})
+    if (a < DSACT_ACT_LINEAR || a > DSACT_ACT_SELU) return fail(DSACT_EINVAL, "unknown output activation %d", a);
+  // std_type "parameter": the log_std half is the learnable row, which the reference does not activate
+  const bool ls_row = h->engine == ENGINE_MLP ? mlp(h)->cfg.policy_std == DSACT_STD_PARAMETER
+                                              : static_cast<HeadsHandle*>(h)->pi.ls_row >= 0;
+  h->oa = OutActs{value_act, policy_act, ls_row ? (int)DSACT_ACT_LINEAR : policy_act};
   return DSACT_OK;
 }
 

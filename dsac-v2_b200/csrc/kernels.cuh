@@ -8,6 +8,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "gemm_simt.cuh"   // act_fwd / act_bwd
+
 namespace dsact {
 
 constexpr float TG_EPS = 1e-6f;          // utils/act_distribution_cls.py:3
@@ -343,6 +345,13 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
   }
 }
 
+// Output activations of the networks (networks/mlp.py, networks/cnn.py: `output_activation` of the last layer), as
+// ACT_* codes: the output GEMMs stay linear and write z; the row kernels read y = act(z) and multiply every output
+// gradient they write by act'(z).  q: every critic output; mean / ls: the two halves of the policy's (mean | log_std)
+// row (ls is linear for std_type "parameter", whose log_std row the reference does not activate).  The row kernels
+// take a compile-time OUTACT switch: the linear instantiation never reads these codes.
+struct OutActs { int q, mean, ls; };
+
 // TanhGaussDistribution.rsample (utils/act_distribution_cls.py:44-54) on the raw policy-head output
 // (mean | log_std), with StochaPolicy's std = exp(clamp(log_std)) (networks/mlp.py:89-92) folded in.
 // blockIdx.y = 0: online policy on obs with eps1 (+ the two logged means, dsac_v2.py:155-157);
@@ -363,6 +372,7 @@ struct SampleArgs {
   int gauss;               // 1: GaussDistribution (utils/act_distribution_cls.py:82-116): no squashing, no action limits
   int v1_stats = 0;        // 1: DSAC_V1's logged policy_mean / policy_std (dsac_v1.py:142-143): tanh(logits[..., 0]) and
                            // logits[..., 1] of cat(mean, std), i.e. the first mean and the SECOND entry of the 2A-wide row
+  OutActs oa;              // output activations (read by the OUTACT instantiation only)
 };
 // One action component of TanhGaussDistribution.rsample: the squashed, scaled action and its log-prob term
 // (gauss: GaussDistribution.rsample, the raw Gaussian sample and Normal.log_prob).
@@ -386,6 +396,8 @@ __device__ __forceinline__ void sample_elem(float mean, float ls, float eps, flo
   tanh_mean = tanhf(mean);
   sd_out = sd;
 }
+// OUTACT: the (mean | log_std) row and the critics' raw std go through the output activations `a.oa` first
+template <bool OUTACT>
 __global__ void sample_kernel(const __grid_constant__ SampleArgs a) {
   pdl_sync();
   __shared__ float red[2 * 32];
@@ -400,15 +412,17 @@ __global__ void sample_kernel(const __grid_constant__ SampleArgs a) {
     float lp = 0.f;
     for (int j = lane; j < A; j += 32) {
       float act, lpj, tm, sd;
-      sample_elem(logits[(size_t)row * 2 * A + j], logits[(size_t)row * 2 * A + A + j], eps[(size_t)row * A + j], a.hi[j], a.lo[j],
-                  a.min_log_std, a.max_log_std, act, lpj, tm, sd, a.gauss != 0);
+      float mean = logits[(size_t)row * 2 * A + j], ls = logits[(size_t)row * 2 * A + A + j];
+      if constexpr (OUTACT) { mean = act_fwd(mean, a.oa.mean); ls = act_fwd(ls, a.oa.ls); }
+      sample_elem(mean, ls, eps[(size_t)row * A + j], a.hi[j], a.lo[j], a.min_log_std, a.max_log_std, act, lpj, tm, sd, a.gauss != 0);
       a.act[which][(size_t)row * A + j] = act;
       img_put(a.img[which], row, j, act);
       lp += lpj;
       if (!a.v1_stats) { sums[0] += tm; sums[1] += sd; }
       else {
         if (j == 0) sums[0] += tm;
-        if (A == 1 ? j == 0 : j == 1) sums[1] += A == 1 ? sd : logits[(size_t)row * 2 * A + j];
+        // (j == 1 < A: the mean of action component 1)
+        if (A == 1 ? j == 0 : j == 1) sums[1] += A == 1 ? sd : (OUTACT ? mean : logits[(size_t)row * 2 * A + j]);
       }
     }
     lp = warp_sum(lp);
@@ -423,8 +437,13 @@ __global__ void sample_kernel(const __grid_constant__ SampleArgs a) {
   } else {
     float sd[2] = {0.f, 0.f};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.B; i += gridDim.x * blockDim.x) {
-      sd[0] += softplus_f(a.out_q[0][2 * i + 1]);
-      sd[1] += softplus_f(a.out_q[1][2 * i + 1]);
+      if constexpr (OUTACT) {
+        sd[0] += softplus_f(act_fwd(a.out_q[0][2 * i + 1], a.oa.q));
+        sd[1] += softplus_f(act_fwd(a.out_q[1][2 * i + 1], a.oa.q));
+      } else {
+        sd[0] += softplus_f(a.out_q[0][2 * i + 1]);
+        sd[1] += softplus_f(a.out_q[1][2 * i + 1]);
+      }
     }
     block_sum<2>(sd, red);
     if (threadIdx.x == 0) {
@@ -468,6 +487,7 @@ struct LossArgs {
   float gamma, inv_global_batch;
   ImgOut img_q[2], img_qa[2];
   StepScalars sc;
+  int act_q;                // output activation of the critics (OUTACT instantiation)
 };
 // Everything the loss needs of ONE sample (dsac_v2.py:218-318): gradients w.r.t. the critics' outputs on (s,a) and on
 // (s,a~), the per-sample loss terms and the logged values.  m[k] = mean_std of critic k, alpha = temperature in use.
@@ -477,11 +497,14 @@ struct LossRow {
   float q[2], sd[2];           // Q_k(s,a) mean and softplus std
   float loss_q, loss_pi, logp_new;
 };
+// OUTACT: every critic output is read as y = act(z) (a.act_q), and every gradient w.r.t. one is multiplied by act'(z)
+template <bool OUTACT>
 __device__ __forceinline__ LossRow loss_row(const LossArgs& a, int i, const float (&m)[2], float alpha) {
   LossRow R;
   const float invB = a.inv_global_batch;
-  const float q1n = a.out_qt[0][2 * i], s1n = softplus_f(a.out_qt[0][2 * i + 1]);
-  const float q2n = a.out_qt[1][2 * i], s2n = softplus_f(a.out_qt[1][2 * i + 1]);
+  auto outq = [&](float z) { if constexpr (OUTACT) return act_fwd(z, a.act_q); else return z; };
+  const float q1n = outq(a.out_qt[0][2 * i]), s1n = softplus_f(outq(a.out_qt[0][2 * i + 1]));
+  const float q2n = outq(a.out_qt[1][2 * i]), s2n = softplus_f(outq(a.out_qt[1][2 * i + 1]));
   const float zc3 = fminf(fmaxf(a.z3[i], -3.f), 3.f), zc4 = fminf(fmaxf(a.z4[i], -3.f), 3.f);
   const float qn = fminf(q1n, q2n);
   const float qn_s = q1n < q2n ? q1n + zc3 * s1n : q2n + zc4 * s2n;  // dsac_v2.py:252-253
@@ -491,7 +514,8 @@ __device__ __forceinline__ LossRow loss_row(const LossArgs& a, int i, const floa
   R.loss_q = 0.f;
 #pragma unroll
   for (int k = 0; k < 2; ++k) {
-    const float q = a.out_q[k][2 * i], raw = a.out_q[k][2 * i + 1];
+    const float zq = a.out_q[k][2 * i], zraw = a.out_q[k][2 * i + 1];
+    const float q = outq(zq), raw = outq(zraw);
     const float sd = softplus_f(raw);
     const float b3 = 3.f * m[k];
     const float yb = q + fminf(fmaxf(ys - q, -b3), b3);  // dsac_v2.py:299-301
@@ -502,17 +526,23 @@ __device__ __forceinline__ LossRow loss_row(const LossArgs& a, int i, const floa
     R.g_mean[k] = w * fminf(fmaxf(dq, -HUBER_DELTA), HUBER_DELTA) * invB;
     const float dsoft = raw > 20.f ? 1.f : 1.f / (1.f + expf(-raw));
     R.g_raw[k] = w * sterm * invB * dsoft;
+    if constexpr (OUTACT) { R.g_mean[k] *= act_bwd(zq, a.act_q); R.g_raw[k] *= act_bwd(zraw, a.act_q); }
     R.q[k] = q;
     R.sd[k] = sd;
   }
   // actor: L_pi = mean(alpha*logp - min(q1pi, q2pi)), dsac_v2.py:304-310; ties split like torch.min
-  const float q1p = a.out_qa[0][2 * i], q2p = a.out_qa[1][2 * i];
+  const float q1p = outq(a.out_qa[0][2 * i]), q2p = outq(a.out_qa[1][2 * i]);
   R.logp_new = a.logp_new[i];
   R.loss_pi = alpha * R.logp_new - fminf(q1p, q2p);
   R.g_pa[0] = q1p < q2p ? -invB : (q1p == q2p ? -0.5f * invB : 0.f);
   R.g_pa[1] = q2p < q1p ? -invB : (q1p == q2p ? -0.5f * invB : 0.f);
+  if constexpr (OUTACT) {
+    R.g_pa[0] *= act_bwd(a.out_qa[0][2 * i], a.act_q);
+    R.g_pa[1] *= act_bwd(a.out_qa[1][2 * i], a.act_q);
+  }
   return R;
 }
+template <bool OUTACT>
 __global__ void loss_kernel(const __grid_constant__ LossArgs a) {
   pdl_sync();
   __shared__ float red[10 * 32];
@@ -523,7 +553,7 @@ __global__ void loss_kernel(const __grid_constant__ LossArgs a) {
   float gb_q2_raw = 0.f;
   float mn[2] = {__int_as_float(0x7f800000), __int_as_float(0x7f800000)};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.B; i += gridDim.x * blockDim.x) {
-    const LossRow R = loss_row(a, i, m, alpha);
+    const LossRow R = loss_row<OUTACT>(a, i, m, alpha);
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       a.d_out_q[k][2 * i] = R.g_mean[k];
@@ -575,6 +605,7 @@ struct LossV1Args {
   float gamma, inv_global_batch, td_bound;
   StepScalars sc;
   ImgOut img_q, img_qa;                   // bf16 images of d_out_q / d_out_qa (the MLP engine's dgrad chain reads them)
+  int act_q;                              // output activation of the critic (OUTACT instantiation)
 };
 
 // __compute_loss_q / __compute_target_q / __compute_loss_policy of dsac_v1.py:195-248, one thread per sample:
@@ -582,17 +613,20 @@ struct LossV1Args {
 //   bound:  L = mean( -(target - q)/(sigma^2 + 0.1) q - ((q - target_b)^2 - sigma^2)/(sigma^3 + 0.1) sigma )   (coefficients detached)
 //   else:   L = mean( -log N(target; q, sigma) )
 //   actor:  L_pi = mean( alpha logp - q(s,a~) )
+// OUTACT: the critic's outputs are read as y = act(z) (a.act_q), and every gradient w.r.t. one is multiplied by act'(z)
+template <bool OUTACT>
 __global__ void loss_v1_kernel(const __grid_constant__ LossV1Args a) {
   pdl_sync();
   __shared__ float red[6 * 32];
   const float alpha = step_alpha(a.sc);
   const float invB = a.inv_global_batch;
+  auto outq = [&](float z) { if constexpr (OUTACT) return act_fwd(z, a.act_q); else return z; };
   float s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // q, sigma, loss_pi, logp, gb_mean, gb_raw
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.B; i += gridDim.x * blockDim.x) {
-    const float qn = a.out_qt[2 * i], sn = softplus_f(a.out_qt[2 * i + 1]);
+    const float qn = outq(a.out_qt[2 * i]), sn = softplus_f(outq(a.out_qt[2 * i + 1]));
     const float zc = fminf(fmaxf(a.z[i], -3.f), 3.f);
     const float target = a.rew[i] + (1.f - a.done[i]) * a.gamma * ((qn + zc * sn) - alpha * a.logp2[i]);
-    const float q = a.out_q[2 * i], raw = a.out_q[2 * i + 1];
+    const float q = outq(a.out_q[2 * i]), raw = outq(a.out_q[2 * i + 1]);
     const float sd = softplus_f(raw);
     float g_mean, g_sd;
     if (a.bound) {
@@ -606,15 +640,21 @@ __global__ void loss_v1_kernel(const __grid_constant__ LossV1Args a) {
       g_sd = (1.f / sd - d * d / (sd * sd * sd)) * invB;
     }
     const float dsoft = raw > 20.f ? 1.f : 1.f / (1.f + expf(-raw));
-    const float g_raw = g_sd * dsoft;
+    float g_raw = g_sd * dsoft;
+    float g_qa = -invB;
+    if constexpr (OUTACT) {
+      g_mean *= act_bwd(a.out_q[2 * i], a.act_q);
+      g_raw *= act_bwd(a.out_q[2 * i + 1], a.act_q);
+      g_qa *= act_bwd(a.out_qa[2 * i], a.act_q);
+    }
     a.d_out_q[2 * i] = g_mean;
     a.d_out_q[2 * i + 1] = g_raw;
     img_put(a.img_q, i, 0, g_mean); img_put(a.img_q, i, 1, g_raw);
     const float lp = a.logp_new[i];
-    a.d_out_qa[2 * i] = -invB;
+    a.d_out_qa[2 * i] = g_qa;
     a.d_out_qa[2 * i + 1] = 0.f;
-    img_put(a.img_qa, i, 0, -invB); img_put(a.img_qa, i, 1, 0.f);
-    s[0] += q; s[1] += sd; s[2] += alpha * lp - a.out_qa[2 * i]; s[3] += lp; s[4] += g_mean; s[5] += g_raw;
+    img_put(a.img_qa, i, 0, g_qa); img_put(a.img_qa, i, 1, 0.f);
+    s[0] += q; s[1] += sd; s[2] += alpha * lp - outq(a.out_qa[2 * i]); s[3] += lp; s[4] += g_mean; s[5] += g_raw;
   }
   block_sum<6>(s, red);
   if (threadIdx.x == 0) {
@@ -645,15 +685,19 @@ struct PolicyGradArgs {
   int ls_col;        // head), an image of its own at column 0 (a separate log_std head), or none (a log_std row)
   StepScalars sc;
   int gauss;         // 1: GaussDistribution (a~ = u, log-prob of the Normal only)
+  OutActs oa;        // output activations of the two halves (OUTACT instantiation)
 };
 // d(actor loss)/d(mean_j, log_std_j) of one row (chain rule through a~ = scale tanh(u) + shift and the log-prob).
-// NQ: critics whose action gradients add up (DSAC-T 2, DSAC_V1 on the MLP engine 1)
-template <int NQ>
+// NQ: critics whose action gradients add up (DSAC-T 2, DSAC_V1 on the MLP engine 1).  OUTACT: the row holds z, the
+// distribution reads act(z) (a.oa.mean / a.oa.ls), and the gradients are taken w.r.t. z.
+template <int NQ, bool OUTACT>
 __device__ __forceinline__ void pgrad_elem(const PolicyGradArgs& a, int row, int j, float coef, float& gu, float& gls) {
   const int A = a.A;
   const float scale = 0.5f * (a.hi[j] - a.lo[j]);
-  const float mean = a.logits[(size_t)row * 2 * A + j];
-  const float ls = a.logits[(size_t)row * 2 * A + A + j];
+  const float zm = a.logits[(size_t)row * 2 * A + j];
+  const float zl = a.logits[(size_t)row * 2 * A + A + j];
+  float mean = zm, ls = zl;
+  if constexpr (OUTACT) { mean = act_fwd(zm, a.oa.mean); ls = act_fwd(zl, a.oa.ls); }
   const bool inside = ls >= a.min_log_std && ls <= a.max_log_std;
   const float sd = expf(fminf(fmaxf(ls, a.min_log_std), a.max_log_std));
   const float e = a.eps[(size_t)row * A + j];
@@ -661,15 +705,16 @@ __device__ __forceinline__ void pgrad_elem(const PolicyGradArgs& a, int row, int
   if (a.gauss) {   // a~ = u; d logp / d mean = 0, d logp / d sd = -1/sd
     gu = da;
     gls = inside ? (gu * e - coef / sd) * sd : 0.f;
-    return;
+  } else {
+    const float th = tanhf(mean + sd * e);
+    const float om = 1.f - th * th;
+    gu = da * scale * om + coef * (2.f * th * om / (1.f + TG_EPS - th * th));
+    const float gsd = gu * e - coef / sd;
+    gls = inside ? gsd * sd : 0.f;
   }
-  const float th = tanhf(mean + sd * e);
-  const float om = 1.f - th * th;
-  gu = da * scale * om + coef * (2.f * th * om / (1.f + TG_EPS - th * th));
-  const float gsd = gu * e - coef / sd;
-  gls = inside ? gsd * sd : 0.f;
+  if constexpr (OUTACT) { gu *= act_bwd(zm, a.oa.mean); gls *= act_bwd(zl, a.oa.ls); }
 }
-template <int NQ>
+template <int NQ, bool OUTACT>
 __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
   pdl_sync();
   extern __shared__ float gb[];   // [2A] block-local bias-gradient sums
@@ -683,7 +728,7 @@ __global__ void policy_grad_kernel(const __grid_constant__ PolicyGradArgs a) {
     float gb_mean = 0.f, gb_ls = 0.f;
     for (int row = blockIdx.x * wpb + warp; j < A && row < a.B; row += gridDim.x * wpb) {
       float gu, gls;
-      pgrad_elem<NQ>(a, row, j, coef, gu, gls);
+      pgrad_elem<NQ, OUTACT>(a, row, j, coef, gu, gls);
       a.d_logits[(size_t)row * 2 * A + j] = gu;
       a.d_logits[(size_t)row * 2 * A + A + j] = gls;
       img_put(a.img, row, j, gu);

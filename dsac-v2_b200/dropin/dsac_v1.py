@@ -7,6 +7,7 @@ with `dsact_gemm` the MLP engine (`dsact_v1_create`: wgmma layer chains or fp32 
   DSAC-T) + `log_alpha`; on a CUDA device the parameters are views into the engine's flat buffers [q | policy | log_alpha].
   Approximators: MLP with policy std_type "mlp_shared" / "mlp_separated" / "parameter", or CNN (`type_1` / `type_2`,
   one conv_type for both networks, as in example_train/dsacv1_cnn_carracing_offasync.py).
+  `value_output_activation` / `policy_output_activation` end the networks as in the reference, on either engine.
 * `DSAC_V1.local_update(data, iteration) -> tb_info` runs the whole update in the CUDA library; no CPU fallback.
   `get_remote_update_info` / `remote_update` (the gradient-message seam of the reference's asynchronous trainers) are not
   part of this engine and raise.
@@ -68,8 +69,8 @@ class ApproxContainer(nn.Module):
             for p in net.parameters():
                 p.requires_grad = False
         self.log_alpha = nn.Parameter(torch.tensor(1, dtype=torch.float32))
-        if q_args["output_activation"] != "linear" or pi_args["output_activation"] != "linear":
-            raise NotImplementedError("the CUDA engine implements linear output activations")
+        # the last layers' activations: the engine's row kernels read act(z) of the linear output layers
+        self._out_acts = (q_args["output_activation"], pi_args["output_activation"])
         if pi_args["action_distribution_cls"].__name__ not in _lib.ACT_DISTS:
             raise NotImplementedError("the CUDA engine implements TanhGaussDistribution and GaussDistribution")
         self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
@@ -139,7 +140,8 @@ class ApproxContainer(nn.Module):
         if eng is None:
             cfg = self._make(max_batch=self._max_batch, **self._cfg_args)
             lim = (self.policy.act_high_lim, self.policy.act_low_lim)
-            eng = self._engine = CnnEngine(cfg, device, *lim) if self._gemm is None else Engine(cfg, device, *lim, v1=self._v1)
+            oa = dict(output_activations=self._out_acts)
+            eng = self._engine = CnnEngine(cfg, device, *lim, **oa) if self._gemm is None else Engine(cfg, device, *lim, v1=self._v1, **oa)
             eng.seed(0x5DEECE66D if self._user_seed is None else int(self._user_seed))
         train, targ = self._flat_groups()
         with torch.no_grad():

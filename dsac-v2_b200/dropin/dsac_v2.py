@@ -8,6 +8,8 @@ the CUDA engine (libdsact.so) instead of eager PyTorch.
 * `DSAC_V2.local_update(data, iteration) -> tb_info` runs the whole update
   (losses, three backward passes, Adam, delayed Polyak) in the CUDA library.
   There is no CPU fallback: on a CPU module it raises.
+* `value_output_activation` / `policy_output_activation` (any hidden-activation
+  name) end the networks as in the reference, on every engine the module picks.
 * `get_remote_update_info` / `remote_update` keep the gradient-message seam
   (reference :107-138); with `torch.distributed` initialised the step is
   data-parallel (all-reduce of the two critic-std sums and of the flat gradients).
@@ -101,8 +103,8 @@ class ApproxContainer(nn.Module):
                 act_q=q_args["hidden_activation"], act_pi=pi_args["hidden_activation"],
                 gemm_mode=kwargs.get("dsact_gemm", "bf16x3"), use_graph=kwargs.get("dsact_graph", True),
                 policy_std=pi_args["std_type"], **common)
-        if q_args["output_activation"] != "linear" or pi_args["output_activation"] != "linear":
-            raise NotImplementedError("the CUDA engine implements linear output activations")
+        # the last layers' activations: the engine's row kernels read act(z) of the linear output layers
+        self._out_acts = (q_args["output_activation"], pi_args["output_activation"])
         self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
         self._engine = None
         # seed of the device generator (noise + replay indices): the run's `seed` kwarg (reference utils/init_args.py
@@ -135,11 +137,13 @@ class ApproxContainer(nn.Module):
         if eng is None and self._cnn:
             make = make_heads_config if self._heads_std else make_cnn_config
             cfg = make(max_batch=self._max_batch, **self._cfg_args)
-            eng = self._engine = CnnEngine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim)
+            eng = self._engine = CnnEngine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim,
+                                           output_activations=self._out_acts)
             eng.seed(self.device_seed())
         elif eng is None:
             cfg = make_config(max_batch=self._max_batch, **self._cfg_args)
-            eng = self._engine = Engine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim)
+            eng = self._engine = Engine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim,
+                                        output_activations=self._out_acts)
             eng.seed(self.device_seed())
         train, targ = self._flat_groups()
         with torch.no_grad():
@@ -181,7 +185,7 @@ class ApproxContainer(nn.Module):
             old = self._engine
             self._max_batch = int(batch)
             cfg = make_config(max_batch=self._max_batch, **self._cfg_args)
-            new = Engine(cfg, old.device, self.policy.act_high_lim, self.policy.act_low_lim)
+            new = Engine(cfg, old.device, self.policy.act_high_lim, self.policy.act_low_lim, output_activations=self._out_acts)
             with torch.no_grad():
                 for name in ("params", "targets", "adam_m", "adam_v", "state"):
                     getattr(new, name).copy_(getattr(old, name))

@@ -7,6 +7,7 @@ path runs in the CUDA library.
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from typing import Dict, Optional, Sequence
 
 import numpy as np
@@ -102,11 +103,20 @@ class Engine:
     _query, _create = "dsact_query_layout", "dsact_create"
 
     def __init__(self, cfg: Config, device: torch.device, act_high: torch.Tensor, act_low: torch.Tensor, *,
-                 workspace_fill: float = 0.0, v1: Optional[V1Options] = None):
+                 workspace_fill: float = 0.0, v1: Optional[V1Options] = None,
+                 output_activations: Sequence[str] = ("linear", "linear")):
         """`workspace_fill`: the value the scratch workspace holds when it is bound.  No step depends on it: every region a
         step reads is written first by that step, or by dsact_bind (arena_views()["slabs"]).
         `v1` (`make_v1_options`): a DSAC_V1 handle of the MLP engine (dsact_v1_create): one critic, flat layout
-        [q | policy | log_alpha], the reference's `dsac_v1.ApproxContainer` names."""
+        [q | policy | log_alpha], the reference's `dsac_v1.ApproxContainer` names.
+        `output_activations`: (value, policy) names of `_lib.ACTIVATIONS`, the reference's value_output_activation /
+        policy_output_activation: the activation of the critics' and the policy's last layer (with policy std_type
+        "parameter" the learnable log_std row is not activated; dsact_set_output_activations in include/dsact.h)."""
+        out_q, out_pi = output_activations
+        for name in (out_q, out_pi):
+            if name not in _lib.ACTIVATIONS:
+                raise ValueError(f"unsupported output activation {name!r}")
+        self.output_activations = (out_q, out_pi)
         if not torch.cuda.is_available():
             raise _lib.DsactError("the DSAC-T update engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
@@ -137,6 +147,8 @@ class Engine:
             else:
                 check(self.lib.dsact_v1_create(C.byref(cfg), C.byref(v1), self.device.index, C.byref(h)))
             self.h = h
+            if self.output_activations != ("linear", "linear"):
+                check(self.lib.dsact_set_output_activations(h, _lib.ACTIVATIONS[out_q], _lib.ACTIVATIONS[out_pi]))
             self._stats_host = torch.zeros(_lib.NUM_STATS, dtype=torch.float32).pin_memory()
             self._bind()
             check(self.lib.dsact_set_carry(self.h, -1.0, -1.0, 0, 0, self._stream()))
@@ -687,7 +699,10 @@ class Engine:
         with torch.cuda.device(self.device):
             check(self.lib.dsact_test_dp_attach(self.h, int(rank), len(peers), arr, C.byref(buf), C.byref(n)))
         self.dp_world = len(peers)
-        self._dp_peers = list(peers)
+        # weak references: the peers hold this engine too, and a reference cycle would leave a closed world's handles to
+        # the cyclic garbage collector, whose dsact_destroy (cudaFree synchronises the device) can then run in the middle
+        # of another world's rank enqueues while their kernels wait on each other
+        self._dp_peers = [weakref.proxy(p) for p in peers]
         return _device_view(buf.value, int(n.value), self.device)   # the library owns it: valid while this handle lives
 
     def test_dp(self, op: str, kind: int = 0, grads: Optional[torch.Tensor] = None, slabs: Optional[torch.Tensor] = None,

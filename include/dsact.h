@@ -143,6 +143,14 @@ int dsact_create(const dsact_config *cfg, int device, dsact_handle **out);
 void dsact_destroy(dsact_handle *h);
 int dsact_bind(dsact_handle *h, const dsact_buffers *bufs);
 
+/* The networks' output activations (the reference's value_output_activation / policy_output_activation: the
+ * `output_activation` of every network's last layer, networks/mlp.py and networks/cnn.py), as DSACT_ACT_* codes.
+ * value_act applies to every critic output (mean and raw std, before the softplus).  policy_act applies to the policy's
+ * outputs: all 2A of "mlp_shared", both networks of "mlp_separated", the mean network only of "parameter" (its log_std
+ * row is not activated), and every head of the CNN approximators.  Works on a handle of any create call; call it
+ * between create and dsact_bind (DSACT_ESTATE after bind).  DSACT_EINVAL for an unknown code.  Default: both linear. */
+int dsact_set_output_activations(dsact_handle *h, int32_t value_act, int32_t policy_act);
+
 /* seed / counter of the device noise generator and of replay index sampling */
 int dsact_seed(dsact_handle *h, uint64_t seed);
 
