@@ -30,17 +30,11 @@ from typing import Dict
 import torch
 import torch.nn as nn
 
-import networks.cnn as _cnn
-import networks.mlp as _mlp
 from dsact_host import TB_TAGS as tb_tags
 from dsact_host import full_state_dict as _full_state
 from dsact_host import load_full_state_dict as _load_full_state
-from dsact_host import net_kwargs
 from dsact_host import replay_updates_on_engine
-
-from dsac_v2_b200 import _lib
-from dsac_v2_b200.engine import Engine, make_config, make_v1_options
-from dsac_v2_b200.engine_cnn import CnnEngine, make_cnn_config, make_heads_config
+from dsact_route import EngineContainer, network_classes
 
 # where the engine's 16-slot statistics carry DSAC_V1's tb_info (dsac_v1.py:172-181)
 _V1_KEYS = (("DSAC/critic_avg_q-RL iter", 0), ("DSAC/critic_avg_std-RL iter", 2), (tb_tags["loss_actor"], 6),
@@ -48,19 +42,14 @@ _V1_KEYS = (("DSAC/critic_avg_q-RL iter", 0), ("DSAC/critic_avg_std-RL iter", 2)
             ("DSAC/alpha-RL iter", 11))
 
 
-class ApproxContainer(nn.Module):
+class ApproxContainer(EngineContainer):
     """One critic, one policy, their targets and log_alpha (reference dsac_v1.py:17-52)."""
+
+    algorithm, critics = "DSAC_V1", ("q",)
 
     def __init__(self, **kwargs):
         super().__init__()
-        q_args, pi_args = net_kwargs("value", kwargs), net_kwargs("policy", kwargs)
-        if q_args["apprfunc"] != pi_args["apprfunc"]:
-            raise NotImplementedError("value and policy approximators must be of the same type (both MLP or both CNN)")
-        cnn = q_args["apprfunc"] == "CNN"
-        mod = _cnn if cnn else _mlp
-        q_cls, pi_cls = getattr(mod, q_args["name"], None), getattr(mod, pi_args["name"], None)
-        if q_cls is None or pi_cls is None:
-            raise NotImplementedError("This apprfunc is not properly defined")
+        q_args, pi_args, q_cls, pi_cls = network_classes(self.algorithm, kwargs)
         self.q = q_cls(**q_args)                      # construction order = the reference's RNG consumption (:28-34)
         self.q_target = deepcopy(self.q)
         self.policy = pi_cls(**pi_args)
@@ -69,108 +58,7 @@ class ApproxContainer(nn.Module):
             for p in net.parameters():
                 p.requires_grad = False
         self.log_alpha = nn.Parameter(torch.tensor(1, dtype=torch.float32))
-        # the last layers' activations: the engine's row kernels read act(z) of the linear output layers
-        self._out_acts = (q_args["output_activation"], pi_args["output_activation"])
-        if pi_args["action_distribution_cls"].__name__ not in _lib.ACT_DISTS:
-            raise NotImplementedError("the CUDA engine implements TanhGaussDistribution and GaussDistribution")
-        self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
-        self._engine = None
-        self._user_seed = kwargs.get("seed", None)
-        self._attachments = []
-        self._register_state_dict_hook(_detach_state_dict)
-        self._gemm = kwargs.get("dsact_gemm", None)
-        if self._gemm is not None:   # the MLP engine (dsact_v1_create)
-            if cnn or pi_args["std_type"] != "mlp_shared":
-                raise NotImplementedError(
-                    "dsact_gemm: DSAC_V1 runs on the MLP engine with MLP approximators and the policy std_type 'mlp_shared' "
-                    "(TanhGaussDistribution or GaussDistribution) only; drop dsact_gemm for the head-wise fp32 engine")
-            if self._gemm not in _lib.GEMM_MODES:
-                raise ValueError(f"dsact_gemm must be one of {sorted(_lib.GEMM_MODES)}, got {self._gemm!r}")
-            self._cfg_args = dict(
-                obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"], hidden_q=q_args["hidden_sizes"],
-                hidden_pi=pi_args["hidden_sizes"], act_q=q_args["hidden_activation"], act_pi=pi_args["hidden_activation"],
-                gemm_mode=self._gemm, use_graph=kwargs.get("dsact_graph", True), gamma=kwargs.get("gamma", 0.99),
-                tau=kwargs.get("tau", 0.005), delay_update=kwargs.get("delay_update", 2), auto_alpha=kwargs.get("auto_alpha", True),
-                alpha=kwargs.get("alpha", 0.2), lr_q=kwargs["value_learning_rate"], lr_pi=kwargs["policy_learning_rate"],
-                lr_alpha=kwargs["alpha_learning_rate"], min_log_std=pi_args["min_log_std"], max_log_std=pi_args["max_log_std"],
-                act_dist=pi_args["action_distribution_cls"].__name__)
-            self._v1 = make_v1_options(kwargs.get("bound", True), kwargs.get("TD_bound", 20))
-            self._make = make_config
-            return
-        if q_args["hidden_activation"] != pi_args["hidden_activation"]:
-            raise NotImplementedError("the head-wise engine takes one hidden activation for critic and policy")
-        common = dict(gamma=kwargs.get("gamma", 0.99), tau=kwargs.get("tau", 0.005), delay_update=kwargs.get("delay_update", 2),
-                      auto_alpha=kwargs.get("auto_alpha", True), alpha=kwargs.get("alpha", 0.2), lr_q=kwargs["value_learning_rate"],
-                      lr_pi=kwargs["policy_learning_rate"], lr_alpha=kwargs["alpha_learning_rate"],
-                      min_log_std=pi_args["min_log_std"], max_log_std=pi_args["max_log_std"],
-                      act_dist=pi_args["action_distribution_cls"].__name__, act_hidden=q_args["hidden_activation"],
-                      algo="DSAC_V1", bound=kwargs.get("bound", True), td_bound=kwargs.get("TD_bound", 20))
-        if cnn:
-            if q_args["conv_type"] != pi_args["conv_type"]:
-                raise NotImplementedError("the CNN engine takes one conv_type for critic and policy")
-            t = _cnn.CONV_TYPES[q_args["conv_type"]]
-            self._make = make_cnn_config
-            self._cfg_args = dict(obs_shape=tuple(q_args["obs_dim"]), act_dim=q_args["act_dim"], kernels=t["kernels"],
-                                  channels=t["channels"], strides=t["strides"], hidden=t["heads"], **common)
-        else:
-            if q_args["hidden_sizes"] != pi_args["hidden_sizes"]:
-                raise NotImplementedError("the head-wise engine takes one hidden_sizes list for critic and policy")
-            self._make = make_heads_config
-            self._cfg_args = dict(obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"], hidden=q_args["hidden_sizes"],
-                                  std_type=pi_args["std_type"], **common)
-
-    def create_action_distributions(self, logits):
-        return self.policy.get_act_dist(logits)
-
-    def _flat_groups(self):
-        train = [p for n in ("q", "policy") for p in getattr(self, n).parameters()] + [self.log_alpha]
-        targ = [p for n in ("q", "policy") for p in getattr(self, n + "_target").parameters()]
-        return train, targ
-
-    def _apply(self, fn, recurse=True):
-        super()._apply(fn, recurse)
-        if self.log_alpha.device.type == "cuda":
-            self._attach(self.log_alpha.device)
-        return self
-
-    def _attach(self, device):
-        eng = self._engine
-        if eng is not None and eng.device != torch.device(device):
-            self._engine = eng = None
-        if eng is None:
-            cfg = self._make(max_batch=self._max_batch, **self._cfg_args)
-            lim = (self.policy.act_high_lim, self.policy.act_low_lim)
-            oa = dict(output_activations=self._out_acts)
-            eng = self._engine = CnnEngine(cfg, device, *lim, **oa) if self._gemm is None else Engine(cfg, device, *lim, v1=self._v1, **oa)
-            eng.seed(0x5DEECE66D if self._user_seed is None else int(self._user_seed))
-        train, targ = self._flat_groups()
-        with torch.no_grad():
-            for flat, group in ((eng.params, train), (eng.targets, targ)):
-                off = 0
-                for p in group:
-                    n = p.numel()
-                    view = flat[off:off + n].view(p.shape)
-                    if p.data.data_ptr() != view.data_ptr():
-                        view.copy_(p.data)
-                        p.data = view
-                    off += n
-                assert off == flat.numel(), "flat layout does not match the module"
-
-    def engine(self, batch: int = 0) -> Engine:
-        if self.log_alpha.device.type != "cuda" or self._engine is None:
-            raise _lib.DsactError(
-                "DSAC_V1's update path runs only on the CUDA engine (libdsact.so, sm_90a); "
-                "move the networks to the GPU first (`alg.networks.cuda()`). There is no CPU fallback.")
-        if batch > self._max_batch:
-            raise ValueError(f"batch {batch} > dsact_max_batch / replay_batch_size {self._max_batch}")
-        return self._engine
-
-
-def _detach_state_dict(module, state_dict, prefix, local_metadata):
-    for k, v in list(state_dict.items()):
-        if isinstance(v, torch.Tensor):
-            state_dict[k] = v.detach().clone()
-    return state_dict
+        self._route(kwargs)
 
 
 class DSAC_V1:
@@ -221,7 +109,7 @@ class DSAC_V1:
         tb_info mappings, fetched with one copy of the [n, 16] block on first access.  The head-wise engine takes the n
         rounds one by one."""
         eng = self.networks.engine(batch_size)
-        if self.networks._gemm is None:
+        if self.networks.route.engine != "mlp":
             return [self.local_update(buffer.sample_batch(batch_size), iteration + k) for k in range(n)]
         return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, _V1_KEYS)
 

@@ -30,37 +30,24 @@ from typing import Dict, Tuple
 import torch
 import torch.nn as nn
 
-import networks.cnn as _cnn
-import networks.mlp as _mlp
 from dsact_host import TB_TAGS as tb_tags
 from dsact_host import full_state_dict as _full_state
 from dsact_host import replay_updates_on_engine
 from dsact_host import load_full_state_dict as _load_full_state
-from dsact_host import net_kwargs
+from dsact_route import EngineContainer, network_classes
 
 from dsac_v2_b200 import _lib, dp
-from dsac_v2_b200.engine import STAT_KEYS, Engine, make_config
-from dsac_v2_b200.engine_cnn import CnnEngine, make_cnn_config, make_heads_config
-
-_TRAINABLE = ("q1", "q2", "policy")
+from dsac_v2_b200.engine import STAT_KEYS
 
 
-class ApproxContainer(nn.Module):
+class ApproxContainer(EngineContainer):
     """Six networks + log_alpha (reference dsac_v2.py:19-62)."""
+
+    algorithm, critics = "DSAC_V2", ("q1", "q2")
 
     def __init__(self, **kwargs):
         super().__init__()
-        if kwargs.get("cnn_shared", False):
-            raise NotImplementedError("cnn_shared feature nets are not part of the CUDA update path")
-        q_args, pi_args = net_kwargs("value", kwargs), net_kwargs("policy", kwargs)
-        if q_args["apprfunc"] != pi_args["apprfunc"]:
-            raise NotImplementedError("value and policy approximators must be of the same type (both MLP or both CNN)")
-        self._cnn = q_args["apprfunc"] == "CNN"   # BASELINE config 5: conv encoder + separate mean / log_std heads
-        self._heads_std = None
-        mod = _cnn if self._cnn else _mlp
-        q_cls, pi_cls = getattr(mod, q_args["name"], None), getattr(mod, pi_args["name"], None)
-        if q_cls is None or pi_cls is None:
-            raise NotImplementedError("This apprfunc is not properly defined")
+        q_args, pi_args, q_cls, pi_cls = network_classes(self.algorithm, kwargs)
         # construction order q1, q2, policy = the reference's consumption of torch's RNG (:31-39)
         self.q1 = q_cls(**q_args)
         self.q2 = q_cls(**q_args)
@@ -72,94 +59,11 @@ class ApproxContainer(nn.Module):
             for p in net.parameters():
                 p.requires_grad = False
         self.log_alpha = nn.Parameter(torch.tensor(1, dtype=torch.float32))
-
-        if pi_args["action_distribution_cls"].__name__ not in _lib.ACT_DISTS:
-            raise NotImplementedError("the CUDA engine implements TanhGaussDistribution and GaussDistribution")
-        common = dict(gamma=kwargs.get("gamma", 0.99), tau=kwargs.get("tau", 0.005), tau_b=kwargs.get("tau_b", None),
-                      delay_update=kwargs.get("delay_update", 2), auto_alpha=kwargs.get("auto_alpha", True),
-                      alpha=kwargs.get("alpha", 0.2), lr_q=kwargs["value_learning_rate"], lr_pi=kwargs["policy_learning_rate"],
-                      lr_alpha=kwargs["alpha_learning_rate"], min_log_std=pi_args["min_log_std"], max_log_std=pi_args["max_log_std"],
-                      act_dist=pi_args["action_distribution_cls"].__name__)
-        if self._cnn:
-            if q_args["conv_type"] != pi_args["conv_type"] or q_args["hidden_activation"] != pi_args["hidden_activation"]:
-                raise NotImplementedError("the CNN engine takes one conv_type / head activation for critics and policy")
-            t = _cnn.CONV_TYPES[q_args["conv_type"]]
-            self._cfg_args = dict(obs_shape=tuple(q_args["obs_dim"]), act_dim=q_args["act_dim"], kernels=t["kernels"],
-                                  channels=t["channels"], strides=t["strides"], hidden=t["heads"],
-                                  act_hidden=q_args["hidden_activation"], **common)
-        elif pi_args["std_type"] != "mlp_shared" and "dsact_gemm" not in kwargs:
-            # separate mean / log_std (reference networks/mlp.py:43-72): the head-wise fp32 engine without an encoder,
-            # unless the caller names the MLP engine's arithmetic (`dsact_gemm`), as for DSAC_V1
-            if q_args["hidden_sizes"] != pi_args["hidden_sizes"] or q_args["hidden_activation"] != pi_args["hidden_activation"]:
-                raise NotImplementedError("policy std_type != 'mlp_shared': critics and policy take one hidden_sizes / activation")
-            self._cnn = True     # same engine class and entry points as the CNN approximators
-            self._heads_std = pi_args["std_type"]
-            self._cfg_args = dict(obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"], hidden=q_args["hidden_sizes"],
-                                  std_type=pi_args["std_type"], act_hidden=q_args["hidden_activation"], **common)
-        else:
-            self._cfg_args = dict(
-                obs_dim=q_args["obs_dim"], act_dim=q_args["act_dim"],
-                hidden_q=q_args["hidden_sizes"], hidden_pi=pi_args["hidden_sizes"],
-                act_q=q_args["hidden_activation"], act_pi=pi_args["hidden_activation"],
-                gemm_mode=kwargs.get("dsact_gemm", "bf16x3"), use_graph=kwargs.get("dsact_graph", True),
-                policy_std=pi_args["std_type"], **common)
-        # the last layers' activations: the engine's row kernels read act(z) of the linear output layers
-        self._out_acts = (q_args["output_activation"], pi_args["output_activation"])
-        self._max_batch = int(kwargs.get("dsact_max_batch", kwargs.get("replay_batch_size", 256)))
-        self._engine = None
-        # seed of the device generator (noise + replay indices): the run's `seed` kwarg (reference utils/init_args.py
-        # seeds torch/numpy with it) mixed with the data-parallel rank, so that seeds and ranks draw independent streams
-        self._user_seed = kwargs.get("seed", None)
-        self._attachments = []   # objects holding a reference to the engine (ReplayBuffer): re-bound when the engine is rebuilt
-        self._register_state_dict_hook(_detach_state_dict)
-
-    def create_action_distributions(self, logits):
-        return self.policy.get_act_dist(logits)
-
-    # ---- flat-buffer plumbing -----------------------------------------------------
-    def _flat_groups(self):
-        """(flat tensor name, [parameters in layout order]) — include/dsact.h layout."""
-        train = [p for n in _TRAINABLE for p in getattr(self, n).parameters()] + [self.log_alpha]
-        targ = [p for n in _TRAINABLE for p in getattr(self, n + "_target").parameters()]
-        return train, targ
-
-    def _apply(self, fn, recurse=True):
-        super()._apply(fn, recurse)
-        if self.log_alpha.device.type == "cuda":
-            self._attach(self.log_alpha.device)
-        return self
-
-    def _attach(self, device):
-        """Make every parameter a view into the engine's flat buffers on `device`."""
-        eng = self._engine
-        if eng is not None and eng.device != torch.device(device):
-            self._engine = eng = None  # moved to another GPU: rebuild there
-        if eng is None and self._cnn:
-            make = make_heads_config if self._heads_std else make_cnn_config
-            cfg = make(max_batch=self._max_batch, **self._cfg_args)
-            eng = self._engine = CnnEngine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim,
-                                           output_activations=self._out_acts)
-            eng.seed(self.device_seed())
-        elif eng is None:
-            cfg = make_config(max_batch=self._max_batch, **self._cfg_args)
-            eng = self._engine = Engine(cfg, device, self.policy.act_high_lim, self.policy.act_low_lim,
-                                        output_activations=self._out_acts)
-            eng.seed(self.device_seed())
-        train, targ = self._flat_groups()
-        with torch.no_grad():
-            for flat, group in ((eng.params, train), (eng.targets, targ)):
-                off = 0
-                for p in group:
-                    n = p.numel()
-                    view = flat[off:off + n].view(p.shape)
-                    if p.data.data_ptr() != view.data_ptr():
-                        view.copy_(p.data)
-                        p.data = view
-                    off += n
-                assert off == flat.numel(), "flat layout does not match the module"
+        self._route(kwargs)
 
     def device_seed(self) -> int:
-        """64-bit seed of the engine's Philox generator: splitmix64 of (user seed, data-parallel rank)."""
+        """64-bit seed of the engine's Philox generator: splitmix64 of (user seed, data-parallel rank), so that seeds and
+        ranks draw independent streams."""
         rank = 0
         try:
             import torch.distributed as dist
@@ -167,60 +71,10 @@ class ApproxContainer(nn.Module):
                 rank = dist.get_rank()
         except Exception:   # noqa: BLE001
             rank = 0
-        base = 0x5DEECE66D if self._user_seed is None else int(self._user_seed)
-        z = (base * 0x9E3779B97F4A7C15 + (rank + 1) * 0xBF58476D1CE4E5B9) & (2 ** 64 - 1)
+        z = (super().device_seed() * 0x9E3779B97F4A7C15 + (rank + 1) * 0xBF58476D1CE4E5B9) & (2 ** 64 - 1)
         z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & (2 ** 64 - 1)
         z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & (2 ** 64 - 1)
         return z ^ (z >> 31)
-
-    def engine(self, batch: int = 0) -> Engine:
-        """The bound engine; raises when the module is not on a CUDA device."""
-        if self.log_alpha.device.type != "cuda" or self._engine is None:
-            raise _lib.DsactError(
-                "DSAC_V2's update path runs only on the CUDA engine (libdsact.so, sm_90a); "
-                "move the networks to the GPU first (`alg.networks.cuda()`). There is no CPU fallback.")
-        if batch > self._max_batch and self._cnn:
-            raise ValueError(f"batch {batch} > dsact_max_batch / replay_batch_size {self._max_batch} (the CNN engine does not regrow)")
-        if batch > self._max_batch:  # grow the activation arena, keep weights / Adam state / carry
-            old = self._engine
-            self._max_batch = int(batch)
-            cfg = make_config(max_batch=self._max_batch, **self._cfg_args)
-            new = Engine(cfg, old.device, self.policy.act_high_lim, self.policy.act_low_lim, output_activations=self._out_acts)
-            with torch.no_grad():
-                for name in ("params", "targets", "adam_m", "adam_v", "state"):
-                    getattr(new, name).copy_(getattr(old, name))
-            new.seed(old._seed)            # a seed restored by load_full_state_dict survives the rebuild
-            self._engine = new
-            for p in self.parameters():  # force re-pointing
-                p.data = p.data.clone()
-            self._attach(old.device)
-            for ref in list(self._attachments):   # replay rings move with their rows; peers reconnect on the next update
-                obj = ref()
-                if obj is not None:
-                    obj.rebind(old, new)
-            old.close()
-        return self._engine
-
-    def grad_views(self):
-        """Per-parameter views of the flat gradient buffer, grouped like get_remote_update_info."""
-        eng = self.engine()
-        out, off = {}, 0
-        for name in _TRAINABLE:
-            views = []
-            for p in getattr(self, name).parameters():
-                views.append(eng.grads[off:off + p.numel()].view(p.shape))
-                off += p.numel()
-            out[name] = views
-        out["log_alpha"] = eng.grads[off]
-        return out
-
-
-def _detach_state_dict(module, state_dict, prefix, local_metadata):
-    # checkpoints must not alias the flat buffers (torch.save would serialise the whole storage per view)
-    for k, v in list(state_dict.items()):
-        if isinstance(v, torch.Tensor):
-            state_dict[k] = v.detach().clone()
-    return state_dict
 
 
 class _LazyTbInfo(Mapping):
@@ -273,7 +127,7 @@ class DSAC_V2:
         # "peer": exchanges inside the step's kernels over NVLink peer memory (falls back to NCCL if the ranks cannot
         # map each other's buffers); "nccl": torch.distributed all-reduces between three graph launches
         self.dp_transport = kwargs.get("dsact_dp_transport", "peer")
-        if not self.networks._cnn and kwargs.get("policy_std_type", "mlp_shared") != "mlp_shared":
+        if self.networks.route.engine == "mlp" and kwargs.get("policy_std_type", "mlp_shared") != "mlp_shared":
             self.dp_transport = "nccl"   # the MLP engine's peer-memory step serves mlp_shared only (dsact_dp_step refuses)
         self._peer_dp, self._peer_eng = None, None
         self._slots, self._owners, self._cursor = None, [None] * self._RING, 0
@@ -365,7 +219,7 @@ class DSAC_V2:
         block on first access.  The head-wise engine and data-parallel runs take the n rounds one by one."""
         eng = self.networks.engine(batch_size)
         _, world = self._world()
-        if self.networks._cnn or world > 1:
+        if self.networks.route.engine != "mlp" or world > 1:
             return [self.local_update(buffer.sample_batch(batch_size), iteration + k) for k in range(n)]
         return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, list(zip(STAT_KEYS, range(14))))
 

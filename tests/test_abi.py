@@ -118,11 +118,7 @@ def _head_wise(variant):
         over = {"algorithm": "DSAC_V1"} if variant == "v1_mlp" else {"policy_std_type": variant}
         kw = synth.reference_kwargs(cfg, replay_batch_size=4, **over)
     net = (dsac_v1 if variant.startswith("v1") else dsac_v2).ApproxContainer(**kw)
-    make = net._make if variant.startswith("v1") else None
-    if make is None:
-        from dsac_v2_b200.engine_cnn import make_cnn_config, make_heads_config
-        make = make_heads_config if net._heads_std else make_cnn_config
-    return net, make(max_batch=4, **net._cfg_args)
+    return net, net.route.config(4)
 
 
 @pytest.mark.parametrize("variant", HEAD_WISE)

@@ -36,9 +36,8 @@ def test_schema_names_every_float_once_in_the_modules_order(name, std_type):
     import dsac_v2
     cfg = synth.mlp_config(name)
     net = dsac_v2.ApproxContainer(**synth.reference_kwargs(cfg, policy_std_type=std_type, replay_batch_size=4, dsact_gemm="fp32"))
-    assert not net._cnn and net._heads_std is None   # the MLP engine, with the networks' own shapes
-    from dsac_v2_b200.engine import make_config
-    c = make_config(max_batch=4, **net._cfg_args)
+    assert net.route.engine == "mlp"   # the MLP engine, with the networks' own shapes
+    c = net.route.config(4)
     lay = query_layout(c)
 
     class Probe:   # _schema only reads the config
@@ -61,7 +60,7 @@ def test_without_dsact_gemm_the_head_wise_engine_is_still_chosen():
     cfg = synth.CONFIGS["ragged"]
     for std_type in STD_TYPES:
         net = dsac_v2.ApproxContainer(**synth.reference_kwargs(cfg, policy_std_type=std_type, replay_batch_size=4))
-        assert net._cnn and net._heads_std == std_type
+        assert net.route.engine == "heads" and net.route.cfg_args["std_type"] == std_type
     with pytest.raises(NotImplementedError):   # the head-wise engine takes one shape for critics and policy
         dsac_v2.ApproxContainer(**synth.reference_kwargs(synth.mlp_config("asym"), policy_std_type="parameter", replay_batch_size=4))
 

@@ -106,7 +106,7 @@ def test_dsact_gemm_takes_different_critic_and_policy_networks():
     with pytest.raises(NotImplementedError):   # the head-wise engine: one hidden_sizes / activation
         dsac_v1.ApproxContainer(**kw)
     net = dsac_v1.ApproxContainer(**dict(kw, dsact_gemm="bf16x3", dsact_graph=False))
-    assert net._cfg_args["gemm_mode"] == "bf16x3" and net._cfg_args["use_graph"] is False
+    assert net.route.cfg_args["gemm_mode"] == "bf16x3" and net.route.cfg_args["use_graph"] is False
 
 
 @pytest.mark.parametrize("name", NEW_GOLDENS)
