@@ -334,6 +334,10 @@ def make_engine(case: Case, mode: str):
                   act_dist=case.act_dist)
     if case.engine == "mlp":
         from dsac_v2_b200.engine import Engine, make_config
+        if case.std_type != "mlp_shared" or case.algo != "DSAC_V2":
+            # this builder makes DSAC-T mlp_shared handles only; tests/gradmatrix.py builds the others through the drop-in's route
+            raise ValueError(f"{case.name}: the MLP-engine case builder takes DSAC_V2 with std_type 'mlp_shared' only, "
+                             f"not {case.algo} / {case.std_type!r}")
         act_q, act_pi = synth.activations(cfg)
         c = make_config(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), act_q=act_q, act_pi=act_pi, gemm_mode=mode,
                         use_graph=False, **common)
@@ -352,29 +356,46 @@ def engine_grads(name, mode: str):
     case named `name` (or the Case itself).  DSAC-T runs the gradient-message seam (`compute_grads`); DSAC_V1 has none, so
     it runs one whole step, which leaves the step's gradients in the gradient buffer and the statistics of its forward
     pass."""
-    from dsac_v2_b200.engine import STAT_KEYS
     case = name if isinstance(name, Case) else CASES[name]
     w, b, n = inputs(case)
-    eng = make_engine(case, "fp32" if mode == "heads" else mode)
+    return step0_grads(make_engine(case, "fp32" if mode == "heads" else mode), case.algo, w, b, noise_for_engine(case, n))
+
+
+def step0_grads(eng, algo: str, w: dict, b: dict, noise):
+    """(gradients, tb_info) of `eng` (closed on return) loaded with `w`, for the minibatch `b` and the engine's four noise
+    arrays: engine_grads on an engine built elsewhere."""
+    from dsac_v2_b200.engine import STAT_KEYS
     try:
         eng.load_weights(w)
         bt = {k: torch.from_numpy(v).cuda() for k, v in b.items()}
-        nz = tuple(torch.from_numpy(x).cuda() for x in noise_for_engine(case, n))
-        if case.algo == "DSAC_V1":
+        nz = tuple(torch.from_numpy(x).cuda() for x in noise)
+        if algo == "DSAC_V1":
             eng.step(bt, 0, nz)
         else:
             eng.compute_grads(bt, nz)
         g = eng.export_weights(grads=True)
-        s = eng.read_stats(case.batch)
+        s = eng.read_stats(len(b["rew"]))
     finally:
         eng.close()
-    if case.algo == "DSAC_V1":
+    if algo == "DSAC_V1":
         from oracle.dsact_oracle import V1_TB_KEYS
         vals = [s[k] for k in STAT_KEYS]
         tb = {k: vals[c] for k, c in zip(V1_TB_KEYS, V1_COLS)}
     else:
         tb = {k: s[k] for k in STAT_KEYS[:14]}
     return g, tb
+
+
+def tb_deviations(r: Reference, tb: Dict[str, float], mode: str):
+    """The engine's tb_info entries [(key, got, want, tol)] farther from float64 than the fp32 oracle, up to the factor of
+    the mode's gate; never tighter than TB_RTOL."""
+    c = GATES[mode][0]
+    bad = []
+    for k, want in r.tb64.items():
+        tol = max(TB_RTOL * max(1.0, abs(want)), c * abs(r.tb32[k] - want))
+        if not abs(tb[k] - want) <= tol:
+            bad.append((k, tb[k], want, tol))
+    return bad
 
 
 def compare(name: str, mode: str):
@@ -384,10 +405,4 @@ def compare(name: str, mode: str):
     g, tb = engine_grads(name, mode)
     gate = gates(name, mode)
     out = {k: (rel(g[k], r.g64[k]), gate[k], r.ref[k], r.signal[k]) for k in r.g64}
-    c = GATES[mode][0]
-    bad_tb = []
-    for k, want in r.tb64.items():   # as close to float64 as the fp32 oracle, up to the same factor; never tighter than 1e-4
-        tol = max(TB_RTOL * max(1.0, abs(want)), c * abs(r.tb32[k] - want))
-        if not abs(tb[k] - want) <= tol:
-            bad_tb.append((k, tb[k], want, tol))
-    return out, g, bad_tb
+    return out, g, tb_deviations(r, tb, mode)

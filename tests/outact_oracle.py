@@ -93,9 +93,10 @@ class OracleDSACV1CNN(_Cnn, OV1.OracleDSACV1CNN):
     pass
 
 
-def build(cfg: dict, over: dict, **extra):
+def build(cfg: dict, over: dict, weights=None, **extra):
     """The oracle of a golden case: `cfg` a synth config, `over` the case's overrides (the algorithm, std type and action
-    distribution pick the class; the rest are hyperparameters).  Returns (oracle, weights)."""
+    distribution pick the class; the rest are hyperparameters), on `weights` (default: synth's weights of the case's
+    schema).  Returns (oracle, weights)."""
     from dsac_v2_b200 import synth
     hyper = dict(synth.HYPER)
     hyper.update(over)
@@ -105,16 +106,17 @@ def build(cfg: dict, over: dict, **extra):
     lim = [cfg["act_lim"]] * cfg["act_dim"]
     lims = (lim, [-x for x in lim])
     if "conv_type" in cfg:
-        w = synth.make_cnn_weights_v1(cfg) if v1 else synth.make_cnn_weights(cfg)
+        w = weights if weights is not None else synth.make_cnn_weights_v1(cfg) if v1 else synth.make_cnn_weights(cfg)
         cls = OracleDSACV1CNN if v1 else OracleDSACTCNN
         return cls(cfg["obs_dim"], cfg["act_dim"], synth.CONV_TYPES[cfg["conv_type"]]["strides"], *lims, w, **hyper), w
-    if std_type != "mlp_shared":
-        w = synth.make_weights_std_v1(cfg, std_type) if v1 else synth.make_weights_std(cfg, std_type)
-        cls = OracleDSACV1Std if v1 else OracleDSACTStd
-        return cls(cfg["obs_dim"], cfg["act_dim"], cfg["hidden"], cfg["hidden"], *lims, w, std_type=std_type, **hyper), w
-    w = synth.make_weights_v1(cfg) if v1 else synth.make_weights(cfg)
     if "hidden_activation" not in hyper:
         act_q, act_pi = synth.activations(cfg)
         hyper = dict(dict(value_hidden_activation=act_q, policy_hidden_activation=act_pi), **hyper)
+    if std_type != "mlp_shared":   # critics and policy may differ in shape (std_mlp_common.std_weights)
+        from std_mlp_common import std_weights
+        w = weights if weights is not None else synth.to_v1_schema(std_weights(cfg, std_type)) if v1 else std_weights(cfg, std_type)
+        cls = OracleDSACV1Std if v1 else OracleDSACTStd
+        return cls(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), *lims, w, std_type=std_type, **hyper), w
+    w = weights if weights is not None else synth.make_weights_v1(cfg) if v1 else synth.make_weights(cfg)
     cls = OracleDSACV1 if v1 else OracleDSACT
     return cls(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), *lims, w, **hyper), w

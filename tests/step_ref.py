@@ -515,6 +515,7 @@ def row_inputs(A: int, B: int, seed: int, hy: dict):
 
 # kind, A, B, mode, auto_alpha, mean_std carried (else unset), bound, max_blocks, global batch factor
 ROW_CASES = {}
+GAUSS_KINDS = ("gauss", "mlp_gauss")   # the row kinds whose policy samples the plain Gaussian
 for _A in (1, 2, 3, 17, 32, 33, 96):
     ROW_CASES[f"mlp_fp32_A{_A}"] = ("mlp", _A, 65, "fp32", _A % 2 == 1, _A % 3 == 0, True, 0, 1)
 for _B in (1, 7, 8, 9, 63, 64):
@@ -531,6 +532,9 @@ ROW_CASES.update({
     "separated": ("separated", 3, 65, "fp32", True, True, True, 0, 1),
     "parameter": ("parameter", 2, 63, "fp32", False, False, True, 0, 1),
     "gauss": ("gauss", 3, 65, "fp32", True, True, True, 0, 1),
+    # the plain Gaussian on MLP-engine handles (the log_std half in the policy's 2A outputs; bf16x3 images of the rows)
+    "mlp_gauss": ("mlp_gauss", 3, 65, "fp32", True, True, True, 0, 1),
+    "mlp_gauss_bf16x3": ("mlp_gauss", 17, 63, "bf16x3", False, False, True, 0, 2),
     "heads_v1_bound": ("heads_v1", 3, 65, "fp32", True, False, True, 0, 1),
     "heads_v1_nll": ("heads_v1", 3, 9, "fp32", False, False, False, 2, 1),
     "mlp_past_grid": ("mlp", 2, "grid", "fp32", True, True, True, 0, 1),

@@ -11,7 +11,7 @@ activated input, one column at a time, and every act' by its error bound moves t
 Every non-linear code runs on the critics and, with another code, on the policy, for each row-kernel route: DSAC-T on the
 MLP engine (fp32; bf16x3, whose bf16 images must hold the split of the kernel's own fp32 outputs; the mlp_separated and
 "parameter" std types), DSAC_V1 on the MLP engine, and the head-wise engine with separate critic / policy heads, the
-"parameter" std type, the plain Gaussian, and DSAC_V1 with the bounded and the Gaussian NLL loss.  With "parameter" (on
+"parameter" std type, the plain Gaussian (on both engines, in fp32 and bf16x3 on the MLP engine), and DSAC_V1 with the bounded and the Gaussian NLL loss.  With "parameter" (on
 either engine) the log_std half is the learnable row, which is not activated.  The rows put z at 0 and below (the
 relu kink, act' = 0), saturate tanh / sigmoid, push the activated log_std past both clamp bounds, and lift the activated
 raw std above softplus's threshold of 20.  Outputs start as NaN and sentinel rows past the batch must stay untouched."""
@@ -29,7 +29,7 @@ HY = dict(gamma=0.99, tau=0.005, tau_b=0.005, alpha=0.2, min_log_std=-0.8, max_l
           lr_alpha=3e-4, delay_update=2, td_bound=20.0)
 CODES = ["relu", "gelu", "tanh", "sigmoid", "elu", "selu"]
 KINDS = ["mlp", "mlp_bf16x3", "v1", "mlp_separated", "mlp_parameter", "separated", "parameter", "gauss", "heads_v1",
-         "heads_v1_nll"]
+         "heads_v1_nll", "mlp_gauss", "mlp_gauss_bf16x3"]
 CASES = [(k, q, CODES[(i + 1) % len(CODES)]) for k in KINDS for i, q in enumerate(CODES)]
 A, B = 3, 37
 U = 2.0 ** -23
@@ -71,9 +71,11 @@ def _engine(kind, acts):
     kw = dict(max_batch=B, auto_alpha=True, gamma=HY["gamma"], tau=HY["tau"], alpha=HY["alpha"], min_log_std=HY["min_log_std"],
               max_log_std=HY["max_log_std"])
     dev, oa = torch.device("cuda", 0), dict(output_activations=acts)
-    if kind in ("mlp", "mlp_bf16x3", "v1", "mlp_separated", "mlp_parameter"):
+    if kind in ("mlp", "mlp_bf16x3", "v1", "mlp_separated", "mlp_parameter", "mlp_gauss", "mlp_gauss_bf16x3"):
         std = {"mlp_separated": "mlp_separated", "mlp_parameter": "parameter"}.get(kind, "mlp_shared")
-        cfg = make_config(5, A, (16,), (16,), gemm_mode="bf16x3" if kind == "mlp_bf16x3" else "fp32", policy_std=std, **kw)
+        dist = "GaussDistribution" if kind.startswith("mlp_gauss") else "TanhGaussDistribution"
+        cfg = make_config(5, A, (16,), (16,), gemm_mode="bf16x3" if kind.endswith("bf16x3") else "fp32", policy_std=std,
+                          act_dist=dist, **kw)
         return Engine(cfg, dev, hi, lo, v1=make_v1_options(True) if kind == "v1" else None, **oa), hi, lo
     if kind == "separated":
         return CnnEngine(make_cnn_config((5, 1, 1), A, (), (), (), (16,), q_heads=2, pi_std="head", **kw), dev, hi, lo, **oa), hi, lo
@@ -140,9 +142,9 @@ def test_row_kernels_with_output_activations(kind, act_q, act_pi):
     eng, hi, lo = _engine(kind, (act_q, act_pi))
     act_ls = "linear" if kind in ("parameter", "mlp_parameter") else act_pi
     v1 = kind in ("v1", "heads_v1", "heads_v1_nll")
-    gauss = kind == "gauss"
+    gauss = kind in ("gauss", "mlp_gauss", "mlp_gauss_bf16x3")
     nq = 1 if v1 else 2
-    planes = 2 if kind == "mlp_bf16x3" else 0
+    planes = 2 if kind.endswith("bf16x3") else 0
     sc = R.scalars(HY)
     x = _inputs(7 + CODES.index(act_q))
     x["hi"], x["lo"] = R.f32(hi), R.f32(lo)

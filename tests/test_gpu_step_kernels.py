@@ -53,8 +53,9 @@ def _engine(kind, A, max_batch, mode="fp32", auto=True, bound=True, obs=5, hidde
     lo = R.f32(-1.0 + 0.125 * (torch.arange(A) % 2)).float()
     kw = dict(max_batch=max_batch, auto_alpha=auto, gamma=HY["gamma"], tau=HY["tau"], alpha=HY["alpha"])
     dev = torch.device("cuda", 0)
-    if kind in ("mlp", "v1"):
-        cfg = make_config(obs, A, hidden, hidden, gemm_mode=mode, **kw)
+    if kind in ("mlp", "v1", "mlp_gauss"):
+        dist = "GaussDistribution" if kind == "mlp_gauss" else "TanhGaussDistribution"
+        cfg = make_config(obs, A, hidden, hidden, gemm_mode=mode, act_dist=dist, **kw)
         return Engine(cfg, dev, hi, lo, v1=make_v1_options(bound) if kind == "v1" else None)
     if kind == "separated":   # separate mean / std heads of the critics and the policy
         return CnnEngine(make_cnn_config((obs, 1, 1), A, (), (), (), hidden, q_heads=2, pi_std="head", **kw), dev, hi, lo)
@@ -100,12 +101,12 @@ def test_row_kernels_against_float64(name):
         B = 4 * _sm_count() * 64 + 1
     gb = B * gbf
     v1 = kind in ("v1", "heads_v1")
-    gauss = kind == "gauss"
+    gauss = kind in R.GAUSS_KINDS
     nq = 1 if v1 else 2
     hy = dict(HY, td_bound=20.0)
     sc = R.scalars(hy)
     eng = _engine(kind, A, max(B, 16), mode, auto, bound)
-    planes = {"fp32": 0, "bf16x3": 2, "bf16": 1}[mode] if kind in ("mlp", "v1") else 0
+    planes = {"fp32": 0, "bf16x3": 2, "bf16": 1}[mode] if kind in ("mlp", "v1", "mlp_gauss") else 0
     x = R.case_inputs(name, B, hy)
     rows = B + SENT
     log_alpha = R.c32(-1.3)

@@ -119,7 +119,7 @@ def _row_outputs(name, fault=None):
     on the rows it does not skip), with the loss fed the restated sample and std sums as the kernels feed it."""
     kind, A, B, mode, auto, carried, bound, cap, gbf = R.ROW_CASES[name]
     gb = B * gbf
-    v1, gauss = kind in ("v1", "heads_v1"), kind == "gauss"
+    v1, gauss = kind in ("v1", "heads_v1"), kind in R.GAUSS_KINDS
     sc = R.scalars(GPU_HY)
     x = R.case_inputs(name, B, GPU_HY)
     res = {}
@@ -165,11 +165,11 @@ def _margin(ok, bad):
     return best
 
 
-_DSACT = ("mlp", "separated", "parameter", "gauss")
+_DSACT = ("mlp", "separated", "parameter", "gauss", "mlp_gauss")
 _V1 = ("v1", "heads_v1")
 ROW_FAULTS = {   # fault: (emulated fault, the cases of ROW_CASES it applies to)
-    "tg_eps_logp": ("tg_eps_logp", lambda c: c[0] != "gauss"),
-    "tg_eps_grad": ("tg_eps_grad", lambda c: c[0] != "gauss"),
+    "tg_eps_logp": ("tg_eps_logp", lambda c: c[0] not in R.GAUSS_KINDS),
+    "tg_eps_grad": ("tg_eps_grad", lambda c: c[0] not in R.GAUSS_KINDS),
     "clamp_mask_exclusive": ("clamp_mask_exclusive", lambda c: True),
     "no_clamp_sample": ("no_clamp_sample", lambda c: True),
     "tie_gpa_one": ("tie_gpa_one", lambda c: c[0] in _DSACT),
@@ -182,7 +182,7 @@ ROW_FAULTS = {   # fault: (emulated fault, the cases of ROW_CASES it applies to)
     "v1_no_td_clamp": ("v1_no_td_clamp", lambda c: c[0] in _V1 and c[6]),
     "v1_gsd_sign_bound": ("v1_gsd_sign", lambda c: c[0] in _V1 and c[6]),
     "v1_gsd_sign_nll": ("v1_gsd_sign", lambda c: c[0] in _V1 and not c[6]),
-    "gauss_squash": ("gauss_squash", lambda c: c[0] == "gauss"),
+    "gauss_squash": ("gauss_squash", lambda c: c[0] in R.GAUSS_KINDS),
     "v1_stats_pick_A1": ("v1_stats_pick", lambda c: c[0] in _V1 and c[1] == 1),
     "v1_stats_pick_A2plus": ("v1_stats_pick", lambda c: c[0] in _V1 and c[1] >= 2),
 }
