@@ -454,8 +454,6 @@ static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsac
   enqueue_begin_step(h, c);
   if (!noise) enqueue_noise(h, B, c);
   const dsact_noise nz = step_noise(h, noise);
-  h->pending = bt; h->pending_batch = B;
-  h->pending_eps1 = nz.eps1; h->pending_z3 = nz.z3; h->pending_z4 = nz.z4;
 
   // ---- encoders: pi(s), pi'(s'), Q_k features of s, Q'_k features of s'
   cnn_conv_forward(h, pi, Ppi, bt.obs, h->convP, B, c);
@@ -502,13 +500,13 @@ static void cnn_enqueue_phase1(HeadsHandle* h, const dsact_batch& bt, const dsac
   c.check();
 }
 
-// phase 2: losses, the head and encoder backward passes, and phase2_tail_kernel, on the rows phase 1 ran.  Every batch
-// mean is a sum over these rows times 1/global_batch; phase2_tail_kernel keeps rows = B (this shard), so that the log_alpha
-// gradient it writes is this rank's additive share -(sum_local logp + B * H) / global_batch (see tail_grad_log_alpha).
-static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
+// phase 2: losses, the head and encoder backward passes, and phase2_tail_kernel, on the rows `bt` and noise `nz` phase 1
+// ran.  Every batch mean is a sum over these rows times 1/global_batch; phase2_tail_kernel keeps rows = B (this shard), so
+// that the log_alpha gradient it writes is this rank's additive share -(sum_local logp + B * H) / global_batch (see
+// tail_grad_log_alpha).
+static void cnn_enqueue_phase2(HeadsHandle* h, const dsact_batch& bt, const dsact_noise& nz, int64_t global_batch, Ctx& c) {
   const CnnGeom &q = h->q, &pi = h->pi;
   const StepSlots& s = h->slot;
-  const dsact_batch& bt = h->pending;
   const int B = bt.batch, A = h->act_dim, nq = h->nq();
   float* W = h->W();
   float* P = h->buf.params; float* G = h->buf.grads;
@@ -519,7 +517,7 @@ static void cnn_enqueue_phase2(HeadsHandle* h, int64_t global_batch, Ctx& c) {
 
   // ---- losses and head-output gradients
   const StepScalars sc = step_scalars(h, global_batch);
-  RowIo io = step_rows(h, bt, dsact_noise{h->pending_eps1, nullptr, h->pending_z3, h->pending_z4});
+  RowIo io = step_rows(h, bt, nz);
   for (int k = 0; k < 2; ++k) {
     io.gbias_q[k] = Gq[k] + q.head_off[0] + q.head.b[q.head.L];                                       // output bias of the mean head
     io.gbias_q_raw[k] = q.nheads == 2 ? Gq[k] + q.head_off[1] + q.head.b[q.head.L] : nullptr;   // ... of the std head (one head: the next element)
@@ -602,7 +600,7 @@ static HeadsHandle* heads(dsact_handle* h) { return static_cast<HeadsHandle*>(h)
 // dsact_step: phase 1, phase 2 and the update on its own rows
 static void cnn_enqueue_step(HeadsHandle* h, const dsact_batch& bt, const dsact_noise* noise, Ctx& c) {
   cnn_enqueue_phase1(h, bt, noise, c);
-  cnn_enqueue_phase2(h, bt.batch, c);
+  cnn_enqueue_phase2(h, bt, step_noise(h, noise), bt.batch, c);
   cnn_enqueue_apply(h, c, 1, false);
 }
 
@@ -613,7 +611,7 @@ static void cnn_enqueue_dp_step(HeadsHandle* h, const dsact_batch& bt, const dsa
   float* state = h->buf.state;
   cnn_enqueue_phase1(h, bt, noise, c);
   enqueue_dp_exchange(h->dp, state, 0, c);
-  cnn_enqueue_phase2(h, global_batch, c);
+  cnn_enqueue_phase2(h, bt, step_noise(h, noise), global_batch, c);
   {   // phase 2 already wrote the log_alpha share: a plain copy of the flat gradients into this rank's block
     TailArgs none;
     memset(&none, 0, sizeof(none));

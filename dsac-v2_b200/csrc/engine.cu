@@ -16,6 +16,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <tuple>
 
 #include <vector>
 
@@ -177,10 +178,21 @@ struct Arena : StepSlots {
   }
 };
 
+// Everything the work captured for an update call depends on that is not read from device memory when the graph runs
+// (graph_key derives it from the call)
 struct GraphKey {
-  int kind; const void* p[9]; int32_t batch; int64_t gb; int64_t size; const void* idx;
-  int64_t n_steps; const void* out;   // dsact_replay_steps: updates per call, per-update statistics rows
-  bool operator==(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) == 0; }
+  int run; bool replay, dp;                              // what the call runs (UpdateCall)
+  const float *obs, *act, *rew, *obs2, *done; int32_t batch;   // its rows
+  const float *eps1, *eps2, *z3, *z4;                    // its noise (null: device noise)
+  int64_t global_batch;
+  bool imaged;                                           // the inputs' images were already written (not by the prologue)
+  const int64_t* idx;                                    // replay indices (null: drawn on the device)
+  int32_t n_steps; const float* stats_out;
+  auto tie() const {
+    return std::tie(run, replay, dp, obs, act, rew, obs2, done, batch, eps1, eps2, z3, z4, global_batch, imaged, idx,
+                    n_steps, stats_out);
+  }
+  bool operator==(const GraphKey& o) const { return tie() == o.tie(); }
 };
 struct GraphEntry { GraphKey key; cudaGraphExec_t exec; int launches; uint64_t stamp; };
 
@@ -215,9 +227,8 @@ struct dsact_handle {
   bool rb_codes = false;        // rb_frames and fr.frames holds uint8 codes, decoded through fr_table
   float* fr_table = nullptr;    // the coded ring's device table [256]
   DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
-  int32_t pending_batch = 0; // rows of the shard phase1 processed (phase2 must match)
-  dsact_batch pending = {};  // batch pointers of phase1
-  const float *pending_eps1 = nullptr, *pending_z3 = nullptr, *pending_z4 = nullptr;  // noise phase1 used (phase2 needs it again)
+  dsact_batch pending = {};  // the rows the last phase 1 ran on (batch 0: none); dsact_grad_phase2 runs on them
+  dsact_noise pending_noise = {};   // ... and its noise (the arena's slots for device noise)
   int64_t launches = 0;
   int32_t last_launches = 0;
   explicit dsact_handle(int e) : engine(e) {}
@@ -229,8 +240,6 @@ struct MlpHandle : dsact_handle {
   dsact_config cfg;
   Net q, pi;
   Arena ar;
-  bool join_pending = false; // a forked branch of the current enqueue has not been joined yet
-  bool apply_early = false;  // phase 2 of the current enqueue already ran the critics' part of the update
   bool arena_imaged;         // the last dsact_replay_sample left bf16 images of obs/obs2/act beside the arena batch
   cudaStream_t cap_stream;   // capture-only stream
   cudaStream_t side_stream;  // second branch inside a step (critic weight gradients || policy backward chain)
@@ -251,7 +260,6 @@ struct MlpHandle : dsact_handle {
   float* in2 = nullptr;
   int64_t in2_obs = 0, in2_obs2 = 0, in2_act = 0, in2_rew = 0, in2_done = 0, in2_logp = 0;
   ImgSlot in2_img[3];
-  int in_set = 0;            // the input set the passes being enqueued read
   cudaStream_t gather_stream = nullptr;   // the next update's gather, forked beside a captured update's backward
   cudaEvent_t ev_gather_fork = nullptr, ev_gather_join = nullptr;
   bool tc_attr_done = false, chain_attr_done = false, wgrad_attr_done = false;   // cudaFuncSetAttribute is per device:
@@ -951,15 +959,15 @@ static Wt weight(const MlpHandle* h, const NetInst& n, int j) {   // layer j of 
   return Wt{n.P + n.net->w[j], n.P + n.net->b[j], h->img(n.wimg[j], n.net->s[j + 1])};
 }
 
-static StepPasses step_passes(const MlpHandle* h, const dsact_batch& bt) {
+// the passes of one update on the rows `bt`, whose images are those of input set `set`
+static StepPasses step_passes(const MlpHandle* h, const dsact_batch& bt, int set) {
   const Arena& ar = h->ar;
   float* W = h->W();
   const int B = bt.batch, O = h->cfg.obs_dim, A = h->cfg.act_dim;
   StepPasses s;
   s.I = net_insts(h);
-  const int in = h->in_set;
-  const Ten obs{const_cast<float*>(bt.obs), h->input_img(in, 0, B)}, obs2{const_cast<float*>(bt.obs2), h->input_img(in, 1, B)};
-  const Ten act{const_cast<float*>(bt.act), h->input_img(in, 2, B)};
+  const Ten obs{const_cast<float*>(bt.obs), h->input_img(set, 0, B)}, obs2{const_cast<float*>(bt.obs2), h->input_img(set, 1, B)};
+  const Ten act{const_cast<float*>(bt.act), h->input_img(set, 2, B)};
   const Ten new_act = ten(h, W + ar.new_act, ar.i_new_act, B), act2 = ten(h, W + ar.act2, ar.i_act2, B);
   // the arena holds critic pass Q_k(s,a) at slot k, Q'_k(s',a') at 2 + k and Q_k(s,a~) at 4 + k
   auto critic = [&](const NetInst& n, int p, const Ten& in, const Ten& a, bool store_z, bool keep) {
@@ -1391,13 +1399,29 @@ static dsact_batch arena_batch(const dsact_handle* h, int32_t batch) {
 }
 
 // ---- enqueue: pieces of one MLP update -------------------------------------------
+// Where an update's prologue is enqueued: by its phase 1, forked beside the replay gather (phase 1 joins it), or on c.s
+// before phase 1
+enum { PRO_HERE = 0, PRO_FORKED = 1, PRO_DONE = 2 };
+// One MLP update as the enqueue pieces see it
+struct UpdatePlan {
+  dsact_batch bt;            // its rows
+  const dsact_noise* nz;     // its noise (null: device noise)
+  int64_t global_batch;      // rows of the whole update (every rank's, dp)
+  bool dp;                   // gradients and statistics reduced over the peers (dsact_dp_connect) instead of locally
+  bool imaged;               // the bf16 images of obs / obs2 / act are in place (the prologue does not write them)
+  int set;                   // the input set whose images the passes read (dsact_replay_steps)
+  int prologue;              // PRO_*
+};
+
 // Everything of a step that depends on neither the minibatch gather nor a forward pass: accumulator clears, the
 // gradient memset, the bf16 images of all weights (and of a caller-supplied batch), the device noise.
-static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged) {
+static void enqueue_prologue(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
   float* W = h->W();
+  const dsact_batch& bt = u.bt;
+  const dsact_noise* nz = u.nz;
   const int B = bt.batch, O = cf.obs_dim, A = cf.act_dim;
   const bool tc = h->tc();
   const int nq = h->nq();
@@ -1423,13 +1447,13 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
     const bool two_heads = cf.policy_std == DSACT_STD_SEPARATED;
     ib.reserve(h, c, pi.L + 2);
     add_weights(I.pi);
-    if (!inputs_imaged) ib.add(bt.obs, O, h->img(ar.i_obs, B), B, O);
+    if (!u.imaged) ib.add(bt.obs, O, h->img(ar.i_obs, B), B, O);
     if (two_heads) add_weights(I.pi_ls);
     for (int k = 0; k < nq; ++k) add_weights(I.qt[k]);
     if (two_heads) add_weights(I.pit_ls);
     ib.reserve(h, c, pi.L + 3);
     add_weights(I.pit);
-    if (!inputs_imaged) {
+    if (!u.imaged) {
       ib.add(bt.obs2, O, h->img(ar.i_obs2, B), B, O);
       ib.add(bt.act, A, h->img(ar.i_act, B), B, A);
     }
@@ -1458,11 +1482,11 @@ static void enqueue_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_no
 }
 
 // In a captured step the prologue runs as its own branch next to whatever the main stream does first (the replay
-// gather); returns true if it was forked and must be joined (enqueue_phase1 does) before the first forward pass.
-static bool fork_prologue(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged) {
-  if (!c.side) return false;
-  fork_branch(c, h->ev_pro_fork, h->ev_pro_join, [&](Ctx& cs) { enqueue_prologue(h, bt, nz, cs, inputs_imaged); });
-  return true;
+// gather); returns PRO_FORKED if it was forked and must be joined (enqueue_phase1 does) before the first forward pass.
+static int fork_prologue(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
+  if (!c.side) return PRO_HERE;
+  fork_branch(c, h->ev_pro_fork, h->ev_pro_join, [&](Ctx& cs) { enqueue_prologue(h, u, cs); });
+  return PRO_FORKED;
 }
 
 static void enqueue_dp_reduce_scatter(const DpPeer& dp, const float* state, int num_sms, Ctx& c) {
@@ -1560,30 +1584,26 @@ static void dp_peer_release(DpPeer& dp) {
   dp = DpPeer();
 }
 
-// `dp_std_exchange`: the std sums are complete once sample_kernel has run, one whole forward chain before the loss needs
-// them: in a captured step their exchange (kernel + NVLink flag round trip + whatever the ranks are skewed by) runs as a
-// side branch under that chain.  `prologue_done`: the caller has enqueued the prologue on c.s already.
-static void enqueue_phase1(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, Ctx& c, bool inputs_imaged = false,
-                           bool prologue_forked = false, bool dp_std_exchange = false, bool prologue_done = false) {
+// Forward passes and sampling of update `u`.  With `u.dp` the std sums are complete once sample_kernel has run, one whole
+// forward chain before the loss needs them: in a captured step their exchange (kernel + NVLink flag round trip + whatever
+// the ranks are skewed by) runs as a side branch under that chain.
+static void enqueue_phase1(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
+  const dsact_batch& bt = u.bt;
   const int B = bt.batch;
-  if (prologue_forked) {
-    cudaStreamWaitEvent(c.s, h->ev_pro_join, 0);
-  } else if (!prologue_done) {
-    enqueue_prologue(h, bt, nz, c, inputs_imaged);
-  }
+  if (u.prologue == PRO_FORKED) cudaStreamWaitEvent(c.s, h->ev_pro_join, 0);
+  else if (u.prologue == PRO_HERE) enqueue_prologue(h, u, c);
 
-  const dsact_noise noise = step_noise(h, nz);   // device noise: sample_kernel steps the counter
-  const StepPasses sp = step_passes(h, bt);
+  const dsact_noise noise = step_noise(h, u.nz);   // device noise: sample_kernel steps the counter
+  const StepPasses sp = step_passes(h, bt, u.set);
   enqueue_fwd(h, sp.a, sp.na, B, c);
   RowIo io = step_rows(h, bt, noise);
   io.img_act[0] = img_out(h, h->ar.i_new_act); io.img_act[1] = img_out(h, h->ar.i_act2);
-  enqueue_sample(h, io, B, !nz, c);
-  const bool dp_forked = dp_std_exchange && c.side != nullptr;
+  enqueue_sample(h, io, B, !u.nz, c);
+  const bool dp_forked = u.dp && c.side != nullptr;
   if (dp_forked) fork_branch(c, h->ev_dp_fork, h->ev_dp_join, [&](Ctx& cs) { enqueue_dp_exchange(h, 0, cs); });
-  else if (dp_std_exchange) enqueue_dp_exchange(h, 0, c);
+  else if (u.dp) enqueue_dp_exchange(h, 0, c);
   enqueue_fwd(h, sp.b, sp.nb, B, c);
   if (dp_forked) cudaStreamWaitEvent(c.s, h->ev_dp_join, 0);
-  h->pending_eps1 = noise.eps1; h->pending_z3 = noise.z3; h->pending_z4 = noise.z4;
   c.check();
 }
 
@@ -1598,13 +1618,15 @@ static TailArgs tail_args(const dsact_handle* h, int64_t global_batch, int rows)
   return t;
 }
 static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail, bool dp, int part);
-// `tail` == null (split API): the weight-gradient slabs are folded into the gradient buffer here and phase2_tail_kernel
-// closes the backward.  Otherwise (single-call steps) the kernels that follow do both: enqueue_apply (dp = false), or
-// dp_grad_fold into this rank's exchange block (dp = true).  Single-GPU fused steps also update the critics on the side
-// branch as soon as their weight gradients are complete, beside the policy backward; the caller's enqueue_apply then
-// does the rest.
-static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_batch, Ctx& c, const TailArgs* tail = nullptr,
-                           bool dp = false) {
+// Losses and backward of update `u`.  `tail` == null (split API): the weight-gradient slabs are folded into the gradient
+// buffer here and phase2_tail_kernel closes the backward.  Otherwise (single-call steps) the kernels that follow do both:
+// enqueue_apply (u.dp = false), or dp_grad_fold into this rank's exchange block (u.dp = true).  Single-GPU fused steps
+// also update the critics on the side branch as soon as their weight gradients are complete, beside the policy backward;
+// returns true when it did, and the caller's enqueue_apply then does the rest (part 2).
+static bool enqueue_phase2(MlpHandle* h, const UpdatePlan& u, Ctx& c, const TailArgs* tail) {
+  const dsact_batch& bt = u.bt;
+  const int64_t global_batch = u.global_batch;
+  const bool dp = u.dp;
   const dsact_config& cf = h->cfg;
   const Net &q = h->q, &pi = h->pi;
   const Arena& ar = h->ar;
@@ -1613,11 +1635,11 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const bool tc = h->tc();
   float* G_ = h->buf.grads;
   const long long n_flat = h->n_params;
-  const StepPasses sp = step_passes(h, bt);
+  const StepPasses sp = step_passes(h, bt, u.set);
   const NetInsts& I = sp.I;
 
   const StepScalars sc = step_scalars(h, global_batch);
-  RowIo io = step_rows(h, bt, dsact_noise{h->pending_eps1, nullptr, h->pending_z3, h->pending_z4});
+  RowIo io = step_rows(h, bt, step_noise(h, u.nz));
   for (int k = 0; k < h->nq(); ++k) {   // one two-output layer per critic: the std output's bias follows the mean's
     io.gbias_q[k] = I.q[k].G + q.b[q.L];
     io.img_q[k] = img_out(h, ar.i_dOut[k]); io.img_qa[k] = img_out(h, ar.i_dOut[4 + k]);
@@ -1637,6 +1659,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   const bool chained = enqueue_dgrad(h, sp.q, sp.nqb, B, c, ga);
   add_wgrads(gw, h, sp.q, sp.nqb, B);
   const bool forked = chained && c.side != nullptr;
+  bool applied = false;
   if (forked) {
     fork_branch(c, h->ev_fork, h->ev_join, [&](Ctx& cs) {
       // the policy backward chain needs ceil(B/64) whole SMs: keep them free of weight-gradient CTAs
@@ -1645,14 +1668,13 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
       launch_group(h, gw, V_WGRAD, cs, cap >= h->num_sms / 2 ? cap : 0);
       if (tail && !dp && slabs_foldable(h)) {   // Adam + Polyak of the critics beside the policy backward: every critic gradient is final here
         enqueue_apply(h, cs, tail, false, 1);
-        h->apply_early = true;
+        applied = true;
       }
     });
   } else {
     launch_group(h, gw, V_WGRAD, c);
   }
   launch_group(h, ga, V_DGRAD, c);
-  h->join_pending = forked;
 
   enqueue_policy_grad(h, io, B, sc, c);
   Group gwp, no_act;   // (the policy passes have no action segment)
@@ -1660,7 +1682,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   add_wgrads(gwp, h, sp.pi, sp.npb, B);
   launch_group(h, gwp, V_WGRAD, c);
 
-  if (h->join_pending) { cudaStreamWaitEvent(c.s, h->ev_join, 0); h->join_pending = false; }
+  if (forked) cudaStreamWaitEvent(c.s, h->ev_join, 0);
   if (tc && !dp && !(tail && slabs_foldable(h))) {  // fold the weight-gradient split slabs into the flat gradient buffer
     const long long n = n_flat;
     int blocks = (int)((n + 255) / 256); if (blocks > 4 * h->num_sms) blocks = 4 * h->num_sms;
@@ -1673,6 +1695,7 @@ static void enqueue_phase2(MlpHandle* h, const dsact_batch& bt, int64_t global_b
   if (dp)  // local total (bias gradients + slabs + log_alpha) -> this rank's block of the exchange buffer
     enqueue_dp_fold(h, G_, tc ? W + ar.slabs : G_, tc ? ar.nslabs : 0, tc ? ar.slab_stride : 4, n_flat, *tail, c);
   c.check();
+  return applied;
 }
 
 // The MLP engine's apply of `part` (see apply_part) with the Adam scalars `scalars_ready` (see ApplyArgs), the step's
@@ -1688,25 +1711,28 @@ static ApplyArgs mlp_apply_args(const MlpHandle* h, int scalars_ready, const Tai
 // `tail` != null: this apply also does the end-of-backward bookkeeping of the step (see TailArgs) and, single-GPU, folds
 // the weight-gradient split slabs.  `dp`: the gradients are the rank-ordered sum of the exchange blocks.
 static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail = nullptr, bool dp = false, int part = 0) {
-  if (part == 0 && h->apply_early) { part = 2; h->apply_early = false; }   // phase 2 already updated the critics
   // split API: the Adam scalars are formed here; single-call steps: precomputed by the previous apply / prologue if stamped
   const int nslabs = tail && !dp && slabs_foldable(h) ? h->ar.nslabs : 0;
   launch_apply(h, mlp_apply_args(h, tail ? 2 : 0, tail, dp, part, nslabs), c);
 }
 
-// One whole update of the single-call steps: phase 1, phase 2 over `global_batch` rows, then (dp) the logged-sum exchange
-// (also the "every rank's block is complete" barrier) and the reduce-scatter from 6 ranks up, then Adam / Polyak.
-// `dp`: the gradients and statistics are reduced over the peers (dsact_dp_connect) instead of locally.
-static void enqueue_update(MlpHandle* h, const dsact_batch& bt, const dsact_noise* nz, int64_t global_batch, bool dp,
-                           bool inputs_imaged, bool prologue_forked, Ctx& c) {
-  enqueue_phase1(h, bt, nz, c, inputs_imaged, prologue_forked, dp);
-  const TailArgs ta = tail_args(h, global_batch, bt.batch);
-  enqueue_phase2(h, bt, global_batch, c, &ta, dp);
-  if (dp) {
+// One whole update of the single-call steps: phase 1, phase 2 over `u.global_batch` rows, then (u.dp) the logged-sum
+// exchange (also the "every rank's block is complete" barrier) and the reduce-scatter from 6 ranks up, then Adam / Polyak.
+static void enqueue_update(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
+  enqueue_phase1(h, u, c);
+  const TailArgs ta = tail_args(h, u.global_batch, u.bt.batch);
+  const bool critics_applied = enqueue_phase2(h, u, c, &ta);
+  if (u.dp) {
     enqueue_dp_exchange(h, 1, c);
     if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, h->buf.state, h->num_sms, c);
   }
-  enqueue_apply(h, c, &ta, dp);
+  enqueue_apply(h, c, &ta, u.dp, critics_applied ? 2 : 0);
+}
+
+// the generator counter step of a call whose last draw is the gather's (no sample_kernel after it steps it)
+static void enqueue_rng_advance(const dsact_handle* h, Ctx& c) {
+  launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state);
+  c.done();
 }
 
 // the replay gather with the bf16 images of obs / obs2 / act.  `images_only`: the caller is a fused tensor-core step,
@@ -1759,6 +1785,11 @@ static void stats_scales(const dsact_handle* h, int64_t global_batch, float* inv
   *inv_policy = (float)(1.0 / pol);
 }
 
+// noise of update k of a call whose caller noise `np` holds n updates' draws back to back
+static dsact_noise update_noise(const dsact_noise& np, int k, int B, int A) {
+  return dsact_noise{np.eps1 + (size_t)k * B * A, np.eps2 + (size_t)k * B * A, np.z3 + (size_t)k * B, np.z4 + (size_t)k * B};
+}
+
 // Updates k = 0 .. n-1, each one dsact_replay_step on its slice of idx / noise.  Update k reads input set k & 1; the gather
 // of update k + 1 into the other set needs only the generator counter update k's sample_kernel leaves, so it is forked
 // (captured: onto its own stream) once update k's forward passes are enqueued and runs beside update k's backward; the
@@ -1766,12 +1797,9 @@ static void stats_scales(const dsact_handle* h, int64_t global_batch, float* inv
 // scalars) reads what update k's apply writes and follows it on the main stream with programmatic dependent launch.
 // stats_out: row k = update k's finalised tb_info, written before update k + 1 clears the accumulators.
 static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx, const dsact_noise* np, float* stats_out, Ctx& c) {
-  const int64_t A = h->cfg.act_dim;
+  const int A = h->cfg.act_dim;
   const bool fused = h->fused();
   const bool fork = c.side != nullptr;
-  auto noise_of = [&](int k) {
-    return dsact_noise{np->eps1 + (size_t)k * B * A, np->eps2 + (size_t)k * B * A, np->z3 + (size_t)k * B, np->z4 + (size_t)k * B};
-  };
   auto idx_of = [&](int k) { return idx ? idx + (size_t)k * B : nullptr; };
   // gather of update k into input set k & 1 (+ the counter step a drawn-index, caller-noise update takes after it)
   auto gather = [&](int k, Ctx& cg) {
@@ -1780,27 +1808,24 @@ static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx,
     const ImgOut img[3] = {img_out_of(h, h->input_img(set, 0, B)), img_out_of(h, h->input_img(set, 1, B)),
                            img_out_of(h, h->input_img(set, 2, B))};
     enqueue_gather(h, B, idx_of(k), img, !fused, cg, &dst);
-    if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, cg, h->buf.state); cg.done(); }
+    if (!idx && np) enqueue_rng_advance(h, cg);
   };
   float inv_b, inv_pol;
   stats_scales(h, B, &inv_b, &inv_pol);
   bool gather_forked = false;
   for (int k = 0; k < n; ++k) {
     const int set = k & 1;
-    h->in_set = set;
-    const dsact_batch bt = input_batch(h, set, B);
     dsact_noise nk;
-    const dsact_noise* npk = nullptr;
-    if (np) { nk = noise_of(k); npk = &nk; }
+    if (np) nk = update_noise(*np, k, B, A);
+    UpdatePlan u{input_batch(h, set, B), np ? &nk : nullptr, B, false, true, set, PRO_DONE};
     if (k == 0) {   // as dsact_replay_step: the prologue beside the gather
-      const bool forked = fork_prologue(h, bt, npk, c, true);
+      u.prologue = fork_prologue(h, u, c);
       gather(0, c);
-      enqueue_phase1(h, bt, npk, c, true, forked);
     } else {
-      enqueue_prologue(h, bt, npk, c, true);
+      enqueue_prologue(h, u, c);
       if (gather_forked) cudaStreamWaitEvent(c.s, h->ev_gather_join, 0);
-      enqueue_phase1(h, bt, npk, c, true, false, false, true);
     }
+    enqueue_phase1(h, u, c);
     gather_forked = false;
     if (k + 1 < n) {
       if (fork) {
@@ -1811,21 +1836,17 @@ static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx,
       }
     }
     const TailArgs ta = tail_args(h, B, B);
-    enqueue_phase2(h, bt, B, c, &ta, false);
-    enqueue_apply(h, c, &ta, false);
+    const bool critics_applied = enqueue_phase2(h, u, c, &ta);
+    enqueue_apply(h, c, &ta, false, critics_applied ? 2 : 0);
     if (stats_out) {
       launch_k(finalize_stats_kernel, 1, 32, 0, c, h->buf.state, inv_b, inv_pol, stats_out + (size_t)k * DSACT_NUM_STATS);
       c.done();
     }
   }
-  h->in_set = 0;
   c.check();
 }
 
 // ---- graph cache -------------------------------------------------------------
-enum { K_STEP = 1, K_PHASE1 = 2, K_PHASE2 = 3, K_APPLY = 4, K_GRADS = 5, K_SAMPLE = 6, K_REPLAY_STEP = 7, K_DP_STEP = 8, K_DP_REPLAY_STEP = 9,
-       K_REPLAY_STEPS = 10 };
-
 static void drop_graphs(MlpHandle* h) {
   for (auto& e : h->graphs) cudaGraphExecDestroy(e.exec);
   h->graphs.clear();
@@ -1882,14 +1903,37 @@ static int run(MlpHandle* h, cudaStream_t user, const GraphKey& key, F enqueue) 
   return DSACT_OK;
 }
 
-static GraphKey make_key(int kind, const dsact_batch* b, const dsact_noise* n, int64_t gb) {
-  GraphKey k;
-  memset(&k, 0, sizeof(k));
-  k.kind = kind;
-  if (b) { k.p[0] = b->obs; k.p[1] = b->act; k.p[2] = b->rew; k.p[3] = b->obs2; k.p[4] = b->done; k.batch = b->batch; }
-  if (n) { k.p[5] = n->eps1; k.p[6] = n->eps2; k.p[7] = n->z3; k.p[8] = n->z4; }
-  k.gb = gb;
-  return k;
+// dsact_profile_step: one eager enqueue on `s` with an event after every launch (no side stream: the critics' update is
+// not split off), synchronised, and the time, FLOPs and launches per class into `out`
+template <typename F>
+static int run_profiled(MlpHandle* h, cudaStream_t s, dsact_profile* out, F enqueue) {
+  Prof prof;
+  Ctx c{s, 0, cudaSuccess};
+  c.pdl = h->tc();
+  c.prof = &prof;
+  cudaEvent_t e0;
+  CUDA_TRY(cudaEventCreate(&e0));
+  CUDA_TRY(cudaEventRecord(e0, s));
+  enqueue(c);
+  cudaError_t e = cudaStreamSynchronize(s);
+  memset(out, 0, sizeof(*out));
+  cudaEvent_t prev = e0;
+  for (size_t i = 0; i < prof.ev.size(); ++i) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, prev, prof.ev[i]);
+    out->ms[prof.cls[i]] += ms;
+    out->flops[prof.cls[i]] += prof.flops[i];
+    out->launches[prof.cls[i]] += 1;
+    out->total_ms += ms;
+    prev = prof.ev[i];
+  }
+  cudaEventDestroy(e0);
+  for (auto ev : prof.ev) cudaEventDestroy(ev);
+  if (c.err != cudaSuccess || e != cudaSuccess)
+    return fail(DSACT_ECUDA, "profile step failed: %s", cudaGetErrorString(c.err != cudaSuccess ? c.err : e));
+  h->launches += c.launches;
+  h->last_launches = c.launches;
+  return DSACT_OK;
 }
 
 // true when `bt` is the arena minibatch that the preceding dsact_replay_sample gathered (images already there)
@@ -1967,6 +2011,156 @@ static int check_sm90(int device, int* num_sms) {
 }
 
 #include "cnn_engine.cuh"
+
+// ---- one path for every update entry point (both engines) -----------------------------------------------------------
+// What an update call runs: phase 1, phase 2, both, Adam / Polyak, a whole update, n_steps replay-fed updates, or the
+// replay gather alone
+enum { RUN_PHASE1, RUN_PHASE2, RUN_GRADS, RUN_APPLY, RUN_STEP, RUN_STEPS, RUN_GATHER };
+
+// One update call as its entry point describes it
+struct UpdateCall {
+  const char* fn;                       // the entry point (refusals name it)
+  int run;                              // RUN_*
+  const dsact_batch* batch = nullptr;   // the caller's rows; null: the replay gather's (replay), or (phase 2) the last phase 1's
+  bool replay = false;                  // rows gathered from the replay ring: `rows` of them, ring rows idx[i] (null: drawn on
+  int32_t rows = 0;                     // the device) among the first `size`
+  int64_t size = 0;
+  const int64_t* idx = nullptr;
+  const dsact_noise* noise = nullptr;   // null: device noise
+  int64_t iteration = 0;                // RUN_APPLY, RUN_STEP, RUN_STEPS: the iteration of the (first) update
+  int64_t global_batch = 0;             // rows of the whole update (0: its own rows)
+  bool dp = false;                      // the data-parallel step over the peers (dsact_dp_connect)
+  int32_t n_steps = 1;                  // updates (RUN_STEPS)
+  float* stats_out = nullptr;           // RUN_STEPS: row k = update k's statistics (null: none)
+  bool profiled = false;                // dsact_profile_step: eager, an event after every launch, timings into `prof`
+  dsact_profile* prof = nullptr;
+  dsact_batch* out = nullptr;           // RUN_GATHER: the arena views of the gathered rows (null: none)
+  UpdateCall(const char* f, int r) : fn(f), run(r) {}
+  bool split() const { return run <= RUN_APPLY; }   // the split calls (DSAC-T only)
+  bool iterates() const { return run == RUN_APPLY || run == RUN_STEP || run == RUN_STEPS; }
+};
+
+// the refusals of call `u`, each with the code its entry point has always returned for it
+static int check_call(const dsact_handle* h, const UpdateCall& u) {
+  int rc = u.profiled || (u.replay && u.run != RUN_GATHER) ? check_mlp(h, u.fn) : DSACT_OK;
+  if (rc) return rc;
+  if (u.batch) {
+    if ((rc = check_batch(h, u.batch))) return rc;
+  } else if (!h || !h->bound || (u.replay && !h->rb_bound)) {
+    return fail(DSACT_ESTATE, "not bound");
+  }
+  if (u.run == RUN_STEPS && (u.n_steps < 1 || u.n_steps > DSACT_MAX_REPLAY_STEPS))
+    return fail(DSACT_EINVAL, "n_steps %d outside [1, %d]", u.n_steps, DSACT_MAX_REPLAY_STEPS);
+  if (u.replay && (u.rows < 1 || u.rows > h->max_batch)) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
+  if (u.run == RUN_STEPS && u.iteration + u.n_steps - 1 > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
+  if ((rc = check_noise(u.noise))) return rc;
+  if (u.split() && (rc = check_v2(h))) return rc;
+  if (u.dp) {
+    if ((rc = check_dp(h))) return rc;
+    if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
+  }
+  if (u.run == RUN_PHASE2 && h->pending.batch < 1)
+    return fail(DSACT_ESTATE, "dsact_grad_phase2 without a preceding dsact_grad_phase1");
+  const int32_t local = u.run == RUN_PHASE2 ? h->pending.batch : u.batch ? u.batch->batch : u.rows;
+  if ((u.dp || u.run == RUN_PHASE2) && u.global_batch < local)
+    return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)u.global_batch, local);
+  if (u.profiled && !u.prof) return fail(DSACT_EINVAL, "null out");
+  return DSACT_OK;
+}
+
+// The captured graph of call `u` on plan `p`: the call's kind, and every input of its work that is not device state
+static GraphKey graph_key(const UpdateCall& u, const UpdatePlan& p) {
+  const dsact_noise n = p.nz ? *p.nz : dsact_noise{};
+  return GraphKey{u.run, u.replay, u.dp, p.bt.obs, p.bt.act, p.bt.rew, p.bt.obs2, p.bt.done, p.bt.batch,
+                  n.eps1, n.eps2, n.z3, n.z4, p.global_batch, p.imaged, u.idx, u.n_steps, u.stats_out};
+}
+
+// The MLP engine's enqueue of call `u`, whose (first) update is `p`
+static void enqueue_call(MlpHandle* h, const UpdateCall& u, UpdatePlan p, Ctx& c) {
+  const int B = p.bt.batch;
+  switch (u.run) {
+    case RUN_PHASE1: enqueue_phase1(h, p, c); break;
+    case RUN_PHASE2: enqueue_phase2(h, p, c, nullptr); break;
+    case RUN_GRADS: enqueue_phase1(h, p, c); enqueue_phase2(h, p, c, nullptr); break;
+    case RUN_APPLY: enqueue_apply(h, c); break;
+    case RUN_STEPS: enqueue_replay_steps(h, u.n_steps, B, u.idx, p.nz, u.stats_out, c); break;
+    case RUN_GATHER:
+      enqueue_gather_imaged(h, B, u.idx, c, false);
+      if (!u.idx) enqueue_rng_advance(h, c);
+      break;
+    case RUN_STEP:
+      if (u.replay) {   // weight images, noise, clears: beside the gather
+        p.prologue = fork_prologue(h, p, c);
+        enqueue_gather_imaged(h, B, u.idx, c, h->fused());
+        if (!u.idx && p.nz) enqueue_rng_advance(h, c);   // device noise: phase 1 advances the counter after the join
+      }
+      enqueue_update(h, p, c);
+      break;
+  }
+}
+
+// Every update entry point: the checks, the device, the ring-size and iteration syncs, the rows and noise, the engine's
+// enqueue (captured, eager or profiled), then what the handle records about it
+static int update(dsact_handle* h, const UpdateCall& u, void* stream) {
+  int rc = check_call(h, u);
+  if (rc) return rc;
+  CUDA_TRY(cudaSetDevice(h->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  MlpHandle* m = h->engine == ENGINE_MLP ? mlp(h) : nullptr;
+  if (u.run == RUN_STEPS && (rc = ensure_input_set2(m))) return rc;
+  if (u.replay && (rc = sync_rb_size(h, u.size, s))) return rc;
+  if (u.iterates() && (rc = sync_iteration(h, u.iteration, s))) return rc;
+
+  // the rows and noise: the caller's, the arena's (replay), or (phase 2) those of the last phase 1
+  dsact_batch bt = {};
+  dsact_noise nz = u.noise ? *u.noise : dsact_noise{};
+  const dsact_noise* np = u.noise ? &nz : nullptr;
+  if (u.batch) bt = *u.batch;
+  else if (u.replay) bt = arena_batch(h, u.rows);
+  else if (u.run == RUN_PHASE2) { bt = h->pending; nz = h->pending_noise; np = &nz; }
+  const int64_t gb = u.global_batch > 0 ? u.global_batch : bt.batch;
+
+  if (!m) {
+    HeadsHandle* hh = heads(h);
+    rc = run_eager(h, s, false, [&](Ctx& c) {
+      switch (u.run) {
+        case RUN_PHASE1: cnn_enqueue_phase1(hh, bt, np, c); break;
+        case RUN_PHASE2: cnn_enqueue_phase2(hh, bt, nz, gb, c); break;
+        case RUN_GRADS: cnn_enqueue_phase1(hh, bt, np, c); cnn_enqueue_phase2(hh, bt, step_noise(h, np), gb, c); break;
+        case RUN_APPLY: cnn_enqueue_apply(hh, c, 0, false); break;
+        case RUN_STEP:
+          if (u.dp) cnn_enqueue_dp_step(hh, bt, np, gb, c);
+          else cnn_enqueue_step(hh, bt, np, c);
+          break;
+        case RUN_GATHER: {
+          const ImgOut none[3] = {NO_IMG, NO_IMG, NO_IMG};
+          enqueue_gather(h, u.rows, u.idx, none, true, c);
+          if (!u.idx) enqueue_rng_advance(h, c);
+          break;
+        }
+      }
+    });
+  } else {
+    // the inputs' images: written by this call's gather, left by the preceding dsact_replay_sample, or written by the
+    // prologue (take_arena_images, the one place that tracks what the arena's images hold)
+    const UpdatePlan p{bt, np, gb, u.dp, u.replay || (u.batch && take_arena_images(m, bt)), 0, PRO_HERE};
+    auto enqueue = [&](Ctx& c) { enqueue_call(m, u, p, c); };
+    rc = u.profiled ? run_profiled(m, s, u.prof, enqueue) : run(m, s, graph_key(u, p), enqueue);
+  }
+  if (rc) return rc;
+
+  // the arena's images (and, in the fused modes, only they) now belong to this call's gather
+  if (m && u.replay) m->arena_imaged = u.run == RUN_GATHER;
+  if (u.run == RUN_GATHER) {
+    if (u.out) *u.out = bt;
+  } else if (u.run != RUN_PHASE2 && u.run != RUN_APPLY) {   // the rows and noise of the (last) phase 1, for dsact_grad_phase2
+    const int k = u.n_steps - 1;   // (dsact_replay_steps: update k read input set k & 1)
+    h->pending = u.run == RUN_STEPS ? input_batch(m, k & 1, bt.batch) : bt;
+    h->pending_noise = np ? update_noise(nz, k, bt.batch, h->act_dim) : step_noise(h, nullptr);
+  }
+  if (u.iterates()) h->dev_iter = u.iteration + u.n_steps;
+  return DSACT_OK;
+}
 
 // ---- C ABI ---------------------------------------------------------------------
 extern "C" {
@@ -2154,111 +2348,33 @@ int dsact_set_carry(dsact_handle* h, float m1, float m2, int64_t tq, int64_t tp,
 }
 
 int dsact_grad_phase1(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
-  int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise)) || (rc = check_v2(h))) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  const dsact_batch bt = *batch;
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  if (h->engine == ENGINE_HEADS) {
-    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_phase1(heads(h), bt, np, c); });
-  } else {
-    MlpHandle* m = mlp(h);
-    const bool imaged = take_arena_images(m, bt);
-    rc = run(m, s, make_key(K_PHASE1, &bt, np, imaged ? 1 : 0), [&](Ctx& c) { enqueue_phase1(m, bt, np, c, imaged); });
-    if (rc == DSACT_OK) {  // (a replayed graph does not run enqueue_phase1, so record the noise pointers here as well)
-      const dsact_noise n = step_noise(m, np);
-      m->pending_eps1 = n.eps1; m->pending_z3 = n.z3; m->pending_z4 = n.z4;
-    }
-  }
-  if (rc) return rc;
-  h->pending = bt;
-  h->pending_batch = bt.batch;
-  return DSACT_OK;
+  UpdateCall u("dsact_grad_phase1", RUN_PHASE1);
+  u.batch = batch; u.noise = noise;
+  return update(h, u, stream);
 }
 
 int dsact_grad_phase2(dsact_handle* h, int64_t global_batch, void* stream) {
-  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
-  int rc = check_v2(h);
-  if (rc) return rc;
-  if (h->pending_batch < 1) return fail(DSACT_ESTATE, "dsact_grad_phase2 without a preceding dsact_grad_phase1");
-  if (global_batch < h->pending_batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, h->pending_batch);
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  if (h->engine == ENGINE_HEADS) return run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_phase2(heads(h), global_batch, c); });
-  MlpHandle* m = mlp(h);
-  const dsact_batch bt = h->pending;
-  dsact_noise nz{h->pending_eps1, nullptr, h->pending_z3, h->pending_z4};
-  GraphKey key = make_key(K_PHASE2, &bt, &nz, global_batch);
-  return run(m, s, key, [&](Ctx& c) { enqueue_phase2(m, bt, global_batch, c); });
+  UpdateCall u("dsact_grad_phase2", RUN_PHASE2);
+  u.global_batch = global_batch;
+  return update(h, u, stream);
 }
 
 int dsact_compute_grads(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, void* stream) {
-  int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise)) || (rc = check_v2(h))) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  const dsact_batch bt = *batch;
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  if (h->engine == ENGINE_HEADS) {
-    rc = run_eager(h, s, false, [&](Ctx& c) {
-      cnn_enqueue_phase1(heads(h), bt, np, c);
-      cnn_enqueue_phase2(heads(h), bt.batch, c);
-    });
-  } else {
-    MlpHandle* m = mlp(h);
-    const bool imaged = take_arena_images(m, bt);
-    GraphKey gkey = make_key(K_GRADS, &bt, np, bt.batch);
-    gkey.size = imaged ? 1 : 0;
-    rc = run(m, s, gkey, [&](Ctx& c) {
-      enqueue_phase1(m, bt, np, c, imaged);
-      enqueue_phase2(m, bt, bt.batch, c);
-    });
-  }
-  if (rc) return rc;
-  h->pending = bt; h->pending_batch = bt.batch;
-  return DSACT_OK;
+  UpdateCall u("dsact_compute_grads", RUN_GRADS);
+  u.batch = batch; u.noise = noise;
+  return update(h, u, stream);
 }
 
 int dsact_apply(dsact_handle* h, int64_t iteration, void* stream) {
-  if (!h || !h->bound) return fail(DSACT_ESTATE, "not bound");
-  int rc = check_v2(h);
-  if (rc) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  if ((rc = sync_iteration(h, iteration, s))) return rc;
-  if (h->engine == ENGINE_HEADS) rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_apply(heads(h), c, 0, false); });
-  else rc = run(mlp(h), s, make_key(K_APPLY, nullptr, nullptr, 0), [&](Ctx& c) { enqueue_apply(mlp(h), c); });
-  if (rc) return rc;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  UpdateCall u("dsact_apply", RUN_APPLY);
+  u.iteration = iteration;
+  return update(h, u, stream);
 }
 
 int dsact_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration, void* stream) {
-  int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise))) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  rc = sync_iteration(h, iteration, s);
-  if (rc) return rc;
-  const dsact_batch bt = *batch;
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  if (h->engine == ENGINE_HEADS) {
-    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_step(heads(h), bt, np, c); });
-  } else {
-    MlpHandle* m = mlp(h);
-    const bool imaged = take_arena_images(m, bt);
-    GraphKey skey = make_key(K_STEP, &bt, np, bt.batch);
-    skey.size = imaged ? 1 : 0;
-    rc = run(m, s, skey, [&](Ctx& c) { enqueue_update(m, bt, np, bt.batch, false, imaged, false, c); });
-  }
-  if (rc) return rc;
-  h->pending = bt; h->pending_batch = bt.batch;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  UpdateCall u("dsact_step", RUN_STEP);
+  u.batch = batch; u.noise = noise; u.iteration = iteration;
+  return update(h, u, stream);
 }
 
 // ---- host minibatches: staging on a private copy stream -------------------------------------------------------
@@ -2493,88 +2609,24 @@ int dsact_replay_add(dsact_handle* h, const float* obs, const float* obs2, const
 }
 
 int dsact_replay_sample(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, dsact_batch* out, void* stream) {
-  if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if (batch < 1 || batch > h->max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  int rc = sync_rb_size(h, size, s);
-  if (rc) return rc;
-  ImgOut img[3] = {NO_IMG, NO_IMG, NO_IMG};
-  auto gather = [&](Ctx& c) {
-    enqueue_gather(h, batch, idx, img, true, c);
-    if (!idx) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-  };
-  if (h->engine == ENGINE_HEADS) {
-    rc = run_eager(h, s, false, gather);
-  } else {
-    MlpHandle* m = mlp(h);
-    img[0] = img_out(m, m->ar.i_obs); img[1] = img_out(m, m->ar.i_obs2); img[2] = img_out(m, m->ar.i_act);
-    GraphKey key = make_key(K_SAMPLE, nullptr, nullptr, 0);
-    key.batch = batch; key.idx = idx;
-    rc = run(m, s, key, gather);
-    if (rc == DSACT_OK) m->arena_imaged = true;
-  }
-  if (rc) return rc;
-  if (out) *out = arena_batch(h, batch);
-  return DSACT_OK;
+  UpdateCall u("dsact_replay_sample", RUN_GATHER);
+  u.replay = true; u.rows = batch; u.size = size; u.idx = idx; u.out = out;
+  return update(h, u, stream);
 }
 
-int dsact_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
+int dsact_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
                       int64_t iteration, void* stream) {
-  int rc = check_mlp(hh, "dsact_replay_step");
-  if (rc) return rc;
-  MlpHandle* h = mlp(hh);
-  if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
-  rc = check_noise(noise);
-  if (rc) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  if ((rc = sync_rb_size(h, size, (cudaStream_t)stream))) return rc;
-  if ((rc = sync_iteration(h, iteration, (cudaStream_t)stream))) return rc;
-  const dsact_batch bt = arena_batch(h, batch);
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  GraphKey key = make_key(K_REPLAY_STEP, &bt, np, batch);
-  key.idx = idx;
-  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) {
-    const bool forked = fork_prologue(h, bt, np, c, true);   // weight images, noise, clears: beside the gather
-    enqueue_gather_imaged(h, batch, idx, c, h->fused());
-    if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-    enqueue_update(h, bt, np, batch, false, true, forked, c);  // device noise (np == null): phase1 advances the counter after the join
-  });
-  if (rc) return rc;
-  h->pending = bt; h->pending_batch = batch;
-  h->arena_imaged = false;   // the arena's images (and, in the fused modes, only they) now belong to this step's gather
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  UpdateCall u("dsact_replay_step", RUN_STEP);
+  u.replay = true; u.rows = batch; u.size = size; u.idx = idx; u.noise = noise; u.iteration = iteration;
+  return update(h, u, stream);
 }
 
-int dsact_replay_steps(dsact_handle* hh, int32_t n_steps, int32_t batch, int64_t size, const int64_t* idx,
+int dsact_replay_steps(dsact_handle* h, int32_t n_steps, int32_t batch, int64_t size, const int64_t* idx,
                        const dsact_noise* noise, float* stats_out, int64_t iteration, void* stream) {
-  int rc = check_mlp(hh, "dsact_replay_steps");
-  if (rc) return rc;
-  MlpHandle* h = mlp(hh);
-  if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if (n_steps < 1 || n_steps > DSACT_MAX_REPLAY_STEPS) return fail(DSACT_EINVAL, "n_steps %d outside [1, %d]", n_steps, DSACT_MAX_REPLAY_STEPS);
-  if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
-  if (iteration + n_steps - 1 > 0x7fffffff) return fail(DSACT_EINVAL, "iteration out of range");
-  rc = check_noise(noise);
-  if (rc) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  if ((rc = ensure_input_set2(h))) return rc;
-  if ((rc = sync_rb_size(h, size, (cudaStream_t)stream))) return rc;
-  if ((rc = sync_iteration(h, iteration, (cudaStream_t)stream))) return rc;
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  const dsact_batch bt = arena_batch(h, batch);
-  GraphKey key = make_key(K_REPLAY_STEPS, &bt, np, batch);
-  key.idx = idx; key.n_steps = n_steps; key.out = stats_out;
-  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) { enqueue_replay_steps(h, n_steps, batch, idx, np, stats_out, c); });
-  if (rc) return rc;
-  h->pending = input_batch(h, (n_steps - 1) & 1, batch); h->pending_batch = batch;
-  h->arena_imaged = false;
-  h->dev_iter = iteration + n_steps;
-  return DSACT_OK;
+  UpdateCall u("dsact_replay_steps", RUN_STEPS);
+  u.replay = true; u.rows = batch; u.size = size; u.idx = idx; u.noise = noise; u.iteration = iteration;
+  u.n_steps = n_steps; u.stats_out = stats_out;
+  return update(h, u, stream);
 }
 
 // ---- data parallelism over peer memory (dp_peer.cuh) ------------------------------------------------------------
@@ -2600,106 +2652,24 @@ int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* h
 // gradient + statistics exchange, Adam on the rank-ordered global sum.  Every rank must call it for the same iteration.
 int dsact_dp_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t global_batch, int64_t iteration,
                   void* stream) {
-  int rc = check_batch(h, batch);
-  if (rc || (rc = check_noise(noise)) || (rc = check_dp(h))) return rc;
-  if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
-  if (global_batch < batch->batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch->batch);
-  CUDA_TRY(cudaSetDevice(h->device));
-  const cudaStream_t s = (cudaStream_t)stream;
-  if ((rc = sync_iteration(h, iteration, s))) return rc;
-  const dsact_batch bt = *batch;
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  if (h->engine == ENGINE_HEADS) {
-    rc = run_eager(h, s, false, [&](Ctx& c) { cnn_enqueue_dp_step(heads(h), bt, np, global_batch, c); });
-  } else {
-    MlpHandle* m = mlp(h);
-    const bool imaged = take_arena_images(m, bt);
-    GraphKey key = make_key(K_DP_STEP, &bt, np, global_batch);
-    key.size = imaged ? 1 : 0;
-    rc = run(m, s, key, [&](Ctx& c) { enqueue_update(m, bt, np, global_batch, true, imaged, false, c); });
-  }
-  if (rc) return rc;
-  h->pending = bt; h->pending_batch = bt.batch;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  UpdateCall u("dsact_dp_step", RUN_STEP);
+  u.batch = batch; u.noise = noise; u.iteration = iteration; u.global_batch = global_batch; u.dp = true;
+  return update(h, u, stream);
 }
 
-int dsact_dp_replay_step(dsact_handle* hh, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
+int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int64_t* idx, const dsact_noise* noise,
                          int64_t global_batch, int64_t iteration, void* stream) {
-  int rc = check_mlp(hh, "dsact_dp_replay_step");
-  if (rc) return rc;
-  MlpHandle* h = mlp(hh);
-  if (!h || !h->bound || !h->rb_bound) return fail(DSACT_ESTATE, "not bound");
-  if ((rc = check_dp(h))) return rc;
-  if (!h->dp.ready) return fail(DSACT_ESTATE, "dsact_dp_connect has not been called");
-  if (batch < 1 || batch > h->cfg.max_batch) return fail(DSACT_EINVAL, "batch outside [1, max_batch]");
-  if (global_batch < batch) return fail(DSACT_EINVAL, "global_batch %lld < local batch %d", (long long)global_batch, batch);
-  rc = check_noise(noise);
-  if (rc) return rc;
-  CUDA_TRY(cudaSetDevice(h->device));
-  if ((rc = sync_rb_size(h, size, (cudaStream_t)stream))) return rc;
-  if ((rc = sync_iteration(h, iteration, (cudaStream_t)stream))) return rc;
-  const dsact_batch bt = arena_batch(h, batch);
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  GraphKey key = make_key(K_DP_REPLAY_STEP, &bt, np, global_batch);
-  key.idx = idx;
-  rc = run(h, (cudaStream_t)stream, key, [&](Ctx& c) {
-    const bool forked = fork_prologue(h, bt, np, c, true);
-    enqueue_gather_imaged(h, batch, idx, c, h->fused());
-    if (!idx && np) { launch_k(rng_advance_kernel, 1, 32, 0, c, h->buf.state); c.done(); }
-    enqueue_update(h, bt, np, global_batch, true, true, forked, c);
-  });
-  if (rc) return rc;
-  h->pending = bt; h->pending_batch = batch;
-  h->arena_imaged = false;   // the arena's images (and, in the fused modes, only they) now belong to this step's gather
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  UpdateCall u("dsact_dp_replay_step", RUN_STEP);
+  u.replay = true; u.rows = batch; u.size = size; u.idx = idx; u.noise = noise; u.iteration = iteration;
+  u.global_batch = global_batch; u.dp = true;
+  return update(h, u, stream);
 }
 
-int dsact_profile_step(dsact_handle* hh, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration,
+int dsact_profile_step(dsact_handle* h, const dsact_batch* batch, const dsact_noise* noise, int64_t iteration,
                        void* stream, dsact_profile* out) {
-  int rc = check_mlp(hh, "dsact_profile_step");
-  if (rc || (rc = check_batch(hh, batch)) || (rc = check_noise(noise))) return rc;
-  if (!out) return fail(DSACT_EINVAL, "null out");
-  MlpHandle* h = mlp(hh);
-  CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  rc = sync_iteration(h, iteration, s);
-  if (rc) return rc;
-  const dsact_batch bt = *batch;
-  dsact_noise nz; const dsact_noise* np = nullptr;
-  if (noise) { nz = *noise; np = &nz; }
-  Prof prof;
-  Ctx c{s, 0, cudaSuccess};
-  c.pdl = h->tc();
-  c.prof = &prof;
-  cudaEvent_t e0;
-  CUDA_TRY(cudaEventCreate(&e0));
-  CUDA_TRY(cudaEventRecord(e0, s));
-  enqueue_update(h, bt, np, bt.batch, false, false, false, c);   // no side stream: the critics' update is not split off
-  cudaError_t e = cudaStreamSynchronize(s);
-  memset(out, 0, sizeof(*out));
-  cudaEvent_t prev = e0;
-  for (size_t i = 0; i < prof.ev.size(); ++i) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, prev, prof.ev[i]);
-    out->ms[prof.cls[i]] += ms;
-    out->flops[prof.cls[i]] += prof.flops[i];
-    out->launches[prof.cls[i]] += 1;
-    out->total_ms += ms;
-    prev = prof.ev[i];
-  }
-  cudaEventDestroy(e0);
-  for (auto ev : prof.ev) cudaEventDestroy(ev);
-  if (c.err != cudaSuccess || e != cudaSuccess)
-    return fail(DSACT_ECUDA, "profile step failed: %s", cudaGetErrorString(c.err != cudaSuccess ? c.err : e));
-  h->launches += c.launches;
-  h->last_launches = c.launches;
-  h->pending = bt; h->pending_batch = bt.batch;
-  h->dev_iter = iteration + 1;
-  return DSACT_OK;
+  UpdateCall u("dsact_profile_step", RUN_STEP);
+  u.batch = batch; u.noise = noise; u.iteration = iteration; u.profiled = true; u.prof = out;
+  return update(h, u, stream);
 }
 
 int64_t dsact_launch_count(const dsact_handle* h) { return h ? h->launches : 0; }

@@ -266,51 +266,50 @@ class Engine:
         keep = (eps1, eps2, z3, z4)
         return C.byref(Noise(eps1.data_ptr(), eps2.data_ptr(), z3.data_ptr(), z4.data_ptr())), keep
 
-    # ---- the path ---------------------------------------------------------------
-    def step(self, data, iteration: int, noise=None):
-        """DSAC_V2.local_update (reference dsac_v2.py:102-105) on device tensors."""
+    def _update(self, fn: str, data=None, noise=None, *, replay=None, args=(), out=None, host_fn=None, release=True):
+        """One update call `fn` of the C ABI: its rows (the minibatch `data`, or with `replay` = (batch, size, idx) the
+        replay gather's), `noise`, the other arguments `args`, the stream, then `out` if given.  `host_fn`: the entry point
+        that takes a host minibatch itself (`data` on the CPU).  `release`: no later call reads a staged host minibatch."""
         with torch.cuda.device(self.device):
-            if data["obs"].device.type == "cpu":   # the reference-facing call with a host minibatch: one C call
-                b = self._host_batch(data)
-                n, keep = self._noise(noise, b.batch)
-                self._keep_noise = keep
-                check(self.lib.dsact_step_host(self.h, C.byref(b), n, int(iteration), self._stream()))
+            if replay is not None:
+                B, size, idx = replay
+                if idx is not None:
+                    idx = idx.to(device=self.device, dtype=torch.int64).contiguous()
+                    self._keep_idx = idx
+                rows = (int(B), int(size), _ptr(idx))
             else:
-                b = self._batch(data)
-                n, keep = self._noise(noise, b.batch)
-                self._keep_noise = keep
-                check(self.lib.dsact_step(self.h, C.byref(b), n, int(iteration), self._stream()))
-        self.last_batch = b.batch
+                if host_fn is not None and data["obs"].device.type == "cpu":
+                    b, fn = self._host_batch(data), host_fn
+                else:
+                    b = self._batch(data)
+                B, rows = b.batch, (C.byref(b),)
+            n, self._keep_noise = self._noise(noise, int(B))
+            check(getattr(self.lib, fn)(self.h, *rows, n, *args, self._stream(), *(() if out is None else (out,))))
+            if release:
+                self._mark_staged_done()
+        self.last_batch = int(B)
+
+    # ---- the path ---------------------------------------------------------------
+    # the step on a host minibatch in one C call (None: the minibatch goes through _batch)
+    _step_host = "dsact_step_host"
+
+    def step(self, data, iteration: int, noise=None):
+        """DSAC_V2.local_update (reference dsac_v2.py:102-105), or DSAC_V1's, on a host or device minibatch."""
+        self._update("dsact_step", data, noise, args=(int(iteration),), host_fn=self._step_host)
 
     def profile_step(self, data, iteration: int, noise=None) -> dict:
         """One eager step with per-launch CUDA events (bench.py's roofline leg)."""
         out = _lib.Profile()
-        with torch.cuda.device(self.device):
-            b = self._batch(data)
-            n, keep = self._noise(noise, b.batch)
-            check(self.lib.dsact_profile_step(self.h, C.byref(b), n, int(iteration), self._stream(), C.byref(out)))
-            self._mark_staged_done()
-        self.last_batch = b.batch
+        self._update("dsact_profile_step", data, noise, args=(int(iteration),), out=C.byref(out))
         names = ("other", "gemm_fwd", "gemm_dgrad", "gemm_wgrad")
         return {"total_ms": out.total_ms,
                 **{k: {"ms": out.ms[i], "flops": out.flops[i], "launches": out.launches[i]} for i, k in enumerate(names)}}
 
     def compute_grads(self, data, noise=None):
-        with torch.cuda.device(self.device):
-            b = self._batch(data)
-            n, keep = self._noise(noise, b.batch)
-            self._keep_noise = keep
-            check(self.lib.dsact_compute_grads(self.h, C.byref(b), n, self._stream()))
-            self._mark_staged_done()
-        self.last_batch = b.batch
+        self._update("dsact_compute_grads", data, noise)
 
     def grad_phase1(self, data, noise=None):
-        with torch.cuda.device(self.device):
-            b = self._batch(data)
-            n, keep = self._noise(noise, b.batch)
-            self._keep_noise = keep
-            check(self.lib.dsact_grad_phase1(self.h, C.byref(b), n, self._stream()))
-        self.last_batch = b.batch
+        self._update("dsact_grad_phase1", data, noise, release=False)   # grad_phase2 reads the rows as well
 
     def grad_phase2(self, global_batch: int):
         with torch.cuda.device(self.device):
@@ -461,14 +460,7 @@ class Engine:
         return self.arena_batch(out)
 
     def replay_step(self, batch: int, size: int, iteration: int, idx: Optional[torch.Tensor] = None, noise=None):
-        with torch.cuda.device(self.device):
-            if idx is not None:
-                idx = idx.to(device=self.device, dtype=torch.int64).contiguous()
-                self._keep_idx = idx
-            n, keep = self._noise(noise, batch)
-            self._keep_noise = keep
-            check(self.lib.dsact_replay_step(self.h, int(batch), int(size), _ptr(idx), n, int(iteration), self._stream()))
-        self.last_batch = int(batch)
+        self._update("dsact_replay_step", noise=noise, replay=(batch, size, idx), args=(int(iteration),))
 
     def _steps_buffer(self, name: str, src: torch.Tensor, dtype) -> torch.Tensor:
         """`src` as a contiguous device tensor.  Host data is staged into a buffer kept per name and shape, so that a
@@ -536,25 +528,11 @@ class Engine:
 
     def dp_step(self, data, iteration: int, global_batch: int, noise=None):
         """dsact_step on this rank's shard with the exchanges done in-kernel over peer memory."""
-        with torch.cuda.device(self.device):
-            b = self._batch(data)
-            n, keep = self._noise(noise, b.batch)
-            self._keep_noise = keep
-            check(self.lib.dsact_dp_step(self.h, C.byref(b), n, int(global_batch), int(iteration), self._stream()))
-            self._mark_staged_done()
-        self.last_batch = b.batch
+        self._update("dsact_dp_step", data, noise, args=(int(global_batch), int(iteration)))
 
     def dp_replay_step(self, batch: int, size: int, iteration: int, global_batch: int, idx: Optional[torch.Tensor] = None,
                        noise=None):
-        with torch.cuda.device(self.device):
-            if idx is not None:
-                idx = idx.to(device=self.device, dtype=torch.int64).contiguous()
-                self._keep_idx = idx
-            n, keep = self._noise(noise, batch)
-            self._keep_noise = keep
-            check(self.lib.dsact_dp_replay_step(self.h, int(batch), int(size), _ptr(idx), n, int(global_batch), int(iteration),
-                                                self._stream()))
-        self.last_batch = int(batch)
+        self._update("dsact_dp_replay_step", noise=noise, replay=(batch, size, idx), args=(int(global_batch), int(iteration)))
 
     # ---- weights in the reference's state_dict schema -----------------------------------
     def _schema(self):

@@ -5,13 +5,12 @@ minibatches is `engine.Engine`'s: the same buffers, and the same dsact_* calls o
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional, Sequence
 
 import torch
 
 from . import _lib
-from ._lib import Batch, CnnConfig, check
+from ._lib import Batch, CnnConfig
 from .engine import Engine
 
 
@@ -60,6 +59,7 @@ class CnnEngine(Engine):
     replay-fused steps, `profile_step` and `test_gemm` raise `DsactError`."""
 
     _query, _create = "dsact_cnn_query_layout", "dsact_cnn_create"
+    _step_host = None   # _batch copies host minibatches to the device
 
     @property
     def obs_elems(self) -> int:
@@ -117,14 +117,6 @@ class CnnEngine(Engine):
             raise ValueError("minibatch shapes do not match the configured observation / action shape")
         self._keep = t
         return Batch(t["obs"].data_ptr(), t["act"].data_ptr(), t["rew"].data_ptr(), t["obs2"].data_ptr(), t["done"].data_ptr(), B, None)
-
-    def step(self, data: Dict[str, torch.Tensor], iteration: int, noise=None):
-        """DSAC_V2.local_update (reference dsac_v2.py:102-105), or DSAC_V1's, on a host or device minibatch."""
-        with torch.cuda.device(self.device):
-            b = self._batch(data)
-            n, self._keep_noise = self._noise(noise, b.batch)
-            check(self.lib.dsact_step(self.h, C.byref(b), n, int(iteration), self._stream()))
-        self.last_batch = b.batch
 
     def replay_sample(self, batch: int, size: int, idx: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         out = super().replay_sample(batch, size, idx)

@@ -257,6 +257,31 @@ def test_replay_sample_then_step_reads_the_gathered_images():
     eng.close()
 
 
+@pytest.mark.parametrize("use_graph", [False, True])
+def test_step_on_sampled_views_after_a_profiled_step_images_them_again(use_graph):
+    """replay_sample, then profile_step on another minibatch, then step on the sampled arena views, in bf16x3 at B = 16.
+    The profiled step wrote its own rows' images into the arena's input image slots, so the step must image the views
+    again: its parameters, targets, Adam moments and state equal, bit for bit, a twin engine's step on a copy of the
+    sampled rows (up to 16 rows an update is bit-reproducible, DESIGN §9 item 6)."""
+    cfg, B, a, host, size = setup("tiny", "bf16x3", use_graph)
+    b = make_engine(cfg, B, use_graph=use_graph, gemm_mode="bf16x3")
+    b.seed(SEED)
+    bind_ring(b, host)
+    other = {k: torch.from_numpy(v).cuda() for k, v in synth.make_batch(cfg, B, 7).items()}
+    noise = [tuple(torch.from_numpy(n[i]).cuda() for i in (0, 1, 4, 5)) for n in (synth.make_noise(cfg, B, it) for it in (0, 1))]
+    views = a.replay_sample(B, size)
+    copy = {k: v.clone() for k, v in views.items()}
+    b.replay_sample(B, size)   # the same draws: the generator counters stay equal
+    for e in (a, b):
+        e.profile_step(other, 0, noise[0])
+    a.step(views, 1, noise[1])
+    b.step(copy, 1, noise[1])
+    torch.cuda.synchronize()
+    for k in ("params", "targets", "adam_m", "adam_v", "state"):
+        assert torch.equal(getattr(a, k), getattr(b, k)), k
+    a.close(); b.close()
+
+
 def test_headwise_replay_sample_draws_and_gathers_exactly():
     """The head-wise engine's gather on carracing rows (27648 floats: many float4 trips per row)."""
     from dsac_v2_b200.engine_cnn import CnnEngine, make_cnn_config
