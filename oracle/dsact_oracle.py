@@ -293,6 +293,38 @@ class OracleDSACT:
         self.apply(iteration)
         return tb
 
+    # ---- the whole state between two updates -----------------------------
+    def _online_keys(self) -> Dict[str, List[str]]:
+        """{net: the state_dict keys of its parameters, in the order of self.p[net]}."""
+        sd = list(self.state_dict())
+        return {net: [k for k in sd if k.startswith(net + ".")] for net in self.NETS}
+
+    def load_state(self, params, m, v, mean_std, steps_q: int, steps_pi: int) -> None:
+        """Replace the state one update starts from: `params` in the state_dict schema (online, `*_target` and
+        log_alpha), the Adam moments `m` / `v` keyed like the online parameters plus "log_alpha", the carried mean_std
+        pair (None or a negative value: unset, as dsac_v2.py:88-89) and the step counters of the critics' optimizers and
+        of the policy and temperature optimizers (they step together, dsac_v2.py:327-333)."""
+        c = lambda x: torch.as_tensor(x).detach().clone().to(device=self.device, dtype=self.dtype)
+        for net, keys in self._online_keys().items():
+            tkeys = [net + "_target" + k[len(net):] for k in keys]
+            self.p[net] = [c(params[k]).requires_grad_(True) for k in keys]
+            self.t[net] = [c(params[k]) for k in tkeys]
+            self.m[net], self.v[net] = [c(m[k]) for k in keys], [c(v[k]) for k in keys]
+            self.steps[net] = int(steps_pi if net == "policy" else steps_q)
+        self.log_alpha = c(params["log_alpha"]).reshape(()).requires_grad_(True)
+        self.m["log_alpha"], self.v["log_alpha"] = [c(m["log_alpha"]).reshape(())], [c(v["log_alpha"]).reshape(())]
+        self.steps["log_alpha"] = int(steps_pi)
+        self.mean_std = [None if x is None or float(x) < 0 else c(float(x)).reshape(()) for x in mean_std]
+
+    def moments(self):
+        """(m, v): the Adam moments in the schema `load_state` takes."""
+        out = []
+        for mv in (self.m, self.v):
+            d = {k: mv[net][i].detach() for net, keys in self._online_keys().items() for i, k in enumerate(keys)}
+            d["log_alpha"] = mv["log_alpha"][0].detach()
+            out.append(d)
+        return tuple(out)
+
     # ---- views in the reference's state_dict schema ----------------------
     def state_dict(self) -> Dict[str, torch.Tensor]:
         inner = {"q1": "q", "q2": "q", "policy": "policy"}

@@ -325,7 +325,8 @@ def engagement(name: str) -> Dict[str, float]:
 
 
 # ---- the CUDA side --------------------------------------------------------------------------------------------------
-def make_engine(case: Case, mode: str):
+def make_engine(case: Case, mode: str, use_graph: bool = False):
+    """The case's engine on cuda:0; `use_graph`: the MLP engine captures its steps in CUDA graphs."""
     cfg, B, h = case.cfg, case.batch, case.hyperparameters
     lim = torch.full((cfg["act_dim"],), cfg["act_lim"])
     common = dict(max_batch=B, gamma=h["gamma"], tau=h["tau"], delay_update=h["delay_update"], auto_alpha=h["auto_alpha"],
@@ -340,7 +341,7 @@ def make_engine(case: Case, mode: str):
                              f"not {case.algo} / {case.std_type!r}")
         act_q, act_pi = synth.activations(cfg)
         c = make_config(cfg["obs_dim"], cfg["act_dim"], *synth.hidden_sizes(cfg), act_q=act_q, act_pi=act_pi, gemm_mode=mode,
-                        use_graph=False, **common)
+                        use_graph=use_graph, **common)
         return Engine(c, torch.device("cuda", 0), lim, -lim)
     from dsac_v2_b200.engine_cnn import CnnEngine, make_cnn_config, make_heads_config
     if case.cnn:
