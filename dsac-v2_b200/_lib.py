@@ -173,6 +173,9 @@ SYMBOLS = {
     "dsact_replay_bind_coded_frames": (C.c_int, [C.c_void_p, C.POINTER(FrameReplay), C.c_void_p]),
     "dsact_replay_add_coded_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int32]
                                       + [C.c_void_p] * 6 + [C.c_int64, C.c_int64, C.c_void_p]),
+    "dsact_replay_bind_coded16_frames": (C.c_int, [C.c_void_p, C.POINTER(FrameReplay), C.c_void_p]),
+    "dsact_replay_add_coded16_frames": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int32]
+                                        + [C.c_void_p] * 6 + [C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_replay_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Batch), C.c_void_p]),
     "dsact_replay_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_int64, C.c_void_p]),
     "dsact_replay_steps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_void_p,

@@ -224,8 +224,9 @@ struct dsact_handle {
   dsact_replay rb = {};
   dsact_frame_replay fr = {};   // the frame ring, when rb_frames (binding either ring kind replaces the other)
   bool rb_frames = false;
-  bool rb_codes = false;        // rb_frames and fr.frames holds uint8 codes, decoded through fr_table
-  float* fr_table = nullptr;    // the coded ring's device table [256]
+  int rb_code_bytes = 0;        // rb_frames: fr.frames holds fp32 values (0), or uint8 (1) / uint16 (2) codes decoded
+                                // through fr_table
+  float* fr_table = nullptr;    // a coded ring's device table [256 or 65 536]
   DpPeer dp;                 // peer-memory data parallelism (dp_peer.cuh)
   dsact_batch pending = {};  // the rows the last phase 1 ran on (batch 0: none); dsact_grad_phase2 runs on them
   dsact_noise pending_noise = {};   // ... and its noise (the arena's slots for device noise)
@@ -1373,7 +1374,8 @@ static void enqueue_gather(const dsact_handle* h, int B, const int64_t* idx, con
   int blocks = (B + 7) / 8; if (blocks > 8 * h->num_sms) blocks = 8 * h->num_sms;
   if (h->rb_frames) {
     const dsact_frame_replay& r = h->fr;
-    launch_k(h->rb_codes ? gather_kernel<true, true> : gather_kernel<true>, blocks, 256, 0, c, (const float*)r.frames,
+    launch_k(h->rb_code_bytes == 2 ? gather_kernel<true, 2> : h->rb_code_bytes == 1 ? gather_kernel<true, 1> : gather_kernel<true>,
+             blocks, 256, 0, c, (const float*)r.frames,
              (const float*)r.frames, r.act, r.rew, r.done,
              r.logp, idx, d[0], d[1], d[2], d[3], d[4], d[5], B, (int)h->obs_elems, h->act_dim,
              img[0], img[1], img[2], draw, (unsigned long long)h->seed, (const float*)h->buf.state, write_f32 ? 1 : 0,
@@ -2459,7 +2461,7 @@ int dsact_replay_bind(dsact_handle* h, const dsact_replay* rb) {
   h->rb = *rb;
   h->rb_bound = true;
   h->rb_frames = false;
-  h->rb_codes = false;
+  h->rb_code_bytes = 0;
   if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
   return DSACT_OK;
 }
@@ -2478,12 +2480,12 @@ static int check_frame_ring(const dsact_handle* h, const dsact_frame_replay* rb)
   return DSACT_OK;
 }
 
-static int bind_frame_ring(dsact_handle* h, const dsact_frame_replay* rb, const float* table) {
+static int bind_frame_ring(dsact_handle* h, const dsact_frame_replay* rb, const float* table, int code_bytes) {
   h->fr = *rb;
   h->fr_table = const_cast<float*>(table);
   h->rb_bound = true;
   h->rb_frames = true;
-  h->rb_codes = table != nullptr;
+  h->rb_code_bytes = code_bytes;
   if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));
   return DSACT_OK;
 }
@@ -2491,14 +2493,22 @@ static int bind_frame_ring(dsact_handle* h, const dsact_frame_replay* rb, const 
 int dsact_replay_bind_frames(dsact_handle* h, const dsact_frame_replay* rb) {
   if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
   if (int rc = check_frame_ring(h, rb)) return rc;
-  return bind_frame_ring(h, rb, nullptr);
+  return bind_frame_ring(h, rb, nullptr, 0);
 }
 
-int dsact_replay_bind_coded_frames(dsact_handle* h, const dsact_frame_replay* rb, const float* table) {
+static int bind_coded_ring(dsact_handle* h, const dsact_frame_replay* rb, const float* table, int code_bytes) {
   if (!h || !rb) return fail(DSACT_EINVAL, "null argument");
   if (int rc = check_frame_ring(h, rb)) return rc;
   if (!table) return fail(DSACT_EINVAL, "null table");
-  return bind_frame_ring(h, rb, table);
+  return bind_frame_ring(h, rb, table, code_bytes);
+}
+
+int dsact_replay_bind_coded_frames(dsact_handle* h, const dsact_frame_replay* rb, const float* table) {
+  return bind_coded_ring(h, rb, table, 1);
+}
+
+int dsact_replay_bind_coded16_frames(dsact_handle* h, const dsact_frame_replay* rb, const float* table) {
+  return bind_coded_ring(h, rb, table, 2);
 }
 
 // the first n entries of a HOST frame-id table (nullptr: not host memory, or an id outside [0, frame_capacity))
@@ -2561,18 +2571,23 @@ int dsact_replay_add_frames(dsact_handle* h, const float* frames, int64_t n_fram
                             const int32_t* obs_frames, const int32_t* obs2_frames, const float* act, const float* rew,
                             const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
   if (!h || !h->rb_bound || !h->rb_frames) return fail(DSACT_ESTATE, "frame replay ring not bound");
-  if (h->rb_codes) return fail(DSACT_ESTATE, "a coded frame ring is bound: frames go in through dsact_replay_add_coded_frames");
+  if (h->rb_code_bytes)
+    return fail(DSACT_ESTATE, "a coded frame ring is bound: frames go in through dsact_replay_add_coded%s_frames",
+                h->rb_code_bytes == 2 ? "16" : "");
   if (int rc = check_frame_rows(h, frames, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr)) return rc;
   return put_frame_rows(h, frames, sizeof(float), n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr,
                         (cudaStream_t)stream);
 }
 
-int dsact_replay_add_coded_frames(dsact_handle* h, const uint8_t* codes, int64_t n_frames, int64_t frame_ptr,
-                                  const float* table, int32_t n_codes, const int32_t* obs_frames, const int32_t* obs2_frames,
-                                  const float* act, const float* rew, const float* done, const float* logp, int64_t n,
-                                  int64_t ptr, void* stream) {
-  if (!h || !h->rb_bound || !h->rb_codes) return fail(DSACT_ESTATE, "coded frame replay ring not bound");
-  if (n_codes < 0 || n_codes > 256) return fail(DSACT_EINVAL, "n_codes %d outside [0, 256]", (int)n_codes);
+// an add to a coded ring of `Code` codes (uint8_t: dsact_replay_add_coded_frames, uint16_t: ..._coded16_frames)
+extern "C++" template <typename Code>
+int add_coded_frames(dsact_handle* h, const Code* codes, int64_t n_frames, int64_t frame_ptr, const float* table,
+                     int32_t n_codes, const int32_t* obs_frames, const int32_t* obs2_frames, const float* act,
+                     const float* rew, const float* done, const float* logp, int64_t n, int64_t ptr, void* stream) {
+  constexpr int bytes = (int)sizeof(Code), max_codes = 1 << (8 * bytes);
+  if (!h || !h->rb_bound || h->rb_code_bytes != bytes)
+    return fail(DSACT_ESTATE, "%scoded frame replay ring not bound", bytes == 2 ? "16-bit " : "");
+  if (n_codes < 0 || n_codes > max_codes) return fail(DSACT_EINVAL, "n_codes %d outside [0, %d]", (int)n_codes, max_codes);
   if (n_codes > 0 && !table) return fail(DSACT_EINVAL, "null table");
   if (int rc = check_frame_rows(h, codes, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr)) return rc;
   if (n_frames > 0) {   // the gather decodes through these codes: every one is checked before anything is copied
@@ -2585,7 +2600,23 @@ int dsact_replay_add_coded_frames(dsact_handle* h, const uint8_t* codes, int64_t
   }
   const cudaStream_t s = (cudaStream_t)stream;
   if (n_codes > 0) CUDA_TRY(cudaMemcpyAsync(h->fr_table, table, n_codes * sizeof(float), cudaMemcpyDefault, s));
-  return put_frame_rows(h, codes, 1, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr, s);
+  return put_frame_rows(h, codes, bytes, n_frames, frame_ptr, obs_frames, obs2_frames, act, rew, done, logp, n, ptr, s);
+}
+
+int dsact_replay_add_coded_frames(dsact_handle* h, const uint8_t* codes, int64_t n_frames, int64_t frame_ptr,
+                                  const float* table, int32_t n_codes, const int32_t* obs_frames, const int32_t* obs2_frames,
+                                  const float* act, const float* rew, const float* done, const float* logp, int64_t n,
+                                  int64_t ptr, void* stream) {
+  return add_coded_frames(h, codes, n_frames, frame_ptr, table, n_codes, obs_frames, obs2_frames, act, rew, done, logp, n,
+                          ptr, stream);
+}
+
+int dsact_replay_add_coded16_frames(dsact_handle* h, const uint16_t* codes, int64_t n_frames, int64_t frame_ptr,
+                                    const float* table, int32_t n_codes, const int32_t* obs_frames,
+                                    const int32_t* obs2_frames, const float* act, const float* rew, const float* done,
+                                    const float* logp, int64_t n, int64_t ptr, void* stream) {
+  return add_coded_frames(h, codes, n_frames, frame_ptr, table, n_codes, obs_frames, obs2_frames, act, rew, done, logp, n,
+                          ptr, stream);
 }
 
 int dsact_replay_add(dsact_handle* h, const float* obs, const float* obs2, const float* act, const float* rew,

@@ -8,6 +8,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "gemm_simt.cuh"   // act_fwd / act_bwd
 
 namespace dsact {
@@ -203,9 +205,13 @@ __device__ __forceinline__ int64_t replay_index(int row, uint32_t step, int64_t 
 // FRAMES = false: the flat ring (dsact_replay), rows r_obs / r_obs2 [capacity, O].
 // FRAMES = true: the frame ring (dsact_frame_replay): r_obs = r_obs2 = the frame store [frame_capacity, F = O / K]; frame
 // k of row src's obs is frame f_obs[src * K + k] (obs2: f_obs2), i.e. floats [k * F, (k + 1) * F) of the observation.
-// CODES = true (with FRAMES): the coded frame ring: the frame store holds uint8 codes [frame_capacity, F] (r_obs points to
-// them) and value c decodes to table[c] (256 floats); every other read and every write is the fp32 frame ring's.
-template <bool FRAMES, bool CODES = false>
+// CODE = 1 or 2 (with FRAMES): a coded frame ring: the frame store holds CODE-byte codes [frame_capacity, F] (r_obs points
+// to them) and value c decodes to table[c]; every other read and every write is the fp32 frame ring's.  CODE = 1: uint8
+// codes, the 256 table floats staged in shared memory.  CODE = 2: uint16 codes, 65 536 table floats (256 KiB, more than
+// shared memory holds), every lookup through the read-only path from L1 / L2 (faster on every measured stream than
+// staging the table's first 4096 entries in shared memory, DESIGN §7).  The kernel never reads how many table entries
+// are in use: a captured graph stays valid while the table grows.
+template <bool FRAMES, int CODE = 0>
 __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __restrict__ r_obs2,
                               const float* __restrict__ r_act, const float* __restrict__ r_rew,
                               const float* __restrict__ r_done, const float* __restrict__ r_logp,
@@ -215,7 +221,10 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
                               int64_t* __restrict__ draw_idx, uint64_t seed, const float* __restrict__ state, int write_f32,
                               const int32_t* __restrict__ f_obs, const int32_t* __restrict__ f_obs2, int K,
                               const float* __restrict__ table) {
-  static_assert(FRAMES || !CODES, "codes index frames");
+  static_assert(FRAMES || CODE == 0, "codes index frames");
+  static_assert(CODE >= 0 && CODE <= 2, "codes are 1 or 2 bytes");
+  using Code = typename std::conditional<CODE == 2, uint16_t, uint8_t>::type;
+  constexpr int PER = CODE == 2 ? 8 : 16;   // codes per 16-byte load
   pdl_sync();
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
@@ -226,26 +235,41 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
     const int k = e / F;
     return r_obs + (int64_t)__ldg(fs + k) * F + (e - k * F);
   };
-  const float* tab = nullptr;   // CODES: the decode table, staged in shared memory
-  if constexpr (CODES) {
+  const float* tab = nullptr;   // CODE = 1: the decode table, staged in shared memory
+  if constexpr (CODE == 1) {
     __shared__ float s_table[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_table[i] = __ldg(table + i);
     __syncthreads();
     tab = s_table;
   }
+  // the value of code c
+  auto dec = [&](auto c) -> float {
+    if constexpr (CODE == 1) return tab[c];
+    else return __ldg(table + c);
+  };
   // address of code e of row src's observation in the coded frame store
   auto code_at = [&](const int32_t* fs, int e) {
     const int k = e / F;
-    return reinterpret_cast<const uint8_t*>(r_obs) + (int64_t)__ldg(fs + k) * F + (e - k * F);
+    return reinterpret_cast<const Code*>(r_obs) + (int64_t)__ldg(fs + k) * F + (e - k * F);
   };
-  // 16 codes (one 16-byte load) -> floats [e, e + 16) of a destination row and its images
+  // PER codes (one 16-byte load) -> floats [e, e + PER) of a destination row and its images
   auto put16 = [&](const uint4 q, float* dst, const ImgOut& img, size_t row, int e) {
     const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+    if constexpr (CODE == 1) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float4 v = make_float4(tab[w[j] & 0xff], tab[(w[j] >> 8) & 0xff], tab[(w[j] >> 16) & 0xff], tab[w[j] >> 24]);
-      if (write_f32) reinterpret_cast<float4*>(dst + e)[j] = v;
-      img_put4(img, row, e + 4 * j, v);
+      for (int j = 0; j < 4; ++j) {
+        const float4 v = make_float4(tab[w[j] & 0xff], tab[(w[j] >> 8) & 0xff], tab[(w[j] >> 16) & 0xff], tab[w[j] >> 24]);
+        if (write_f32) reinterpret_cast<float4*>(dst + e)[j] = v;
+        img_put4(img, row, e + 4 * j, v);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const float4 v = make_float4(dec(w[2 * j] & 0xffff), dec(w[2 * j] >> 16), dec(w[2 * j + 1] & 0xffff),
+                                     dec(w[2 * j + 1] >> 16));
+        if (write_f32) reinterpret_cast<float4*>(dst + e)[j] = v;
+        img_put4(img, row, e + 4 * j, v);
+      }
     }
   };
   // draw_idx != null: no index list was given; every warp draws its row's index itself  and records it in draw_idx
@@ -270,29 +294,29 @@ __global__ void gather_kernel(const float* __restrict__ r_obs, const float* __re
     const int32_t* fo2 = FRAMES ? f_obs2 + src * K : nullptr;
     float* dobs = obs + (size_t)row * O;
     float* dobs2 = obs2 + (size_t)row * O;
-    if constexpr (CODES) {
-      if ((F & 15) == 0) {
-        // 16 codes per 16-byte load (a load never straddles two frames); three of obs and of obs2 in flight per lane, as
+    if constexpr (CODE > 0) {
+      if ((F & (PER - 1)) == 0) {
+        // PER codes per 16-byte load (a load never straddles two frames); three of obs and of obs2 in flight per lane, as
         // the fp32 path keeps
-        for (int c0 = lane; c0 < O / 16; c0 += 96) {
+        for (int c0 = lane; c0 < O / PER; c0 += 96) {
           uint4 a[3], b[3];
 #pragma unroll
           for (int u = 0; u < 3; ++u) {
             const int c = c0 + 32 * u;
-            if (c < O / 16) {
-              a[u] = __ldg(reinterpret_cast<const uint4*>(code_at(fo, 16 * c)));
-              b[u] = __ldg(reinterpret_cast<const uint4*>(code_at(fo2, 16 * c)));
+            if (c < O / PER) {
+              a[u] = __ldg(reinterpret_cast<const uint4*>(code_at(fo, PER * c)));
+              b[u] = __ldg(reinterpret_cast<const uint4*>(code_at(fo2, PER * c)));
             }
           }
 #pragma unroll
           for (int u = 0; u < 3; ++u) {
             const int c = c0 + 32 * u;
-            if (c < O / 16) { put16(a[u], dobs, i_obs, row, 16 * c); put16(b[u], dobs2, i_obs2, row, 16 * c); }
+            if (c < O / PER) { put16(a[u], dobs, i_obs, row, PER * c); put16(b[u], dobs2, i_obs2, row, PER * c); }
           }
         }
       } else {
         for (int c = lane; c < O; c += 32) {
-          const float a = tab[__ldg(code_at(fo, c))], b = tab[__ldg(code_at(fo2, c))];
+          const float a = dec(__ldg(code_at(fo, c))), b = dec(__ldg(code_at(fo2, c)));
           if (write_f32) { dobs[c] = a; dobs2[c] = b; }
           img_put(i_obs, row, c, a); img_put(i_obs2, row, c, b);
         }

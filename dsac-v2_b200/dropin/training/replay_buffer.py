@@ -20,6 +20,10 @@ float32 values (the coded frame ring): a quarter of the frame bytes, for observa
 (8-bit images scaled to floats, such as `gym_carracingraw`'s rgb / 255).  Values are matched bit for bit; a store that
 brings a 257th distinct value raises ValueError and leaves the buffer as it was.  The minibatches are still bit for bit
 those of the flat ring.
+
+`dsact_replay_codes=16` (with `dsact_replay_frames`) stores 16-bit codes into a table of at most 65 536 values: half the
+frame bytes, for sources such as `gym_carracing`'s stacked grey frames (`dot(rgb, [0.299, 0.587, 0.114]) / 128 - 1`)
+whose stream uses at most 65 536 distinct values.  A store that brings a 65 537th value is refused the same way.
 """
 __all__ = ["ReplayBuffer"]
 
@@ -51,10 +55,13 @@ class ReplayBuffer:
         if self.frames_per_obs is not None:
             self.planner = FramePlanner(self.max_size, int(self.frames_per_obs), self.obs_elems)
         self.coder = None
-        if kwargs.get("dsact_replay_codes"):
+        codes = kwargs.get("dsact_replay_codes")
+        if codes is not None and codes is not False:
+            if codes is not True and (isinstance(codes, bool) or codes != 16):
+                raise ValueError(f"dsact_replay_codes={codes!r}: True (8-bit codes) or 16 (16-bit codes)")
             if self.planner is None:
                 raise ValueError("dsact_replay_codes codes the frames of the frame ring: it needs dsact_replay_frames")
-            self.coder = FrameCoder()
+            self.coder = FrameCoder(8 if codes is True else 16)
         self.ptr, self.size = 0, 0
         self.engine = None
         self._stage = None      # pinned staging buffers
@@ -79,15 +86,17 @@ class ReplayBuffer:
                            for _ in range(self._STAGES)]
         else:
             pl = self.planner
-            engine.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K, coded=self.coder is not None)
+            self._bind_frames(engine, pl.frame_capacity)
             ids = lambda: torch.zeros(R, pl.K, dtype=torch.int32).pin_memory()
-            # up to 2K new frames per row: the same bytes as the flat ring's obs + obs2 staging (a quarter when coded)
-            fdt = torch.float32 if self.coder is None else torch.uint8
+            # up to 2K new frames per row: the same bytes as the flat ring's obs + obs2 staging (a quarter with 8-bit codes,
+            # a half with 16-bit codes, held in int16 and written through a uint16 view)
+            fdt = {None: torch.float32, 8: torch.uint8, 16: torch.int16}[self._code_bits()]
             self._stage = [dict(frames=torch.zeros(2 * R * pl.K, pl.F, dtype=fdt).pin_memory(), obs_frames=ids(),
                                 obs2_frames=ids(), act=pin(R, A), rew=pin(R), done=pin(R), logp=pin(R))
                            for _ in range(self._STAGES)]
             self._nframes, self._frame_ptr = 0, 0
-        self._np = [{k: v.numpy() for k, v in s.items()} for s in self._stage]
+        self._np = [{k: v.numpy().view(np.uint16) if v.dtype == torch.int16 else v.numpy() for k, v in s.items()}
+                    for s in self._stage]
         self._events = [None] * self._STAGES
         pending, self._pending = self._pending, []
         for row in pending:
@@ -102,10 +111,17 @@ class ReplayBuffer:
         if self.planner is None:
             new.bind_replay(self.max_size)
         else:
-            new.bind_replay_frames(self.max_size, self.planner.frame_capacity, self.planner.K, coded=self.coder is not None)
+            self._bind_frames(new, self.planner.frame_capacity)
         for k, v in old.replay.items():
             new.replay[k].copy_(v)
         self.engine = new
+
+    def _code_bits(self):
+        return None if self.coder is None else self.coder.code_bits
+
+    def _bind_frames(self, eng, frame_capacity: int):
+        eng.bind_replay_frames(self.max_size, frame_capacity, self.planner.K, coded=self.coder is not None,
+                               code_bits=self._code_bits() or 8)
 
     def _require_engine(self):
         if self.engine is None:
@@ -117,10 +133,11 @@ class ReplayBuffer:
 
     def __get_RAM__(self):
         """MB of device memory holding valid transitions (frame ring: the frames they refer to, and their frame ids; coded
-        frame ring: one byte per frame value, and the table)."""
+        frame rings: one or two bytes per frame value, and the table)."""
         if self.planner is not None:
             pl = self.planner
-            frames = 4 * pl.F * pl.held() if self.coder is None else pl.F * pl.held() + 4 * FrameCoder.N
+            c = self.coder
+            frames = 4 * pl.F * pl.held() if c is None else c.code_bits // 8 * pl.F * pl.held() + 4 * c.N
             return (frames + 4 * (2 * pl.K + self.act_dim + 3) * self.size) / 1e6
         row_bytes = 4 * (2 * self.obs_elems + self.act_dim + 3)
         return row_bytes * self.size / 1e6
@@ -189,8 +206,9 @@ class ReplayBuffer:
             if self.coder is None:
                 self.engine.replay_add_frames(st["frames"], self._nframes, self._frame_ptr, st, n, self.ptr)
             else:
-                self.engine.replay_add_coded_frames(st["frames"], self._nframes, self._frame_ptr, self.coder.table,
-                                                    self.coder.n, st, n, self.ptr)
+                e = self.engine
+                add = e.replay_add_coded_frames if self.coder.code_bits == 8 else e.replay_add_coded16_frames
+                add(st["frames"], self._nframes, self._frame_ptr, self.coder.table, self.coder.n, st, n, self.ptr)
             self._nframes = 0
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.engine.device))
@@ -206,7 +224,7 @@ class ReplayBuffer:
         with torch.cuda.device(eng.device):
             old = eng.replay
             src, dst = (torch.from_numpy(x).to(eng.device) for x in pl.moves(frame_capacity))
-            eng.bind_replay_frames(self.max_size, frame_capacity, pl.K, coded=self.coder is not None)
+            self._bind_frames(eng, frame_capacity)
             eng.replay["frames"][dst] = old["frames"][src]
             for k in ("act", "rew", "done", "logp") + (("table",) if self.coder is not None else ()):
                 eng.replay[k].copy_(old[k])
@@ -246,15 +264,18 @@ class ReplayBuffer:
         self._require_engine()
         if state["max_size"] != self.max_size:
             raise ValueError("replay capacity differs from the checkpoint")
-        if ("frame_planner" in state) != (self.planner is not None) or ("frame_coder" in state) != (self.coder is not None):
-            raise ValueError("the checkpoint's replay ring kind (flat / frame / coded frame ring) differs from this buffer's")
+        coder = state.get("frame_coder")
+        if ("frame_planner" in state, None if coder is None else coder.get("code_bits", 8)) != \
+                (self.planner is not None, self._code_bits()):
+            raise ValueError("the checkpoint's replay ring kind (flat / frame / 8-bit or 16-bit coded frame ring) differs "
+                             "from this buffer's")
         self.ptr, self.size, self._fill = int(state["ptr"]), int(state["size"]), 0
         if self.planner is not None:
             pl = self.planner
             pl.load_state_dict(state["frame_planner"])
             eng = self.engine
             if eng.replay["frames"].shape[0] != pl.frame_capacity:
-                eng.bind_replay_frames(self.max_size, pl.frame_capacity, pl.K, coded=self.coder is not None)
+                self._bind_frames(eng, pl.frame_capacity)
             self._nframes = 0
             self._put_ids()
             if self.coder is not None:

@@ -363,32 +363,37 @@ class Engine:
             check(self.lib.dsact_replay_bind(self.h, C.byref(rb)))
         self.capacity = int(capacity)
 
-    def bind_replay_frames(self, capacity: int, frame_capacity: int, frames_per_obs: int, coded: bool = False):
+    def bind_replay_frames(self, capacity: int, frame_capacity: int, frames_per_obs: int, coded: bool = False,
+                           code_bits: int = 8):
         """Bind a frame ring (dsact_replay_bind_frames): `capacity` rows whose obs / obs2 are `frames_per_obs` (K) frame
         ids each into a store of `frame_capacity` frames of obs_elems / K floats.  `replay` then holds `frames`,
         `obs_frames`, `obs2_frames` (int32 [capacity, K]), `act`, `rew`, `done`, `logp`.
-        coded: the coded frame ring (dsact_replay_bind_coded_frames): `frames` holds uint8 codes, and `table` (256
-        floats, zeros until replay_add_coded_frames fills them) their values."""
+        coded: a coded frame ring, `frames` holding codes of `code_bits` bits and `table` (2^code_bits floats, zeros until
+        an add fills them) their values.  code_bits 8 (dsact_replay_bind_coded_frames): uint8 codes; 16
+        (dsact_replay_bind_coded16_frames): uint16 codes, held in an int16 tensor."""
         O, A, K = self.obs_elems, self.cfg.act_dim, int(frames_per_obs)
         capacity, frame_capacity = int(capacity), int(frame_capacity)
         if not 1 <= K <= 64 or O % K:
             raise ValueError(f"frames_per_obs {K} must be in [1, 64] and divide the observation's {O} floats")
         if not K <= frame_capacity <= 2 ** 31 - 1 or capacity < 1:
             raise ValueError(f"frame_capacity {frame_capacity} outside [{K}, 2^31 - 1] or capacity {capacity} < 1")
+        if coded and code_bits not in (8, 16):
+            raise ValueError(f"code_bits {code_bits!r}: the coded frame rings take 8- or 16-bit codes")
         with torch.cuda.device(self.device):
             z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)
             ids = lambda: torch.zeros(capacity, K, dtype=torch.int32, device=self.device)
-            frames = (torch.zeros(frame_capacity, O // K, dtype=torch.uint8, device=self.device) if coded
-                      else z(frame_capacity, O // K))
+            frames = (torch.zeros(frame_capacity, O // K, dtype=torch.uint8 if code_bits == 8 else torch.int16,
+                                  device=self.device) if coded else z(frame_capacity, O // K))
             self.replay = dict(frames=frames, obs_frames=ids(), obs2_frames=ids(), act=z(capacity, A),
                                rew=z(capacity), done=z(capacity), logp=z(capacity))
             if coded:
-                self.replay["table"] = z(256)
+                self.replay["table"] = z(1 << code_bits)
             r = self.replay
             rb = _lib.FrameReplay(*(r[k].data_ptr() for k in ("frames", "obs_frames", "obs2_frames", "act", "rew", "done",
                                                               "logp")), capacity, frame_capacity, K)
             if coded:
-                check(self.lib.dsact_replay_bind_coded_frames(self.h, C.byref(rb), r["table"].data_ptr()))
+                bind = self.lib.dsact_replay_bind_coded_frames if code_bits == 8 else self.lib.dsact_replay_bind_coded16_frames
+                check(bind(self.h, C.byref(rb), r["table"].data_ptr()))
             else:
                 check(self.lib.dsact_replay_bind_frames(self.h, C.byref(rb)))
         self.capacity = capacity
@@ -402,18 +407,27 @@ class Engine:
         """dsact_replay_add_coded_frames: `n_frames` frames of codes (contiguous uint8 HOST tensor) -> frame slots
         (frame_ptr + i) % frame_capacity, table[:n_codes] (float32, host) -> the device table; the rows as in
         replay_add_frames."""
+        self._add_coded(self.lib.dsact_replay_add_coded_frames, (torch.uint8,), codes, n_frames, frame_ptr, table, n_codes,
+                        rows, n, ptr)
+
+    def replay_add_coded16_frames(self, codes: Optional[torch.Tensor], n_frames: int, frame_ptr: int, table: np.ndarray,
+                                  n_codes: int, rows: Dict[str, torch.Tensor], n: int, ptr: int):
+        """dsact_replay_add_coded16_frames: replay_add_coded_frames with 16-bit codes (a contiguous int16 or uint16 HOST
+        tensor holding the uint16 codes) and up to 65 536 table entries."""
+        self._add_coded(self.lib.dsact_replay_add_coded16_frames, (torch.int16, torch.uint16), codes, n_frames, frame_ptr,
+                        table, n_codes, rows, n, ptr)
+
+    def _add_coded(self, fn, code_dtypes, codes, n_frames, frame_ptr, table, n_codes, rows, n, ptr):
         r = rows
-        for k, dt, t in (("codes", torch.uint8, codes), ("obs_frames", torch.int32, r["obs_frames"]),
-                         ("obs2_frames", torch.int32, r["obs2_frames"])):
-            if t is not None and (t.device.type != "cpu" or t.dtype != dt or not t.is_contiguous()):
-                raise ValueError(f"{k} must be a contiguous {dt} host tensor")
+        for k, dts, t in (("codes", code_dtypes, codes), ("obs_frames", (torch.int32,), r["obs_frames"]),
+                          ("obs2_frames", (torch.int32,), r["obs2_frames"])):
+            if t is not None and (t.device.type != "cpu" or t.dtype not in dts or not t.is_contiguous()):
+                raise ValueError(f"{k} must be a contiguous {' or '.join(map(str, dts))} host tensor")
         table = np.ascontiguousarray(table, np.float32)
         with torch.cuda.device(self.device):
-            check(self.lib.dsact_replay_add_coded_frames(self.h, _ptr(codes), int(n_frames), int(frame_ptr),
-                                                         table.ctypes.data, int(n_codes), r["obs_frames"].data_ptr(),
-                                                         r["obs2_frames"].data_ptr(), r["act"].data_ptr(),
-                                                         r["rew"].data_ptr(), r["done"].data_ptr(), r["logp"].data_ptr(),
-                                                         int(n), int(ptr), self._stream()))
+            check(fn(self.h, _ptr(codes), int(n_frames), int(frame_ptr), table.ctypes.data, int(n_codes),
+                     r["obs_frames"].data_ptr(), r["obs2_frames"].data_ptr(), r["act"].data_ptr(), r["rew"].data_ptr(),
+                     r["done"].data_ptr(), r["logp"].data_ptr(), int(n), int(ptr), self._stream()))
 
     def replay_add_frames(self, frames: Optional[torch.Tensor], n_frames: int, frame_ptr: int, rows: Dict[str, torch.Tensor],
                           n: int, ptr: int):

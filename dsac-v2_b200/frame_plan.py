@@ -137,41 +137,59 @@ class FramePlanner:
 
 
 class FrameCoder:
-    """Host coder of the coded frame ring (dsact_replay_bind_coded_frames): float32 values -> uint8 codes through a table
-    of up to 256 values.  Values are matched on their bit patterns (so -0.0 and 0.0, and NaNs of different payloads, are
-    different values) and take codes in order of first appearance.  The table is a bijection between codes and the bit
-    patterns seen, so comparing codes is comparing values.
+    """Host coder of the coded frame rings (dsact_replay_bind_coded_frames, dsact_replay_bind_coded16_frames): float32
+    values -> codes of `code_bits` bits (8: uint8, up to 256 values; 16: uint16, up to 65 536) through a table.  Values
+    are matched on their bit patterns (so -0.0 and 0.0, and NaNs of different payloads, are different values) and take
+    codes in order of first appearance.  The table is a bijection between codes and the bit patterns seen, so comparing
+    codes is comparing values.
 
-    Lookup: a multiplicative hash (bits * mul mod 2^32) >> 16 into 65536 slots, with `mul` chosen so that no two table
-    entries share a slot; a value is known when its slot holds its own bit pattern.  A few vector operations per value,
-    and no Python loop over values."""
-    N = 256
+    Lookup, with no Python loop over values.  8 bits: a multiplicative hash (bits * mul mod 2^32) >> 16 into 65536 slots,
+    with `mul` chosen so that no two table entries share a slot; a value is known when its slot holds its own bit
+    pattern.  16 bits: a table that large cannot be placed collision-free in such a hash, so a binary search
+    (np.searchsorted) over the patterns held, kept sorted beside their codes."""
     _SHIFT = 16
 
-    def __init__(self):
+    def __init__(self, code_bits: int = 8):
+        if code_bits not in (8, 16):
+            raise ValueError(f"code_bits {code_bits!r}: the coded frame rings take 8- or 16-bit codes")
+        self.code_bits = code_bits
+        self.N = 1 << code_bits
+        self.dtype = np.uint8 if code_bits == 8 else np.uint16
         self.bits = np.zeros(self.N, np.uint32)   # table: code -> bit pattern
         self.n = 0
-        self._mul = np.uint32(0x9E3779B1)
-        self._used = np.zeros(1 << (32 - self._SHIFT), bool)    # slot -> (holds an entry, its pattern, its code)
-        self._slot_bits = np.zeros(1 << (32 - self._SHIFT), np.uint32)
-        self._slot_code = np.zeros(1 << (32 - self._SHIFT), np.uint8)
+        if code_bits == 8:
+            self._mul = np.uint32(0x9E3779B1)
+            self._used = np.zeros(1 << (32 - self._SHIFT), bool)    # slot -> (holds an entry, its pattern, its code)
+            self._slot_bits = np.zeros(1 << (32 - self._SHIFT), np.uint32)
+            self._slot_code = np.zeros(1 << (32 - self._SHIFT), np.uint8)
+        else:
+            self._sorted = np.zeros(0, np.uint32)        # the patterns held, ascending, and their codes
+            self._sorted_code = np.zeros(0, np.uint16)
 
     @property
     def table(self) -> np.ndarray:
-        """float32 [256]: code -> value (entries from n on are unused)."""
+        """float32 [N]: code -> value (entries from n on are unused)."""
         return self.bits.view(np.float32)
 
     def _slots(self, flat: np.ndarray, mul) -> np.ndarray:
         return (flat * mul) >> np.uint32(self._SHIFT)
 
+    def _find(self, flat: np.ndarray):
+        """(known: bool per value, codes: a writable code array, valid where known)."""
+        if self.code_bits == 8:
+            s = self._slots(flat, self._mul)
+            return self._used[s] & (self._slot_bits[s] == flat), self._slot_code[s]
+        if self.n == 0:
+            return np.zeros(flat.shape, bool), np.zeros(flat.shape, np.uint16)
+        i = np.minimum(np.searchsorted(self._sorted, flat), self.n - 1)
+        return self._sorted[i] == flat, self._sorted_code[i]
+
     def encode(self, values: np.ndarray):
-        """(uint8 codes of `values`' shape, bit patterns the table does not hold yet, in order of first appearance).
-        Changes nothing; ValueError when the table would need more than 256 entries."""
+        """(codes of `values`' shape, bit patterns the table does not hold yet, in order of first appearance).
+        Changes nothing; ValueError when the table would need more than N entries."""
         b = np.ascontiguousarray(values, np.float32).view(np.uint32)
         flat = b.reshape(-1)
-        s = self._slots(flat, self._mul)
-        known = self._used[s] & (self._slot_bits[s] == flat)
-        codes = self._slot_code[s]
+        known, codes = self._find(flat)
         if known.all():
             return codes.reshape(b.shape), flat[:0]
         miss = ~known
@@ -180,20 +198,27 @@ class FrameCoder:
         new = uniq[order]
         if self.n + len(new) > self.N:
             v = new[self.N - self.n]
-            raise ValueError(f"the coded replay ring holds at most {self.N} distinct observation values; "
-                             f"{np.array(v, np.uint32).view(np.float32).item()!r} (bits 0x{int(v):08x}) would be value "
-                             f"{self.N + 1}: the observations are not 8-bit quantised")
+            raise ValueError(f"the {self.code_bits}-bit coded replay ring holds at most {self.N} distinct observation "
+                             f"values; {np.array(v, np.uint32).view(np.float32).item()!r} (bits 0x{int(v):08x}) would be "
+                             f"value {self.N + 1}: the observations are not {self.code_bits}-bit quantised")
         rank = np.empty(len(uniq), np.int64)
         rank[order] = np.arange(len(uniq))
-        codes[miss] = (self.n + rank[inv.reshape(-1)]).astype(np.uint8)
+        codes[miss] = (self.n + rank[inv.reshape(-1)]).astype(self.dtype)
         return codes.reshape(b.shape), new
 
     def commit(self, new: np.ndarray) -> None:
         """Append the patterns `encode` returned to the table."""
         if len(new) == 0:
             return
+        start = self.n
         self.bits[self.n:self.n + len(new)] = new
         self.n += len(new)
+        if self.code_bits == 16:
+            o = np.argsort(new)
+            pos = np.searchsorted(self._sorted, new[o])
+            self._sorted = np.insert(self._sorted, pos, new[o])
+            self._sorted_code = np.insert(self._sorted_code, pos, (start + o).astype(np.uint16))
+            return
         bits = self.bits[:self.n]
         mul, g = self._mul, np.random.default_rng(self.n)
         while len(np.unique(self._slots(bits, mul))) != self.n:   # a collision: another odd multiplier
@@ -206,12 +231,19 @@ class FrameCoder:
         self._slot_code[s] = np.arange(self.n).astype(np.uint8)
 
     def state_dict(self) -> dict:
-        return {"bits": self.bits[:self.n].copy()}
+        st = {"bits": self.bits[:self.n].copy()}
+        if self.code_bits != 8:   # (8-bit states keep the form they always had)
+            st["code_bits"] = self.code_bits
+        return st
 
     def load_state_dict(self, st: dict) -> None:
+        if st.get("code_bits", 8) != self.code_bits:
+            raise ValueError(f"frame coder state of {st.get('code_bits', 8)}-bit codes, not {self.code_bits}-bit")
         bits = np.asarray(st["bits"], np.uint32)
         if len(bits) > self.N or len(np.unique(bits)) != len(bits):
-            raise ValueError("frame coder state: not a table of at most 256 distinct values")
+            raise ValueError(f"frame coder state: not a table of at most {self.N} distinct values")
         self.bits[:] = 0
         self.n = 0
+        if self.code_bits == 16:
+            self._sorted, self._sorted_code = self._sorted[:0], self._sorted_code[:0]
         self.commit(bits)

@@ -247,6 +247,22 @@ int dsact_replay_add_coded_frames(dsact_handle *h, const uint8_t *codes, int64_t
                                   const float *table, int32_t n_codes, const int32_t *obs_frames,
                                   const int32_t *obs2_frames, const float *act, const float *rew, const float *done,
                                   const float *logp, int64_t n, int64_t ptr, void *stream);
+/* ---- coded frame replay ring: frames of 16-bit codes ----
+ * The coded ring with one uint16 code per value (rb->frames points to uint16 [frame_capacity, obs_elems /
+ * frames_per_obs]) and a device table of 65 536 floats: half the fp32 frame ring's bytes, for sources with at most 65 536
+ * distinct values, such as CarRacing's stacked grey frames (dot(rgb, [0.299, 0.587, 0.114]) / 128 - 1 take up to
+ * 247 024 float32 values over all RGB triples; a stream that uses at most 65 536 of them fits).  Every gather yields bit
+ * for bit what the fp32 frame ring holding the decoded frames would, and never reads how many table entries are in use,
+ * so a captured replay step stays valid while the table grows.
+ * dsact_replay_bind_coded16_frames: the checks of dsact_replay_bind_coded_frames. */
+int dsact_replay_bind_coded16_frames(dsact_handle *h, const dsact_frame_replay *rb, const float *table);
+/* dsact_replay_add_coded_frames for a 16-bit coded ring: HOST uint16 codes, n_codes in [0, 65 536], the same checks
+ * before anything is copied.  Each ring kind's add call refuses every other ring kind (DSACT_ESTATE): the 8-bit and the
+ * 16-bit coded rings refuse each other's calls. */
+int dsact_replay_add_coded16_frames(dsact_handle *h, const uint16_t *codes, int64_t n_frames, int64_t frame_ptr,
+                                    const float *table, int32_t n_codes, const int32_t *obs_frames,
+                                    const int32_t *obs2_frames, const float *act, const float *rew, const float *done,
+                                    const float *logp, int64_t n, int64_t ptr, void *stream);
 /* sample_batch(): gather rows idx[i] (device int64, or NULL = draw uniformly in [0,size) on
  * the device) into the engine's batch arena; `out` receives the arena's device pointers */
 int dsact_replay_sample(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx,
