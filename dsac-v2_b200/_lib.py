@@ -185,6 +185,8 @@ SYMBOLS = {
     "dsact_dp_step": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.POINTER(Noise), C.c_int64, C.c_int64, C.c_void_p]),
     "dsact_dp_replay_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_int64, C.c_int64,
                                        C.c_void_p]),
+    "dsact_dp_replay_steps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.POINTER(Noise), C.c_int64,
+                                        C.c_void_p, C.c_int64, C.c_void_p]),
     "dsact_v1_query_layout": (C.c_int, [C.POINTER(Config), C.POINTER(V1Options), C.POINTER(Layout)]),
     "dsact_v1_create": (C.c_int, [C.POINTER(Config), C.POINTER(V1Options), C.c_int, C.POINTER(C.c_void_p)]),
     "dsact_cnn_query_layout": (C.c_int, [C.POINTER(CnnConfig), C.POINTER(Layout)]),

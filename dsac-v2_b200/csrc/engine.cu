@@ -1718,10 +1718,9 @@ static void enqueue_apply(MlpHandle* h, Ctx& c, const TailArgs* tail = nullptr, 
   launch_apply(h, mlp_apply_args(h, tail ? 2 : 0, tail, dp, part, nslabs), c);
 }
 
-// One whole update of the single-call steps: phase 1, phase 2 over `u.global_batch` rows, then (u.dp) the logged-sum
+// The rest of a single-call update after its phase 1: phase 2 over `u.global_batch` rows, then (u.dp) the logged-sum
 // exchange (also the "every rank's block is complete" barrier) and the reduce-scatter from 6 ranks up, then Adam / Polyak.
-static void enqueue_update(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
-  enqueue_phase1(h, u, c);
+static void enqueue_phase2_apply(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
   const TailArgs ta = tail_args(h, u.global_batch, u.bt.batch);
   const bool critics_applied = enqueue_phase2(h, u, c, &ta);
   if (u.dp) {
@@ -1729,6 +1728,12 @@ static void enqueue_update(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
     if (dp_two_shot(h->dp)) enqueue_dp_reduce_scatter(h->dp, h->buf.state, h->num_sms, c);
   }
   enqueue_apply(h, c, &ta, u.dp, critics_applied ? 2 : 0);
+}
+
+// One whole update of the single-call steps
+static void enqueue_update(MlpHandle* h, const UpdatePlan& u, Ctx& c) {
+  enqueue_phase1(h, u, c);
+  enqueue_phase2_apply(h, u, c);
 }
 
 // the generator counter step of a call whose last draw is the gather's (no sample_kernel after it steps it)
@@ -1744,7 +1749,7 @@ static void enqueue_gather_imaged(MlpHandle* h, int B, const int64_t* idx, Ctx& 
   enqueue_gather(h, B, idx, img, !images_only, c);
 }
 
-// ---- n replay-fed updates in one submission (dsact_replay_steps) ----------------------------------------------------
+// ---- n replay-fed updates in one submission (dsact_replay_steps, dsact_dp_replay_steps) ------------------------------
 // the minibatch of input set `set` (0: the arena's, 1: the library-owned second set)
 static dsact_batch input_batch(const MlpHandle* h, int set, int32_t batch) {
   if (set == 0) return arena_batch(h, batch);
@@ -1797,8 +1802,16 @@ static dsact_noise update_noise(const dsact_noise& np, int k, int B, int A) {
 // (captured: onto its own stream) once update k's forward passes are enqueued and runs beside update k's backward; the
 // set it overwrites was last read by update k - 1.  The prologue of update k + 1 (weight images, noise, clears, Adam
 // scalars) reads what update k's apply writes and follows it on the main stream with programmatic dependent launch.
-// stats_out: row k = update k's finalised tb_info, written before update k + 1 clears the accumulators.
-static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx, const dsact_noise* np, float* stats_out, Ctx& c) {
+// stats_out: row k = update k's finalised tb_info over `global_batch` rows, written before update k + 1 clears the
+// accumulators (slot 14: the peer-timeout flag as update k left it).
+// `dp`: every update is dsact_dp_replay_step's, the data-parallel body of enqueue_update: the std-sum exchange on the side
+// branch under phase 1's second forward chain, phase 2 over `global_batch` rows ending in dp_grad_fold, the logged-sum
+// exchange, the reduce-scatter from 6 ranks up, the apply on the exchanged sums.  Each update bumps the exchange epoch as
+// its single call does.  The exchange branch is joined inside phase 1, before the gather branch is forked, and the
+// gather branch is joined before the next update's phase 1 forks the exchange again: neither pair of fork / join events
+// is recorded again while the branch it bounds is open.
+static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx, const dsact_noise* np, int64_t global_batch,
+                                 bool dp, float* stats_out, Ctx& c) {
   const int A = h->cfg.act_dim;
   const bool fused = h->fused();
   const bool fork = c.side != nullptr;
@@ -1813,13 +1826,13 @@ static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx,
     if (!idx && np) enqueue_rng_advance(h, cg);
   };
   float inv_b, inv_pol;
-  stats_scales(h, B, &inv_b, &inv_pol);
+  stats_scales(h, global_batch, &inv_b, &inv_pol);
   bool gather_forked = false;
   for (int k = 0; k < n; ++k) {
     const int set = k & 1;
     dsact_noise nk;
     if (np) nk = update_noise(*np, k, B, A);
-    UpdatePlan u{input_batch(h, set, B), np ? &nk : nullptr, B, false, true, set, PRO_DONE};
+    UpdatePlan u{input_batch(h, set, B), np ? &nk : nullptr, global_batch, dp, true, set, PRO_DONE};
     if (k == 0) {   // as dsact_replay_step: the prologue beside the gather
       u.prologue = fork_prologue(h, u, c);
       gather(0, c);
@@ -1837,9 +1850,7 @@ static void enqueue_replay_steps(MlpHandle* h, int n, int B, const int64_t* idx,
         gather(k + 1, c);
       }
     }
-    const TailArgs ta = tail_args(h, B, B);
-    const bool critics_applied = enqueue_phase2(h, u, c, &ta);
-    enqueue_apply(h, c, &ta, false, critics_applied ? 2 : 0);
+    enqueue_phase2_apply(h, u, c);
     if (stats_out) {
       launch_k(finalize_stats_kernel, 1, 32, 0, c, h->buf.state, inv_b, inv_pol, stats_out + (size_t)k * DSACT_NUM_STATS);
       c.done();
@@ -2085,7 +2096,7 @@ static void enqueue_call(MlpHandle* h, const UpdateCall& u, UpdatePlan p, Ctx& c
     case RUN_PHASE2: enqueue_phase2(h, p, c, nullptr); break;
     case RUN_GRADS: enqueue_phase1(h, p, c); enqueue_phase2(h, p, c, nullptr); break;
     case RUN_APPLY: enqueue_apply(h, c); break;
-    case RUN_STEPS: enqueue_replay_steps(h, u.n_steps, B, u.idx, p.nz, u.stats_out, c); break;
+    case RUN_STEPS: enqueue_replay_steps(h, u.n_steps, B, u.idx, p.nz, p.global_batch, p.dp, u.stats_out, c); break;
     case RUN_GATHER:
       enqueue_gather_imaged(h, B, u.idx, c, false);
       if (!u.idx) enqueue_rng_advance(h, c);
@@ -2661,6 +2672,16 @@ int dsact_replay_steps(dsact_handle* h, int32_t n_steps, int32_t batch, int64_t 
 }
 
 // ---- data parallelism over peer memory (dp_peer.cuh) ------------------------------------------------------------
+// After a (re)connect: captured data-parallel steps hold the previous peer map, and the MLP engine allocates the second
+// input set of dsact_dp_replay_steps here rather than in the first call.  There its cudaMalloc and cudaMemset would sit
+// between the ranks' enqueues, and CUDA does not run work issued before such calls beside work issued after them: ranks
+// that share a device would wait on each other until their exchanges timed out.
+static int dp_connected(dsact_handle* h) {
+  if (h->engine != ENGINE_MLP) return DSACT_OK;
+  drop_graphs(mlp(h));
+  return ensure_input_set2(mlp(h));
+}
+
 int dsact_dp_export(dsact_handle* h, void* handle_out, int64_t* bytes_out) {
   if (!h || !handle_out) return fail(DSACT_EINVAL, "null argument");
   int rc = check_dp(h);
@@ -2675,8 +2696,7 @@ int dsact_dp_connect(dsact_handle* h, int32_t rank, int32_t world, const void* h
   if (rc) return rc;
   if (!h->dp.buf) return fail(DSACT_ESTATE, "dsact_dp_export has not been called");
   rc = dp_peer_connect(h->dp, h->device, h->buf.state, rank, world, handles);
-  if (rc == DSACT_OK && h->engine == ENGINE_MLP) drop_graphs(mlp(h));   // captured data-parallel steps hold the previous peer map
-  return rc;
+  return rc ? rc : dp_connected(h);
 }
 
 // One data-parallel update as one submission: forward, std-sum exchange, losses + backward scaled by 1/global_batch,
@@ -2693,6 +2713,14 @@ int dsact_dp_replay_step(dsact_handle* h, int32_t batch, int64_t size, const int
   UpdateCall u("dsact_dp_replay_step", RUN_STEP);
   u.replay = true; u.rows = batch; u.size = size; u.idx = idx; u.noise = noise; u.iteration = iteration;
   u.global_batch = global_batch; u.dp = true;
+  return update(h, u, stream);
+}
+
+int dsact_dp_replay_steps(dsact_handle* h, int32_t n_steps, int32_t batch, int64_t size, const int64_t* idx,
+                          const dsact_noise* noise, int64_t global_batch, float* stats_out, int64_t iteration, void* stream) {
+  UpdateCall u("dsact_dp_replay_steps", RUN_STEPS);
+  u.replay = true; u.rows = batch; u.size = size; u.idx = idx; u.noise = noise; u.iteration = iteration;
+  u.n_steps = n_steps; u.stats_out = stats_out; u.global_batch = global_batch; u.dp = true;
   return update(h, u, stream);
 }
 
@@ -3037,8 +3065,7 @@ int dsact_test_dp_attach(dsact_handle* h, int32_t rank, int32_t world, dsact_han
   }
   if ((rc = dp_peer_reset(h->dp, h->device, rank, world))) return rc;
   for (int r = 0; r < world; ++r) h->dp.comm.peer[r] = peers[r]->dp.buf;
-  if ((rc = dp_peer_start(h->dp, h->buf.state))) return rc;
-  if (h->engine == ENGINE_MLP) drop_graphs(mlp(h));   // as dsact_dp_connect: captured steps hold the previous peer map
+  if ((rc = dp_peer_start(h->dp, h->buf.state)) || (rc = dp_connected(h))) return rc;
   if (buffer) *buffer = h->dp.buf;
   if (floats) *floats = DP_GRADS_OFF + 2 * h->dp.npad();
   return DSACT_OK;

@@ -157,6 +157,14 @@ class DSAC_V2:
     def _world(self):
         return dp.world() if self.data_parallel else (None, 1)
 
+    def _peers(self, eng, dist) -> bool:
+        """True when `eng`'s data-parallel updates run over peer memory.  The first data-parallel update (or the first
+        after the engine was rebuilt) maps the exchange buffers: a collective call."""
+        if self._peer_dp is None or self._peer_eng is not eng:
+            self._peer_dp = self.dp_transport != "nccl" and dp.connect_peers(eng, dist)
+            self._peer_eng = eng
+        return self._peer_dp
+
     def _stats(self, eng, global_batch, t0):
         if self._slots is None:
             self._slots = [torch.zeros(_lib.NUM_STATS, dtype=torch.float32).pin_memory() for _ in range(self._RING)]
@@ -201,10 +209,7 @@ class DSAC_V2:
         if world == 1:
             eng.step(data, iteration, self._noise(B))
             return self._stats(eng, B, t0)
-        if self._peer_dp is None or self._peer_eng is not eng:   # first data-parallel update (or the engine was rebuilt):
-            self._peer_dp = self.dp_transport != "nccl" and dp.connect_peers(eng, dist)   # map the exchange buffers (collective)
-            self._peer_eng = eng
-        if self._peer_dp:           # one graph launch; exchanges inside the step's kernels over NVLink peer memory
+        if self._peers(eng, dist):   # one graph launch; exchanges inside the step's kernels over NVLink peer memory
             eng.dp_step(data, iteration, B * world, self._noise(B))
             return self._stats(eng, B * world, t0)
         gb = self._gradients(data, eng)
@@ -215,13 +220,26 @@ class DSAC_V2:
         """n rounds of `local_update(buffer.sample_batch(batch_size), iteration + k)`, k = 0 .. n-1, as ONE engine call
         (Engine.replay_steps) where the engine has one: the same host draws in the same order (numpy indices, torch CPU
         noise), the same results.  Device draws take one generator counter per update (as replay_step), not two as a
-        sample_batch + local_update round does: same distribution, other numbers.  Returns the n tb_info mappings; their values are fetched with one copy of the [n, 16]
-        block on first access.  The head-wise engine and data-parallel runs take the n rounds one by one."""
+        sample_batch + local_update round does: same distribution, other numbers.  Returns the n tb_info mappings; their
+        values are fetched with one copy of the [n, 16] block on first access.
+        Under torch.distributed with the peer transport the call is one Engine.dp_replay_steps on every rank, each rank
+        drawing `batch_size` rows from its own buffer, with the same rules: host draws give the results of the n
+        data-parallel rounds, device draws take one generator counter per update.  The "nccl" transport and the head-wise
+        engine take the n rounds one by one."""
         eng = self.networks.engine(batch_size)
-        _, world = self._world()
-        if self.networks.route.engine != "mlp" or world > 1:
-            return [self.local_update(buffer.sample_batch(batch_size), iteration + k) for k in range(n)]
-        return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, list(zip(STAT_KEYS, range(14))))
+        dist, world = self._world()
+        keys = list(zip(STAT_KEYS, range(14)))
+        if self.networks.route.engine != "mlp":
+            return self._rounds(buffer, batch_size, iteration, n)
+        if world == 1:
+            return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, keys)
+        if not self._peers(eng, dist):
+            return self._rounds(buffer, batch_size, iteration, n)
+        return replay_updates_on_engine(eng, buffer, batch_size, iteration, n, self._noise, keys,
+                                        global_batch=batch_size * world)
+
+    def _rounds(self, buffer, batch_size: int, iteration: int, n: int) -> list:
+        return [self.local_update(buffer.sample_batch(batch_size), iteration + k) for k in range(n)]
 
     def get_remote_update_info(self, data: Dict, iteration: int) -> Tuple[dict, dict]:
         t0 = time.time()

@@ -228,6 +228,9 @@ class LazyStatsRow(Mapping):
     def _materialise(self) -> dict:
         if self._vals is None:
             row = self._block.get()[self._k]
+            if row[14] != 0.0:   # include/dsact.h: tb_info slot 14 = 1 + rank of a peer that never arrived
+                from dsac_v2_b200._lib import DsactError
+                raise DsactError(f"data-parallel exchange timed out waiting for rank {int(row[14]) - 1}")
             vals = {tag: row[c] for tag, c in self._keys}
             vals[TB_TAGS["alg_time"]] = self._alg_ms
             self._vals, self._block = vals, None
@@ -243,9 +246,10 @@ class LazyStatsRow(Mapping):
         return len(self._keys) + 1
 
 
-def replay_updates_on_engine(eng, buffer, batch: int, iteration: int, n: int, noise_fn, keys) -> list:
-    """replay_updates on the MLP engine: the host draws of n rounds, one Engine.replay_steps call, one lazy tb_info
-    mapping per update (`keys`: (tag, column of the 16 statistics) pairs)."""
+def replay_updates_on_engine(eng, buffer, batch: int, iteration: int, n: int, noise_fn, keys, global_batch=None) -> list:
+    """replay_updates on the MLP engine: the host draws of n rounds, one Engine.replay_steps call (with `global_batch`:
+    one Engine.dp_replay_steps call over that many rows of every rank), one lazy tb_info mapping per update (`keys`: (tag,
+    column of the 16 statistics) pairs)."""
     t0 = time.time()
     if buffer.engine is not eng:
         raise ValueError("the replay buffer is not attached to this algorithm's engine")
@@ -253,7 +257,10 @@ def replay_updates_on_engine(eng, buffer, batch: int, iteration: int, n: int, no
         raise ValueError("cannot sample from an empty replay buffer")
     buffer.flush()
     idx, noise = host_draws(buffer, batch, n, noise_fn)
-    stats = eng.replay_steps(n, batch, buffer.size, iteration, idx=idx, noise=noise)
+    if global_batch is None:
+        stats = eng.replay_steps(n, batch, buffer.size, iteration, idx=idx, noise=noise)
+    else:
+        stats = eng.dp_replay_steps(n, batch, buffer.size, iteration, global_batch, idx=idx, noise=noise)
     block = LazyStatsRow.Block(stats)
     alg_ms = (time.time() - t0) * 1000 / n
     return [LazyStatsRow(block, k, keys, alg_ms) for k in range(n)]

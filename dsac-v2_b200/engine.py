@@ -497,6 +497,10 @@ class Engine:
         `idx`: None (device draws) or int64 [n, batch]; `noise`: None or (eps1, eps2 [n, batch, A], z3, z4 [n, batch]).
         Returns the [n, 16] device tensor of per-update tb_info rows (valid until the next call with the same n), or None
         with stats=False."""
+        return self._replay_steps("dsact_replay_steps", n, batch, size, iteration, idx, noise, stats)
+
+    def _replay_steps(self, fn: str, n: int, batch: int, size: int, iteration: int, idx, noise, stats: bool, dp_args=()):
+        """replay_steps through entry point `fn`, whose `dp_args` follow the noise."""
         n, B, A = int(n), int(batch), self.cfg.act_dim
         with torch.cuda.device(self.device):
             if idx is not None:
@@ -517,8 +521,8 @@ class Engine:
                     outs[n] = torch.zeros(n, _lib.NUM_STATS, dtype=torch.float32, device=self.device)
                 out = outs[n]
             self._keep_idx = idx
-            check(self.lib.dsact_replay_steps(self.h, n, B, int(size), _ptr(idx), nz, _ptr(out), int(iteration),
-                                              self._stream()))
+            check(getattr(self.lib, fn)(self.h, n, B, int(size), _ptr(idx), nz, *dp_args, _ptr(out), int(iteration),
+                                        self._stream()))
         self.last_batch = B
         return out
 
@@ -547,6 +551,14 @@ class Engine:
     def dp_replay_step(self, batch: int, size: int, iteration: int, global_batch: int, idx: Optional[torch.Tensor] = None,
                        noise=None):
         self._update("dsact_dp_replay_step", noise=noise, replay=(batch, size, idx), args=(int(global_batch), int(iteration)))
+
+    def dp_replay_steps(self, n: int, batch: int, size: int, iteration: int, global_batch: int,
+                        idx: Optional[torch.Tensor] = None, noise=None, stats: bool = True) -> Optional[torch.Tensor]:
+        """n dp_replay_step calls in one submission (dsact_dp_replay_steps): replay_steps with every update's exchanges
+        over the peers, over `global_batch` rows.  The same `idx` / `noise` layouts, staging buffers and [n, 16] return
+        as replay_steps; row k's statistics are over `global_batch` rows, slot 14 the peer-timeout flag."""
+        return self._replay_steps("dsact_dp_replay_steps", n, batch, size, iteration, idx, noise, stats,
+                                  dp_args=(int(global_batch),))
 
     # ---- weights in the reference's state_dict schema -----------------------------------
     def _schema(self):

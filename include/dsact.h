@@ -274,7 +274,8 @@ int dsact_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int64_
  * iteration .. iteration+n_steps-1, each drawing from the ring of `size` rows, with the same generator counters, delayed-
  * update phases and resulting device state as the n single calls (the off_idx slot holds the last update's indices,
  * dsact_read_stats returns the last update's statistics).  The gather of update k+1 runs beside update k's backward, into
- * a second minibatch input set the library allocates on the first call (for max_batch rows; freed by dsact_destroy).
+ * a second minibatch input set the library allocates on the first call, or in dsact_dp_connect (for max_batch rows; freed
+ * by dsact_destroy).
  *   idx:       NULL (each update draws its own indices on the device) or device int64 [n_steps, batch].
  *   noise:     NULL (device draws) or arrays with a leading n_steps dimension: eps1/eps2 [n_steps, batch, act_dim],
  *              z3/z4 [n_steps, batch].
@@ -297,7 +298,7 @@ int dsact_replay_steps(dsact_handle *h, int32_t n_steps, int32_t batch, int64_t 
  * sums, the gradients and the logged sums reduced over all ranks inside the step's own kernels (rank-ordered sums: the
  * replicas stay bit-identical).  `global_batch` = sum of the ranks' batch sizes.  A peer that never arrives makes
  * tb_info slot 14 non-zero (1 + its rank) after DSACT_DP_TIMEOUT_MS (default 10 s) instead of hanging the GPU.
- * MLP-engine handles with policy_std != DSACT_STD_SHARED return DSACT_EINVAL from all four calls (reduce between the split
+ * MLP-engine handles with policy_std != DSACT_STD_SHARED return DSACT_EINVAL from all five calls (reduce between the split
  * calls dsact_grad_phase1/2 and dsact_apply instead). */
 #define DSACT_IPC_HANDLE_BYTES 64
 #define DSACT_DP_MAX_RANKS 8
@@ -307,6 +308,17 @@ int dsact_dp_step(dsact_handle *h, const dsact_batch *batch, const dsact_noise *
                   int64_t iteration, void *stream);
 int dsact_dp_replay_step(dsact_handle *h, int32_t batch, int64_t size, const int64_t *idx, const dsact_noise *noise,
                          int64_t global_batch, int64_t iteration, void *stream);
+/* n_steps consecutive dsact_dp_replay_step calls in one submission: dsact_replay_steps with every update data-parallel.
+ * Updates for iterations iteration .. iteration+n_steps-1, each with its exchanges inside its kernels, in the order and
+ * with the exchange epochs, generator counters and device state of the n single calls.  idx and noise as in
+ * dsact_replay_steps ([n_steps, batch] and n_steps draws back to back; NULL: device draws, one generator counter per
+ * update).  stats_out: NULL or device float [n_steps, DSACT_NUM_STATS]; row k holds update k's finalised tb_info over
+ * `global_batch` rows, slot 14 included: what dsact_read_stats(h, global_batch, ...) returns after the k-th single call.
+ * Every rank must make the same call (n_steps, iteration, global_batch).  Refused as its siblings refuse: head-wise and
+ * DSAC_V1 handles, policy_std != DSACT_STD_SHARED, no dsact_dp_connect (DSACT_ESTATE), n_steps outside
+ * [1, DSACT_MAX_REPLAY_STEPS], global_batch below batch. */
+int dsact_dp_replay_steps(dsact_handle *h, int32_t n_steps, int32_t batch, int64_t size, const int64_t *idx,
+                          const dsact_noise *noise, int64_t global_batch, float *stats_out, int64_t iteration, void *stream);
 
 /* ---- DSAC_V1 on the MLP engine ---------------------------------------------------------------------------------------
  * DSAC_V1 (reference dsac_v1.py:56-273: ONE distributional critic, fixed TD bound) with MLP approximators and the policy's
@@ -342,7 +354,7 @@ int dsact_v1_create(const dsact_config *cfg, const dsact_v1_options *v1, int dev
  * the "mlp_shared" policy also runs on the MLP engine (dsact_v1_create above), with its tensor-core modes, captured steps,
  * host staging and replay-fused steps.
  * dsact_cnn_create returns a dsact_handle that every dsact_* entry point above takes, with the same semantics, except:
- *  - dsact_step_host, dsact_stage_host / _release, dsact_replay_step, dsact_dp_replay_step, dsact_profile_step and
+ *  - dsact_step_host, dsact_stage_host / _release, dsact_replay_step(s), dsact_dp_replay_step(s), dsact_profile_step and
  *    dsact_test_gemm / dsact_test_chain return DSACT_EINVAL (the MLP engine implements them);
  *  - a DSAC_V1 handle (algo = 1) returns DSACT_EINVAL from the split and data-parallel calls (dsact_grad_phase1/2,
  *    dsact_compute_grads, dsact_apply, dsact_dp_export / _connect / _step);
